@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- the hot path of BASELINE.json measured on B200.
+"""bench.py -- the hot path of BASELINE.json measured on an H100.
 
 Workload (config 2 of BASELINE.json, the one the metric is quoted on):
   Bayesian logistic regression, synthetic X[1e6, 32] fp32, 64 vectorised particles, Trace_ELBO,
@@ -7,7 +7,8 @@ Workload (config 2 of BASELINE.json, the one the metric is quoted on):
   (guide sampling, model, fused scoring, backward, fused optimiser, loss read-back).
 
     python bench.py --gpus N --steps K --warmup W          # our arm  (torchrun for N > 1)
-    python bench.py --impl reference ...                   # reference arm: UNMODIFIED Pyro (baseline/_ref) on the host cores
+    python bench.py --impl reference ...                   # reference arm: UNMODIFIED Pyro (oracle/_ref) on the host cores
+    python bench.py ... --dump-outputs DIR                 # also write the last timed step's results as DIR/*.npy
 
 One JSON line on stdout (rank 0).  Keys follow the driver contract; extra keys:
   roofline      dominant kernel of the measured path: algorithmic bytes per launch / its average
@@ -44,7 +45,7 @@ def peaks():
         with open(path) as f:
             p = json.load(f)
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 def make_data(device, dtype=torch.float32, n=N_ROWS, seed=0):
@@ -124,7 +125,7 @@ def bind_near_gpu(index):
 def build_svi(path, particles, lr=0.01, sharded=False):
     """Every path runs the SAME, unchanged model (tests/models.py::logistic_model is the reference's
     tests/infer/mcmc/test_hmc.py:189-198 with `w.squeeze(-2) @ X.T + b`).  "glm": latent values reach the
-    model as lazy-aware tensors, so the likelihood site is scored by the fused tcgen05 kernel
+    model as lazy-aware tensors, so the likelihood site is scored by the fused wgmma kernel
     (pyro_b200/lazy.py); "site": that mechanism is switched off and the [P, N] logits are materialised
     (cuBLAS) and scored by the per-site kernel."""
     import models
@@ -196,6 +197,22 @@ def time_steps(svi, args, steps, warmup, device, flush, sync_each=True):
     return ms, loss
 
 
+def dump_outputs(out_dir, loss):
+    """The results of the last timed step: its loss (float64) and the guide parameters it updated
+    (constrained values, float32), one ``<name>.npy`` each (a few hundred bytes in all).  Inputs are seeded,
+    so two builds run with the same arguments can be compared file by file."""
+    import numpy as np
+    import pyro_b200 as pyro
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray(float(loss), dtype=np.float64))
+    store = pyro.get_param_store()
+    for name in store.keys():
+        v = store[name]
+        if hasattr(v, "dense"):       # positive parameters are handed out as a deferred exp(u)
+            v = v.dense()
+        np.save(os.path.join(out_dir, name + ".npy"), v.detach().float().cpu().numpy())
+
+
 def kernel_time_ms(fn, iters, flush):
     """Average device time of one launch sequence ``fn``: CUDA events on the launching stream
     around a replay of the sequence captured in a CUDA graph (so the Python wrapper cost of the
@@ -245,7 +262,7 @@ def roofline_for(path, X, y, particles, flush):
         name = "site_vec_kernel<BernoulliLogits,float,GRAD>"
     ach = alg / (ms * 1e-3) / 1e9
     traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")  # dram read+write per launch, from ncu --set full
+    tpath = os.path.join(ROOT, "profiles", "traffic.json")  # optional: DRAM read+write bytes per launch by kernel
     if os.path.exists(tpath):
         with open(tpath) as f:
             traffic = json.load(f).get(name.split(" ")[0].split("<")[0])
@@ -253,10 +270,10 @@ def roofline_for(path, X, y, particles, flush):
            "frac": round(ach / peak, 4), "traffic": traffic, "ms_per_launch": round(ms, 4),
            "algorithmic_bytes": alg, "peak_source": how}
     if "glm" in path:
-        # this kernel is not HBM-bound: 3 SFU ops per (row, particle) at 16/clk/SM, and the K = 8 TF32
-        # tcgen05 instructions are bound by their shared-memory operand fetch (profiles/glm_tc_r2.md)
-        sfu_us = 3.0 * n * P / (148 * 16 * 1.965e9) * 1e6
-        out["note"] = ("tcgen05/TMA kernel, shared-memory/tensor-pipe bound (ncu: tensor pipe active 89 %%): "
+        # this kernel is not HBM-bound: 3 SFU ops per (row, particle) at 16/clk/SM (H100 SXM: 132 SMs,
+        # 1.98 GHz maximum SM clock)
+        sfu_us = 3.0 * n * P / (132 * 16 * 1.98e9) * 1e6
+        out["note"] = ("wgmma/TMA kernel: "
                        "MUFU floor %.0f us, HBM floor %.0f us, measured %.0f us incl. the finish kernel; "
                        "4*N*D*P = %.1f GFLOP nominal (x2 for the W hi+lo split) = %.0f TFLOP/s nominal"
                        % (sfu_us, alg / peak / 1e3, ms * 1e3, 4.0 * n * D_FEAT * P / 1e9,
@@ -265,19 +282,19 @@ def roofline_for(path, X, y, particles, flush):
 
 
 class _RefPyroSVI:
-    """UNMODIFIED reference Pyro (pyro 1.9.1, pip-installed from /root/reference into baseline/_ref by
-    __graft_entry__.build(), plus the stand-in for its absent opt_einsum dependency) running the same
+    """UNMODIFIED reference Pyro (pyro 1.9.1, copied into oracle/_ref by __graft_entry__.build() through
+    oracle/build_ref.py, plus the stand-in for its absent opt_einsum dependency) running the same
     workload through its own public API on CPU tensors: pyro.infer.SVI / Trace_ELBO(num_particles=64,
     vectorize_particles=True) / pyro.optim.ClippedAdam.  None of this repo's kernels is involved."""
 
     def __init__(self):
         from pyro_b200 import bind
         if not bind.add_reference_to_path():
-            raise RuntimeError("baseline/_ref is missing")
+            raise RuntimeError("oracle/_ref is missing")
         import pyro
         import pyro.distributions as dist
         from torch.distributions import constraints
-        assert "baseline" in pyro.__file__ and pyro.__version__.startswith("1.9")
+        assert "_ref" in pyro.__file__ and pyro.__version__.startswith("1.9")
         pyro.clear_param_store()
 
         def model(X, y):
@@ -307,7 +324,7 @@ class _RefPyroSVI:
 
 
 def _ref_pyro_nuts(y, sigma, warmup=100, samples=100):
-    """eight_schools through UNMODIFIED reference Pyro (baseline/_ref): pyro.infer.MCMC(pyro.infer.NUTS(model)),
+    """eight_schools through UNMODIFIED reference Pyro (oracle/_ref): pyro.infer.MCMC(pyro.infer.NUTS(model)),
     one chain on the host; leapfrogs counted at pyro.ops.integrator.potential_grad (one call per leapfrog,
     pyro/ops/integrator.py:45-65).  None when the reference is not importable."""
     try:
@@ -317,7 +334,7 @@ def _ref_pyro_nuts(y, sigma, warmup=100, samples=100):
         import pyro
         import pyro.distributions as dist
         import pyro.ops.integrator as integ
-        assert "baseline" in pyro.__file__
+        assert "_ref" in pyro.__file__
     except Exception:  # noqa: BLE001
         return None
 
@@ -474,9 +491,7 @@ def nuts_section(dev, quick=False):
     chain.run(torch.zeros(10, dtype=torch.float64), 100, 100)
     dt = time.perf_counter() - t0
     out["cpu_baseline"] = {"leapfrog_per_sec": round(chain.num_leapfrogs / dt, 1), "cores": 1, "kind": "port",
-                           "sample": "eight_schools, 1 chain, 100 warm-up + 100 samples, oracle/mcmc.py NUTSChain "
-                                     "(reference Pyro itself measured 522-541 leapfrog/s in the build container, "
-                                     "tests/golden/make_golden.py)"}
+                           "sample": "eight_schools, 1 chain, 100 warm-up + 100 samples, oracle/mcmc.py NUTSChain"}
     torch.set_num_threads(os.cpu_count())
     return out
 
@@ -532,7 +547,7 @@ def nuts_multirank(dev, rank, world):
 
 
 def config3_section(dev):
-    """BASELINE config 3: GaussianHMM SVI step, H = 512, O = 4, T = 10 000, one B200 (structure of
+    """BASELINE config 3: GaussianHMM SVI step, H = 512, O = 4, T = 10 000, one GPU (structure of
     profiler/gaussianhmm.py:12-56): learnable parameters for the five parts, empty guide, Trace_ELBO,
     ClippedAdam.  The contraction runs on library GEMMs (cuBLAS / cuSOLVER through torch) -- see DESIGN.md."""
     from torch.distributions import constraints
@@ -638,6 +653,9 @@ def main():
     ap.add_argument("--cpu-steps", type=int, default=4)
     ap.add_argument("--no-nuts", action="store_true")
     ap.add_argument("--no-configs", action="store_true", help="skip the config 3 / config 5 sections")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (loss) and updated (the guide parameters) "
+                         "as DIR/<name>.npy")
     a = ap.parse_args()
     a.warmup = max(a.warmup, 3)
     rank = int(os.environ.get("RANK", "0"))
@@ -647,10 +665,10 @@ def main():
     if a.impl == "reference":
         if rank != 0:
             return
-        steps = min(a.steps, 20)
+        steps = a.steps
         v, ms, threads, loss = cpu_reference(steps, min(a.warmup, 2))
         kind = cpu_reference.kind
-        what = ("pyro.infer.SVI.step of unmodified Pyro (baseline/_ref)" if kind == "reference"
+        what = ("pyro.infer.SVI.step of unmodified Pyro (oracle/_ref)" if kind == "reference"
                 else "oracle/svi.py LogisticSVIMatmul")
         out = {"impl": "reference", "metric": METRIC, "value": round(v, 4), "unit": UNIT, "n_gpus": a.gpus,
                "steps": steps, "warmup": min(a.warmup, 2), "ms_per_step": round(ms, 3),
@@ -682,7 +700,7 @@ def main():
     torch.manual_seed(1234)
     P_local = PARTICLES
     X, y = make_data(dev)
-    flush = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device=dev)  # 256 MB > 126 MB L2
+    flush = torch.empty(64 * 1024 * 1024, dtype=torch.float32, device=dev)  # 256 MB > 50 MB L2
     path = a.path
     sharded = world > 1
     step_args = (X, y)
@@ -710,6 +728,8 @@ def main():
         time.sleep(0.15)
     ms, loss = time_steps(svi, step_args, a.steps, a.warmup + 2, dev, flush)
     torch.cuda.synchronize(dev)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, loss)
     if world > 1:
         dist.barrier()
     total_ms = torch.tensor([sum(ms)], device=dev, dtype=torch.float64)
@@ -810,14 +830,14 @@ def main():
            "config": {"workload": WORKLOAD, "global_particles": PARTICLES,
                       "model": "tests/models.py::logistic_model -- the reference model unchanged "
                                "(w.squeeze(-2) @ X.T + b -> Bernoulli(logits)); no repo-specific API in the model",
-                      "precision": "fp32 storage and accumulation; the two contractions run on tcgen05 tensor cores "
+                      "precision": "fp32 storage and accumulation; the two contractions run on wgmma tensor cores "
                                    "with TF32 operands, W split hi+lo (removes the row-coherent rounding error): "
                                    "sum / dW / db within 2e-5 / 2e-4 of fp64 (tests/test_gpu_tier2.py, N=1e6)",
                       "parallelism": ("data plate (rows) sharded over %d ranks, same particles on every rank, "
                                       "1 all-reduce of [loss, grads] (67 floats) per step between two "
                                       "CUDA graphs" % world) if world > 1 else "single GPU",
                       "path": path, "l2": "256 MB flush write between timed steps (outside the timed interval); "
-                                          "inputs 132 MB > 126 MB L2",
+                                          "inputs 132 MB > 50 MB L2",
                       "timing": "per-step CUDA events on the launching stream around SVI.step_async (loss stays on the device; "
                                 "no host wait inside the loop), summed; max over ranks"},
            "final_loss": round(float(loss), 3),
@@ -859,7 +879,7 @@ def main():
         out["cpu_baseline"] = {"value": round(v, 4), "unit": UNIT, "cores": threads, "kind": cpu_reference.kind,
                                "sample": "%d full-size steps (N=1e6, P=64) of %s, torch CPU ops, the fastest of "
                                          "several host thread counts" % (
-                                             a.cpu_steps, "pyro.infer.SVI.step of unmodified Pyro (baseline/_ref)"
+                                             a.cpu_steps, "pyro.infer.SVI.step of unmodified Pyro (oracle/_ref)"
                                              if cpu_reference.kind == "reference" else "oracle/svi.py LogisticSVIMatmul"),
                                "ms_per_step": round(cms, 2)}
         if not a.no_nuts:

@@ -1,4 +1,4 @@
-"""BASELINE config 3 (GaussianHMM, H = 512 hidden dims, O = 4, T = 10 000, SVI on one B200):
+"""BASELINE config 3 (GaussianHMM, H = 512 hidden dims, O = 4, T = 10 000, SVI on one GPU):
 `SVI.step` with learnable parameters for the five parts, empty guide, Trace_ELBO, ClippedAdam
 (structure of profiler/gaussianhmm.py:12-56 and pyro/contrib/timeseries/lgssm.py:72-95), plus the bare
 log_prob forward / forward+backward.  The steady-state path (time-invariant parameters: covariance

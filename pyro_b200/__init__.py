@@ -1,7 +1,7 @@
-"""pyro_b200 -- B200-native numerics behind Pyro's two hot paths.
+"""pyro_b200 -- native CUDA numerics behind Pyro's two hot paths, for the H100.
 
 The Trace_ELBO SVI step and the NUTS/HMC leapfrog of pyro-ppl/pyro 1.9.1, re-built on
-hand-written sm_100a CUDA kernels behind a C ABI (include/pyro_b200.h).  The Python here is the
+hand-written sm_90a CUDA kernels behind a C ABI (include/pyro_b200.h).  The Python here is the
 host-side mirror of the reference's interface for those paths (same names, arguments and error
 behaviour: ``sample/param/plate``, ``poutine``, ``distributions``, ``infer.SVI/Trace_ELBO/MCMC/NUTS``,
 ``optim.ClippedAdam``), so model and guide code written for Pyro runs unchanged with

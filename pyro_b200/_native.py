@@ -147,7 +147,7 @@ def lib():
                     raise RuntimeError(
                         "pyro_b200: native library %s is missing. Build it with "
                         "`python -c 'import __graft_entry__ as g; g.build()'` "
-                        "(nvcc, sm_100a). There is no CPU fallback." % LIB_PATH)
+                        "(nvcc, sm_90a). There is no CPU fallback." % LIB_PATH)
                 L = ctypes.CDLL(LIB_PATH)
                 for name, (res, args) in SIGNATURES.items():
                     fn = getattr(L, name)
@@ -178,7 +178,7 @@ _DTYPES = {torch.float32: B2_F32, torch.float64: B2_F64, torch.int64: B2_I64, to
 def require_cuda(t, what):
     if not t.is_cuda:
         raise RuntimeError(
-            "pyro_b200: %s needs CUDA tensors (got device %s). The B200 backend has no CPU "
+            "pyro_b200: %s needs CUDA tensors (got device %s). The CUDA backend has no CPU "
             "path; move the inputs to the GPU." % (what, t.device))
 
 

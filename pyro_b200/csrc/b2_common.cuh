@@ -10,7 +10,7 @@
 namespace b2 {
 
 constexpr int kMaxD = 6;          // dims kept after host-side coalescing
-constexpr int kNumSMs = 148;      // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;      // H100 SXM
 constexpr int kMaxRed = 8;        // reduction slots per launch (sum, dvalue, dparams[4], spare)
 constexpr int kMaxPartialBlocks = 8192;
 

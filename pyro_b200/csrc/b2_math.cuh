@@ -114,8 +114,7 @@ B2_HD T digamma(T x) {
 // ---- fp32 device fast paths -------------------------------------------------------------------
 // On the device, fp32 kernels use the SFU approximations (MUFU.EX2 / LG2 / RCP: ~2 ulp) instead
 // of the libm-accurate expf / log1pf / IEEE division, whose ~50 instructions per element made the
-// HBM-bound kernels issue-bound (measured: Bernoulli site kernel 22% of HBM peak before, see
-// profiles/).  Absolute error of each result stays below 4e-7, inside the stated fp32 tolerance
+// HBM-bound kernels issue-bound.  Absolute error of each result stays below 4e-7, inside the stated fp32 tolerance
 // |d| <= 1e-5 * max(1, |lp|).  fp64 and the host build keep the accurate functions.
 B2_HD float fast_exp(float x) {
 #ifdef __CUDA_ARCH__
@@ -169,9 +168,8 @@ B2_HD double fast_log1p_unit(double e) { return log1p(e); }
 // Stirling / asymptotic series at x >= 4 (truncation below 7e-8 there).  The shift is closed form:
 //   p = x(x+3),  (x)(x+1)(x+2)(x+3) = p(p+2),   sum_{i<4} 1/(x+i) = (2x+3)(2p+2) / (p(p+2))
 // so lgamma + digamma cost two logs and two reciprocals in total (libm's lgammaf alone is ~100
-// instructions and made the Gamma/Beta/Poisson kernels issue-bound at 10-25% of HBM peak,
-// profiles/micro_logprob_r1_before_fastgamma.txt; a per-unit shift loop to x >= 8 still left Gamma at
-// 44%).  Absolute error ~1e-6 for lgamma, relative ~1e-6 for digamma / trigamma: inside the fp32
+// instructions and made the Gamma/Beta/Poisson kernels issue-bound; a per-unit shift loop to x >= 8
+// costs more instructions than the closed form).  Absolute error ~1e-6 for lgamma, relative ~1e-6 for digamma / trigamma: inside the fp32
 // tolerance.  Non-positive arguments (never produced by valid parameters) take the accurate route.
 // The accurate route is OUT OF LINE on purpose: inlined into the 16-element unrolled loop bodies of the vector
 // kernels it made them 6-18 k instructions (Beta: 259 KB of SASS, far beyond the instruction cache) although it
@@ -567,7 +565,7 @@ struct ValueAux {
 
 // log(k!) and digamma(k + 1) for k = 0..63, correctly rounded: Poisson observations are small counts, and a
 // cached 512-byte gather replaces the two logarithms, the reciprocal and ~25 FMA-pipe instructions of the
-// series per element (the Poisson kernel sat at 41 % of the HBM peak, issue-bound).
+// series per element (the Poisson kernel is otherwise issue-bound).
 #if defined(__CUDACC__)
 static __device__ const float kLogFactorialF32[64] = {0.0f, 0.0f, 0.693147181f, 1.79175947f, 3.17805383f, 4.78749174f, 6.57925121f, 8.52516136f, 10.6046029f, 12.8018275f, 15.1044126f, 17.5023078f, 19.9872145f, 22.5521639f, 25.1912212f, 27.8992714f, 30.6718601f, 33.5050735f, 36.3954452f, 39.3398842f, 42.3356165f, 45.3801389f, 48.4711814f, 51.6066756f, 54.7847294f, 58.0036052f, 61.2617018f, 64.5575386f, 67.8897431f, 71.257039f, 74.6582363f, 78.0922236f, 81.5579595f, 85.054467f, 88.5808275f, 92.1361756f, 95.7196945f, 99.3306125f, 102.968199f, 106.63176f, 110.32064f, 114.034212f, 117.771881f, 121.533082f, 125.317271f, 129.123934f, 132.952575f, 136.802723f, 140.673924f, 144.565744f, 148.477767f, 152.409593f, 156.360836f, 160.331128f, 164.320112f, 168.327445f, 172.352797f, 176.395848f, 180.456291f, 184.533829f, 188.628173f, 192.739047f, 196.866182f, 201.009316f};
 static __device__ const float kDigammaIntF32[64] = {-0.577215665f, 0.422784335f, 0.922784335f, 1.25611767f, 1.50611767f, 1.70611767f, 1.87278434f, 2.01564148f, 2.14064148f, 2.25175259f, 2.35175259f, 2.44266168f, 2.52599501f, 2.60291809f, 2.67434666f, 2.74101333f, 2.80351333f, 2.86233686f, 2.91789241f, 2.97052399f, 3.02052399f, 3.06814304f, 3.11359759f, 3.15707585f, 3.19874251f, 3.23874251f, 3.27720405f, 3.31424109f, 3.34995537f, 3.38443813f, 3.41777147f, 3.45002953f, 3.48127953f, 3.51158256f, 3.54099433f, 3.56956575f, 3.59734353f, 3.62437056f, 3.65068635f, 3.67632737f, 3.70132737f, 3.72571762f, 3.74952714f, 3.77278296f, 3.79551023f, 3.81773245f, 3.83947158f, 3.86074818f, 3.88158151f, 3.90198967f, 3.92198967f, 3.94159752f, 3.96082829f, 3.97969621f, 3.99821473f, 4.01639655f, 4.03425369f, 4.05179755f, 4.06903893f, 4.08598808f, 4.10265475f, 4.11904819f, 4.13517722f, 4.15105024f};

@@ -194,8 +194,7 @@ __global__ void __launch_bounds__(256) categorical_kernel(const EventArgs a) {
 // A row is K consecutive elements per operand, so a warp covers 32 consecutive rows = one contiguous
 // span of memory: every fetched line is fully used (through L1 across the k loop), the K special
 // functions of a row are independent work for one thread (ILP without shuffles), and there is no
-// per-row integer division.  The sub-warp-group kernels above measured 7-12% of the HBM peak at
-// K = 8 (profiles/micro_logprob_r1.txt).
+// per-row integer division; the sub-warp-group kernels above waste most of their lanes at small K.
 template <typename T>
 B2_HD T xlogy_fast(T c, T x) {
   if (sizeof(T) == 4) return (c == (T)0) ? (T)0 : c * fast_log(x);
@@ -322,7 +321,7 @@ __global__ void __launch_bounds__(256) categorical_rowthread_kernel(const EventA
 // w = L^-T z for the gradients) live in NSLOT registers per lane: NSLOT = 4 covers n <= 128 (round 1),
 // NSLOT = 16 / 32 cover n <= 512 / 1024 (round 2: the MVN sizes of BASELINE config 3, H = 512).  The
 // per-pivot work is an O(n) dot product read straight from L (L2-resident when the factor is shared by
-// the batch), so the kernel is latency-bound, not a tensor-core GEMM; a blocked TRSM on tcgen05 only
+// the batch), so the kernel is latency-bound, not a tensor-core GEMM; a blocked TRSM on wgmma only
 // pays off for thousands of right-hand sides per factor, which no BASELINE config has. ----------
 constexpr int kMvnMaxN = 1024;
 template <typename T, bool GRAD, int NSLOT = 4>
@@ -439,9 +438,8 @@ __global__ void __launch_bounds__(256) mvn_tril_kernel(const EventArgs a) {
 // Lane j holds ROW j of the factor (Lr[k] = L[j][k]), so forward substitution is a chain of broadcasts:
 //   pivot i:  z_i = r_i / L_ii is final on lane i -> one shuffle -> every lane j > i does r_j -= L[j][i] z_i
 // i.e. ~35 cycles per pivot (shuffle + FMA) instead of the five dependent shuffle/add steps of a group
-// reduction per pivot, which is what a column-owning lane needs (mvn_warp32_kernel of round 1: ~6 us per 32x32
-// row, 16 warps resident -> 19 % of the HBM peak; the thread-per-row kernel for n <= 8 walked L with 4-byte
-// loads 4*n*n bytes apart across a warp and ran fully unrolled to 8 whatever n was: 26 % at n = 8).  Rows are read
+// reduction per pivot, which is what a column-owning lane needs (the thread-per-row kernel for n <= 8 walks L with
+// 4-byte loads 4*n*n bytes apart across a warp and runs fully unrolled to 8 whatever n is).  Rows are read
 // coalesced: G <= 8 as 16-byte (8-byte for G = 2) chunks of consecutive lanes, G = 32 as 32 row-major 128-byte
 // lines staged through a padded shared-memory tile and read back transposed.  The gradient pass needs the
 // columns as well (w = L^-T z is a broadcast chain for COLUMN owners); they come from the same tile / from L1.
@@ -642,7 +640,7 @@ __global__ void __launch_bounds__(256) reduce_to_kernel(const ReduceArgs a) {
 // Column reduction: the kept dims are the trailing, contiguous ones (dst[C] = sum over R rows of
 // src[R, C], row stride C) -- the gradient of a parameter that is broadcast over particles / chains.
 // Threads own columns (coalesced), grid.y splits the rows; fixed summation order.  The one-CTA-per-
-// output kernel above reads this layout with a 4*C-byte stride between lanes (75 us for [256, 61440]).
+// output kernel above reads this layout with a 4*C-byte stride between lanes.
 template <typename T>
 __global__ void __launch_bounds__(256) reduce_cols_kernel(const T* __restrict__ src, T* __restrict__ dst,
                                                           double* __restrict__ partials, int64_t R,
@@ -698,10 +696,8 @@ __global__ void reduce_to_finish_kernel(const ReduceArgs a) {
 // G = min(32, K/V/4) lanes own a row and each lane takes kChunks = 4 16-byte chunks per step, for two rows
 // (row, row + ngroups) at once: 8 independent 16-byte loads in flight per thread, and the per-row overhead --
 // the group reductions, the row's own special functions, offsets, the mask -- is spread over >= 16 elements per
-// lane.  History: scalar sub-warp groups measured 9-13 % of the HBM peak at K = 64 (round 1); one chunk per lane
-// (G = K/V lanes) 33-36 %: ncu showed that version ISSUE-bound, not memory-bound (issue slots 75-81 % busy at 51
-// (Categorical) / 91 (Dirichlet) instructions per element, most of them per-row work amortised over only 4
-// elements per lane) -- requesting the next rows early changed nothing (profiles/micro_logprob_r2.md).
+// lane.  With one chunk per lane (G = K/V lanes) the kernel is issue-bound, not memory-bound: most of its
+// instructions are per-row work amortised over only 4 elements per lane.
 constexpr int kChunks = 4;
 
 template <typename T, bool GRAD>
@@ -911,7 +907,7 @@ __global__ void __launch_bounds__(256) categorical_vec_kernel(const EventArgs a)
 
 // ---- MVN, event size n <= 8: one thread per row ------------------------------------------------------
 // The warp-per-row kernel above spends 32 lanes and n warp reductions on a 2x2 .. 8x8 triangular
-// solve (1.5-4% of the HBM peak, profiles/micro_logprob_r1.txt).  For small n the whole solve fits
+// solve.  For small n the whole solve fits
 // one thread's registers: z = L^-1 (x - mu) by forward substitution, w = L^-T z by back substitution,
 // all loops fully unrolled over NMAX with predicates on the runtime n; a warp covers 32 consecutive
 // rows, i.e. one contiguous span of each operand.
@@ -1117,7 +1113,7 @@ extern "C" int b2_event_score(int family, const b2_tensor* value, const b2_tenso
     if (family == B2_DIRICHLET) vec_rows_ok = vec_rows_ok && al(a.x.ptr, a.x.st[0]) && al(a.gx.ptr, a.gx.st[0]);
   }
   if (family == B2_MVN_TRIL && cd <= 1 && event_size <= 4 && nb >= 1024) {
-    // tiny events: one thread per row (measured at n = 2: 43 % of the HBM peak against 37 % for lane groups)
+    // tiny events: one thread per row (no group reductions at all)
     blocks = (nb + 255) / 256;
     if (blocks > cap * 2) blocks = cap * 2;
     if (dtype == B2_F32) {
@@ -1160,8 +1156,6 @@ extern "C" int b2_event_score(int family, const b2_tensor* value, const b2_tenso
   }
   else if (family != B2_MVN_TRIL && cd <= 1 && !rowthread && vec_rows_ok) {
     // lanes per row: the largest power of two <= K/V/4 (each lane takes 4 chunks per step), at most a warp
-    // (measured: doubling the lanes costs Categorical K = 64 53 -> 37 %, halving them gains Dirichlet K = 64
-    // 60 -> 64 % but costs Categorical 53 -> 51 %; profiles/micro_logprob_r2.md)
     int lgv = 0;
     const int V = (dtype == B2_F32) ? 4 : 2;
     while (lgv < 5 && (2 << lgv) <= event_size / V / 4) ++lgv;

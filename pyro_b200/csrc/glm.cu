@@ -135,7 +135,7 @@ __global__ void __launch_bounds__(256) glm_bernoulli_kernel(const float* __restr
 
 // second stage: fixed-order sum over the CTAs' partials; applies weight / scale.
 // One WARP per entry of the [P, D+2] table: lanes stride over the CTAs (L2-resident partials),
-// then a shuffle tree -- a thread-per-entry loop over ~300 dependent loads took 35 us.
+// then a shuffle tree (a thread-per-entry loop is a chain of ~300 dependent loads).
 __global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict__ partials,
                                                          int nblocks, int P, int D, double scale,
                                                          double weight, float* __restrict__ sum_p,
@@ -189,7 +189,7 @@ __global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict
 int glm_mma_grid_x(int64_t N);
 void launch_glm_mma(const float* X, const float* y, const float* W, const float* b, int64_t N, int P,
                     float* partials, int gx, cudaStream_t s);
-// tcgen05 + TMA variant (glm_tc.cu)
+// wgmma + TMA variant (glm_tc.cu)
 int glm_tc_grid_x(int64_t N);
 int launch_glm_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int P,
                   float* partials, int gx, int mode, cudaStream_t s);
@@ -236,7 +236,7 @@ extern "C" int b2_glm_bernoulli_logits(const float* X, const float* y, const flo
   float* partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
   if (use_tc) {
     // default: W split; below 64 Ki rows the incoherent X rounding has not averaged out yet -> full 3xTF32
-    // B2_FLAG_GLM_BF16_GRAD (opt-in): BF16 gradient contraction on MN-major operands (MODE 3)
+    // B2_FLAG_GLM_BF16_GRAD (opt-in): BF16 gradient contraction (MODE 3)
     const int mode = (flags & B2_FLAG_GLM_TF32) ? 0
                      : ((flags & B2_FLAG_GLM_BF16_GRAD) ? 3
                         : (((flags & B2_FLAG_GLM_3XTF32) || N < 65536) ? 2 : 1));

@@ -15,14 +15,12 @@
 // flash-attention uses between Q K^T and P V).  The B fragments of both GEMMs are read from the same
 // shared-memory X tile (row pitch 36 floats: both access patterns are bank-conflict free).
 //
-// Why mma.sync and not tcgen05 here: with K = D = 32 and N = P = 64 the contractions are ~40 us of
-// tensor work even on the legacy path, below the SFU floor of this kernel (3 MUFU per (row, particle)
-// = 43 us) and comparable to its HBM floor (20 us); a TMEM/tcgen05 pipeline would not move the
-// bound.  See DESIGN.md (kernel table) for the measured numbers.
+// This is the legacy tensor-core path (B2_FLAG_GLM_MMA_SYNC); the default for D == 32 is the
+// wgmma/TMA kernel of glm_tc.cu.  Both are bounded by the SFU work of the epilogue (3 MUFU per
+// (row, particle)) rather than by the contractions.
 //
 // Precision: TF32 operands (10-bit mantissa, round-to-nearest) perturb each logit by ~1e-3 relative;
-// the errors are unbiased and average out over the N-term sums (measured ELBO deviation < 1e-5
-// relative at N = 1e6).  The fp32 SIMT kernel in glm.cu stays available (flag B2_GLM_FP32).
+// the errors are unbiased and average out over the N-term sums.  The fp32 SIMT kernel in glm.cu stays available (flag B2_GLM_FP32).
 #include <cuda_pipeline.h>
 
 #include "b2_common.cuh"
@@ -37,7 +35,7 @@ constexpr int kMmaParticles = 64;                // particles per CTA (blockIdx.
 
 // fp32 -> tf32 with round-to-nearest (ties away), done with two integer ALU ops.  cvt.rna.tf32.f32
 // executes on the same 16-lane pipe as MUFU; at 3 conversions per (row, particle) it doubled the
-// load of the pipe that bounds this kernel (ncu: profiles/ncu_glm_mma_r1.txt).
+// load of the pipe that bounds this kernel.
 __device__ __forceinline__ uint32_t to_tf32(float x) {
   return (__float_as_uint(x) + 0x1000u) & 0xffffe000u;
 }

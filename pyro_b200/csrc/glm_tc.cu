@@ -1,5 +1,5 @@
-// glm_tc.cu -- Blackwell-native fused logistic-regression likelihood kernel (BASELINE config 2):
-// TMA tile loads, tcgen05.mma with TMEM accumulators, warp-specialised persistent CTAs.
+// glm_tc.cu -- Hopper fused logistic-regression likelihood kernel (BASELINE config 2):
+// TMA tile loads completing on mbarriers, wgmma with register accumulators, persistent CTAs.
 //
 // Same contract as glm_bernoulli_kernel (glm.cu): ONE pass over X[N,32] and y[N] gives, for up to 64
 // weight vectors (particles) per CTA slab, sum_n log Bernoulli(y_n | logits = x_n.w_p + b_p), dW and
@@ -7,48 +7,38 @@
 // torch/distributions/bernoulli.py:121-125 (log_prob), pyro/poutine/trace_struct.py:264-278 (.sum())
 // and the autograd backward of all three.
 //
-// Per 128-row tile (one persistent CTA per SM, tiles round-robin over CTAs):
+// Per 64-row tile (one persistent CTA per SM, tiles round-robin over CTAs, and inside a CTA round-robin
+// over its three warpgroups; each warpgroup owns a whole tile):
 //
-//   GEMM 1   D1[n, p] = sum_d X[n, d] W[p, d] + b[p]      M = 128 rows, N = 64 particles, K = 32
+//   split    the warpgroup rounds its X tile to nearest TF32 in place (MODE 2: X_hi / X_lo split) and
+//            writes the transposed X^T[d][n] (plus 8 rows of ones) as the K-major B operand of GEMM 2.
+//   GEMM 1   D1[n, p] = sum_d X[n, d] W[p, d] + b[p]      wgmma m64n64k8, K = 32, accumulator = bias.
 //            default (MODE 1): W split hi + lo, two TF32 MMAs per k-step -- the rounding of W is the only
 //            error of a TF32 GEMM 1 that is COHERENT over rows (it shifts all N logits of a particle the
-//            same way and survives the N-term sums); X is rounded to nearest in place (incoherent,
-//            averages as 1/sqrt(N)).  MODE 2 splits X as well (every logit exact to ~1e-6), MODE 0 is
-//            single-pass TF32.  fp32 accumulation in TMEM; the bias enters through one more MMA
-//            (A = ones, B = [b_hi, b_lo, 0...]).
-//   epilogue sixteen warps tcgen05.ld the 128 x 64 logits (thread = row, 16 particles each), evaluate
-//            lp = y*l - softplus(l), g = y - sigmoid(l) (3 MUFU + ~12 FMA-pipe ops per element, in
-//            batches of 8 so the MUFU latency is covered inside the warp), keep the per-particle lp sums
-//            in registers and store g^T (rounded to nearest TF32) into shared memory as the K-major A
-//            operand of GEMM 2.
-//   GEMM 2   [dW | db][p, :] += sum_n g[n, p] [X | 1][n, :]   M = 64, N = 40 (32 columns of X^T and 8 rows
-//            of ones), K = 128: single-pass TF32 on round-to-nearest operands (unbiased;
-//            |err| <= 2^-11 sum|g x|, measured 4e-6 relative at N = 1e6); one accumulator per 32-row
-//            k-block, summed once at the end of the kernel.
+//            same way and survives the N-term sums); X is rounded to nearest (incoherent, averages as
+//            1/sqrt(N)).  MODE 2 splits X as well (every logit exact to ~1e-6), MODE 0 is single-pass TF32.
+//   epilogue each thread holds 2 rows x 16 particles of D1 in registers, evaluates lp = y*l - softplus(l),
+//            g = y - sigmoid(l) (3 MUFU + ~12 FMA-pipe ops per element, in batches of 8 so the MUFU latency
+//            is covered inside the warp), keeps per-particle lp sums in registers and stores g^T (rounded to
+//            nearest TF32) into shared memory as the K-major A operand of GEMM 2.
+//   GEMM 2   [dW | db][p, :] += sum_n g[n, p] [X | 1][n, :]   wgmma m64n40k8, K = 64: single-pass TF32 on
+//            round-to-nearest operands (unbiased; |err| <= 2^-11 sum|g x|).  The accumulator stays in
+//            registers for the whole kernel; GEMM 2 of a tile runs while the warpgroup waits for its next
+//            tile, and the three warpgroups of a CTA overlap each other's phases.
+//            MODE 3 (B2_FLAG_GLM_BF16_GRAD, opt-in): GEMM 2 in BF16 (m64n40k16, half the MMAs).
 //
-// TF32 MN-major operands only exist in the 32-byte-atom swizzle, so instead of re-reading the X tile
-// in a second layout, four "split" warps transform each TMA tile once: RN-rounded X in place (plus X_lo
-// in MODE 2) for GEMM 1 and the transposed X^T[d, n] for GEMM 2.  All operand tiles are K-major
-// SWIZZLE_128B, the layout TMA writes natively.
+// TF32 wgmma operands must be K-major, so the split pass transposes X once per tile in shared memory.
+// Every operand tile is K-major SWIZZLE_128B (the layout TMA writes natively for the X tile).
 //
-// Warp roles (704 threads): warp 0 TMA producer, warp 1 MMA issuer + TMEM owner (the whole warp walks
-// the loop, one elected lane issues; the issue order of a batch is static so consecutive MMAs are 1-3
-// instructions apart), warps 2-17 epilogue (TMEM sub-partition = warp % 4), warps 18-21 split pass.
-// Pipelines (all mbarriers): TMA ring of 4 X stages, X^T/y ring of 3 stages, D1 double-buffered in TMEM
-// with GEMM 1 running TWO tiles ahead (it is issued interleaved with GEMM 2 of tile j as soon as the
-// epilogue of tile j is done), g^T double-buffered in shared memory.
+// 384 threads = three warpgroups and no producer warp: registers are allocated to groups of 4 warps, so a
+// 13th warp would cost the consumers 40 registers each.  Each warpgroup double-buffers its own X/y tiles:
+// one thread issues the TMA load of tile j+2 into the stage of tile j as soon as GEMM 1 has read it (an
+// mbarrier per stage counts the transaction bytes); g^T, X^T and X_lo are private to each warpgroup.
 //
-// What bounds it (B200, N = 1e6, P = 64; profiles/glm_tc_r2.md): 89 us.  An isolated tcgen05.mma of these
-// shapes costs (A bytes + B bytes) / 128 B per clock -- 51 cycles for 128x64x8, 28 for 64x40x8
-// (profiles/umma_bench.cu) -- i.e. the K = 8 TF32 instruction is bound by the shared-memory operand
-// fetch, and that same 128 B/clk port also carries the split pass, the g^T stores and the TMA writes:
-// ~200 KB of shared-memory traffic per 16 KB tile, >= 1600 cycles, against 1536 cycles of MUFU work.
-// ncu: tensor pipe active 89 %, issue slots 65 %, XU pipe 56 %, DRAM 1.0x the algorithmic bytes.
-//
-// Determinism: every CTA writes its partials once; glm_finish_kernel adds them in a fixed order.
+// Determinism: every CTA writes its partials once (warpgroups summed in a fixed order); glm_finish_kernel
+// adds the CTA partials in a fixed order.
 #include <cuda.h>
 #include <cuda_bf16.h>
-#include <cuda/std/type_traits>
 #include <stdlib.h>
 
 #include "b2_common.cuh"
@@ -56,77 +46,35 @@
 namespace b2 {
 namespace tc {
 
-constexpr int kRows = 128;
+constexpr int kRows = 64;                       // rows per tile = M of one wgmma
 constexpr int kD = 32;
 constexpr int kP = 64;
-constexpr int kMaxStagesT = 3;
-constexpr int kEpiWarp0 = 2, kEpiWarps = 16;       // 4 per SM sub-partition: latency hiding for the MUFU chains
-constexpr int kEpiCols = kP * 4 / kEpiWarps;        // particles (TMEM columns) per epilogue thread
-constexpr int kSplitWarp0 = kEpiWarp0 + kEpiWarps, kSplitWarps = 4;
-constexpr int kThreads = (kSplitWarp0 + kSplitWarps) * 32;
-constexpr int kMaxStagesX = 4;
+constexpr int kWG = 3;                          // warpgroups
+constexpr int kStages = 2 * kWG;                // two X/y stages per warpgroup
+constexpr int kThreads = kWG * 128;
 
-constexpr uint32_t kTile = kRows * kD * 4;                    // 16 KB
-constexpr uint32_t kXStage = kTile + 512;                     // bytes per TMA transaction: X tile + 128 y values
-constexpr uint32_t kGBuf = 4 * kP * 128;                      // g^T: [kb 4][p 64][32 n] fp32 = 32 KB
-constexpr uint32_t kXtBlock = (kD + 8) * 128;                 // X^T k-block: 32 rows of d + 8 rows of ones
-constexpr uint32_t kXtStage = 4 * kXtBlock;                   // 20 KB
+constexpr uint32_t kTile = kRows * kD * 4;      // 8 KB X tile
+constexpr uint32_t kYBytes = kRows * 4;         // 256 B of y
+constexpr uint32_t kXtBlock = (kD + 8) * 128;   // X^T k-block: 32 rows of d + 8 rows of ones, 32 n each (5 KB)
+constexpr uint32_t kGBlock = kP * 128;          // g^T k-block: 64 rows of p, 32 n each (8 KB)
 
-// MODE 0: single-pass TF32 logits.  MODE 1 (default): W split hi/lo -- the rounding error of W is the
-// only COHERENT error of a TF32 GEMM 1 (it is the same for all rows, so it does not average out over
-// the N-term sums); X is rounded to nearest in place (incoherent, averages as 1/sqrt(N)).
-// MODE 2: full 3xTF32 (X split as well): every logit exact to ~1e-6, at the price of a shallower TMA
-// ring (the X_lo tiles take the shared memory of two X stages).
-// MODE 3: logits as MODE 1; GEMM 2 in BF16 (kind::f16, K = 16 per instruction) on MN-major operands -- g and
-// X keep their natural [row][column] layout (no transposition pass, vector stores), half the bytes, half the
-// MMAs.  Operand rounding 2^-9 (round to nearest, unbiased): 3e-5 of the largest entry of dW at N = 1e6 for
-// generic W, but a noise floor of ~1e-3 sqrt(N) that matters when the gradient itself is O(sqrt(N)); opt-in
-// (B2_FLAG_GLM_BF16_GRAD), 90 us instead of 100 us.
-template <int MODE>
-struct Layout {
-  static constexpr bool kBf16 = (MODE == 3);
-  static constexpr int kStagesX = (MODE == 2) ? 2 : 4;             // TMA ring: X tile (hi in place) + y
-  static constexpr int kStagesL = (MODE == 2) ? 2 : 0;             // X_lo ring
-  static constexpr int kStagesT = 3;                               // GEMM 2 B-operand (+ y) ring: split pass -> GEMM 2
-                                                                   // (>= 3: GEMM 1 runs two tiles ahead)
-  static constexpr uint32_t kXtStage = kBf16 ? kTile : b2::tc::kXtStage;   // bf16 [128 n][64 cols] = 16 KB
-  static constexpr uint32_t kGBuf = kBf16 ? kTile : b2::tc::kGBuf;         // bf16 [128 n][64 p]   = 16 KB
-  static constexpr uint32_t OFF_X = 0;
-  static constexpr uint32_t OFF_XLO = OFF_X + kStagesX * kTile;
-  static constexpr uint32_t OFF_XT = OFF_XLO + kStagesL * kTile;   // [stage][kb 4][d 32 + 8 ones][32 n] fp32
-  static constexpr uint32_t OFF_G = OFF_XT + kStagesT * kXtStage;
-  // the g buffers double as the [128][65] fp32 scratch of the final reduction (33 280 bytes)
-  static constexpr uint32_t kGRegion = (2 * kGBuf > 34816u) ? 2 * kGBuf : 34816u;
-  static constexpr uint32_t OFF_WHI = OFF_G + kGRegion;           // [p 64][32 d] SW128, 8 KB
-  static constexpr uint32_t OFF_WLO = OFF_WHI + 8192;
-  static constexpr uint32_t OFF_WB = OFF_WLO + 8192;               // bias tile (k = 0: b_hi, k = 1: b_lo)
-  static constexpr uint32_t OFF_ONES = OFF_WB + 8192;              // 4 KB of 1.0f (no-swizzle operand)
-  static constexpr uint32_t OFF_Y = OFF_ONES + 4096;               // [stage T][128] fp32 (epilogue reads)
-  static constexpr uint32_t OFF_YX = OFF_Y + kStagesT * 512;       // [stage X][128] fp32 (TMA target)
-  static constexpr uint32_t OFF_BAR = OFF_YX + kStagesX * 512;
-  static constexpr uint32_t kSmemBytes = OFF_BAR + 256 + 1024;     // + slack for the 1024-byte alignment
-};
-static_assert(Layout<1>::kSmemBytes <= 232448 && Layout<2>::kSmemBytes <= 232448 &&
-                  Layout<3>::kSmemBytes <= 232448, "shared memory budget");
-
-// barrier slots (8 bytes each)
-enum : int {
-  BAR_XFULL = 0,                         // [kMaxStagesX] TMA landed
-  BAR_XREADY = BAR_XFULL + kMaxStagesX,  // [kMaxStagesX] split pass done
-  BAR_XEMPTY = BAR_XREADY + kMaxStagesX, // [kMaxStagesX] GEMM 1 finished reading the X tile
-  BAR_LEMPTY = BAR_XEMPTY + kMaxStagesX, // [2] GEMM 1 finished reading X_lo (MODE 2)
-  BAR_TEMPTY = BAR_LEMPTY + 2,           // [kStagesT] GEMM 2 finished reading X^T
-  BAR_D1FULL = BAR_TEMPTY + kMaxStagesT, // [2]
-  BAR_D1EMPTY = BAR_D1FULL + 2,          // [2]
-  BAR_GFULL = BAR_D1EMPTY + 2,           // [2]
-  BAR_GEMPTY = BAR_GFULL + 2,            // [2]
-  BAR_DONE = BAR_GEMPTY + 2,
-  BAR_COUNT
-};
-static_assert(BAR_COUNT * 8 + 8 <= 256, "barrier block overflow");
-
-constexpr uint32_t kTmemCols = 512;
-constexpr uint32_t kColD1 = 0, kColD2 = 128;   // D2[kb]: 40 columns each (32 of dW + 8 equal columns of db), kb = 0..3
+// per-warpgroup region
+constexpr uint32_t WG_G = 0;                        // g^T  [kb 2][p 64][32 n] fp32 (BF16: [p 64][64 n])
+constexpr uint32_t WG_XT = WG_G + 2 * kGBlock;      // X^T  [kb 2][c 40][32 n] fp32 (BF16: [c 40][64 n])
+constexpr uint32_t WG_XLO = WG_XT + 2 * kXtBlock;   // X_lo [n 64][32 d] fp32 (MODE 2)
+constexpr uint32_t kWGBytes = WG_XLO + kTile;
+// CTA layout (every operand region 1024-byte aligned: the 128-byte swizzle pattern is taken from address bits)
+constexpr uint32_t OFF_X = 0;
+constexpr uint32_t OFF_Y = OFF_X + kStages * kTile;
+constexpr uint32_t OFF_WHI = OFF_Y + 2048;          // [p 64][32 d] SW128, 8 KB
+constexpr uint32_t OFF_WLO = OFF_WHI + 8192;
+constexpr uint32_t OFF_WG = OFF_WLO + 8192;
+constexpr uint32_t OFF_BAR = OFF_WG + kWG * kWGBytes;
+constexpr uint32_t kSmemBytes = OFF_BAR + 256 + 1024;   // + slack for the 1024-byte alignment
+static_assert(kStages * kYBytes <= 2048 && kSmemBytes <= 232448, "shared memory budget");
+static_assert(kWGBytes % 1024 == 0 && kXtBlock % 1024 == 0, "operand alignment");
+// the final reduction reuses the X ring: [kWG][64 p][33] + [kWG * 4 warps][64 p] floats
+static_assert((kWG * kP * 33 + kWG * 4 * kP) * 4 <= kStages * kTile, "reduction scratch");
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);
@@ -134,33 +82,29 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
+// The retry loop lives inside the asm block: a C++ loop around try_wait is a divergent branch to ptxas, and
+// wgmma accumulators live across a divergent path make it serialise every wgmma of the kernel (C7520).
+// After 2^26 failed tries it traps: a protocol bug must not hang the device.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok = 0, spins = 0;
-  for (;;) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (ok) return;
-    if (++spins > (1u << 26)) __trap();   // a protocol bug must not hang the device
-  }
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t.reg .u32 n;\n\t"
+      "mov.u32 n, 0;\n"
+      "WAIT:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+      "@p bra.uni DONE;\n\t"
+      "add.u32 n, n, 1;\n\t"
+      "setp.lt.u32 p, n, 67108864;\n\t"
+      "@p bra.uni WAIT;\n\t"
+      "trap;\n"
+      "DONE:\n\t}"
+      ::"r"(bar), "r"(parity)
+      : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
   asm volatile(
@@ -174,57 +118,67 @@ __device__ __forceinline__ void tma_load_1d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(map), "r"(c0), "r"(bar)
       : "memory");
 }
-
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout): start address >> 4 in
-// [0,14), leading byte offset >> 4 in [16,30), stride byte offset >> 4 in [32,46), version 1 in
-// [46,48), layout type in [61,64) (0 = no swizzle, 2 = SWIZZLE_128B).
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo, uint32_t layout) {
-  return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo >> 4) & 0x3FFFu) << 16) |
-         ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32) | (1ull << 46) | ((uint64_t)layout << 61);
-}
-// K-major SWIZZLE_128B tile of 128-byte rows: 8-row groups are 1024 bytes apart
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) { return make_desc(saddr, 0, 1024, 2); }
-
-// instruction descriptor, kind::tf32, fp32 accumulate, both operands K-major
-__host__ __device__ constexpr uint32_t idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wg_bar(int id) {   // named barrier of one warpgroup (ids 1..kWG)
+  asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory");
 }
 
-// kind::f16 with BF16 operands (format code 1), both MN-major (bits 15 / 16), fp32 accumulate
-__host__ __device__ constexpr uint32_t idesc_bf16_mn(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
+// wgmma shared-memory matrix descriptor: start address >> 4 in [0,14), leading byte offset >> 4 in [16,30)
+// (unused for swizzled K-major operands), stride byte offset >> 4 in [32,46) (8-row groups are 1024 bytes
+// apart), layout type in [62,64) (1 = SWIZZLE_128B).  A k-step inside the 128-byte atom adds 32 bytes (+2).
+__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
+  return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void mma_bf16(uint32_t d_tmem, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from touching accumulator registers while an asynchronous wgmma owns them
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+
+// D[64 x 64] += A[64 x 8] B[64 x 8]^T, TF32, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_n64_tf32(float (&d)[32], uint64_t a, uint64_t b) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a), "l"(b), "r"(idesc), "r"(acc)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(1)
       : "memory");
 }
-
-__device__ __forceinline__ void mma_tf32(uint32_t d_tmem, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
+// D[64 x 40] += A[64 x 8] B[40 x 8]^T, TF32
+__device__ __forceinline__ void wgmma_n40_tf32(float (&d)[20], uint64_t a, uint64_t b) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a), "l"(b), "r"(idesc), "r"(acc)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %22, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n40k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19}, "
+      "%20, %21, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
+      : "l"(a), "l"(b), "r"(1)
       : "memory");
 }
-
-// one lane of a converged warp (the pattern the compiler needs to emit warp-uniform tcgen05 issue code
-// without a per-instruction election loop)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
+// D[64 x 40] += A[64 x 16] B[40 x 16]^T, BF16, both operands K-major
+__device__ __forceinline__ void wgmma_n40_bf16(float (&d)[20], uint64_t a, uint64_t b) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred)
-      :
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %22, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n40k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19}, "
+      "%20, %21, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
+      : "l"(a), "l"(b), "r"(1)
       : "memory");
-  return pred != 0;
 }
 
 __device__ __forceinline__ float ex2f(float x) {
@@ -249,23 +203,11 @@ __device__ __forceinline__ float tf32_rn(float x) {
 
 // B elements at once, stage by stage: the MUFU results are consumed a whole stage (>= B instructions)
 // after they were issued, so their latency is covered inside the warp instead of by warp switching.
-// g[n][p] as bf16, natural layout (MN-major A operand of the BF16 GEMM 2): 8 values = one 16-byte chunk
-__device__ __forceinline__ void store_g_bf16(uint8_t* gt, int r, int chunk, const float (&g)[8]) {
-  __nv_bfloat162 a = __floats2bfloat162_rn(g[0], g[1]), b = __floats2bfloat162_rn(g[2], g[3]);
-  __nv_bfloat162 c = __floats2bfloat162_rn(g[4], g[5]), d = __floats2bfloat162_rn(g[6], g[7]);
-  uint4 v;
-  v.x = *reinterpret_cast<uint32_t*>(&a);
-  v.y = *reinterpret_cast<uint32_t*>(&b);
-  v.z = *reinterpret_cast<uint32_t*>(&c);
-  v.w = *reinterpret_cast<uint32_t*>(&d);
-  *reinterpret_cast<uint4*>(gt + r * 128 + ((chunk ^ (r & 7)) << 4)) = v;
-}
-
 template <bool MASK, int B, bool RAW = false>
-__device__ __forceinline__ void epi_batch(const uint32_t* lr, float y, float vw, float* acc, float* g) {
+__device__ __forceinline__ void epi_batch(const float* lr, float y, float vw, float* acc, float* g) {
   float e[B], den[B], inv[B], lg[B];
 #pragma unroll
-  for (int j = 0; j < B; ++j) e[j] = ex2f(-1.4426950408889634f * fabsf(__uint_as_float(lr[j])));
+  for (int j = 0; j < B; ++j) e[j] = ex2f(-1.4426950408889634f * fabsf(lr[j]));
 #pragma unroll
   for (int j = 0; j < B; ++j) den[j] = 1.f + e[j];
 #pragma unroll
@@ -274,7 +216,7 @@ __device__ __forceinline__ void epi_batch(const uint32_t* lr, float y, float vw,
   for (int j = 0; j < B; ++j) lg[j] = lg2f(den[j]);
 #pragma unroll
   for (int j = 0; j < B; ++j) {
-    const float l = __uint_as_float(lr[j]);
+    const float l = lr[j];
     if (MASK) {
       acc[j] = fmaf(vw, fmaf(y, l, -fmaxf(l, 0.f)), acc[j]);
     } else {
@@ -284,7 +226,7 @@ __device__ __forceinline__ void epi_batch(const uint32_t* lr, float y, float vw,
   }
 #pragma unroll
   for (int j = 0; j < B; ++j) {
-    const float l = __uint_as_float(lr[j]);
+    const float l = lr[j];
     const float sg = (l >= 0.f) ? inv[j] : e[j] * inv[j];
     float gg = y - sg;
     if (MASK) {
@@ -297,28 +239,25 @@ __device__ __forceinline__ void epi_batch(const uint32_t* lr, float y, float vw,
   }
 }
 
+// MODE 0: single-pass TF32 logits.  MODE 1 (default): W split hi/lo.  MODE 2: full 3xTF32 (X split as
+// well).  MODE 3: logits as MODE 1, GEMM 2 in BF16 (operand rounding 2^-9, unbiased; opt-in).
+//
+// wgmma accumulator fragment (m64nN, f32): thread (warp w4 of the warpgroup, lane = 4 gid + t4) holds
+// d[4j + 2h + e] = D[16 w4 + gid + 8h][8j + 2 t4 + e].
 template <int MODE>
 __global__ void __launch_bounds__(kThreads, 1)
 glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_y,
                         const float* __restrict__ W, const float* __restrict__ bvec, int64_t N, int P,
-                        float* __restrict__ partials, long long* __restrict__ trace) {
+                        float* __restrict__ partials) {
   pdl_enter();   // lets glm_finish_kernel be resident (blocked in its griddepcontrol.wait) before this kernel ends
-  using L = Layout<MODE>;
-  // optional event trace of CTA (0, 0): trace[it * 16 + k] = SM clock of event k of tile it (first 64 tiles)
-  const bool tr = (trace != nullptr) && blockIdx.x == 0 && blockIdx.y == 0;
-#define TRACE(it_, k_) do { if (tr && (it_) < 64) trace[(it_) * 16 + (k_)] = clock64(); } while (0)
-  constexpr int SX = L::kStagesX;
-  constexpr int kStagesT = L::kStagesT;
-  constexpr bool BF = L::kBf16;              // GEMM 2 in BF16 on MN-major operands
+  constexpr bool BF = (MODE == 3);           // GEMM 2 in BF16
   constexpr int LM = BF ? 1 : MODE;          // precision mode of the logits (GEMM 1)
-  constexpr uint32_t kXtStage = L::kXtStage, kGBuf = L::kGBuf;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* sm = smem_raw + (base - raw);
-  const uint32_t bar0 = base + L::OFF_BAR;
-  auto bar = [&](int i) { return bar0 + 8u * (uint32_t)i; };
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(sm + L::OFF_BAR + 8 * BAR_COUNT);
+  const uint32_t bar0 = base + OFF_BAR;
+  auto bar_full = [&](int s) { return bar0 + 8u * (uint32_t)s; };
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int slab = blockIdx.y;
@@ -328,34 +267,13 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
 
   // ---- one-time setup --------------------------------------------------------------------------------
   if (tid == 0) {
-    for (int i = 0; i < kMaxStagesX; ++i) {
-      mbar_init(bar(BAR_XFULL + i), 1);
-      mbar_init(bar(BAR_XREADY + i), kSplitWarps * 32);
-      mbar_init(bar(BAR_XEMPTY + i), 1);
-    }
-    for (int i = 0; i < 2; ++i) mbar_init(bar(BAR_LEMPTY + i), 1);
-    for (int i = 0; i < kMaxStagesT; ++i) mbar_init(bar(BAR_TEMPTY + i), 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(bar(BAR_D1FULL + i), 1);
-      mbar_init(bar(BAR_D1EMPTY + i), kEpiWarps * 32);
-      mbar_init(bar(BAR_GFULL + i), kEpiWarps * 32);
-      mbar_init(bar(BAR_GEMPTY + i), 1);
-    }
-    mbar_init(bar(BAR_DONE), 1);
+    for (int s = 0; s < kStages; ++s) mbar_init(bar_full(s), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     base + L::OFF_BAR + 8 * BAR_COUNT),
-                 "r"(kTmemCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  // weight / bias / ones tiles (generic-proxy writes, made visible to the MMA unit below)
   {
-    float* whi = reinterpret_cast<float*>(sm + L::OFF_WHI);
-    float* wlo = reinterpret_cast<float*>(sm + L::OFF_WLO);
-    float* wb = reinterpret_cast<float*>(sm + L::OFF_WB);
+    // weight tiles (generic-proxy writes, made visible to the tensor cores below)
+    float* whi = reinterpret_cast<float*>(sm + OFF_WHI);
+    float* wlo = reinterpret_cast<float*>(sm + OFF_WLO);
     for (int e = tid; e < kP * kD; e += kThreads) {
       const int p = e >> 5, d = e & 31;
       const int gp = slab * kP + p;
@@ -364,368 +282,221 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
       const int off = p * 32 + ((((d >> 2) ^ (p & 7)) << 2) | (d & 3));   // float index, 128B swizzle
       whi[off] = hi;
       wlo[off] = w - hi;
-      float bv = 0.f;
-      if (d < 2 && bvec != nullptr && gp < P) {
-        const float bb = bvec[gp];
-        const float bh = tf32_trunc(bb);
-        bv = (d == 0) ? bh : (bb - bh);
-      }
-      wb[off] = bv;
     }
-    float* ones = reinterpret_cast<float*>(sm + L::OFF_ONES);
-    for (int e = tid; e < 1024; e += kThreads) ones[e] = 1.f;
+    // rows 32..39 of every X^T buffer are ones: GEMM 2 then yields db in column 32 of its accumulator
     if (!BF) {
-      // rows 32..39 of every X^T k-block are ones: GEMM 2 then yields db in columns 32..39 of D2
-      for (int e = tid; e < kStagesT * 4 * 256; e += kThreads) {
-        const int blk = e >> 8, w = e & 255;
-        reinterpret_cast<float*>(sm + L::OFF_XT + blk * kXtBlock + kD * 128)[w] = 1.f;
+      for (int e = tid; e < kWG * 2 * 256; e += kThreads) {
+        const int g = e >> 9, kb = (e >> 8) & 1, w = e & 255;
+        reinterpret_cast<float*>(sm + OFF_WG + g * kWGBytes + WG_XT + kb * kXtBlock + kD * 128)[w] = 1.f;
       }
     } else {
-      // bf16 B operand [128 n][64 columns]: columns 0..31 = x (split pass), column 32 = 1 (-> db in column
-      // 32 of D2), columns 33..63 = 0.  The constant chunks 4..7 of every row are written once here
-      // (16-byte chunk c of row n sits at chunk position c ^ (n & 7): 128-byte swizzle).
-      for (int e = tid; e < kStagesT * kRows * 4; e += kThreads) {
-        const int stg = e / (kRows * 4), rr = (e / 4) % kRows, c = 4 + (e & 3);
-        uint4 v = make_uint4(c == 4 ? 0x00003f80u : 0u, 0u, 0u, 0u);   // bf16 1.0 = 0x3f80 in element 0
-        *reinterpret_cast<uint4*>(sm + L::OFF_XT + stg * kXtStage + rr * 128 + ((c ^ (rr & 7)) << 4)) = v;
+      for (int e = tid; e < kWG * 8 * 64; e += kThreads) {
+        const int g = e >> 9, w = e & 511;
+        reinterpret_cast<__nv_bfloat16*>(sm + OFF_WG + g * kWGBytes + WG_XT + kD * 128)[w] = __float2bfloat16(1.f);
       }
     }
   }
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 0) {
-    // =========================== TMA producer ===========================================================
-    if (lane == 0) {
-      for (int it = 0; it < nt; ++it) {
-        const int sx = it % SX, ux = it / SX;
-        const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
-        mbar_wait(bar(BAR_XEMPTY + sx), (ux & 1) ^ 1);
-        TRACE(it, 0);
-        mbar_expect_tx(bar(BAR_XFULL + sx), kXStage);
-        tma_load_2d(base + L::OFF_X + sx * kTile, &map_x, 0, (int)(tile * kRows), bar(BAR_XFULL + sx));
-        tma_load_1d(base + L::OFF_YX + sx * 512, &map_y, (int)(tile * kRows), bar(BAR_XFULL + sx));
-      }
-    }
-  } else if (warp == 1) {
-    // =========================== MMA issuer =============================================================
-    // The whole warp walks the loop (waits included); one elected lane issues the tcgen05 instructions.
-    // Back-to-back MMAs into the SAME accumulator serialise on the tensor pipe's accumulate latency
-    // (~100 cycles measured, far above the 20-35 cycle issue cost of these small shapes), so the issue
-    // order interleaves five independent chains: GEMM 2 of tile j keeps one accumulator per 32-row
-    // k-block (D2[0..3], summed once at the end of the kernel) and GEMM 1 of tile j+2 is threaded
-    // through them.
-    constexpr uint32_t id1 = idesc_tf32(128, 64);
-    constexpr uint32_t id2 = idesc_tf32(64, 40);
-    const uint64_t d_whi = desc_sw128(base + L::OFF_WHI);
-    const uint64_t d_wlo = desc_sw128(base + L::OFF_WLO);
-    const uint64_t d_wb = desc_sw128(base + L::OFF_WB);
-    const uint64_t d_ones = make_desc(base + L::OFF_ONES, 128, 256, 0);
-    const uint64_t d_x0 = desc_sw128(base + L::OFF_X);
-    const uint64_t d_xl0 = desc_sw128(base + L::OFF_XLO);
-    const uint64_t d_g0 = desc_sw128(base + L::OFF_G);
-    const uint64_t d_xt0 = desc_sw128(base + L::OFF_XT);
-    constexpr int kG1 = (LM == 2) ? 12 : (LM == 1 ? 8 : 4);   // data MMAs of GEMM 1
-    constexpr int n_g1 = kG1 + 1;                                 // + the bias MMA (a zero tile without bias)
+  float lpa[16];                               // per-particle lp sums of the thread's rows (consumers)
+  float acc2[20];                              // GEMM 2 accumulator [p][c]: dW in c < 32, db in c = 32
+#pragma unroll
+  for (int i = 0; i < 16; ++i) lpa[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < 20; ++i) acc2[i] = 0.f;
+  // warp-uniform by construction (a shuffle result), so the tile loop is not a divergent branch to ptxas
+  const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0), w4 = warp & 3, t = tid & 127;
+  const int gid = lane >> 2, t4 = lane & 3;
 
-    // i-th MMA of GEMM 1 (i is a compile-time constant after unrolling); d1 / ax / al: accumulator and
-    // operand descriptors of the tile
-    auto g1_mma = [&](int i, uint32_t d1, uint64_t ax, uint64_t al) {
-      if (i == kG1) {
-        mma_tf32(d1, d_ones, d_wb, id1, 1u);
-        return;
+  {
+    // =========================== consumer warpgroups ====================================================
+    uint8_t* my = sm + OFF_WG + wg * kWGBytes;
+    const uint32_t my_s = base + OFF_WG + wg * kWGBytes;
+    const uint64_t d_whi = desc_sw128(base + OFF_WHI), d_wlo = desc_sw128(base + OFF_WLO);
+    const uint64_t d_xlo = desc_sw128(my_s + WG_XLO);
+    float bias[16];
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int gp = slab * kP + 8 * j + 2 * t4 + e;
+        bias[2 * j + e] = (bvec != nullptr && gp < P) ? bvec[gp] : 0.f;
       }
-      constexpr int per_k = kG1 / 4;
-      const int k = i / per_k, part = i % per_k;
-      if (part == 0) mma_tf32(d1, ax + (uint64_t)(k * 2), d_whi + (uint64_t)(k * 2), id1, k > 0 ? 1u : 0u);
-      else if (part == 1) mma_tf32(d1, ax + (uint64_t)(k * 2), d_wlo + (uint64_t)(k * 2), id1, 1u);
-      else mma_tf32(d1, al + (uint64_t)(k * 2), d_whi + (uint64_t)(k * 2), id1, 1u);
+    // tile it -> X/y stage; one thread of the warpgroup issues the loads
+    auto load = [&](int it, int s) {
+      const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
+      mbar_expect_tx(bar_full(s), kTile + kYBytes);
+      tma_load_2d(base + OFF_X + s * kTile, &map_x, 0, (int)(tile * kRows), bar_full(s));
+      tma_load_1d(base + OFF_Y + s * kYBytes, &map_y, (int)(tile * kRows), bar_full(s));
     };
-    auto g1_commit = [&](int it) {
-      tc_commit(bar(BAR_D1FULL + (it & 1)));
-      tc_commit(bar(BAR_XEMPTY + it % SX));
-      if (LM == 2) tc_commit(bar(BAR_LEMPTY + (it & 1)));
-    };
-    auto g1_wait = [&](int it) {
-      mbar_wait(bar(BAR_XREADY + it % SX), (it / SX) & 1);
-      mbar_wait(bar(BAR_D1EMPTY + (it & 1)), ((it >> 1) & 1) ^ 1);
-    };
-    // GEMM 2 of tile j, with GEMM 1 of tile j+2 threaded through when WITH_G1 (static issue order)
-    auto batch = [&](int j, auto with_g1_tag) {
-      constexpr bool WITH_G1 = decltype(with_g1_tag)::value;
-      const int st = j % kStagesT, bj = j & 1;
-      const int it = j + 2;
-      const uint32_t d1 = tmem + kColD1 + (uint32_t)(it & 1) * 64u;
-      const uint64_t ax = d_x0 + (uint64_t)((uint32_t)(it % SX) * (kTile >> 4));
-      const uint64_t al = d_xl0 + (uint64_t)((uint32_t)(it & 1) * (kTile >> 4));
-      // descriptor start addresses advance in 16-byte units: +2 per k-step of 8 floats inside a 32-float
-      // k-block, + one block (kP*128 resp. kXtBlock bytes) per k-block
-      const uint64_t da0 = d_g0 + (uint64_t)((uint32_t)bj * (kGBuf >> 4));
-      const uint64_t db0 = d_xt0 + (uint64_t)((uint32_t)st * (kXtStage >> 4));
-      const uint32_t acc0 = j > 0 ? 1u : 0u;
-      int gi = 0;
-      if (BF) {
-        // 8 MMAs of K = 16 rows (2048 bytes of both MN-major tiles per step), one accumulator
-        constexpr uint32_t id2b = idesc_bf16_mn(64, 64);
+    if (t == 0)
+      for (int k = 0; k < 2 && wg + k * kWG < nt; ++k) load(wg + k * kWG, 2 * wg + k);
+    for (int k = 0, it = wg; it < nt; ++k, it += kWG) {
+      const int s = 2 * wg + (k & 1);
+      const int64_t row0 = (blockIdx.x + (int64_t)it * gridDim.x) * kRows;
+      mbar_wait(bar_full(s), (uint32_t)(k >> 1) & 1u);
+      // GEMM 2 of this warpgroup's previous tile has finished reading g^T / X^T
+      wgmma_wait0();
+      fence_regs(acc2);
+      // ---- split / transposition pass: thread t owns 16 columns (chunks 4h .. 4h+3) of row r ----------
+      {
+        const int r = t >> 1, hh = t & 1;
+        float4* xs = reinterpret_cast<float4*>(sm + OFF_X + s * kTile);
+        float4* xl = reinterpret_cast<float4*>(my + WG_XLO);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          mma_bf16(tmem + kColD2, da0 + (uint64_t)(k * 128), db0 + (uint64_t)(k * 128), id2b, k > 0 ? 1u : acc0);
-          if (WITH_G1) {
-            const int upto = ((k + 1) * n_g1 + 7) >> 3;
+        for (int c4 = 0; c4 < 4; ++c4) {
+          const int c = hh * 4 + c4;
+          const int idx = r * 8 + (c ^ (r & 7));      // 16-byte chunk holding d = 4c .. 4c+3 of row r
+          const float4 v = xs[idx];
+          const float x[4] = {v.x, v.y, v.z, v.w};
+          float xr[4];
 #pragma unroll
-            for (int q = 0; q < 3; ++q)
-              if (gi < upto) {
-                g1_mma(gi, d1, ax, al);
-                ++gi;
-              }
+          for (int q = 0; q < 4; ++q) xr[q] = tf32_rn(x[q]);
+          if (LM == 2) {
+            float h[4];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) h[q] = tf32_trunc(x[q]);
+            xs[idx] = make_float4(h[0], h[1], h[2], h[3]);
+            xl[idx] = make_float4(x[0] - h[0], x[1] - h[1], x[2] - h[2], x[3] - h[3]);
+          } else {
+            xs[idx] = make_float4(xr[0], xr[1], xr[2], xr[3]);
           }
-        }
-      } else {
-#pragma unroll
-      for (int sstep = 0; sstep < 4; ++sstep) {
-#pragma unroll
-        for (int kb = 0; kb < 4; ++kb) {
-          const uint64_t da = da0 + (uint64_t)(kb * ((kP * 128) >> 4) + sstep * 2);
-          const uint64_t db = db0 + (uint64_t)(kb * (kXtBlock >> 4) + sstep * 2);
-          mma_tf32(tmem + kColD2 + (uint32_t)kb * 40u, da, db, id2, sstep > 0 ? 1u : acc0);
-          if (WITH_G1) {
-            const int upto = ((sstep * 4 + kb + 1) * n_g1 + 15) >> 4;   // spread evenly over the 16 slots
-#pragma unroll
-            for (int q = 0; q < 2; ++q)
-              if (gi < upto) {
-                g1_mma(gi, d1, ax, al);
-                ++gi;
-              }
-          }
-        }
-      }
-      }
-      if (WITH_G1) g1_commit(it);
-      tc_commit(bar(BAR_TEMPTY + st));
-      tc_commit(bar(BAR_GEMPTY + bj));
-    };
-    // prologue: GEMM 1 of the first two tiles
-    for (int it = 0; it < 2 && it < nt; ++it) {
-      g1_wait(it);
-      if (lane == 0) TRACE(it, 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t d1 = tmem + kColD1 + (uint32_t)(it & 1) * 64u;
-        const uint64_t ax = d_x0 + (uint64_t)((uint32_t)(it % SX) * (kTile >> 4));
-        const uint64_t al = d_xl0 + (uint64_t)((uint32_t)(it & 1) * (kTile >> 4));
-#pragma unroll
-        for (int i = 0; i < n_g1; ++i) g1_mma(i, d1, ax, al);
-        g1_commit(it);
-      }
-      __syncwarp();
-      if (lane == 0) TRACE(it, 3);
-    }
-    for (int j = 0; j < nt; ++j) {
-      const bool has_g1 = (j + 2 < nt);
-      if (has_g1) g1_wait(j + 2);                      // long satisfied: split pass / epilogue of older tiles
-      mbar_wait(bar(BAR_GFULL + (j & 1)), (j >> 1) & 1);   // epilogue of tile j has written g^T
-      if (lane == 0) TRACE(j, 4);
-      tc_fence_after();
-      if (elect_one()) {
-        if (has_g1) batch(j, cuda::std::true_type{});
-        else batch(j, cuda::std::false_type{});
-      }
-      __syncwarp();
-      if (lane == 0) TRACE(j, 5);
-    }
-    if (elect_one()) tc_commit(bar(BAR_DONE));
-    __syncwarp();
-  } else if (warp >= kSplitWarp0) {
-    // =========================== split / transposition warps ===========================================
-    const int r = tid - kSplitWarp0 * 32;           // row of the tile owned by this thread
-    const int kb = r >> 5;                          // 32-row k-block of the transposed tile
-    for (int it = 0; it < nt; ++it) {
-      const int sx = it % SX, ux = it / SX;
-      const int st = it % kStagesT, ut = it / kStagesT;
-      mbar_wait(bar(BAR_XFULL + sx), ux & 1);
-      if (r == 0) TRACE(it, 6);
-      mbar_wait(bar(BAR_TEMPTY + st), (ut & 1) ^ 1);           // GEMM 2 of tile it-3 released X^T[st]
-      if (r == 0) TRACE(it, 7);
-      if (LM == 2) mbar_wait(bar(BAR_LEMPTY + (it & 1)), ((it >> 1) & 1) ^ 1);
-      float4* xhi = reinterpret_cast<float4*>(sm + L::OFF_X + sx * kTile);
-      float4* xlo = reinterpret_cast<float4*>(sm + L::OFF_XLO + (it & 1) * kTile);
-      float* xt = reinterpret_cast<float*>(sm + L::OFF_XT + st * kXtStage + kb * kXtBlock);
-      // y travels with the X^T stage (the epilogue reads it after the X stage may have been refilled)
-      reinterpret_cast<float*>(sm + L::OFF_Y + st * 512)[r] =
-          reinterpret_cast<const float*>(sm + L::OFF_YX + sx * 512)[r];
-#pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        const int idx = r * 8 + (c ^ (r & 7));      // 16-byte chunk holding d = 4c .. 4c+3 of row r
-        const float4 v = xhi[idx];
-        float x[4] = {v.x, v.y, v.z, v.w};
-        if (LM == 2) {
-          float4 h, l;
-          h.x = tf32_trunc(v.x); h.y = tf32_trunc(v.y); h.z = tf32_trunc(v.z); h.w = tf32_trunc(v.w);
-          l.x = v.x - h.x; l.y = v.y - h.y; l.z = v.z - h.z; l.w = v.w - h.w;
-          xhi[idx] = h;
-          xlo[idx] = l;
-#pragma unroll
-          for (int q = 0; q < 4; ++q) x[q] = tf32_rn(x[q]);
-        } else {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) x[q] = tf32_rn(x[q]);
-          xhi[idx] = make_float4(x[0], x[1], x[2], x[3]);
-        }
-        if (BF) {
-          // natural layout, bf16: columns 4c .. 4c+3 of row r -> 8 bytes inside 16-byte chunk c/2
-          __nv_bfloat162 lo2 = __floats2bfloat162_rn(v.x, v.y), hi2 = __floats2bfloat162_rn(v.z, v.w);
-          uint2 pk;
-          pk.x = *reinterpret_cast<uint32_t*>(&lo2);
-          pk.y = *reinterpret_cast<uint32_t*>(&hi2);
-          *reinterpret_cast<uint2*>(sm + L::OFF_XT + st * kXtStage + r * 128 + (((c >> 1) ^ (r & 7)) << 4) +
-                                    (c & 1) * 8) = pk;
-        } else {
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             const int d = c * 4 + q;
-            // X^T[d][n = r]: row d of k-block kb, 16-byte chunk (lane >> 2) ^ (d & 7), element lane & 3
-            xt[d * 32 + (((((r & 31) >> 2) ^ (d & 7)) << 2) | (r & 3))] = x[q];
+            if (BF) {
+              // X^T[d][n = r] bf16: 16-byte chunk (r >> 3) ^ (d & 7), element r & 7
+              *reinterpret_cast<__nv_bfloat16*>(my + WG_XT + d * 128 + ((((r >> 3) ^ (d & 7))) << 4) + (r & 7) * 2) =
+                  __float2bfloat16(x[q]);
+            } else {
+              // X^T[d][n = r]: k-block r >> 5, 16-byte chunk ((r & 31) >> 2) ^ (d & 7), element r & 3
+              reinterpret_cast<float*>(my + WG_XT + (r >> 5) * kXtBlock)[d * 32 + (((((r & 31) >> 2) ^ (d & 7)) << 2) |
+                                                                                   (r & 3))] = xr[q];
+            }
           }
         }
       }
+      const float* ys = reinterpret_cast<const float*>(sm + OFF_Y + s * kYBytes);
+      const float y0 = ys[16 * w4 + gid], y1 = ys[16 * w4 + gid + 8];
       fence_proxy_async();
-      mbar_arrive(bar(BAR_XREADY + sx));
-      if (r == 0) TRACE(it, 8);
-    }
-  } else {
-    // =========================== epilogue warps ========================================================
-    const int ew = warp - kEpiWarp0;
-    const int sub = warp & 3;                       // TMEM sub-partition this warp may access
-    const int part = ew >> 2;                       // particles [kEpiCols*part, kEpiCols*(part+1))
-    const int r = sub * 32 + lane;                  // row of the tile
-    float acc[kEpiCols];
+      wg_bar(1 + wg);
+      // ---- GEMM 1: logits, accumulator initialised with the bias --------------------------------------
+      float acc1[32];
 #pragma unroll
-    for (int j = 0; j < kEpiCols; ++j) acc[j] = 0.f;
-    // g^T[p][n = r]: k-block = sub, chunk (lane >> 2) ^ (p & 7); p & 7 == j & 7 because kEpiCols % 8 == 0
-    uint32_t gofs[8];
+      for (int j = 0; j < 8; ++j)
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
-      gofs[j] = (uint32_t)sub * (kP * 128) + (uint32_t)part * (kEpiCols * 128) +
-                ((((uint32_t)(lane >> 2) ^ (uint32_t)j) << 4) | ((uint32_t)(lane & 3) << 2));
-    for (int it = 0; it < nt; ++it) {
-      const int st = it % kStagesT;
-      const int b = it & 1, v = it >> 1;
-      const int64_t row0 = (blockIdx.x + (int64_t)it * gridDim.x) * kRows;
-      // GEMM 2 of tile it-2 (long finished) has released g^T[b]
-      mbar_wait(bar(BAR_GEMPTY + b), (v & 1) ^ 1);
-      if (ew == 0 && lane == 0) TRACE(it, 11);
-      // d1_full implies the split pass of this tile ran (x_ready -> GEMM 1 -> d1_full): y[st] is in place
-      mbar_wait(bar(BAR_D1FULL + b), v & 1);
-      if (ew == 0 && lane == 0) TRACE(it, 9);
-      tc_fence_after();
-      uint32_t lr[kEpiCols];
-      const uint32_t taddr = tmem + ((uint32_t)(sub * 32) << 16) + kColD1 + (uint32_t)b * 64u +
-                             (uint32_t)part * kEpiCols;
-      static_assert(kEpiCols == 16, "the TMEM load below is the .x16 form");
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-          "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-          : "=r"(lr[0]), "=r"(lr[1]), "=r"(lr[2]), "=r"(lr[3]), "=r"(lr[4]), "=r"(lr[5]), "=r"(lr[6]),
-            "=r"(lr[7]), "=r"(lr[8]), "=r"(lr[9]), "=r"(lr[10]), "=r"(lr[11]), "=r"(lr[12]), "=r"(lr[13]),
-            "=r"(lr[14]), "=r"(lr[15])
-          : "r"(taddr)
-          : "memory");
-      const float y = reinterpret_cast<const float*>(sm + L::OFF_Y + st * 512)[r];
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      tc_fence_before();
-      mbar_arrive(bar(BAR_D1EMPTY + b));            // D1[b] is in registers now
-      if (ew == 0 && lane == 0) TRACE(it, 10);
-      uint8_t* gt = sm + L::OFF_G + b * kGBuf;
-      if (row0 + kRows <= N) {
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int j0 = 0; j0 < kEpiCols; j0 += 8) {
-          float g[8];
-          epi_batch<false, 8, BF>(lr + j0, y, 1.f, acc + j0, g);
-          if (BF) store_g_bf16(gt, r, part * (kEpiCols / 8) + (j0 >> 3), g);
-          else {
+          for (int e = 0; e < 2; ++e) acc1[4 * j + 2 * h + e] = bias[2 * j + e];
+      wgmma_fence();
+      const uint64_t d_x = desc_sw128(base + OFF_X + s * kTile);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) *reinterpret_cast<float*>(gt + gofs[j] + (j0 + j) * 128) = g[j];
-          }
+      for (int k = 0; k < 4; ++k) {
+        wgmma_n64_tf32(acc1, d_x + 2 * k, d_whi + 2 * k);
+        if (LM >= 1) wgmma_n64_tf32(acc1, d_x + 2 * k, d_wlo + 2 * k);
+        if (LM == 2) wgmma_n64_tf32(acc1, d_xlo + 2 * k, d_whi + 2 * k);
+      }
+      wgmma_commit();
+      wgmma_wait0();
+      fence_regs(acc1);
+      // GEMM 1 has read the X stage and y is in registers: refill the stage with tile it + 2 kWG
+      if (t == 0 && it + 2 * kWG < nt) load(it + 2 * kWG, s);
+      // ---- epilogue: lp sums in registers, g^T into shared memory -------------------------------------
+      const bool tail = row0 + kRows > N;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int n = 16 * w4 + gid + 8 * h;
+        const float yv = h ? y1 : y0;
+        const float vw = (row0 + n < N) ? 1.f : 0.f;
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          float l[8], g[8];
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) l[2 * jj + e] = acc1[4 * (4 * half + jj) + 2 * h + e];
+          if (tail) epi_batch<true, 8, BF>(l, yv, vw, lpa + 8 * half, g);
+          else epi_batch<false, 8, BF>(l, yv, 1.f, lpa + 8 * half, g);
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int p = 8 * (4 * half + jj) + 2 * t4 + e;
+              if (BF) {
+                *reinterpret_cast<__nv_bfloat16*>(my + WG_G + p * 128 + (((n >> 3) ^ (p & 7)) << 4) + (n & 7) * 2) =
+                    __float2bfloat16(g[2 * jj + e]);
+              } else {
+                *reinterpret_cast<float*>(my + WG_G + (n >> 5) * kGBlock + p * 128 +
+                                          (((((n & 31) >> 2) ^ (p & 7))) << 4) + (n & 3) * 4) = g[2 * jj + e];
+              }
+            }
         }
+      }
+      fence_proxy_async();
+      wg_bar(1 + wg);
+      // ---- GEMM 2: [dW | db] += g^T [X | 1], left running while the next tile is waited for ----------
+      wgmma_fence();
+      if (BF) {
+        const uint64_t da = desc_sw128(my_s + WG_G), db = desc_sw128(my_s + WG_XT);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_n40_bf16(acc2, da + 2 * k, db + 2 * k);
       } else {
-        const float vw = (row0 + r < N) ? 1.f : 0.f;
 #pragma unroll
-        for (int j0 = 0; j0 < kEpiCols; j0 += 8) {
-          float g[8];
-          epi_batch<true, 8, BF>(lr + j0, y, vw, acc + j0, g);
-          if (BF) store_g_bf16(gt, r, part * (kEpiCols / 8) + (j0 >> 3), g);
-          else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) *reinterpret_cast<float*>(gt + gofs[j] + (j0 + j) * 128) = g[j];
-          }
+        for (int k = 0; k < 8; ++k) {
+          const uint64_t da = desc_sw128(my_s + WG_G + (k >> 2) * kGBlock) + 2 * (k & 3);
+          const uint64_t db = desc_sw128(my_s + WG_XT + (k >> 2) * kXtBlock) + 2 * (k & 3);
+          wgmma_n40_tf32(acc2, da, db);
         }
       }
-      fence_proxy_async();
-      mbar_arrive(bar(BAR_GFULL + b));
-      if (ew == 0 && lane == 0) TRACE(it, 12);
-      if (ew == 4 && lane == 0) TRACE(it, 13);
-      if (ew == 3 && lane == 0) TRACE(it, 14);
-      if (ew == 15 && lane == 0) TRACE(it, 15);
+      wgmma_commit();
     }
-    // ---- CTA results: dW, db from TMEM; lp sums through shared memory (fixed order) ---------------------
-    mbar_wait(bar(BAR_DONE), 0);
-    tc_fence_after();
-    float* scratch = reinterpret_cast<float*>(sm + L::OFF_G);    // [128 rows][65]; GEMM 2 is finished with g^T
+    wgmma_wait0();
+    fence_regs(acc2);
 #pragma unroll
-    for (int j = 0; j < kEpiCols; ++j) scratch[r * 65 + part * kEpiCols + j] = acc[j];
-    asm volatile("bar.sync 1, %0;" ::"n"(kEpiWarps * 32) : "memory");
-    float* out = partials + ((int64_t)blockIdx.x * P) * (kD + 2);
-    if (ew < 4) {
-      // M = 64 accumulators: row p lives in lane (p % 16) of sub-partition p / 16
-      float dwf[32], dbf = 0.f;
-#pragma unroll
-      for (int d = 0; d < 32; ++d) dwf[d] = 0.f;
-      const uint32_t t2 = tmem + ((uint32_t)(sub * 32) << 16);
-#pragma unroll
-      for (int kb = 0; kb < (BF ? 1 : 4); ++kb) {
-        uint32_t dw[32], dbv[8];
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(dw[0]), "=r"(dw[1]), "=r"(dw[2]), "=r"(dw[3]), "=r"(dw[4]), "=r"(dw[5]), "=r"(dw[6]),
-              "=r"(dw[7]), "=r"(dw[8]), "=r"(dw[9]), "=r"(dw[10]), "=r"(dw[11]), "=r"(dw[12]), "=r"(dw[13]),
-              "=r"(dw[14]), "=r"(dw[15]), "=r"(dw[16]), "=r"(dw[17]), "=r"(dw[18]), "=r"(dw[19]), "=r"(dw[20]),
-              "=r"(dw[21]), "=r"(dw[22]), "=r"(dw[23]), "=r"(dw[24]), "=r"(dw[25]), "=r"(dw[26]), "=r"(dw[27]),
-              "=r"(dw[28]), "=r"(dw[29]), "=r"(dw[30]), "=r"(dw[31])
-            : "r"(t2 + kColD2 + (uint32_t)kb * 40u)      // BF: one accumulator, dW in columns 0..31, db in 32
-            : "memory");
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                     : "=r"(dbv[0]), "=r"(dbv[1]), "=r"(dbv[2]), "=r"(dbv[3]), "=r"(dbv[4]), "=r"(dbv[5]),
-                       "=r"(dbv[6]), "=r"(dbv[7])
-                     : "r"(t2 + kColD2 + (uint32_t)kb * 40u + 32u)
-                     : "memory");
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int d = 0; d < 32; ++d) dwf[d] += __uint_as_float(dw[d]);
-        dbf += __uint_as_float(dbv[0]);
-      }
-      const int pl = sub * 16 + lane;               // valid for lane < 16
-      const int gp = slab * kP + pl;
-      if (lane < 16 && gp < P) {
-        float s = 0.f;
-        for (int n = 0; n < kRows; ++n) s += scratch[n * 65 + pl];
-        float* o = out + (int64_t)gp * (kD + 2);
-#pragma unroll
-        for (int d = 0; d < kD; ++d) o[d] = dwf[d];
-        o[kD] = dbf;
-        o[kD + 1] = s;
-      }
+    for (int i = 0; i < 16; ++i) {
+      float v = lpa[i];
+      v += __shfl_xor_sync(0xffffffffu, v, 4);
+      v += __shfl_xor_sync(0xffffffffu, v, 8);
+      v += __shfl_xor_sync(0xffffffffu, v, 16);
+      lpa[i] = v;
     }
-    tc_fence_before();
+  }
+  // ---- CTA results through shared memory (the X ring is idle now), fixed summation order -----------------
+  __syncthreads();
+  float* red2 = reinterpret_cast<float*>(sm + OFF_X);     // [kWG][64 p][33]
+  float* redlp = red2 + kWG * kP * 33;                    // [kWG * 4 warps][64 p]
+  {
+#pragma unroll
+    for (int j = 0; j < 5; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int p = 16 * w4 + gid + 8 * h, c = 8 * j + 2 * t4 + e;
+          if (c <= kD) red2[(wg * kP + p) * 33 + c] = acc2[4 * j + 2 * h + e];
+        }
+    if (gid == 0) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) redlp[warp * kP + 8 * j + 2 * t4 + e] = lpa[2 * j + e];
+    }
   }
   __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(kTmemCols) : "memory");
+  if (tid < kP) {
+    const int gp = slab * kP + tid;
+    if (gp < P) {
+      float* o = partials + ((int64_t)blockIdx.x * P + gp) * (kD + 2);
+      for (int c = 0; c <= kD; ++c) {          // dW[0..31], db
+        float v = 0.f;
+        for (int g = 0; g < kWG; ++g) v += red2[(g * kP + tid) * 33 + c];
+        o[c] = v;
+      }
+      float v = 0.f;
+      for (int w = 0; w < kWG * 4; ++w) v += redlp[w * kP + tid];
+      o[kD + 1] = v;
+    }
   }
 }
 
@@ -789,28 +560,21 @@ int launch_glm_tc(const float* X, const float* y, const float* W, const float* b
   }
   static bool attr_set = false;
   if (!attr_set) {
-    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)Layout<0>::kSmemBytes);
-    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)Layout<1>::kSmemBytes);
-    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)Layout<2>::kSmemBytes);
-    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)Layout<3>::kSmemBytes);
+    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
     attr_set = true;
   }
   dim3 grid((unsigned)gx, (unsigned)((P + kP - 1) / kP), 1);
-  // B2_GLM_TC_TRACE = device address (decimal) of a 64 x 16 int64 buffer for the event trace of CTA 0
-  const char* tr_env = getenv("B2_GLM_TC_TRACE");
-  long long* trace = tr_env ? reinterpret_cast<long long*>(strtoull(tr_env, nullptr, 10)) : nullptr;
   if (mode == 3)
-    launch_pdl(glm_bernoulli_tc_kernel<3>, grid, dim3(kThreads), (size_t)Layout<3>::kSmemBytes, s, mx, my, W, b, N, P, partials, trace);
+    launch_pdl(glm_bernoulli_tc_kernel<3>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, W, b, N, P, partials);
   else if (mode == 2)
-    launch_pdl(glm_bernoulli_tc_kernel<2>, grid, dim3(kThreads), (size_t)Layout<2>::kSmemBytes, s, mx, my, W, b, N, P, partials, trace);
+    launch_pdl(glm_bernoulli_tc_kernel<2>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, W, b, N, P, partials);
   else if (mode == 1)
-    launch_pdl(glm_bernoulli_tc_kernel<1>, grid, dim3(kThreads), (size_t)Layout<1>::kSmemBytes, s, mx, my, W, b, N, P, partials, trace);
+    launch_pdl(glm_bernoulli_tc_kernel<1>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, W, b, N, P, partials);
   else
-    launch_pdl(glm_bernoulli_tc_kernel<0>, grid, dim3(kThreads), (size_t)Layout<0>::kSmemBytes, s, mx, my, W, b, N, P, partials, trace);
+    launch_pdl(glm_bernoulli_tc_kernel<0>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, W, b, N, P, partials);
   return 0;
 }
 

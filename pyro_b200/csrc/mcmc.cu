@@ -682,7 +682,7 @@ __global__ void __launch_bounds__(256) nuts_leaf_hier_kernel(const LeafHierArgs 
     T* ck_r = reinterpret_cast<T*>(a.rck);
     T* ck_s = reinterpret_cast<T*>(a.sck);
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    constexpr int UN = 2;  // elements in flight per thread (4 measured slower: 80 k -> 61 k chain-leapfrog/s, 88 regs)
+    constexpr int UN = 2;  // elements in flight per thread (4 raises the register count and lowers occupancy)
     int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     auto elem = [&](int64_t jj, T eta, T rj, T mv, T rsv, T yv, T sv) {
       const T isg = fast_rcp(sv);

@@ -278,12 +278,8 @@ struct VecBody {
 };
 
 // Vectors in flight per operand per thread.  Forward-only fp32 kernels of the cheap families are pure streams: 4
-// vectors (measured 85 % of the HBM copy peak for Normal).  Kernels that also write gradients carry more live
-// registers, and the lgamma families (Gamma, Beta, Poisson) are bound by instruction issue, not by loads in
-// flight: 2 vectors (measured, forward-only: Gamma 64.3 -> 69.5 %, Beta 41.5 -> 45.6 %, Poisson 52.5 -> 55.3 % of
-// the HBM peak against 4 vectors; profiles/micro_logprob_r2.md).
-// (Round 2 also tried 4 vectors in flight for the one-parameter gradient kernels: 128 registers, 2 CTAs per SM,
-// and no gain -- Bernoulli 67.9 -> 69.8 %, HalfCauchy 71.2 -> 69.5 %, Exponential 65.7 -> 64.3 %.)
+// vectors.  Kernels that also write gradients carry more live registers, and the lgamma families (Gamma, Beta,
+// Poisson) are bound by instruction issue, not by loads in flight: 2 vectors (4 would only cost registers).
 template <int FAM, typename T, bool GRAD>
 struct VecUnroll {
   static constexpr bool kHeavy = (FAM == kGamma || FAM == kBeta || FAM == kPoisson);
@@ -526,7 +522,7 @@ __global__ void __launch_bounds__(kSmallThreads) site_small_kernel(const SiteArg
   }
   if (GRAD) {
     // ONE copy of the reduction code, looped over the outputs: these kernels run from a cold
-    // instruction cache (ncu: stall_no_inst on top), so a second inlined copy costs more than the loop
+    // instruction cache, so a second inlined copy costs more than the loop
 #pragma unroll 1
     for (int k = 0; k <= NP; ++k) {
       OutOpnd o = a.gx;

@@ -1,9 +1,9 @@
-"""Distribution classes of the B200 backend.
+"""Distribution classes of the CUDA backend.
 
 Host-side mirror of the reference's distribution protocol (pyro/distributions/distribution.py:29-222,
 pyro/distributions/torch_distribution.py:19-232): ``sample/rsample/log_prob/score_parts/expand/
 mask/to_event/has_rsample/batch_shape/event_shape/support``.  What differs is WHERE the arithmetic
-runs: ``log_prob`` and ``score_parts`` dispatch to the fused sm_100a kernels through the C ABI
+runs: ``log_prob`` and ``score_parts`` dispatch to the fused sm_90a kernels through the C ABI
 (``pyro_b200._native``); there is no ATen fallback -- scoring a CPU tensor raises.
 
 Parameters are kept at their STORED shape; ``expand`` only records the new batch shape, and the

@@ -9,7 +9,7 @@ filter: O(T H^3) work, O(H^2) live state, and every heavy operation is a dense `
 
 Round-1 status: the GEMMs / small Choleskys run through cuBLAS / cuSOLVER (``torch.matmul``,
 ``torch.linalg``) -- plain library contractions, fp32 (or TF32 tensor cores with ``tf32=True``) --
-and gradients come from autograd through the recursion.  There is no hand-written tcgen05 kernel
+and gradients come from autograd through the recursion.  There is no hand-written tensor-core kernel
 for this row yet (DESIGN.md section 7); parity with the reference is pinned by
 tests/golden/hmm.npz.
 """

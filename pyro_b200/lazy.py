@@ -6,7 +6,7 @@ A model such as tests/infer/mcmc/test_hmc.py:189-198 writes its likelihood as
     pyro.sample("y", dist.Bernoulli(logits=logits), obs=y)
 
 Executed literally this materialises ``[P, N]`` logits (cuBLAS), ``[P, N]`` log-probabilities and
-their gradients: 1.3 ms of a 1.34 ms step at BASELINE config 2.  The ELBO hands latent site values
+their gradients, which dominate the step at BASELINE config 2.  The ELBO hands latent site values
 to the model as :class:`SiteValue` tensors instead; every torch operation on them runs exactly as on
 a plain tensor EXCEPT a contraction with a gradient-free data matrix, which returns a
 :class:`LinearPredictorTensor` -- a storage-less tensor that remembers ``(X, w, b)``.  Adding a

@@ -2,7 +2,7 @@
 round 1 only exercised on the CPU stand-ins now run through the real kernels on device tensors --
 score-function ELBO (a10), HMC.sample (b3), warm-up adaptation pieces (b6), r_hat / ESS (b7), optimiser
 checkpoints (f3) -- plus the exactness of the CUDA-graph step, the safety of its input buffers, and
-the unchanged logistic model reaching the tcgen05 GLM kernel (checked against the oracle at D = 32 and at
+the unchanged logistic model reaching the wgmma GLM kernel (checked against the oracle at D = 32 and at
 the full BASELINE size)."""
 import math
 
@@ -231,10 +231,10 @@ def test_captured_step_never_writes_caller_tensors():
     assert svi.optim.get_state()["w_loc"]["state"][0]["step"] == 12
 
 
-# ---- the unchanged model reaches the tcgen05 GLM kernel; parity against the oracle --------------------------
+# ---- the unchanged model reaches the wgmma GLM kernel; parity against the oracle --------------------------
 def test_unchanged_logistic_model_d32_matches_oracle_trajectory():
     """models.logistic_model is the reference model verbatim (`w.squeeze(-2) @ X.T + b`); at D = 32 its
-    likelihood site is scored by the tcgen05 kernel (lazy linear predictor).  Three SVI steps with
+    likelihood site is scored by the wgmma kernel (lazy linear predictor).  Three SVI steps with
     injected noise against oracle/svi.py (itself pinned to reference Pyro's trajectory)."""
     torch.manual_seed(0)
     N_, D, P = 70000, 32, 16          # >= 64 Ki rows: the default (W-split) precision mode
@@ -278,7 +278,7 @@ def test_unchanged_logistic_model_d32_matches_oracle_trajectory():
                                                      ("B2_FLAG_GLM_BF16_GRAD", 2e-5, 2e-4),
                                                      ("B2_FLAG_GLM_TF32", 5e-4, 2e-3)])
 def test_glm_kernel_full_size_against_oracle(flag_name, tol_sum, tol_g):
-    """BASELINE size (N = 1e6, D = 32, P = 64): per-particle sums, dW and db of the tcgen05 kernel against
+    """BASELINE size (N = 1e6, D = 32, P = 64): per-particle sums, dW and db of the wgmma kernel against
     the oracle's fp64 Bernoulli log-density (oracle/dists.py) differentiated by autograd on the CPU.
     Default path: fp32 tolerances (2e-5 on sums, 2e-4 x scale on gradients)."""
     if EMULATE:
@@ -326,13 +326,22 @@ def test_glm_kernel_full_size_against_oracle(flag_name, tol_sum, tol_g):
 @pytest.mark.parametrize("n,P,bias,flag", [(1, 1, True, "B2_FLAG_GLM_3XTF32"), (127, 3, False, "B2_FLAG_GLM_3XTF32"),
                                            (128, 64, True, "B2_FLAG_GLM_3XTF32"), (129, 65, True, "B2_FLAG_GLM_3XTF32"),
                                            (1, 1, True, None), (5000, 130, False, None),
-                                           (8192, 64, True, None), (70001, 64, True, None), (65535, 130, False, None)])
+                                           (8192, 64, True, None), (70001, 64, True, None), (65535, 130, False, None),
+                                           (129, 65, True, "B2_FLAG_GLM_TF32"), (70001, 64, True, "B2_FLAG_GLM_TF32"),
+                                           (129, 65, True, "B2_FLAG_GLM_BF16_GRAD"),
+                                           (70001, 64, True, "B2_FLAG_GLM_BF16_GRAD")])
 def test_glm_tc_kernel_ragged_shapes_against_oracle(n, P, bias, flag):
-    """Edge cases of the tiled kernel: a single row, one row short of / one past a 128-row tile, ragged
-    particle slabs (65, 130), no bias.  With an explicit tensor-core flag the tcgen05 kernel runs at any
-    size and its gradient contraction is single-pass TF32 on round-to-nearest operands: the tolerance is
-    2^-11 of the LARGEST TERM budget (5e-4 x scale) for tiny N, where nothing averages; the default
-    dispatch (flag None: exact fp32 SIMT below 8 Ki rows, tcgen05 above) must meet the fp32 tolerances."""
+    """Edge cases of the tiled kernel (64-row tiles, three warpgroups per CTA): a single row, sizes one row
+    short of / one past a tile boundary and a ragged last tile (70001 = 1093 * 64 + 49), ragged particle
+    slabs (65, 130), no bias.  With an explicit tensor-core flag the wgmma kernel runs at any size and its
+    gradient contraction is single-pass TF32 on round-to-nearest operands: the tolerance is 2^-11 of the
+    LARGEST TERM budget (5e-4 x scale) for tiny N, where nothing averages; the default dispatch (flag None:
+    exact fp32 SIMT below 8 Ki rows, wgmma above) must meet the fp32 tolerances.  Single-pass TF32 logits
+    (B2_FLAG_GLM_TF32) take the TF32 tolerances of the full-size test (5e-4 / 2e-3).  The BF16 gradient
+    contraction (B2_FLAG_GLM_BF16_GRAD) rounds g and x to 2^-9 each, so its dW / db error is bounded
+    elementwise by 2^-8 sum_n |g x| (plus the fp32 tolerance); its logits are those of the default W split
+    at any N (not 3xTF32 below 64 Ki rows), i.e. X rounded to nearest TF32: |d lp / d logit| <= 1 bounds
+    the error of each sum by 2^-12 sum_n sum_d |x w| (2^-11 taken)."""
     if EMULATE:
         pytest.skip("kernel test")
     from pyro_b200 import _native as N
@@ -358,8 +367,18 @@ def test_glm_tc_kernel_ragged_shapes_against_oracle(n, P, bias, flag):
                                             sum_p.data_ptr(), None, dW.data_ptr(), db.data_ptr(), ws.data_ptr(),
                                             ws.numel(), N.stream_ptr(torch.device(DEV))), "b2_glm_bernoulli_logits")
     torch.cuda.synchronize()
-    tol_g = 5e-4 if flag else 2e-4
-    assert float((sum_p.double().cpu() - s_ref).abs().max()) <= 2e-5 * max(1.0, float(s_ref.abs().max()))
+    tol_sum = 5e-4 if flag == "B2_FLAG_GLM_TF32" else 2e-5
+    tol_g = {None: 2e-4, "B2_FLAG_GLM_TF32": 2e-3}.get(flag, 5e-4)
+    if flag == "B2_FLAG_GLM_BF16_GRAD":
+        bound_s = 2.0 ** -11 * (X.double().abs() @ W.double().abs().t()).sum(0) + \
+            tol_sum * max(1.0, float(s_ref.abs().max()))
+        assert bool(((sum_p.double().cpu() - s_ref).abs() <= bound_s).all())
+        bound_W = 2.0 ** -8 * (g.abs() @ X.double().abs()) + tol_g * max(1.0, float(gW.abs().max()))
+        bound_b = 2.0 ** -8 * g.abs().sum(1) + tol_g * max(1.0, float(gb.abs().max()))
+        assert bool(((dW.double().cpu() - gW).abs() <= bound_W).all())
+        assert bool(((db.double().cpu() - gb).abs() <= bound_b).all())
+        return
+    assert float((sum_p.double().cpu() - s_ref).abs().max()) <= tol_sum * max(1.0, float(s_ref.abs().max()))
     assert float((dW.double().cpu() - gW).abs().max()) <= tol_g * max(1.0, float(gW.abs().max()))
     assert float((db.double().cpu() - gb).abs().max()) <= tol_g * max(1.0, float(gb.abs().max()))
 
