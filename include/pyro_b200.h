@@ -106,14 +106,8 @@ typedef struct {
                                     reference's small fixtures) */
 #define B2_FLAG_GLM_FP32 2       /* b2_glm_bernoulli_logits: fp32 SIMT contractions instead of the
                                     tensor-core path */
-#define B2_FLAG_GLM_TF32 8       /* b2_glm_bernoulli_logits: single-pass TF32 logits (opt-in, ~1e-3
-                                    relative per logit) instead of the default 3xTF32 split */
 #define B2_FLAG_GLM_3XTF32 32    /* b2_glm_bernoulli_logits: split X as well as W (every logit exact to
                                     ~1e-6; the default splits W only, see below) */
-#define B2_FLAG_GLM_BF16_GRAD 64 /* b2_glm_bernoulli_logits (opt-in): gradient contraction in BF16 -- half
-                                    the MMAs, operand rounding 2^-9 (see below) */
-#define B2_FLAG_GLM_MMA_SYNC 16  /* b2_glm_bernoulli_logits: the legacy mma.sync kernel (single-pass
-                                    TF32) instead of the wgmma/TMA kernel */
 
 /*
  * b2_site_score -- fused log_prob + score of one sample site for an elementwise family.
@@ -273,17 +267,16 @@ int b2_elbo_combine(const void* const* terms, const double* coeffs, int n, int d
  * X: [N,D] row-major fp32 (16-byte aligned), D in {4, 8, 16, 32}; W: [P,D]; b: [P] (nullable);
  * y: [N] fp32.
  * out_total (nullable): scalar, (=|+=) sum_coeff * scale * SUM_p sum_p[p].
- * For D == 32 the two contractions run on the tensor cores (wgmma) out of TMA-staged tiles with
- * register accumulators (glm_tc.cu).  Default precision: W is split hi + lo (two TF32 MMAs per k-step), which
- * removes the only error that is COHERENT over rows (a rounded W shifts every row's logit the same way
- * and survives the N-term sums); X and g = y - sigmoid are rounded to nearest TF32 (incoherent, averages
- * as 1/sqrt(N)): sum_p, dW, db agree with an fp64 evaluation to ~1e-6 / ~1e-5 relative at N = 1e6.
- * B2_FLAG_GLM_BF16_GRAD (opt-in): the gradient contraction in BF16 (half the MMAs); operand rounding
- * 2^-9, unbiased -- 3e-5 of the largest
- * entry on dW for generic W, but a noise floor of ~1e-3 sqrt(N) that shows when the gradient itself is ~sqrt(N)
- * (balanced data, near a stationary point), which is why it is not the default.
- * B2_FLAG_GLM_3XTF32: X split as well (every logit fp32-exact); B2_FLAG_GLM_TF32: single-pass TF32;
- * B2_FLAG_GLM_MMA_SYNC: the round-1 mma.sync kernel; B2_FLAG_GLM_FP32: the fp32 SIMT kernel.
+ * For D == 32 and N >= 8192 the two contractions run on the tensor cores (wgmma) out of TMA-staged
+ * tiles with register accumulators (glm_tc.cu).  Default precision: W is split hi + lo (two TF32 MMAs per
+ * k-step), which removes the only error that is COHERENT over rows (a rounded W shifts every row's logit
+ * the same way and survives the N-term sums); X and g = y - sigmoid are rounded to nearest TF32
+ * (incoherent, averages as 1/sqrt(N)): sum_p, dW, db agree with an fp64 evaluation to ~1e-6 / ~1e-5
+ * relative at N = 1e6.  Below 65536 rows, and at any N with B2_FLAG_GLM_3XTF32, X is split as well
+ * (every logit fp32-exact).  All other calls run the fp32 SIMT kernel: D != 32, N < 8192 without
+ * B2_FLAG_GLM_3XTF32, B2_FLAG_GLM_FP32, a y that is not 16-byte aligned (the tensor-core kernel loads
+ * y with TMA) and N >= 2^31.  Flag bits 8, 16 and 64 selected variants removed in version 101 and are
+ * ignored.
  * workspace: b2_glm_workspace() bytes, zero-initialised ONCE by the caller (its first 256 bytes
  * hold a ticket counter that the library leaves zeroed).  Two launches: the streaming kernel
  * and a finish kernel that sums the CTA partials in a fixed order (deterministic).

@@ -7,11 +7,12 @@
 // N=1e6, D=32), instead of materialising the [P,N] logits / log_prob / grad tensors that the
 // reference chain (matmul -> Bernoulli.log_prob -> sum -> backward) writes and re-reads.
 //
-// SIMT formulation (first version): CTA = 256 threads = 4 row groups x 64 particles.  Each thread
+// fp32 SIMT kernel (D != 32, N < 8192 rows, B2_FLAG_GLM_FP32, and operands the wgmma kernel of
+// glm_tc.cu cannot load): CTA = 256 threads = 4 row groups x 64 particles.  Each thread
 // keeps W[p,:] and its dW[p,:] accumulator in registers; X tiles are staged through shared memory
 // with cp.async double buffering and read back as warp-wide broadcasts (every lane of a warp has a
 // different particle but the same row, so an LDS.128 serves 4 FMAs x 2 uses for all 32 lanes).
-// FLOPs = 4*N*D*P; at P=64, D=32 the FMA pipe, not HBM, bounds this version (see DESIGN.md).
+// FLOPs = 4*N*D*P; at P=64, D=32 the FMA pipe, not HBM, bounds this kernel (see DESIGN.md).
 #include <cuda_pipeline.h>
 
 #include "b2_common.cuh"
@@ -185,14 +186,10 @@ __global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict
   }
 }
 
-// tensor-core variant (glm_mma.cu)
-int glm_mma_grid_x(int64_t N);
-void launch_glm_mma(const float* X, const float* y, const float* W, const float* b, int64_t N, int P,
-                    float* partials, int gx, cudaStream_t s);
 // wgmma + TMA variant (glm_tc.cu)
 int glm_tc_grid_x(int64_t N);
 int launch_glm_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int P,
-                  float* partials, int gx, int mode, cudaStream_t s);
+                  float* partials, int gx, bool split_x, cudaStream_t s);
 
 inline int glm_grid_x(int64_t N) {
   const int64_t ntiles = (N + kGlmTileRows - 1) / kGlmTileRows;
@@ -224,26 +221,19 @@ extern "C" int b2_glm_bernoulli_logits(const float* X, const float* y, const flo
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   // below 8 Ki rows the single-pass TF32 gradient contraction has not averaged its operand rounding
   // (2^-12 relative per term) below the fp32 tolerance yet: those sizes take the exact fp32 SIMT kernel
-  // unless a tensor-core variant is asked for explicitly
-  const bool forced_tc = flags & (B2_FLAG_GLM_TF32 | B2_FLAG_GLM_3XTF32 | B2_FLAG_GLM_MMA_SYNC | B2_FLAG_GLM_BF16_GRAD);
-  const bool use_tensor = (D == 32) && !(flags & B2_FLAG_GLM_FP32) && (N >= 8192 || forced_tc);
-  const bool use_tc = use_tensor && !(flags & B2_FLAG_GLM_MMA_SYNC) &&
-                      reinterpret_cast<uintptr_t>(y) % 16 == 0 && N < ((int64_t)1 << 31);
-  const bool use_mma = use_tensor && !use_tc;
-  const int gx = use_tc ? glm_tc_grid_x(N) : (use_mma ? glm_mma_grid_x(N) : glm_grid_x(N));
+  // unless the tensor-core kernel is asked for explicitly (B2_FLAG_GLM_3XTF32).  The TMA loads need a
+  // 16-byte aligned y and 32-bit row coordinates; other operands take the SIMT kernel as well.
+  const bool use_tc = (D == 32) && !(flags & B2_FLAG_GLM_FP32) && reinterpret_cast<uintptr_t>(y) % 16 == 0 &&
+                      N < ((int64_t)1 << 31) && (N >= 8192 || (flags & B2_FLAG_GLM_3XTF32));
+  const int gx = use_tc ? glm_tc_grid_x(N) : glm_grid_x(N);
   dim3 grid((unsigned)gx, (unsigned)((P + kGlmParticles - 1) / kGlmParticles), 1);
   unsigned int* ticket = reinterpret_cast<unsigned int*>(workspace);
   float* partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
   if (use_tc) {
     // default: W split; below 64 Ki rows the incoherent X rounding has not averaged out yet -> full 3xTF32
-    // B2_FLAG_GLM_BF16_GRAD (opt-in): BF16 gradient contraction (MODE 3)
-    const int mode = (flags & B2_FLAG_GLM_TF32) ? 0
-                     : ((flags & B2_FLAG_GLM_BF16_GRAD) ? 3
-                        : (((flags & B2_FLAG_GLM_3XTF32) || N < 65536) ? 2 : 1));
-    const int rc = launch_glm_tc(X, y, W, b, N, P, partials, gx, mode, s);
+    const bool split_x = (flags & B2_FLAG_GLM_3XTF32) || N < 65536;
+    const int rc = launch_glm_tc(X, y, W, b, N, P, partials, gx, split_x, s);
     if (rc != 0) return rc;
-  } else if (use_mma) {
-    launch_glm_mma(X, y, W, b, N, P, partials, gx, s);
   } else
   switch (D) {
     case 4: glm_bernoulli_kernel<4><<<grid, 256, 0, s>>>(X, y, W, b, N, P, partials); break;

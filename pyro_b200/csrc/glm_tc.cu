@@ -10,13 +10,13 @@
 // Per 64-row tile (one persistent CTA per SM, tiles round-robin over CTAs, and inside a CTA round-robin
 // over its three warpgroups; each warpgroup owns a whole tile):
 //
-//   split    the warpgroup rounds its X tile to nearest TF32 in place (MODE 2: X_hi / X_lo split) and
+//   split    the warpgroup rounds its X tile to nearest TF32 in place (SPLIT_X: X_hi / X_lo split) and
 //            writes the transposed X^T[d][n] (plus 8 rows of ones) as the K-major B operand of GEMM 2.
 //   GEMM 1   D1[n, p] = sum_d X[n, d] W[p, d] + b[p]      wgmma m64n64k8, K = 32, accumulator = bias.
-//            default (MODE 1): W split hi + lo, two TF32 MMAs per k-step -- the rounding of W is the only
-//            error of a TF32 GEMM 1 that is COHERENT over rows (it shifts all N logits of a particle the
-//            same way and survives the N-term sums); X is rounded to nearest (incoherent, averages as
-//            1/sqrt(N)).  MODE 2 splits X as well (every logit exact to ~1e-6), MODE 0 is single-pass TF32.
+//            W is split hi + lo, two TF32 MMAs per k-step -- the rounding of W is the only error of a
+//            TF32 GEMM 1 that is COHERENT over rows (it shifts all N logits of a particle the same way
+//            and survives the N-term sums); X is rounded to nearest (incoherent, averages as 1/sqrt(N)).
+//            SPLIT_X splits X as well (a third MMA per k-step; every logit exact to ~1e-6).
 //   epilogue each thread holds 2 rows x 16 particles of D1 in registers, evaluates lp = y*l - softplus(l),
 //            g = y - sigmoid(l) (3 MUFU + ~12 FMA-pipe ops per element, in batches of 8 so the MUFU latency
 //            is covered inside the warp), keeps per-particle lp sums in registers and stores g^T (rounded to
@@ -25,7 +25,6 @@
 //            round-to-nearest operands (unbiased; |err| <= 2^-11 sum|g x|).  The accumulator stays in
 //            registers for the whole kernel; GEMM 2 of a tile runs while the warpgroup waits for its next
 //            tile, and the three warpgroups of a CTA overlap each other's phases.
-//            MODE 3 (B2_FLAG_GLM_BF16_GRAD, opt-in): GEMM 2 in BF16 (m64n40k16, half the MMAs).
 //
 // TF32 wgmma operands must be K-major, so the split pass transposes X once per tile in shared memory.
 // Every operand tile is K-major SWIZZLE_128B (the layout TMA writes natively for the X tile).
@@ -38,7 +37,6 @@
 // Determinism: every CTA writes its partials once (warpgroups summed in a fixed order); glm_finish_kernel
 // adds the CTA partials in a fixed order.
 #include <cuda.h>
-#include <cuda_bf16.h>
 #include <stdlib.h>
 
 #include "b2_common.cuh"
@@ -59,9 +57,9 @@ constexpr uint32_t kXtBlock = (kD + 8) * 128;   // X^T k-block: 32 rows of d + 8
 constexpr uint32_t kGBlock = kP * 128;          // g^T k-block: 64 rows of p, 32 n each (8 KB)
 
 // per-warpgroup region
-constexpr uint32_t WG_G = 0;                        // g^T  [kb 2][p 64][32 n] fp32 (BF16: [p 64][64 n])
-constexpr uint32_t WG_XT = WG_G + 2 * kGBlock;      // X^T  [kb 2][c 40][32 n] fp32 (BF16: [c 40][64 n])
-constexpr uint32_t WG_XLO = WG_XT + 2 * kXtBlock;   // X_lo [n 64][32 d] fp32 (MODE 2)
+constexpr uint32_t WG_G = 0;                        // g^T  [kb 2][p 64][32 n] fp32
+constexpr uint32_t WG_XT = WG_G + 2 * kGBlock;      // X^T  [kb 2][c 40][32 n] fp32
+constexpr uint32_t WG_XLO = WG_XT + 2 * kXtBlock;   // X_lo [n 64][32 d] fp32 (SPLIT_X)
 constexpr uint32_t kWGBytes = WG_XLO + kTile;
 // CTA layout (every operand region 1024-byte aligned: the 128-byte swizzle pattern is taken from address bits)
 constexpr uint32_t OFF_X = 0;
@@ -167,19 +165,6 @@ __device__ __forceinline__ void wgmma_n40_tf32(float (&d)[20], uint64_t a, uint6
       : "l"(a), "l"(b), "r"(1)
       : "memory");
 }
-// D[64 x 40] += A[64 x 16] B[40 x 16]^T, BF16, both operands K-major
-__device__ __forceinline__ void wgmma_n40_bf16(float (&d)[20], uint64_t a, uint64_t b) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %22, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n40k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19}, "
-      "%20, %21, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
-      : "l"(a), "l"(b), "r"(1)
-      : "memory");
-}
 
 __device__ __forceinline__ float ex2f(float x) {
   float r;
@@ -203,7 +188,7 @@ __device__ __forceinline__ float tf32_rn(float x) {
 
 // B elements at once, stage by stage: the MUFU results are consumed a whole stage (>= B instructions)
 // after they were issued, so their latency is covered inside the warp instead of by warp switching.
-template <bool MASK, int B, bool RAW = false>
+template <bool MASK, int B>
 __device__ __forceinline__ void epi_batch(const float* lr, float y, float vw, float* acc, float* g) {
   float e[B], den[B], inv[B], lg[B];
 #pragma unroll
@@ -235,23 +220,21 @@ __device__ __forceinline__ void epi_batch(const float* lr, float y, float vw, fl
     } else {
       acc[j] = fmaf(lg[j], -0.6931471805599453f, acc[j]);
     }
-    g[j] = RAW ? gg : tf32_rn(gg);
+    g[j] = tf32_rn(gg);
   }
 }
 
-// MODE 0: single-pass TF32 logits.  MODE 1 (default): W split hi/lo.  MODE 2: full 3xTF32 (X split as
-// well).  MODE 3: logits as MODE 1, GEMM 2 in BF16 (operand rounding 2^-9, unbiased; opt-in).
+// SPLIT_X = false (default): W split hi/lo, X rounded to nearest.  SPLIT_X = true: full 3xTF32, X split
+// hi/lo as well.
 //
 // wgmma accumulator fragment (m64nN, f32): thread (warp w4 of the warpgroup, lane = 4 gid + t4) holds
 // d[4j + 2h + e] = D[16 w4 + gid + 8h][8j + 2 t4 + e].
-template <int MODE>
+template <bool SPLIT_X>
 __global__ void __launch_bounds__(kThreads, 1)
 glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_y,
                         const float* __restrict__ W, const float* __restrict__ bvec, int64_t N, int P,
                         float* __restrict__ partials) {
   pdl_enter();   // lets glm_finish_kernel be resident (blocked in its griddepcontrol.wait) before this kernel ends
-  constexpr bool BF = (MODE == 3);           // GEMM 2 in BF16
-  constexpr int LM = BF ? 1 : MODE;          // precision mode of the logits (GEMM 1)
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
@@ -278,22 +261,15 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
       const int p = e >> 5, d = e & 31;
       const int gp = slab * kP + p;
       const float w = (gp < P) ? W[(int64_t)gp * kD + d] : 0.f;
-      const float hi = (LM >= 1) ? tf32_trunc(w) : tf32_rn(w);
+      const float hi = tf32_trunc(w);
       const int off = p * 32 + ((((d >> 2) ^ (p & 7)) << 2) | (d & 3));   // float index, 128B swizzle
       whi[off] = hi;
       wlo[off] = w - hi;
     }
     // rows 32..39 of every X^T buffer are ones: GEMM 2 then yields db in column 32 of its accumulator
-    if (!BF) {
-      for (int e = tid; e < kWG * 2 * 256; e += kThreads) {
-        const int g = e >> 9, kb = (e >> 8) & 1, w = e & 255;
-        reinterpret_cast<float*>(sm + OFF_WG + g * kWGBytes + WG_XT + kb * kXtBlock + kD * 128)[w] = 1.f;
-      }
-    } else {
-      for (int e = tid; e < kWG * 8 * 64; e += kThreads) {
-        const int g = e >> 9, w = e & 511;
-        reinterpret_cast<__nv_bfloat16*>(sm + OFF_WG + g * kWGBytes + WG_XT + kD * 128)[w] = __float2bfloat16(1.f);
-      }
+    for (int e = tid; e < kWG * 2 * 256; e += kThreads) {
+      const int g = e >> 9, kb = (e >> 8) & 1, w = e & 255;
+      reinterpret_cast<float*>(sm + OFF_WG + g * kWGBytes + WG_XT + kb * kXtBlock + kD * 128)[w] = 1.f;
     }
   }
   fence_proxy_async();
@@ -353,7 +329,7 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
           float xr[4];
 #pragma unroll
           for (int q = 0; q < 4; ++q) xr[q] = tf32_rn(x[q]);
-          if (LM == 2) {
+          if (SPLIT_X) {
             float h[4];
 #pragma unroll
             for (int q = 0; q < 4; ++q) h[q] = tf32_trunc(x[q]);
@@ -365,15 +341,9 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             const int d = c * 4 + q;
-            if (BF) {
-              // X^T[d][n = r] bf16: 16-byte chunk (r >> 3) ^ (d & 7), element r & 7
-              *reinterpret_cast<__nv_bfloat16*>(my + WG_XT + d * 128 + ((((r >> 3) ^ (d & 7))) << 4) + (r & 7) * 2) =
-                  __float2bfloat16(x[q]);
-            } else {
-              // X^T[d][n = r]: k-block r >> 5, 16-byte chunk ((r & 31) >> 2) ^ (d & 7), element r & 3
-              reinterpret_cast<float*>(my + WG_XT + (r >> 5) * kXtBlock)[d * 32 + (((((r & 31) >> 2) ^ (d & 7)) << 2) |
-                                                                                   (r & 3))] = xr[q];
-            }
+            // X^T[d][n = r]: k-block r >> 5, 16-byte chunk ((r & 31) >> 2) ^ (d & 7), element r & 3
+            reinterpret_cast<float*>(my + WG_XT + (r >> 5) * kXtBlock)[d * 32 + (((((r & 31) >> 2) ^ (d & 7)) << 2) |
+                                                                                 (r & 3))] = xr[q];
           }
         }
       }
@@ -394,8 +364,8 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
         wgmma_n64_tf32(acc1, d_x + 2 * k, d_whi + 2 * k);
-        if (LM >= 1) wgmma_n64_tf32(acc1, d_x + 2 * k, d_wlo + 2 * k);
-        if (LM == 2) wgmma_n64_tf32(acc1, d_xlo + 2 * k, d_whi + 2 * k);
+        wgmma_n64_tf32(acc1, d_x + 2 * k, d_wlo + 2 * k);
+        if (SPLIT_X) wgmma_n64_tf32(acc1, d_xlo + 2 * k, d_whi + 2 * k);
       }
       wgmma_commit();
       wgmma_wait0();
@@ -416,20 +386,15 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
           for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
             for (int e = 0; e < 2; ++e) l[2 * jj + e] = acc1[4 * (4 * half + jj) + 2 * h + e];
-          if (tail) epi_batch<true, 8, BF>(l, yv, vw, lpa + 8 * half, g);
-          else epi_batch<false, 8, BF>(l, yv, 1.f, lpa + 8 * half, g);
+          if (tail) epi_batch<true, 8>(l, yv, vw, lpa + 8 * half, g);
+          else epi_batch<false, 8>(l, yv, 1.f, lpa + 8 * half, g);
 #pragma unroll
           for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
               const int p = 8 * (4 * half + jj) + 2 * t4 + e;
-              if (BF) {
-                *reinterpret_cast<__nv_bfloat16*>(my + WG_G + p * 128 + (((n >> 3) ^ (p & 7)) << 4) + (n & 7) * 2) =
-                    __float2bfloat16(g[2 * jj + e]);
-              } else {
-                *reinterpret_cast<float*>(my + WG_G + (n >> 5) * kGBlock + p * 128 +
-                                          (((((n & 31) >> 2) ^ (p & 7))) << 4) + (n & 3) * 4) = g[2 * jj + e];
-              }
+              *reinterpret_cast<float*>(my + WG_G + (n >> 5) * kGBlock + p * 128 +
+                                        (((((n & 31) >> 2) ^ (p & 7))) << 4) + (n & 3) * 4) = g[2 * jj + e];
             }
         }
       }
@@ -437,17 +402,11 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
       wg_bar(1 + wg);
       // ---- GEMM 2: [dW | db] += g^T [X | 1], left running while the next tile is waited for ----------
       wgmma_fence();
-      if (BF) {
-        const uint64_t da = desc_sw128(my_s + WG_G), db = desc_sw128(my_s + WG_XT);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_n40_bf16(acc2, da + 2 * k, db + 2 * k);
-      } else {
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const uint64_t da = desc_sw128(my_s + WG_G + (k >> 2) * kGBlock) + 2 * (k & 3);
-          const uint64_t db = desc_sw128(my_s + WG_XT + (k >> 2) * kXtBlock) + 2 * (k & 3);
-          wgmma_n40_tf32(acc2, da, db);
-        }
+      for (int k = 0; k < 8; ++k) {
+        const uint64_t da = desc_sw128(my_s + WG_G + (k >> 2) * kGBlock) + 2 * (k & 3);
+        const uint64_t db = desc_sw128(my_s + WG_XT + (k >> 2) * kXtBlock) + 2 * (k & 3);
+        wgmma_n40_tf32(acc2, da, db);
       }
       wgmma_commit();
     }
@@ -531,7 +490,7 @@ int glm_tc_grid_x(int64_t N) {
 
 // returns 0 on success, a negative B2_ERR code when the TMA path cannot be used for these operands
 int launch_glm_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int P,
-                  float* partials, int gx, int mode, cudaStream_t s) {
+                  float* partials, int gx, bool split_x, cudaStream_t s) {
   using namespace tc;
   EncodeTiledFn enc = encode_fn();
   if (enc == nullptr) return B2_ERR_LAUNCH;
@@ -560,21 +519,15 @@ int launch_glm_tc(const float* X, const float* y, const float* W, const float* b
   }
   static bool attr_set = false;
   if (!attr_set) {
-    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
     attr_set = true;
   }
   dim3 grid((unsigned)gx, (unsigned)((P + kP - 1) / kP), 1);
-  if (mode == 3)
-    launch_pdl(glm_bernoulli_tc_kernel<3>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, W, b, N, P, partials);
-  else if (mode == 2)
-    launch_pdl(glm_bernoulli_tc_kernel<2>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, W, b, N, P, partials);
-  else if (mode == 1)
-    launch_pdl(glm_bernoulli_tc_kernel<1>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, W, b, N, P, partials);
+  if (split_x)
+    launch_pdl(glm_bernoulli_tc_kernel<true>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, W, b, N, P, partials);
   else
-    launch_pdl(glm_bernoulli_tc_kernel<0>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, W, b, N, P, partials);
+    launch_pdl(glm_bernoulli_tc_kernel<false>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, W, b, N, P, partials);
   return 0;
 }
 

@@ -29,7 +29,7 @@ def test_header_symbols_are_exported():
 
 def test_argument_validation_without_gpu():
     L = N.lib()
-    assert L.b2_version() >= 100
+    assert L.b2_version() >= 101
     assert L.b2_last_error(-3).decode().startswith("unknown distribution family")
     assert L.b2_site_score_workspace() > 0
     t = N.b2_tensor()
