@@ -8,31 +8,39 @@
 // and the autograd backward of all three.
 //
 // Per 64-row tile (one persistent CTA per SM, tiles round-robin over CTAs, and inside a CTA round-robin
-// over its three warpgroups; each warpgroup owns a whole tile):
+// over its four warpgroups; each warpgroup owns a whole tile):
 //
 //   split    the warpgroup rounds its X tile to nearest TF32 in place (SPLIT_X: X_hi / X_lo split) and
-//            writes the transposed X^T[d][n] (plus 8 rows of ones) as the K-major B operand of GEMM 2.
-//   GEMM 1   D1[n, p] = sum_d X[n, d] W[p, d] + b[p]      wgmma m64n64k8, K = 32, accumulator = bias.
+//            writes the transposed X^T[d][n] (plus 8 rows of ones) as the K-major B operand of GEMM 2, with
+//            n permuted inside each group of 8 rows (kt_pos) to match the register layout of g.
+//   GEMM 1   D1^T[p, n] = sum_d W[p, d] X[n, d] + b[p]    wgmma m64n64k8, K = 32, A = W, B = the X tile
+//            (both K-major as they sit in shared memory), accumulator = bias.
 //            W is split hi + lo, two TF32 MMAs per k-step -- the rounding of W is the only error of a
 //            TF32 GEMM 1 that is COHERENT over rows (it shifts all N logits of a particle the same way
 //            and survives the N-term sums); X is rounded to nearest (incoherent, averages as 1/sqrt(N)).
 //            SPLIT_X splits X as well (a third MMA per k-step; every logit exact to ~1e-6).
-//   epilogue each thread holds 2 rows x 16 particles of D1 in registers, evaluates lp = y*l - softplus(l),
-//            g = y - sigmoid(l) (3 MUFU + ~12 FMA-pipe ops per element, in batches of 8 so the MUFU latency
-//            is covered inside the warp), keeps per-particle lp sums in registers and stores g^T (rounded to
-//            nearest TF32) into shared memory as the K-major A operand of GEMM 2.
-//   GEMM 2   [dW | db][p, :] += sum_n g[n, p] [X | 1][n, :]   wgmma m64n40k8, K = 64: single-pass TF32 on
-//            round-to-nearest operands (unbiased; |err| <= 2^-11 sum|g x|).  The accumulator stays in
-//            registers for the whole kernel; GEMM 2 of a tile runs while the warpgroup waits for its next
-//            tile, and the three warpgroups of a CTA overlap each other's phases.
+//   epilogue each thread holds 2 particles x 16 rows of D1^T in registers, evaluates lp = y*l - softplus(l),
+//            g = y - sigmoid(l) (3 MUFU + ~12 FMA-pipe ops per element, in batches of 4 so part of the MUFU
+//            latency is covered inside the warp), keeps its two per-particle lp sums in registers and rounds g to
+//            nearest TF32.  g stays in the registers: it is already the A fragment of GEMM 2.
+//   GEMM 2   [dW | db][p, :] += sum_n g[p, n] [X | 1][n, :]   wgmma m64n40k8, K = 64, A from registers:
+//            single-pass TF32 on round-to-nearest operands (unbiased; |err| <= 2^-11 sum|g x|).  The
+//            accumulator stays in registers for the whole kernel; GEMM 2 of a tile is committed and left
+//            running while the warpgroup waits for its next tile (the wait sits at the top of the tile
+//            loop), and the warpgroups of a CTA overlap each other's phases.
+//
+// No ordinary instruction writes a wgmma accumulator between the start and the end of a wgmma pipeline
+// stage: ptxas would serialise every wgmma of the kernel (C7515).  So GEMM 2's accumulator is started by
+// the first k-step of the warpgroup's first tile with scale-d = 0 rather than zeroed, and the g registers
+// are pinned before wgmma.fence.  tests/test_glm_tc_sass.py checks the SASS for this.
 //
 // TF32 wgmma operands must be K-major, so the split pass transposes X once per tile in shared memory.
-// Every operand tile is K-major SWIZZLE_128B (the layout TMA writes natively for the X tile).
+// Every shared-memory operand tile is K-major SWIZZLE_128B (the layout TMA writes natively for the X tile).
 //
-// 384 threads = three warpgroups and no producer warp: registers are allocated to groups of 4 warps, so a
-// 13th warp would cost the consumers 40 registers each.  Each warpgroup double-buffers its own X/y tiles:
+// 512 threads = four warpgroups and no producer warp, so each scheduler has four warps to switch between
+// while MUFU results are pending; that caps the kernel at 128 registers per thread.  Each warpgroup double-buffers its own X/y tiles:
 // one thread issues the TMA load of tile j+2 into the stage of tile j as soon as GEMM 1 has read it (an
-// mbarrier per stage counts the transaction bytes); g^T, X^T and X_lo are private to each warpgroup.
+// mbarrier per stage counts the transaction bytes); X^T and X_lo are private to each warpgroup.
 //
 // Determinism: every CTA writes its partials once (warpgroups summed in a fixed order); glm_finish_kernel
 // adds the CTA partials in a fixed order.
@@ -47,18 +55,16 @@ namespace tc {
 constexpr int kRows = 64;                       // rows per tile = M of one wgmma
 constexpr int kD = 32;
 constexpr int kP = 64;
-constexpr int kWG = 3;                          // warpgroups
+constexpr int kWG = 4;                          // warpgroups
 constexpr int kStages = 2 * kWG;                // two X/y stages per warpgroup
 constexpr int kThreads = kWG * 128;
 
 constexpr uint32_t kTile = kRows * kD * 4;      // 8 KB X tile
 constexpr uint32_t kYBytes = kRows * 4;         // 256 B of y
 constexpr uint32_t kXtBlock = (kD + 8) * 128;   // X^T k-block: 32 rows of d + 8 rows of ones, 32 n each (5 KB)
-constexpr uint32_t kGBlock = kP * 128;          // g^T k-block: 64 rows of p, 32 n each (8 KB)
 
 // per-warpgroup region
-constexpr uint32_t WG_G = 0;                        // g^T  [kb 2][p 64][32 n] fp32
-constexpr uint32_t WG_XT = WG_G + 2 * kGBlock;      // X^T  [kb 2][c 40][32 n] fp32
+constexpr uint32_t WG_XT = 0;                       // X^T  [kb 2][c 40][32 n] fp32, n permuted (see kt_pos)
 constexpr uint32_t WG_XLO = WG_XT + 2 * kXtBlock;   // X_lo [n 64][32 d] fp32 (SPLIT_X)
 constexpr uint32_t kWGBytes = WG_XLO + kTile;
 // CTA layout (every operand region 1024-byte aligned: the 128-byte swizzle pattern is taken from address bits)
@@ -71,8 +77,8 @@ constexpr uint32_t OFF_BAR = OFF_WG + kWG * kWGBytes;
 constexpr uint32_t kSmemBytes = OFF_BAR + 256 + 1024;   // + slack for the 1024-byte alignment
 static_assert(kStages * kYBytes <= 2048 && kSmemBytes <= 232448, "shared memory budget");
 static_assert(kWGBytes % 1024 == 0 && kXtBlock % 1024 == 0, "operand alignment");
-// the final reduction reuses the X ring: [kWG][64 p][33] + [kWG * 4 warps][64 p] floats
-static_assert((kWG * kP * 33 + kWG * 4 * kP) * 4 <= kStages * kTile, "reduction scratch");
+// the final reduction reuses the X ring: [kWG][64 p][33] + [kWG][64 p] floats
+static_assert((kWG * kP * 33 + kWG * kP) * 4 <= kStages * kTile, "reduction scratch");
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);
@@ -136,6 +142,12 @@ __device__ __forceinline__ void fence_regs(float (&r)[N]) {
 #pragma unroll
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
+// pins register A operands before wgmma.fence (a definition after it makes ptxas insert warpgroup.arrive)
+template <int N>
+__device__ __forceinline__ void fence_regs(uint32_t (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
+}
 
 // D[64 x 64] += A[64 x 8] B[64 x 8]^T, TF32, both operands K-major in shared memory
 __device__ __forceinline__ void wgmma_n64_tf32(float (&d)[32], uint64_t a, uint64_t b) {
@@ -152,17 +164,18 @@ __device__ __forceinline__ void wgmma_n64_tf32(float (&d)[32], uint64_t a, uint6
       : "l"(a), "l"(b), "r"(1)
       : "memory");
 }
-// D[64 x 40] += A[64 x 8] B[40 x 8]^T, TF32
-__device__ __forceinline__ void wgmma_n40_tf32(float (&d)[20], uint64_t a, uint64_t b) {
+// D[64 x 40] = A[64 x 8] B[40 x 8]^T (+ D when acc != 0), TF32, A from registers: thread (warp w4 of the
+// warpgroup, lane = 4 gid + t4) passes a[i] = A[16 w4 + gid + 8 (i & 1)][t4 + 4 (i >> 1)]
+__device__ __forceinline__ void wgmma_n40_tf32_ra(float (&d)[20], const uint32_t (&a)[4], uint64_t b, int acc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %22, 0;\n\t"
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %25, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n40k8.f32.tf32.tf32 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19}, "
-      "%20, %21, p, 1, 1;\n\t}"
+      "{%20, %21, %22, %23}, %24, p, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
         "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
         "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
-      : "l"(a), "l"(b), "r"(1)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
       : "memory");
 }
 
@@ -186,11 +199,14 @@ __device__ __forceinline__ float tf32_rn(float x) {
   return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
 }
 
-// B elements at once, stage by stage: the MUFU results are consumed a whole stage (>= B instructions)
-// after they were issued, so their latency is covered inside the warp instead of by warp switching.
-template <bool MASK, int B>
-__device__ __forceinline__ void epi_batch(const float* lr, float y, float vw, float* acc, float* g) {
-  float e[B], den[B], inv[B], lg[B];
+// Four logits of one particle at once, stage by stage: each MUFU result is consumed a stage (>= 4
+// instructions) after it was issued, and the four warps per scheduler cover the rest of the MUFU latency
+// (a batch of 8 would not fit 128 registers).  Returns the sum of lp = y*l - softplus(l) over the four and
+// writes g = y - sigmoid(l) rounded to nearest TF32.  MASK weights both with vw (0 for rows past N).
+template <bool MASK>
+__device__ __forceinline__ float epi_batch(const float* lr, const float* y, const float* vw, uint32_t* g) {
+  constexpr int B = 4;
+  float e[B], den[B], inv[B], lg[B], lp[B];
 #pragma unroll
   for (int j = 0; j < B; ++j) e[j] = ex2f(-1.4426950408889634f * fabsf(lr[j]));
 #pragma unroll
@@ -202,27 +218,22 @@ __device__ __forceinline__ void epi_batch(const float* lr, float y, float vw, fl
 #pragma unroll
   for (int j = 0; j < B; ++j) {
     const float l = lr[j];
-    if (MASK) {
-      acc[j] = fmaf(vw, fmaf(y, l, -fmaxf(l, 0.f)), acc[j]);
-    } else {
-      acc[j] = fmaf(y, l, acc[j]);
-      acc[j] -= fmaxf(l, 0.f);
-    }
-  }
-#pragma unroll
-  for (int j = 0; j < B; ++j) {
-    const float l = lr[j];
+    lp[j] = fmaf(lg[j], -0.6931471805599453f, fmaf(y[j], l, -fmaxf(l, 0.f)));
     const float sg = (l >= 0.f) ? inv[j] : e[j] * inv[j];
-    float gg = y - sg;
+    float gg = y[j] - sg;
     if (MASK) {
-      gg *= vw;
-      acc[j] = fmaf(vw * lg[j], -0.6931471805599453f, acc[j]);
-    } else {
-      acc[j] = fmaf(lg[j], -0.6931471805599453f, acc[j]);
+      lp[j] *= vw[j];
+      gg *= vw[j];
     }
-    g[j] = tf32_rn(gg);
+    g[j] = __float_as_uint(tf32_rn(gg));
   }
+  return (lp[0] + lp[1]) + (lp[2] + lp[3]);
 }
+
+// Position of tile row n in GEMM 2's k order.  GEMM 1's accumulator gives a thread the rows n = 8j + 2 t4 + e
+// (e = 0, 1) of k-block j, and the register A operand of GEMM 2 takes them as k = t4 + 4e; X^T is stored in
+// that order, so g never leaves the registers.
+__device__ __forceinline__ int kt_pos(int n) { return (n & ~7) | ((n & 7) >> 1) | ((n & 1) << 2); }
 
 // SPLIT_X = false (default): W split hi/lo, X rounded to nearest.  SPLIT_X = true: full 3xTF32, X split
 // hi/lo as well.
@@ -275,12 +286,11 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
   fence_proxy_async();
   __syncthreads();
 
-  float lpa[16];                               // per-particle lp sums of the thread's rows (consumers)
-  float acc2[20];                              // GEMM 2 accumulator [p][c]: dW in c < 32, db in c = 32
-#pragma unroll
-  for (int i = 0; i < 16; ++i) lpa[i] = 0.f;
-#pragma unroll
-  for (int i = 0; i < 20; ++i) acc2[i] = 0.f;
+  float lpa[2] = {0.f, 0.f};                   // lp sums of the thread's two particles
+  // GEMM 2 accumulator [p][c]: dW in c < 32, db in c = 32.  Never written by ordinary instructions before
+  // the tile loop (that serialises every wgmma, C7515): the warpgroup's first GEMM 2 k-step starts it with
+  // scale-d = 0, and a warpgroup without a tile is left out of the CTA reduction.
+  float acc2[20];
   // warp-uniform by construction (a shuffle result), so the tile loop is not a divergent branch to ptxas
   const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0), w4 = warp & 3, t = tid & 127;
   const int gid = lane >> 2, t4 = lane & 3;
@@ -291,14 +301,12 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
     const uint32_t my_s = base + OFF_WG + wg * kWGBytes;
     const uint64_t d_whi = desc_sw128(base + OFF_WHI), d_wlo = desc_sw128(base + OFF_WLO);
     const uint64_t d_xlo = desc_sw128(my_s + WG_XLO);
-    float bias[16];
+    float bias[2];                             // of particles 16 w4 + gid + 8h
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int gp = slab * kP + 8 * j + 2 * t4 + e;
-        bias[2 * j + e] = (bvec != nullptr && gp < P) ? bvec[gp] : 0.f;
-      }
+    for (int h = 0; h < 2; ++h) {
+      const int gp = slab * kP + 16 * w4 + gid + 8 * h;
+      bias[h] = (bvec != nullptr && gp < P) ? bvec[gp] : 0.f;
+    }
     // tile it -> X/y stage; one thread of the warpgroup issues the loads
     auto load = [&](int it, int s) {
       const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
@@ -312,12 +320,12 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
       const int s = 2 * wg + (k & 1);
       const int64_t row0 = (blockIdx.x + (int64_t)it * gridDim.x) * kRows;
       mbar_wait(bar_full(s), (uint32_t)(k >> 1) & 1u);
-      // GEMM 2 of this warpgroup's previous tile has finished reading g^T / X^T
+      // GEMM 2 of this warpgroup's previous tile has finished reading X^T and the g registers
       wgmma_wait0();
       fence_regs(acc2);
       // ---- split / transposition pass: thread t owns 16 columns (chunks 4h .. 4h+3) of row r ----------
       {
-        const int r = t >> 1, hh = t & 1;
+        const int r = t >> 1, hh = t & 1, rk = kt_pos(r);
         float4* xs = reinterpret_cast<float4*>(sm + OFF_X + s * kTile);
         float4* xl = reinterpret_cast<float4*>(my + WG_XLO);
 #pragma unroll
@@ -341,90 +349,78 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             const int d = c * 4 + q;
-            // X^T[d][n = r]: k-block r >> 5, 16-byte chunk ((r & 31) >> 2) ^ (d & 7), element r & 3
-            reinterpret_cast<float*>(my + WG_XT + (r >> 5) * kXtBlock)[d * 32 + (((((r & 31) >> 2) ^ (d & 7)) << 2) |
-                                                                                 (r & 3))] = xr[q];
+            // X^T[d][k = rk]: k-block rk >> 5, 16-byte chunk ((rk & 31) >> 2) ^ (d & 7), element rk & 3
+            reinterpret_cast<float*>(my + WG_XT + (rk >> 5) * kXtBlock)[d * 32 + (((((rk & 31) >> 2) ^ (d & 7)) << 2) |
+                                                                                  (rk & 3))] = xr[q];
           }
         }
       }
-      const float* ys = reinterpret_cast<const float*>(sm + OFF_Y + s * kYBytes);
-      const float y0 = ys[16 * w4 + gid], y1 = ys[16 * w4 + gid + 8];
+      float2 yr[8];                            // y of the thread's rows n = 8j + 2 t4 + e, read before the refill
+#pragma unroll
+      for (int j = 0; j < 8; ++j) yr[j] = reinterpret_cast<const float2*>(sm + OFF_Y + s * kYBytes)[4 * j + t4];
       fence_proxy_async();
       wg_bar(1 + wg);
-      // ---- GEMM 1: logits, accumulator initialised with the bias --------------------------------------
+      // ---- GEMM 1: logits D1^T[p, n] = W X^T + b, accumulator initialised with the bias ---------------
       float acc1[32];
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) acc1[4 * j + 2 * h + e] = bias[2 * j + e];
+      for (int i = 0; i < 32; ++i) acc1[i] = bias[(i >> 1) & 1];
       wgmma_fence();
       const uint64_t d_x = desc_sw128(base + OFF_X + s * kTile);
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        wgmma_n64_tf32(acc1, d_x + 2 * k, d_whi + 2 * k);
-        wgmma_n64_tf32(acc1, d_x + 2 * k, d_wlo + 2 * k);
-        if (SPLIT_X) wgmma_n64_tf32(acc1, d_xlo + 2 * k, d_whi + 2 * k);
+        wgmma_n64_tf32(acc1, d_whi + 2 * k, d_x + 2 * k);
+        wgmma_n64_tf32(acc1, d_wlo + 2 * k, d_x + 2 * k);
+        if (SPLIT_X) wgmma_n64_tf32(acc1, d_whi + 2 * k, d_xlo + 2 * k);
       }
       wgmma_commit();
       wgmma_wait0();
       fence_regs(acc1);
       // GEMM 1 has read the X stage and y is in registers: refill the stage with tile it + 2 kWG
       if (t == 0 && it + 2 * kWG < nt) load(it + 2 * kWG, s);
-      // ---- epilogue: lp sums in registers, g^T into shared memory -------------------------------------
+      // ---- epilogue: lp sums and g, both in registers ----------------------------------------------------
       const bool tail = row0 + kRows > N;
+      uint32_t g[32];                          // indexed like acc1
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int n = 16 * w4 + gid + 8 * h;
-        const float yv = h ? y1 : y0;
-        const float vw = (row0 + n < N) ? 1.f : 0.f;
+      for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          float l[8], g[8];
+        for (int q = 0; q < 4; ++q) {          // k-blocks j = 2q, 2q + 1
+          float l[4], yy[4], vw[4];
+          uint32_t gb[4];
 #pragma unroll
-          for (int jj = 0; jj < 4; ++jj)
+          for (int i = 0; i < 4; ++i) {
+            const int j = 2 * q + (i >> 1), e = i & 1;
+            l[i] = acc1[4 * j + 2 * h + e];
+            yy[i] = e ? yr[j].y : yr[j].x;
+            vw[i] = (row0 + 8 * j + 2 * t4 + e < N) ? 1.f : 0.f;
+          }
+          lpa[h] += tail ? epi_batch<true>(l, yy, vw, gb) : epi_batch<false>(l, yy, vw, gb);
 #pragma unroll
-            for (int e = 0; e < 2; ++e) l[2 * jj + e] = acc1[4 * (4 * half + jj) + 2 * h + e];
-          if (tail) epi_batch<true, 8>(l, yv, vw, lpa + 8 * half, g);
-          else epi_batch<false, 8>(l, yv, 1.f, lpa + 8 * half, g);
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int p = 8 * (4 * half + jj) + 2 * t4 + e;
-              *reinterpret_cast<float*>(my + WG_G + (n >> 5) * kGBlock + p * 128 +
-                                        (((((n & 31) >> 2) ^ (p & 7))) << 4) + (n & 3) * 4) = g[2 * jj + e];
-            }
+          for (int i = 0; i < 4; ++i) g[4 * (2 * q + (i >> 1)) + 2 * h + (i & 1)] = gb[i];
         }
-      }
-      fence_proxy_async();
-      wg_bar(1 + wg);
-      // ---- GEMM 2: [dW | db] += g^T [X | 1], left running while the next tile is waited for ----------
+      // ---- GEMM 2: [dW | db] += g [X | 1], g from registers, left running while the next tile is waited for
+      fence_regs(g);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const uint64_t da = desc_sw128(my_s + WG_G + (k >> 2) * kGBlock) + 2 * (k & 3);
-        const uint64_t db = desc_sw128(my_s + WG_XT + (k >> 2) * kXtBlock) + 2 * (k & 3);
-        wgmma_n40_tf32(acc2, da, db);
+      for (int j = 0; j < 8; ++j) {
+        const uint32_t a[4] = {g[4 * j], g[4 * j + 2], g[4 * j + 1], g[4 * j + 3]};
+        wgmma_n40_tf32_ra(acc2, a, desc_sw128(my_s + WG_XT + (j >> 2) * kXtBlock) + 2 * (j & 3), it != wg || j != 0);
       }
       wgmma_commit();
     }
     wgmma_wait0();
     fence_regs(acc2);
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      float v = lpa[i];
-      v += __shfl_xor_sync(0xffffffffu, v, 4);
-      v += __shfl_xor_sync(0xffffffffu, v, 8);
-      v += __shfl_xor_sync(0xffffffffu, v, 16);
-      lpa[i] = v;
+    for (int h = 0; h < 2; ++h) {
+      float v = lpa[h];
+      v += __shfl_xor_sync(0xffffffffu, v, 1);
+      v += __shfl_xor_sync(0xffffffffu, v, 2);
+      lpa[h] = v;
     }
   }
   // ---- CTA results through shared memory (the X ring is idle now), fixed summation order -----------------
   __syncthreads();
   float* red2 = reinterpret_cast<float*>(sm + OFF_X);     // [kWG][64 p][33]
-  float* redlp = red2 + kWG * kP * 33;                    // [kWG * 4 warps][64 p]
+  float* redlp = red2 + kWG * kP * 33;                    // [kWG][64 p]
   {
 #pragma unroll
     for (int j = 0; j < 5; ++j)
@@ -435,11 +431,9 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
           const int p = 16 * w4 + gid + 8 * h, c = 8 * j + 2 * t4 + e;
           if (c <= kD) red2[(wg * kP + p) * 33 + c] = acc2[4 * j + 2 * h + e];
         }
-    if (gid == 0) {
+    if (t4 == 0) {
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) redlp[warp * kP + 8 * j + 2 * t4 + e] = lpa[2 * j + e];
+      for (int h = 0; h < 2; ++h) redlp[wg * kP + 16 * w4 + gid + 8 * h] = lpa[h];
     }
   }
   __syncthreads();
@@ -449,11 +443,11 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
       float* o = partials + ((int64_t)blockIdx.x * P + gp) * (kD + 2);
       for (int c = 0; c <= kD; ++c) {          // dW[0..31], db
         float v = 0.f;
-        for (int g = 0; g < kWG; ++g) v += red2[(g * kP + tid) * 33 + c];
+        for (int g = 0; g < kWG && g < nt; ++g) v += red2[(g * kP + tid) * 33 + c];
         o[c] = v;
       }
       float v = 0.f;
-      for (int w = 0; w < kWG * 4; ++w) v += redlp[w * kP + tid];
+      for (int g = 0; g < kWG && g < nt; ++g) v += redlp[g * kP + tid];
       o[kD + 1] = v;
     }
   }
