@@ -287,6 +287,34 @@ int b2_glm_bernoulli_logits(const float* X, const float* y, const float* W, cons
                             float* out_db, void* workspace, size_t workspace_bytes, void* stream);
 size_t b2_glm_workspace(int64_t N, int D, int P);
 
+/*
+ * b2_glm_categorical_logits -- fused softmax-regression (multiclass logistic) likelihood term: for P
+ * particles with weights W[p] (K x D) and biases b[p] (K), logits[p,n,k] = <X[n,:], W[p,k,:]> + b[p,k];
+ *   sum_p[p]   = SUM_n ( logits[p,n,y[n]] - logsumexp_k logits[p,n,k] )      (Categorical log_prob)
+ *   dW[p,k,:]  = weight * SUM_n ([k == y[n]] - softmax_k(logits[p,n,:])) * X[n,:]
+ *   db[p,k]    = weight * SUM_n ([k == y[n]] - softmax_k(logits[p,n,:]))
+ * X and y are read from HBM about once for value AND gradient, and no [P,N,K] tensor is written.
+ * X: [N,D] row-major fp32; y: [N] int64 labels; W: [P,K,D]; b: [P,K] (nullable).  Scope: D == 32,
+ * 2 <= K <= 16, P >= 1, 1 <= N < 2^31, X and y 16-byte aligned; any other call returns
+ * B2_ERR_BAD_SHAPE.  A label outside [0, K) makes that particle's sum_p NaN (never an out-of-bounds
+ * read); the other particles are unaffected.
+ * out_total (nullable): scalar, (=|+=) sum_coeff * scale * SUM_p sum_p[p] (B2_FLAG_ACCUMULATE_SUM).
+ * out_sum_p, out_dW, out_db are nullable; dW and db are scaled by weight * scale.
+ * Both contractions run on the tensor cores (wgmma, glm_categorical_tc.cu) with the precision policy of
+ * b2_glm_bernoulli_logits: W is split hi + lo and X rounded to nearest TF32 (incoherent error, averages
+ * as 1/sqrt(N)); below 65536 rows, and at any N with B2_FLAG_GLM_3XTF32, X is split as well (every
+ * logit fp32-exact).  g is rounded to nearest TF32 for the gradient contraction.
+ * workspace: b2_glm_categorical_workspace() bytes, zero-initialised ONCE by the caller (its first 256
+ * bytes hold a ticket counter that the library leaves zeroed).  Two launches: the streaming kernel and
+ * a finish kernel that sums the CTA partials in a fixed order (deterministic, no float atomics).
+ */
+int b2_glm_categorical_logits(const float* X, const int64_t* y, const float* W, const float* b,
+                              int64_t N, int D, int K, int P, double scale, double weight,
+                              double sum_coeff, int flags, float* out_sum_p, float* out_total,
+                              float* out_dW, float* out_db, void* workspace, size_t workspace_bytes,
+                              void* stream);
+size_t b2_glm_categorical_workspace(int64_t N, int D, int K, int P);
+
 /* ---- optimisers --------------------------------------------------------------------------
  * Multi-tensor fused updates replacing PyroOptim's per-parameter Python loop
  * (pyro/optim/optim.py:117-155).  Per-tensor scalar state lives in DEVICE arrays so a captured

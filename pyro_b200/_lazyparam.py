@@ -67,8 +67,12 @@ class LazyExpParam(torch.Tensor):
 def densify(x):
     """What a native kernel (an autograd.Function, opaque to ``__torch_function__``) must be handed: the
     materialised ``exp(u)`` of a :class:`LazyExpParam`; the plain tensor inside a trace-time wrapper that keeps one
-    as ``_t`` (the provenance tags of TraceGraph_ELBO); anything else unchanged."""
+    as ``_t`` (the provenance tags of TraceGraph_ELBO); the materialised logits of a lazy linear predictor
+    (pyro_b200/lazy.py) that reached a distribution other than the fused GLM routes, so that autograd sees its
+    dependence on the weights; anything else unchanged."""
     if isinstance(x, LazyExpParam):
+        return x.dense()
+    if type(x).__name__ == "LinearPredictorTensor":
         return x.dense()
     if type(x) is not torch.Tensor and isinstance(x, torch.Tensor) and hasattr(x, "_provenance"):
         return x._t

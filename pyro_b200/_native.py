@@ -112,6 +112,9 @@ SIGNATURES = {
     "b2_glm_bernoulli_logits": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _f64, _f64, _f64, _i32,
                                        _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2_glm_workspace": (_sz, [_i64, _i32, _i32]),
+    "b2_glm_categorical_logits": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _f64,
+                                         _i32, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "b2_glm_categorical_workspace": (_sz, [_i64, _i32, _i32, _i32]),
     "b2_clipped_adam": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _vp]),
     "b2_adagrad_rmsprop": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _vp]),
     "b2_leapfrog_half_kick_drift": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _i32, _vp]),

@@ -1071,7 +1071,8 @@ class _GlmBernoulliFn(torch.autograd.Function):
 def _lazy_of(logits):
     if isinstance(logits, LinearPredictor):
         return logits
-    return getattr(logits, "_lazy", None) if type(logits).__name__ == "LinearPredictorTensor" else None
+    lz = getattr(logits, "_lazy", None) if type(logits).__name__ == "LinearPredictorTensor" else None
+    return lz if isinstance(lz, LinearPredictor) else None
 
 
 class _BernoulliLinear(Bernoulli):
@@ -1120,7 +1121,163 @@ def _bernoulli_new(cls, probs=None, logits=None, validate_args=None):
 
 
 Bernoulli.__new__ = staticmethod(_bernoulli_new)
-__all__ += ["LinearPredictor", "linear_predictor", "constant"]
+
+
+# ---------------------------------------------------------------------------------------------
+# fused softmax regression: Categorical(logits = X @ W.mT + b)
+# ---------------------------------------------------------------------------------------------
+class ClassLinearPredictor:
+    """Lazy class-axis logits ``X @ W.mT + b`` for K classes: behaves like an ``[N, K]`` logits tensor
+    (``W``: [K, D]) or a ``[P, N, K]`` one (``W``: [P, K, D], vectorised particles) when handed to
+    ``Categorical(logits=...)``, which then scores the site with ONE kernel that reads X and the labels
+    once and emits sum, dW and db (``b2_glm_categorical_logits``).  A separate type from
+    :class:`LinearPredictor`, whose ``[P, D]`` weights are particles, not classes.
+
+    ``Wt`` is the right-hand operand exactly as the model wrote it (``[.., D, K]``, usually the ``W.mT``
+    view); ``b``: None, [K] or [P, 1, K].  ``linear`` records an ``F.linear(X, W[, b])`` call, so that
+    :meth:`dense` repeats the eager computation bit for bit."""
+
+    def __init__(self, X, Wt, b=None, linear=False, linear_bias=False):
+        if type(Wt).__name__ == "SiteValue":
+            Wt = Wt.as_subclass(torch.Tensor)
+        if type(b).__name__ == "SiteValue":
+            b = b.as_subclass(torch.Tensor)
+        self.X, self.Wt, self.b = X, Wt, b
+        self.linear, self.linear_bias = linear, linear_bias
+        self.vectorised = Wt.dim() == 3
+        self.P = Wt.shape[0] if self.vectorised else 1
+        self.K = Wt.shape[-1]
+        n = X.shape[0]
+        self.shape = torch.Size((self.P, n, self.K)) if self.vectorised else torch.Size((n, self.K))
+        self.dtype, self.device = X.dtype, X.device
+
+    @property
+    def W(self):
+        return self.Wt.mT
+
+    def with_bias(self, b):
+        """The predictor plus ``b`` ([K], or [P, 1, K] with vectorised particles), or None."""
+        if self.b is not None or not isinstance(b, torch.Tensor):
+            return None
+        shapes = [(self.K,)] + ([(self.P, 1, self.K)] if self.vectorised else [])
+        if tuple(b.shape) not in shapes or b.dtype != self.dtype or b.device != self.device:
+            return None
+        return ClassLinearPredictor(self.X, self.Wt, b, self.linear)
+
+    def bias_pk(self):
+        """The bias as [P, K] (a view), or None."""
+        return None if self.b is None else self.b.reshape(-1, self.K).expand(self.P, self.K)
+
+    def dense(self):
+        import torch.nn.functional as F
+        if self.linear_bias:
+            return F.linear(self.X, self.W, self.b)
+        out = F.linear(self.X, self.W) if self.linear else self.X @ self.Wt
+        return out if self.b is None else out + self.b
+
+
+def class_linear_predictor(X, W, b=None):
+    """Lazy ``X @ W.mT + b`` with ``W``: [K, D] (logits [N, K]) or [P, K, D] (logits [P, N, K]) and ``b``:
+    None, [K] or [P, 1, K]; other shapes, dtypes or devices raise ValueError."""
+    if not (isinstance(X, torch.Tensor) and X.dim() == 2 and isinstance(W, torch.Tensor) and W.dim() in (2, 3)
+            and W.shape[-1] == X.shape[1] and W.dtype == X.dtype and W.device == X.device):
+        raise ValueError("class_linear_predictor: expected X [N, D] and W [K, D] or [P, K, D] of X's dtype and "
+                         "device, got X %s and W %s" % (tuple(getattr(X, "shape", ())), tuple(getattr(W, "shape", ()))))
+    lp = ClassLinearPredictor(X, W.mT)
+    if b is None:
+        return lp
+    out = lp.with_bias(b.as_subclass(torch.Tensor) if type(b).__name__ == "SiteValue" else b)
+    if out is None:
+        raise ValueError("class_linear_predictor: the bias must be [K]%s of X's dtype and device, got %s"
+                         % (" or [P, 1, K]" if lp.vectorised else "", tuple(getattr(b, "shape", ()))))
+    return out
+
+
+class _GlmCategoricalFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, meta, X, y, W, b):
+        scale, weight, coeff, unit, flags = meta
+        N.require_cuda(X, "fused softmax-regression likelihood")
+        P, K, D = W.shape
+        n = X.shape[0]
+        dev = X.device
+        Wc = W.contiguous()
+        bc = b.contiguous() if b is not None else None
+        total = torch.empty((), dtype=torch.float32, device=dev)
+        dW = torch.empty(P, K, D, dtype=torch.float32, device=dev)
+        db = torch.empty(P, K, dtype=torch.float32, device=dev)
+        need = int(N.lib().b2_glm_categorical_workspace(n, D, K, P))
+        ws = N.workspace(dev, need, tag="glm")
+        N.check(N.lib().b2_glm_categorical_logits(
+            X.data_ptr(), y.data_ptr(), Wc.data_ptr(), bc.data_ptr() if bc is not None else None,
+            n, D, K, P, float(scale), float(weight), float(coeff), int(flags), None, total.data_ptr(),
+            dW.data_ptr(), db.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(dev)),
+            "b2_glm_categorical_logits")
+        ctx.grads = (dW, db if b is not None else None)
+        ctx.unit = unit
+        return total
+
+    @staticmethod
+    def backward(ctx, gout):
+        dW, db = ctx.grads
+        if not ctx.unit:
+            dW = dW * gout
+            db = db * gout if db is not None else None
+        return None, None, None, dW, db
+
+
+def _class_lazy_of(logits):
+    if isinstance(logits, ClassLinearPredictor):
+        return logits
+    lz = getattr(logits, "_lazy", None) if isinstance(logits, torch.Tensor) else None
+    return lz if isinstance(lz, ClassLinearPredictor) else None
+
+
+class _CategoricalLinear(Categorical):
+    """Categorical whose logits are a ClassLinearPredictor (built by ``Categorical(logits=lazy)``, or by an
+    unchanged model whose ``X @ W.mT + b`` was kept lazy by pyro_b200/lazy.py).  ``log_prob``, ``logits``
+    and ``probs`` materialise the logits; the ELBO's site sum takes the fused kernel."""
+
+    def __init__(self, probs=None, logits=None, validate_args=None):
+        lazy = _class_lazy_of(logits)
+        self._lazy = lazy
+        self._dense = None
+        self._num_events = lazy.K
+        Distribution.__init__(self, lazy.shape[:-1])
+
+    @property
+    def _logits_raw(self):
+        if self._dense is None:
+            self._dense = self._lazy.dense()
+        return self._dense
+
+    def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
+        lz = self._lazy
+        X = lz.X
+        n, D = X.shape
+        # D == 32 and N >= 8192: the tensor-core kernel's scope and precision policy (as for Bernoulli)
+        ok = (mask is None and X.dtype == torch.float32 and lz.Wt.dtype == torch.float32
+              and X.is_contiguous() and X.data_ptr() % 16 == 0 and D == 32 and 2 <= lz.K <= 16 and n >= 8192
+              and isinstance(value, torch.Tensor) and value.numel() == n
+              and tuple(self.batch_shape) == tuple(lz.shape[:-1]))
+        if not ok:
+            return super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
+        y = self._value(value).reshape(-1).contiguous()
+        if y.data_ptr() % 16 != 0:
+            y = y.clone()
+        W = lz.W.reshape(lz.P, lz.K, D)
+        return _GlmCategoricalFn.apply((scale, weight, sum_coeff, unit, 0), X, y, W, lz.bias_pk())
+
+
+def _categorical_new(cls, probs=None, logits=None, validate_args=None):
+    # ``Categorical(logits=ClassLinearPredictor)`` builds the fused softmax-regression subclass
+    if cls is Categorical and probs is None and _class_lazy_of(logits) is not None:
+        return object.__new__(_CategoricalLinear)
+    return object.__new__(cls)
+
+
+Categorical.__new__ = staticmethod(_categorical_new)
+__all__ += ["LinearPredictor", "linear_predictor", "ClassLinearPredictor", "class_linear_predictor", "constant"]
 
 from .hmm import GaussianHMM  # noqa: E402,F401
 __all__ += ["GaussianHMM"]

@@ -14,18 +14,24 @@ per-particle bias keeps it lazy; ``Bernoulli(logits=lazy)`` scores the site with
 y (``b2_glm_bernoulli_logits``); any other use materialises ``X @ w + b`` on the spot, so the
 semantics of arbitrary user code are unchanged.
 
+Softmax regression has the same seam: ``X @ W.mT`` (``W.transpose(-1, -2)``, ``torch.matmul``) and
+``F.linear(X, W)`` with a site value ``W[K, D]`` or ``W[P, K, D]`` give ``[N, K]`` / ``[P, N, K]`` class logits
+kept as a :class:`ClassLinearPredictor`; a bias ``[K]`` or ``[P, 1, K]`` keeps them lazy, and
+``Categorical(logits=lazy)`` scores the site with ``b2_glm_categorical_logits``.
+
 This is trace-time pattern matching at the seam where Pyro already passes values around (the replayed
 guide value of pyro/poutine/replay_messenger.py:50-61); nothing in the model is rewritten.
 """
 import torch
 
 from ._lazyparam import LazyExpParam
-from .distributions import LinearPredictor
+from .distributions import ClassLinearPredictor, LinearPredictor
 
 _VIEW_FUNCS = {"squeeze", "unsqueeze", "reshape", "view", "transpose", "t", "permute", "expand",
                "expand_as", "flatten", "contiguous", "__getitem__", "movedim", "swapaxes", "detach_",
                "mT", "T", "narrow", "select", "unflatten"}
 _MATMUL_FUNCS = {"matmul", "__matmul__", "__rmatmul__", "mm", "mv", "linear", "inner"}
+_CLASS_MATMUL_FUNCS = {"matmul", "__matmul__", "__rmatmul__", "mm"}
 _ADD_FUNCS = {"add", "__add__", "__radd__", "__iadd__", "add_"}
 _CHEAP_TRUE = {"eq", "__eq__", "isfinite"}
 _CHEAP_FALSE = {"ne", "__ne__", "isnan", "isinf"}
@@ -88,6 +94,9 @@ class SiteValue(torch.Tensor):
     def __torch_function__(cls, func, types, args=(), kwargs=None):
         kwargs = kwargs or {}
         name = _name(func)
+        if name == "__get__":
+            # a property such as ``W.mT``: name it after the attribute, so a transposed view stays a SiteValue
+            name = getattr(getattr(func, "__self__", None), "__name__", name)
         if name in _MATMUL_FUNCS and not kwargs:
             lazy = _try_lazy_matmul(name, args)
             if lazy is not None:
@@ -111,7 +120,14 @@ def _try_lazy_matmul(name, args):
         if not (_is_data(Xa) and isinstance(wa, SiteValue)):
             return None
         rm = _row_major(Xa)
-        if rm is None or rm[1] or not _weights_of(wa, Xa.shape[1]):
+        if rm is None or rm[1]:
+            return None
+        if wa.dim() == 2:
+            # F.linear(X, W[K, D][, b[K]]) -> [N, K] class logits
+            if not _class_weights_of(wa, Xa) or (bias is not None and not _class_bias_ok(bias, wa.shape[0], Xa)):
+                return None
+            return _make_class(rm[0], wa.mT, bias, linear=True)
+        if wa.dim() != 1 or not _weights_of(wa, Xa.shape[1]):
             return None
         lp = _make(rm[0], wa, None)
         return lp if bias is None else lp + bias
@@ -130,12 +146,34 @@ def _try_lazy_matmul(name, args):
             return None
         return _make(X, a, None)
     if _is_data(a) and isinstance(b, SiteValue):
-        # X [N, D] @ w [D]
         rm = _row_major(a)
-        if rm is None or rm[1] or b.dim() != 1 or b.shape[0] != a.shape[1]:
+        if rm is None or rm[1]:
+            return None
+        if b.dim() in (2, 3) and name in _CLASS_MATMUL_FUNCS:
+            # X [N, D] @ W.mT, W [K, D] or [P, K, D] -> [N, K] / [P, N, K] class logits
+            if b.shape[-2] != a.shape[1] or not _class_weights_of(b.mT, a):
+                return None
+            return _make_class(rm[0], b, None)
+        # X [N, D] @ w [D]
+        if b.dim() != 1 or b.shape[0] != a.shape[1]:
             return None
         return _make(rm[0], b, None)
     return None
+
+
+def _class_weights_of(W, X):
+    """A site value usable as class weights for the data matrix X: [K, D] or [P, K, D], same dtype/device."""
+    return (W.dim() in (2, 3) and W.shape[-1] == X.shape[1] and W.shape[-2] >= 1 and W.dtype == X.dtype
+            and W.device == X.device)
+
+
+def _class_bias_ok(b, K, X):
+    return isinstance(b, torch.Tensor) and not isinstance(b, LinearPredictorTensor) and tuple(b.shape) == (K,) \
+        and b.dtype == X.dtype and b.device == X.device
+
+
+def _make_class(X, Wt, b, linear=False):
+    return LinearPredictorTensor(ClassLinearPredictor(X, Wt, b, linear=linear, linear_bias=b is not None))
 
 
 def _make(X, w, b):
@@ -145,7 +183,8 @@ def _make(X, w, b):
 
 
 class LinearPredictorTensor(torch.Tensor):
-    """``X @ w^T + b`` not yet computed: metadata of a ``[P, N]`` / ``[N]`` tensor, no storage."""
+    """``X @ w^T + b`` not yet computed: metadata of a ``[P, N]`` / ``[N]`` tensor, no storage.  Wrapping a
+    :class:`ClassLinearPredictor` it stands for ``[N, K]`` / ``[P, N, K]`` class logits."""
 
     @staticmethod
     def __new__(cls, lazy):
@@ -169,6 +208,11 @@ class LinearPredictorTensor(torch.Tensor):
 
     def _with_bias(self, b):
         lz = self._lazy
+        if isinstance(lz, ClassLinearPredictor):
+            if isinstance(b, LinearPredictorTensor):
+                return None
+            out = lz.with_bias(b.as_subclass(torch.Tensor) if isinstance(b, SiteValue) else b)
+            return None if out is None else LinearPredictorTensor(out)
         if lz.b is not None:
             return None
         if isinstance(b, (int, float)):
