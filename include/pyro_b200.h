@@ -315,6 +315,35 @@ int b2_glm_categorical_logits(const float* X, const int64_t* y, const float* W, 
                               void* stream);
 size_t b2_glm_categorical_workspace(int64_t N, int D, int K, int P);
 
+/*
+ * b2_glm_potential -- HMC / NUTS potential energy and gradient of Bayesian logistic (kind
+ * B2_GLM_BERNOULLI) or softmax (B2_GLM_CATEGORICAL) regression for C chains, with the likelihood of
+ * every chain computed in one pass over X by the kernels of b2_glm_bernoulli_logits /
+ * b2_glm_categorical_logits (the chains are their particles):
+ *   U[c]       = -( SUM_n log p(y[n] | logits[c,n]) + SUM_i log Normal(w[c,i]; 0, s_w)
+ *                   + SUM_k log Normal(b[c,k]; 0, s_b) )
+ *   grad[c,:]  = dU / dz[c,:]
+ * logits[c,n] = <X[n,:], w[c,:]> + b[c] (Bernoulli, K == 1) or logits[c,n,k] = <X[n,:], W[c,k,:]> + b[c,k]
+ * (Categorical).  z: [C, Dz] fp32 row-major chain state; the weights (K*D values, W row-major [K, D])
+ * start at column w_off, the bias (K values, only if has_bias) at column b_off, and Dz == K*D + (has_bias ? K
+ * : 0).  grad has z's layout.  X: [N, D] fp32 row-major, 16-byte aligned; y: [N] fp32 0/1 (Bernoulli) or
+ * int64 labels, 16-byte aligned (Categorical).
+ * Scope: Bernoulli with K == 1 and D in {4, 8, 16, 32}; Categorical with D == 32 and 2 <= K <= 16;
+ * s_w > 0 and (with a bias) s_b > 0; anything else returns B2_ERR_BAD_SHAPE.
+ * The GLM kernels always run with B2_FLAG_GLM_3XTF32 (every logit fp32-exact).  The prior and the totals
+ * are accumulated in fp64 in a fixed order: results are deterministic.
+ * workspace: b2_glm_potential_workspace() bytes, zero-initialised ONCE by the caller; it must not be
+ * shared with a concurrent call of any GLM entry point.  Four launches (pack, GLM kernel, GLM finish,
+ * potential finish), no host synchronisation: one evaluation can be captured in a CUDA graph.
+ */
+#define B2_GLM_BERNOULLI 0
+#define B2_GLM_CATEGORICAL 1
+int b2_glm_potential(int kind, const float* X, const void* y, int64_t N, int D, int K, int has_bias,
+                     const float* z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, double s_w,
+                     double s_b, float* U, float* grad, void* workspace, size_t workspace_bytes,
+                     void* stream);
+size_t b2_glm_potential_workspace(int kind, int64_t N, int D, int K, int64_t C);
+
 /* ---- optimisers --------------------------------------------------------------------------
  * Multi-tensor fused updates replacing PyroOptim's per-parameter Python loop
  * (pyro/optim/optim.py:117-155).  Per-tensor scalar state lives in DEVICE arrays so a captured

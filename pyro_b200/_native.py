@@ -35,6 +35,7 @@ EMULATE_RSAMPLE = False   # tests/cpu_emulation.py flips this to exercise the fu
 SITE_SMALL_N = 8192   # B2_SITE_SMALL_N: one-CTA kernel with fused stored-shape gradient reductions
 DIRICHLET, CATEGORICAL, MVN_TRIL = 32, 33, 34
 MODEL_HIER_NORMAL, MODEL_LOGISTIC = 0, 1
+GLM_BERNOULLI, GLM_CATEGORICAL = 0, 1
 NUTS_SMALL_MAX_D = 64
 
 
@@ -115,6 +116,9 @@ SIGNATURES = {
     "b2_glm_categorical_logits": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _f64,
                                          _i32, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2_glm_categorical_workspace": (_sz, [_i64, _i32, _i32, _i32]),
+    "b2_glm_potential": (_i32, [_i32, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _i64, _i64, _f64, _f64,
+                                _vp, _vp, _vp, _sz, _vp]),
+    "b2_glm_potential_workspace": (_sz, [_i32, _i64, _i32, _i32, _i64]),
     "b2_clipped_adam": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _vp]),
     "b2_adagrad_rmsprop": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _vp]),
     "b2_leapfrog_half_kick_drift": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _i32, _vp]),

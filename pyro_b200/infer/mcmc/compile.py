@@ -60,7 +60,8 @@ def _sites(trace):
     for name, site in trace.nodes.items():
         if site["type"] != "sample":
             continue
-        if site.get("infer", {}).get("_subsample"):
+        # plates record a subsample site: flagged in pyro_b200, a ``_Subsample`` distribution in Pyro
+        if site.get("infer", {}).get("_subsample") or type(site["fn"]).__name__ == "_Subsample":
             continue
         (observed if site["is_observed"] else latent)[name] = site
     return latent, observed
@@ -180,6 +181,86 @@ def _try_logistic(poutine, model, args, kwargs, latent, observed):
     return LogisticPotential(X, y.to(X.dtype), prior_scale=s, site_name=bname)
 
 
+def _try_glm(poutine, model, args, kwargs, latent, observed):
+    """Logistic regression with an intercept, or softmax regression with or without one, in fp32, within
+    the GLM kernels' scope: Bernoulli D in {4, 8, 16, 32}; Categorical D == 32, 2 <= K <= 16."""
+    from .potential import GlmPotential
+    if len(observed) != 1 or len(latent) not in (1, 2):
+        return None
+    (obs_name, obs), = observed.items()
+    _, kind = _base(obs["fn"])
+    # lazy linear-predictor logits build _BernoulliLinear / _CategoricalLinear (pyro_b200/distributions)
+    kind = {"BernoulliLinear": "Bernoulli", "CategoricalLinear": "Categorical"}.get(kind, kind)
+    if kind not in ("Bernoulli", "Categorical") or not _plain_site(obs):
+        return None
+    y = obs["value"]
+    if not isinstance(y, torch.Tensor) or y.dim() != 1:
+        return None
+    n = y.numel()
+    X = None
+    for a in list(args) + list(kwargs.values()):
+        if isinstance(a, torch.Tensor) and a.dim() == 2 and a.shape[0] == n and a.dtype == torch.float32 \
+                and not a.requires_grad:
+            X = a
+    if X is None or not X.is_contiguous() or X.data_ptr() % 16 != 0:
+        return None
+    D = X.shape[1]
+    scales, shapes = {}, {}
+    for name, site in latent.items():
+        fn, cls = _base(site["fn"])
+        v = site["value"]
+        if cls != "Normal" or not _plain_site(site) or not isinstance(v, torch.Tensor) \
+                or v.dtype != torch.float32 or _const(fn.loc) != 0.0:
+            return None
+        s = _const(fn.scale)
+        if s is None or not s > 0.0:
+            return None
+        scales[name], shapes[name] = s, tuple(v.shape)
+    if kind == "Bernoulli":
+        K = 1
+        wshapes, bshapes = [(D,)], [(), (1,)]
+        if D not in (4, 8, 16, 32) or y.dtype != torch.float32:
+            return None
+    else:
+        wmat = [s for s in shapes.values() if len(s) == 2]
+        K = wmat[0][0] if len(wmat) == 1 else 0
+        wshapes, bshapes = [(K, D)], [(K,)]
+        if D != 32 or not 2 <= K <= 16 or y.dtype != torch.int64:
+            return None
+    weight = [name for name, s in shapes.items() if s in wshapes]
+    bias = [name for name, s in shapes.items() if s in bshapes]
+    if len(weight) != 1 or len(bias) + 1 != len(latent):
+        return None
+    weight, bias = weight[0], (bias[0] if bias else None)
+    if kind == "Bernoulli" and bias is None:
+        return None   # intercept-free logistic regression keeps LogisticPotential's route
+    # ---- functional probe: logits == X @ w + b  /  log_softmax(logits) == log_softmax(X @ W.mT + b) --------
+    gen = torch.Generator(device="cpu").manual_seed(20240302)
+    for _ in range(3):
+        wv = torch.randn(shapes[weight], generator=gen).to(X)
+        bv = torch.randn(shapes[bias], generator=gen).to(X) if bias is not None else None
+        data = {weight: wv} if bias is None else {weight: wv, bias: bv}
+        logits = _probe(poutine, model, args, kwargs, data, obs_name).logits
+        if hasattr(logits, "dense"):
+            logits = logits.dense()
+        if kind == "Bernoulli":
+            want = X @ wv + bv.reshape(())
+        else:
+            want = X @ wv.mT + (bv if bv is not None else 0.0)
+            logits, want = torch.log_softmax(logits, -1), torch.log_softmax(want, -1)
+        if tuple(logits.shape) != tuple(want.shape) or not _close(logits, want, X.dtype):
+            return None
+    off, sites = 0, {}
+    for name in latent:
+        width = 1
+        for d in shapes[name]:
+            width *= d
+        sites[name] = (slice(off, off + width), "identity", shapes[name])
+        off += width
+    return GlmPotential(X, y.detach(), kind, sites, weight, bias, s_w=scales[weight],
+                        s_b=scales[bias] if bias is not None else 1.0)
+
+
 def recognise(model, args=(), kwargs=None, poutine=None):
     """A native potential for ``model`` if it belongs to a compiled class, else None (never raises:
     any surprise means "not recognised")."""
@@ -191,7 +272,7 @@ def recognise(model, args=(), kwargs=None, poutine=None):
         with torch.no_grad():
             proto = poutine.trace(model).get_trace(*args, **kwargs)
             latent, observed = _sites(proto)
-            for attempt in (_try_hier_normal, _try_logistic):
+            for attempt in (_try_hier_normal, _try_logistic, _try_glm):
                 pot = attempt(poutine, model, args, kwargs, latent, observed)
                 if pot is not None:
                     return pot

@@ -110,6 +110,69 @@ class LogisticPotential(NativePotential):
         super().__init__(N.MODEL_LOGISTIC, X.dtype, X.device, n, d, X, y, (prior_scale,), sites)
 
 
+class GlmPotential:
+    """Bayesian logistic or softmax regression with constant-scale Normal priors:
+    ``w ~ Normal(0, s_w)[D]``, ``b ~ Normal(0, s_b)``, ``y ~ Bernoulli(logits = X @ w + b)``, or
+    ``W ~ Normal(0, s_w)[K, D]``, ``b ~ Normal(0, s_b)[K]`` (optional),
+    ``y ~ Categorical(logits = X @ W.mT + b)``.
+
+    ``value_and_grad`` is ``b2_glm_potential``: the likelihood of all chains comes from one pass of the
+    fused GLM kernel over X, the chains being its particles.  ``sites`` maps each site name to
+    ``(slice into z, "identity", value shape)`` in the order and layout ``TracePotential`` gives the same
+    model, so samples, ``initial_params`` and ``full_mass`` behave the same on either.  Every chain is
+    evaluated; the sampler masks inactive chains, as it does for ``TracePotential``."""
+
+    def __init__(self, X, y, kind, sites, weight, bias=None, s_w=1.0, s_b=1.0):
+        N.require_cuda(X, "GlmPotential")
+        if X.dtype != torch.float32 or X.dim() != 2:
+            raise ValueError("GlmPotential needs fp32 X of shape [N, D]")
+        self.X = X.contiguous()
+        self.kind = N.GLM_BERNOULLI if kind == "Bernoulli" else N.GLM_CATEGORICAL
+        # private contiguous copies: the kernels load y with TMA (16-byte aligned)
+        self.y = (y.to(torch.float32) if self.kind == N.GLM_BERNOULLI else y.to(torch.int64)).clone()
+        self.sites = dict(sites)
+        self.weight, self.bias = weight, bias
+        self.n, self.Dx = self.X.shape
+        wshape = self.sites[weight][2]
+        self.K = 1 if self.kind == N.GLM_BERNOULLI else int(wshape[0])
+        self.w_off = self.sites[weight][0].start
+        self.b_off = self.sites[bias][0].start if bias is not None else 0
+        self.has_bias = bias is not None
+        self.s_w, self.s_b = float(s_w), float(s_b)
+        self.D = sum(sl.stop - sl.start for sl, _, _ in self.sites.values())
+        self.dtype = torch.float32
+        self.device = self.X.device
+
+    @property
+    def dim(self):
+        return self.D
+
+    def value_and_grad(self, z, active=None):
+        N.require_cuda(z, "GlmPotential")
+        z = z.detach().to(torch.float32).contiguous()
+        C = z.shape[0]
+        U = torch.empty(C, dtype=torch.float32, device=z.device)
+        g = torch.empty_like(z)
+        lib = N.lib()
+        need = int(lib.b2_glm_potential_workspace(self.kind, self.n, self.Dx, self.K, C))
+        ws = N.workspace(z.device, need, tag="glm_potential")
+        N.check(lib.b2_glm_potential(
+            self.kind, self.X.data_ptr(), self.y.data_ptr(), self.n, self.Dx, self.K, int(self.has_bias),
+            z.data_ptr(), C, self.D, self.w_off, self.b_off, self.s_w, self.s_b, U.data_ptr(), g.data_ptr(),
+            ws.data_ptr(), ws.numel(), N.stream_ptr(z.device)), "b2_glm_potential")
+        return U, g
+
+    def unpack(self, z):
+        return {name: self.unpack_site(name, z[..., sl]) for name, (sl, _, _) in self.sites.items()}
+
+    def unpack_site(self, name, u):
+        return u.reshape(u.shape[:-1] + tuple(self.sites[name][2]))
+
+    def init_uniform(self, num_chains, radius=2.0, generator=None):
+        return (torch.rand(num_chains, self.D, dtype=self.dtype, device=self.device,
+                           generator=generator) * 2 - 1) * radius
+
+
 class TracePotential:
     """Potential of an arbitrary model, evaluated for ``C`` chains per call.
 
