@@ -20,9 +20,10 @@
 //            and survives the N-term sums); X is rounded to nearest (incoherent, averages as 1/sqrt(N)).
 //            SPLIT_X splits X as well (a third MMA per k-step; every logit exact to ~1e-6).
 //   epilogue each thread holds 2 particles x 16 rows of D1^T in registers, evaluates lp = y*l - softplus(l),
-//            g = y - sigmoid(l) (3 MUFU + ~12 FMA-pipe ops per element, in batches of 4 so part of the MUFU
-//            latency is covered inside the warp), keeps its two per-particle lp sums in registers and rounds g to
-//            nearest TF32.  g stays in the registers: it is already the A fragment of GEMM 2.
+//            g = y - sigmoid(l) (2 MUFU per element plus one lg2 per particle and tile on the product of the
+//            softplus denominators, in batches so part of the MUFU latency is covered inside the warp), keeps
+//            its two per-particle lp sums in registers and rounds g to nearest TF32.  g stays in the
+//            registers: it is already the A fragment of GEMM 2.  Only the last, partial tile masks rows.
 //   GEMM 2   [dW | db][p, :] += sum_n g[p, n] [X | 1][n, :]   wgmma m64n40k8, K = 64, A from registers:
 //            single-pass TF32 on round-to-nearest operands (unbiased; |err| <= 2^-11 sum|g x|).  The
 //            accumulator stays in registers for the whole kernel; GEMM 2 of a tile is committed and left
@@ -81,14 +82,23 @@ static_assert(kWGBytes % 1024 == 0 && kXtBlock % 1024 == 0, "operand alignment")
 // the final reduction reuses the X ring: [kWG][64 p][33] + [kWG][64 p] floats
 static_assert((kWG * kP * 33 + kWG * kP) * 4 <= kStages * kTile, "reduction scratch");
 
-// Four logits of one particle at once, stage by stage: each MUFU result is consumed a stage (>= 4
-// instructions) after it was issued, and the four warps per scheduler cover the rest of the MUFU latency
-// (a batch of 8 would not fit 128 registers).  Returns the sum of lp = y*l - softplus(l) over the four and
-// writes g = y - sigmoid(l) rounded to nearest TF32.  MASK weights both with vw (0 for rows past N).
-template <bool MASK>
-__device__ __forceinline__ float epi_batch(const float* lr, const float* y, const float* vw, uint32_t* g) {
-  constexpr int B = 4;
-  float e[B], den[B], inv[B], lg[B], lp[B];
+constexpr int kEpiBatch = 4;                    // logits of one particle per epilogue batch (8 fits, no faster)
+
+// lp = y*l - softplus(l) = y*l - max(l, 0) - ln(1 + e^-|l|).  The epilogue sums the linear part per tile and
+// multiplies the denominators den = 1 + e^-|l| instead of taking a logarithm of each: den is in (1, 2], so
+// the product of a thread's 16 rows of one particle is at most 2^16, and one lg2 per particle and tile
+// replaces 16.  Rounding: each of the 15 products adds at most 2^-24 relative, at most 15 * 2^-24 = 9e-7
+// nats per 16 logits, no worse than the sixteen lg2.approx results it replaces (about 1e-7 nats each).
+//
+// One batch of B logits of one particle, stage by stage: each MUFU result is consumed a stage (>= B
+// instructions) after it was issued, and the four warps per scheduler cover the rest of the MUFU latency.
+// Returns the sum of y*l - max(l, 0) over the batch, multiplies the batch's den into prod and writes
+// g = y - sigmoid(l) rounded to nearest TF32.  MASK weights the linear part and g with vw (0 for rows past
+// N) and gives a masked row the factor 1 exactly.
+template <bool MASK, int B>
+__device__ __forceinline__ float epi_batch(const float* lr, const float* y, const float* vw, float& prod,
+                                           uint32_t* g) {
+  float e[B], den[B], inv[B], f[B], lp[B];
 #pragma unroll
   for (int j = 0; j < B; ++j) e[j] = ex2f(-1.4426950408889634f * fabsf(lr[j]));
 #pragma unroll
@@ -96,11 +106,11 @@ __device__ __forceinline__ float epi_batch(const float* lr, const float* y, cons
 #pragma unroll
   for (int j = 0; j < B; ++j) inv[j] = rcpf(den[j]);
 #pragma unroll
-  for (int j = 0; j < B; ++j) lg[j] = lg2f(den[j]);
+  for (int j = 0; j < B; ++j) f[j] = MASK ? fmaf(vw[j], e[j], 1.f) : den[j];
 #pragma unroll
   for (int j = 0; j < B; ++j) {
     const float l = lr[j];
-    lp[j] = fmaf(lg[j], -0.6931471805599453f, fmaf(y[j], l, -fmaxf(l, 0.f)));
+    lp[j] = fmaf(y[j], l, -fmaxf(l, 0.f));
     const float sg = (l >= 0.f) ? inv[j] : e[j] * inv[j];
     float gg = y[j] - sg;
     if (MASK) {
@@ -109,7 +119,43 @@ __device__ __forceinline__ float epi_batch(const float* lr, const float* y, cons
     }
     g[j] = __float_as_uint(tf32_rn(gg));
   }
-  return (lp[0] + lp[1]) + (lp[2] + lp[3]);
+#pragma unroll
+  for (int w = 1; w < B; w *= 2)
+#pragma unroll
+    for (int j = 0; j < B; j += 2 * w) {
+      lp[j] += lp[j + w];
+      f[j] *= f[j + w];
+    }
+  prod *= f[0];
+  return lp[0];
+}
+
+// The epilogue of one tile: the linear lp sums lin[h] and den products prod[h] of the thread's two particles
+// (16 rows each), and g indexed like acc1.  MASK (the last, partial tile only) zeroes rows past N.
+template <bool MASK>
+__device__ __forceinline__ void epilogue(const float (&acc1)[32], const float2 (&yr)[8], int64_t row0, int64_t N,
+                                         int t4, float (&lin)[2], float (&prod)[2], uint32_t (&g)[32]) {
+  constexpr int B = kEpiBatch;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    prod[h] = 1.f;
+#pragma unroll
+    for (int q = 0; q < 16 / B; ++q) {         // k-blocks j = B/2 q .. B/2 q + B/2 - 1
+      float l[B], yy[B], vw[B];
+      uint32_t gb[B];
+#pragma unroll
+      for (int i = 0; i < B; ++i) {
+        const int j = B / 2 * q + (i >> 1), e = i & 1;
+        l[i] = acc1[4 * j + 2 * h + e];
+        yy[i] = e ? yr[j].y : yr[j].x;
+        vw[i] = MASK ? ((row0 + 8 * j + 2 * t4 + e < N) ? 1.f : 0.f) : 1.f;
+      }
+      const float s = epi_batch<MASK, B>(l, yy, vw, prod[h], gb);
+      lin[h] = q ? lin[h] + s : s;
+#pragma unroll
+      for (int i = 0; i < B; ++i) g[4 * (B / 2 * q + (i >> 1)) + 2 * h + (i & 1)] = gb[i];
+    }
+  }
 }
 
 // SPLIT_X = false (default): W split hi/lo, X rounded to nearest.  SPLIT_X = true: full 3xTF32, X split
@@ -200,20 +246,27 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
       // GEMM 2 of this warpgroup's previous tile has finished reading X^T and the g registers
       wgmma_wait0();
       fence_regs(acc2);
-      // ---- split / transposition pass: thread t owns 16 columns (chunks 4h .. 4h+3) of row r ----------
+      // ---- split / transposition pass ------------------------------------------------------------------
+      // Thread t owns the 16-byte chunk c (d = 4c .. 4c+3) of the four rows n = 8 q8 + 2i + e (i = 0..3):
+      // kt_pos puts them at the consecutive k = 8 q8 + 4e + i, so after a 4x4 transpose in registers each d
+      // is one 16-byte store into X^T.  The eight lanes of a quarter-warp (one phase of a 16-byte access)
+      // take the eight (q8 & 3, e) and eight distinct chunks, chosen so that the 16-byte bank groups of both
+      // the X loads (c ^ (n & 7)) and the X^T stores ((2 (q8 & 3) + e) ^ (d & 7)) are all different.
       {
-        const int r = t >> 1, hh = t & 1, rk = kt_pos(r);
+        const int lam = t & 7, mu = t >> 3;
+        const int e = lam & 1, q8 = ((mu >> 3) << 2) | (lam >> 1);
+        const int c = (((lam & 1) << 2) | (lam >> 1)) ^ (mu & 7);
         float4* xs = reinterpret_cast<float4*>(sm + OFF_X + s * kTile);
         float4* xl = reinterpret_cast<float4*>(my + WG_XLO);
+        float xr[4][4];                        // [i][q] = X[8 q8 + 2i + e][4c + q] rounded to nearest TF32
 #pragma unroll
-        for (int c4 = 0; c4 < 4; ++c4) {
-          const int c = hh * 4 + c4;
+        for (int i = 0; i < 4; ++i) {
+          const int r = 8 * q8 + 2 * i + e;
           const int idx = r * 8 + (c ^ (r & 7));      // 16-byte chunk holding d = 4c .. 4c+3 of row r
           const float4 v = xs[idx];
           const float x[4] = {v.x, v.y, v.z, v.w};
-          float xr[4];
 #pragma unroll
-          for (int q = 0; q < 4; ++q) xr[q] = tf32_rn(x[q]);
+          for (int q = 0; q < 4; ++q) xr[i][q] = tf32_rn(x[q]);
           if (SPLIT_X) {
             float h[4];
 #pragma unroll
@@ -221,15 +274,16 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
             xs[idx] = make_float4(h[0], h[1], h[2], h[3]);
             xl[idx] = make_float4(x[0] - h[0], x[1] - h[1], x[2] - h[2], x[3] - h[3]);
           } else {
-            xs[idx] = make_float4(xr[0], xr[1], xr[2], xr[3]);
+            xs[idx] = make_float4(xr[i][0], xr[i][1], xr[i][2], xr[i][3]);
           }
+        }
+        // X^T[d][k]: k-block k >> 5, 16-byte chunk ((k & 31) >> 2) ^ (d & 7), element k & 3 (= i here)
+        const int kc = 2 * (q8 & 3) + e;
+        float4* xt = reinterpret_cast<float4*>(my + WG_XT + (q8 >> 2) * kXtBlock);
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const int d = c * 4 + q;
-            // X^T[d][k = rk]: k-block rk >> 5, 16-byte chunk ((rk & 31) >> 2) ^ (d & 7), element rk & 3
-            reinterpret_cast<float*>(my + WG_XT + (rk >> 5) * kXtBlock)[d * 32 + (((((rk & 31) >> 2) ^ (d & 7)) << 2) |
-                                                                                  (rk & 3))] = xr[q];
-          }
+        for (int q = 0; q < 4; ++q) {
+          const int d = 4 * c + q;
+          xt[d * 8 + (kc ^ (d & 7))] = make_float4(xr[0][q], xr[1][q], xr[2][q], xr[3][q]);
         }
       }
       float2 yr[8];                            // y of the thread's rows n = 8j + 2 t4 + e, read before the refill
@@ -254,26 +308,15 @@ glm_bernoulli_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_
       fence_regs(acc1);
       // GEMM 1 has read the X stage and y is in registers: refill the stage with tile it + 2 kWG
       if (t == 0 && it + 2 * kWG < nt) load(it + 2 * kWG, s);
-      // ---- epilogue: lp sums and g, both in registers ----------------------------------------------------
-      const bool tail = row0 + kRows > N;
+      // ---- epilogue: lp sums and g, both in registers; the row mask only in the last, partial tile ------
       uint32_t g[32];                          // indexed like acc1
+      float lin[2], prod[2];
+      if (row0 + kRows > N)
+        epilogue<true>(acc1, yr, row0, N, t4, lin, prod, g);
+      else
+        epilogue<false>(acc1, yr, row0, N, t4, lin, prod, g);
 #pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {          // k-blocks j = 2q, 2q + 1
-          float l[4], yy[4], vw[4];
-          uint32_t gb[4];
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int j = 2 * q + (i >> 1), e = i & 1;
-            l[i] = acc1[4 * j + 2 * h + e];
-            yy[i] = e ? yr[j].y : yr[j].x;
-            vw[i] = (row0 + 8 * j + 2 * t4 + e < N) ? 1.f : 0.f;
-          }
-          lpa[h] += tail ? epi_batch<true>(l, yy, vw, gb) : epi_batch<false>(l, yy, vw, gb);
-#pragma unroll
-          for (int i = 0; i < 4; ++i) g[4 * (2 * q + (i >> 1)) + 2 * h + (i & 1)] = gb[i];
-        }
+      for (int h = 0; h < 2; ++h) lpa[h] += fmaf(lg2f(prod[h]), -0.6931471805599453f, lin[h]);
       // ---- GEMM 2: [dW | db] += g [X | 1], g from registers, left running while the next tile is waited for
       fence_regs(g);
       wgmma_fence();
