@@ -316,6 +316,40 @@ int b2_glm_categorical_logits(const float* X, const int64_t* y, const float* W, 
 size_t b2_glm_categorical_workspace(int64_t N, int D, int K, int P);
 
 /*
+ * b2_poisson_product -- fused Poisson matrix-factorisation likelihood term (the bottom layer of the sparse
+ * gamma DEF, Gamma-Poisson NMF): for P particles with latent factors A[p] (N x K) and B[p] (K x J) and shared
+ * counts x (N x J), rate[p,n,j] = SUM_k A[p,n,k] * B[p,k,j];
+ *   sum_p[p]  = SUM_{n,j} ( xlogy(x[n,j], rate) - rate - lgamma(x[n,j] + 1) )       (Poisson log_prob)
+ *   G[p,n,j]  = x[n,j] / rate[p,n,j] - 1
+ *   dA[p]     = weight * scale * G[p] @ B[p]^T      (N x K)
+ *   dB[p]     = weight * scale * A[p]^T @ G[p]      (K x J)
+ * No [P,N,J] tensor is written: A, B and x are read about once per particle and the gradients written once.
+ * A: [P,N,K], B: [P,K,J], x: [N,J], all fp32 row-major, x 16-byte aligned.  Scope: 1 <= K <= 16,
+ * 1 <= N < 2^31, J a multiple of 4, 1 <= P <= 65535; anything else returns B2_ERR_BAD_SHAPE, and a null
+ * A, B or x returns B2_ERR_NULL, both before any CUDA call.
+ * out_total (nullable): scalar, (=|+=) sum_coeff * SUM_p sum_p[p] (B2_FLAG_ACCUMULATE_SUM); sum_p includes
+ * scale.  out_sum_p, out_dA, out_dB are nullable.  At rate == 0 the value and G are those of the Poisson
+ * site family (lp = -inf and G = +inf for x > 0; lp = 0 and G = NaN for x == 0).
+ * All three contractions run on the tensor cores (wgmma, poisson_product_tc.cu).  Both factors are split
+ * hi + lo and the rate takes three TF32 products (every rate fp32-exact), because a rounding error of A or B
+ * is shared by a whole row or column of rates.  The two gradient contractions split G, A and B the same way
+ * (three products each): G = x / rate - 1 has both signs and large entries where the rate is small, so dA and
+ * dB are sums with heavy cancellation.  SUM lgamma(x + 1) is evaluated once per call, not once per particle.
+ * A non-finite G (rate == 0 with x > 0: +inf) makes the factor gradients it enters non-finite, as on the
+ * materialised path, but an entry the materialised path gives as +-inf can be NaN here: the split products
+ * multiply G's +inf by the zero low part of a factor value that TF32 represents exactly.
+ * workspace: b2_poisson_product_workspace() bytes, zero-initialised ONCE by the caller (its first 256 bytes
+ * hold a ticket counter that the library leaves zeroed).  Two launches: the streaming kernel and a finish
+ * kernel that sums the CTA partials in a fixed order (deterministic, no float atomics, no host
+ * synchronisation: the call can be captured in a CUDA graph).
+ */
+int b2_poisson_product(const float* A, const float* B, const float* x, int64_t N, int K, int64_t J, int P,
+                       double scale, double weight, double sum_coeff, int flags, float* out_sum_p,
+                       float* out_total, float* out_dA, float* out_dB, void* workspace, size_t workspace_bytes,
+                       void* stream);
+size_t b2_poisson_product_workspace(int64_t N, int K, int64_t J, int P);
+
+/*
  * b2_glm_potential -- HMC / NUTS potential energy and gradient of Bayesian logistic (kind
  * B2_GLM_BERNOULLI) or softmax (B2_GLM_CATEGORICAL) regression for C chains, with the likelihood of
  * every chain computed in one pass over X by the kernels of b2_glm_bernoulli_logits /

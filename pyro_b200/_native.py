@@ -116,6 +116,9 @@ SIGNATURES = {
     "b2_glm_categorical_logits": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _f64,
                                          _i32, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2_glm_categorical_workspace": (_sz, [_i64, _i32, _i32, _i32]),
+    "b2_poisson_product": (_i32, [_vp, _vp, _vp, _i64, _i32, _i64, _i32, _f64, _f64, _f64, _i32, _vp, _vp, _vp,
+                                  _vp, _vp, _sz, _vp]),
+    "b2_poisson_product_workspace": (_sz, [_i64, _i32, _i64, _i32]),
     "b2_glm_potential": (_i32, [_i32, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _i64, _i64, _f64, _f64,
                                 _vp, _vp, _vp, _sz, _vp]),
     "b2_glm_potential_workspace": (_sz, [_i32, _i64, _i32, _i32, _i64]),

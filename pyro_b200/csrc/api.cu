@@ -21,5 +21,5 @@ extern "C" const char* b2_last_error(int code) {
   }
 }
 
-extern "C" int b2_version(void) { return 103; }
+extern "C" int b2_version(void) { return 104; }
 extern "C" int64_t b2_launch_count(void) { return b2::g_launch_count; }

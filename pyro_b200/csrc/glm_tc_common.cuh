@@ -1,6 +1,6 @@
-// glm_tc_common.cuh -- device helpers shared by the Hopper wgmma GLM kernels (glm_tc.cu,
-// glm_categorical_tc.cu): mbarriers, TMA tile loads, SWIZZLE_128B operand descriptors, the TF32 wgmma
-// wrappers, MUFU wrappers and TF32 rounding, and the host-side tensor-map encoder.
+// glm_tc_common.cuh -- device helpers shared by the Hopper wgmma kernels (glm_tc.cu,
+// glm_categorical_tc.cu, poisson_product_tc.cu): mbarriers, TMA tile loads, SWIZZLE_128B operand
+// descriptors, the TF32 wgmma wrappers, MUFU wrappers and TF32 rounding, and the host-side tensor-map encoder.
 #pragma once
 #include <cuda.h>
 
@@ -106,6 +106,32 @@ __device__ __forceinline__ void wgmma_n40_tf32_ra(float (&d)[20], const uint32_t
         "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
       : "memory");
+}
+
+// D[64 x 16] = A[64 x 8] B[16 x 8]^T (+ D when acc != 0), TF32, both operands K-major in shared memory
+__device__ __forceinline__ void wgmma_n16_tf32(float (&d)[8], uint64_t a, uint64_t b, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "r"(acc)
+      : "memory");
+}
+// D[64 x 16] = A[64 x 8] B[16 x 8]^T (+ D when acc != 0), TF32, A from registers (layout of wgmma_n40_tf32_ra)
+__device__ __forceinline__ void wgmma_n16_tf32_ra(float (&d)[8], const uint32_t (&a)[4], uint64_t b, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
+      : "memory");
+}
+
+// float offset of element (row, col), col < 32, in a K-major SWIZZLE_128B operand of 32-float rows
+__device__ __forceinline__ int sw128(int row, int col) {
+  return row * 32 + ((((col >> 2) ^ (row & 7)) << 2) | (col & 3));
 }
 
 __device__ __forceinline__ float ex2f(float x) {

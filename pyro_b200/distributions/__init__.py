@@ -1277,7 +1277,126 @@ def _categorical_new(cls, probs=None, logits=None, validate_args=None):
 
 
 Categorical.__new__ = staticmethod(_categorical_new)
-__all__ += ["LinearPredictor", "linear_predictor", "ClassLinearPredictor", "class_linear_predictor", "constant"]
+
+
+# ---------------------------------------------------------------------------------------------
+# fused Poisson matrix factorisation: Poisson(rate = A @ B) with both factors latent
+# ---------------------------------------------------------------------------------------------
+class FactorProduct:
+    """Lazy product ``A @ B`` of two latent factors, either ``A`` [N, K] and ``B`` [K, J] or ``A`` [P, N, K] and
+    ``B`` [P, K, J] with the same P (no broadcasting): behaves like an ``[N, J]`` / ``[P, N, J]`` rate tensor when
+    handed to ``Poisson(rate)``, which then scores the site with ONE kernel that emits the sum and the gradients
+    of both factors (``b2_poisson_product``, 1 <= K <= 16) without writing the ``[P, N, J]`` rate.  Other shapes
+    raise ValueError.  ``bmm`` records a ``torch.bmm`` call, so that :meth:`dense` repeats the eager
+    computation bit for bit."""
+
+    def __init__(self, A, B, bmm=False):
+        if type(A).__name__ == "SiteValue":
+            A = A.as_subclass(torch.Tensor)
+        if type(B).__name__ == "SiteValue":
+            B = B.as_subclass(torch.Tensor)
+        if not (isinstance(A, torch.Tensor) and isinstance(B, torch.Tensor) and A.dim() == B.dim()
+                and A.dim() in (2, 3) and B.shape[-2] == A.shape[-1] and A.shape[:-2] == B.shape[:-2]
+                and A.dtype == B.dtype and A.device == B.device):
+            raise ValueError("FactorProduct: expected A [N, K] and B [K, J], or A [P, N, K] and B [P, K, J], of one "
+                             "dtype and device, got A %s and B %s" % (tuple(getattr(A, "shape", ())),
+                                                                      tuple(getattr(B, "shape", ()))))
+        self.A, self.B, self.bmm = A, B, bmm
+        self.vectorised = A.dim() == 3
+        self.P = A.shape[0] if self.vectorised else 1
+        self.K = A.shape[-1]
+        self.shape = A.shape[:-1] + B.shape[-1:]
+        self.dtype, self.device = A.dtype, A.device
+
+    def dense(self):
+        return torch.bmm(self.A, self.B) if self.bmm else torch.matmul(self.A, self.B)
+
+
+class _PoissonProductFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, meta, A, B, x):
+        scale, weight, coeff, unit = meta
+        N.require_cuda(A, "fused Poisson factorisation likelihood")
+        Ac, Bc = A.contiguous(), B.contiguous()
+        n, K = A.shape[-2:]
+        J = B.shape[-1]
+        P = A.shape[0] if A.dim() == 3 else 1
+        dev = A.device
+        total = torch.empty((), dtype=torch.float32, device=dev)
+        dA = torch.empty(Ac.shape, dtype=torch.float32, device=dev)
+        dB = torch.empty(Bc.shape, dtype=torch.float32, device=dev)
+        need = int(N.lib().b2_poisson_product_workspace(n, K, J, P))
+        ws = N.workspace(dev, need, tag="glm")
+        N.check(N.lib().b2_poisson_product(
+            Ac.data_ptr(), Bc.data_ptr(), x.data_ptr(), n, K, J, P, float(scale), float(weight), float(coeff), 0,
+            None, total.data_ptr(), dA.data_ptr(), dB.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(dev)),
+            "b2_poisson_product")
+        ctx.grads = (dA, dB)
+        ctx.unit = unit
+        return total
+
+    @staticmethod
+    def backward(ctx, gout):
+        dA, dB = ctx.grads
+        if not ctx.unit:
+            dA, dB = dA * gout, dB * gout
+        return None, dA, dB, None
+
+
+def _factor_lazy_of(rate):
+    if isinstance(rate, FactorProduct):
+        return rate
+    lz = getattr(rate, "_lazy", None) if isinstance(rate, torch.Tensor) else None
+    return lz if isinstance(lz, FactorProduct) else None
+
+
+class _PoissonProduct(Poisson):
+    """Poisson whose rate is a FactorProduct (built by ``Poisson(lazy)`` when an unchanged model's
+    ``torch.matmul(z, w)`` of two latent values was kept lazy by pyro_b200/lazy.py).  ``rate``, ``log_prob``,
+    ``mean`` and every other use materialise the rate; the ELBO's site sum takes the fused kernel."""
+
+    def __init__(self, rate, validate_args=None, is_sparse=False):
+        lazy = _factor_lazy_of(rate)
+        self._lazy = lazy
+        self._dense = None
+        Distribution.__init__(self, lazy.shape)
+
+    @property
+    def _params(self):
+        if self._dense is None:
+            self._dense = self._lazy.dense()
+        return [self._dense]
+
+    @property
+    def rate(self):
+        return self._params[0]
+
+    def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
+        lz = self._lazy
+        n, J = lz.shape[-2:]
+        # one [N, J] count matrix broadcast over the particles, fp32 on the factors' device
+        ok = (mask is None and isinstance(value, torch.Tensor) and value.dtype == torch.float32
+              and lz.A.dtype == torch.float32 and lz.B.dtype == torch.float32 and tuple(value.shape) == (n, J)
+              and value.device == lz.device and lz.device.type == "cuda" and J % 4 == 0 and 1 <= lz.K <= 16
+              and tuple(self.batch_shape) == tuple(lz.shape))
+        if not ok:
+            return super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
+        x = value.contiguous()
+        if x.data_ptr() % 16 != 0:
+            x = x.clone()
+        return _PoissonProductFn.apply((scale, weight, sum_coeff, unit), lz.A, lz.B, x)
+
+
+def _poisson_new(cls, rate=None, validate_args=None, is_sparse=False):
+    # ``Poisson(FactorProduct)`` builds the fused factorisation subclass
+    if cls is Poisson and _factor_lazy_of(rate) is not None:
+        return object.__new__(_PoissonProduct)
+    return object.__new__(cls)
+
+
+Poisson.__new__ = staticmethod(_poisson_new)
+__all__ += ["LinearPredictor", "linear_predictor", "ClassLinearPredictor", "class_linear_predictor", "FactorProduct",
+            "constant"]
 
 from .hmm import GaussianHMM  # noqa: E402,F401
 __all__ += ["GaussianHMM"]

@@ -19,19 +19,28 @@ Softmax regression has the same seam: ``X @ W.mT`` (``W.transpose(-1, -2)``, ``t
 kept as a :class:`ClassLinearPredictor`; a bias ``[K]`` or ``[P, 1, K]`` keeps them lazy, and
 ``Categorical(logits=lazy)`` scores the site with ``b2_glm_categorical_logits``.
 
+Poisson matrix factorisation (the bottom layer of the sparse gamma DEF) has one more: ``torch.matmul(z, w)``,
+``z @ w`` or ``torch.bmm(z, w)`` of TWO site values ``z[N, K] @ w[K, J]`` or ``z[P, N, K] @ w[P, K, J]``
+(fp32, one CUDA device, 1 <= K <= 16) gives a :class:`FactorProduct`, and ``Poisson(lazy)`` scores the site with
+``b2_poisson_product`` without writing the ``[P, N, J]`` rate.  Any other use, ``+`` included, materialises it.
+
 This is trace-time pattern matching at the seam where Pyro already passes values around (the replayed
 guide value of pyro/poutine/replay_messenger.py:50-61); nothing in the model is rewritten.
 """
 import torch
 
 from ._lazyparam import LazyExpParam
-from .distributions import ClassLinearPredictor, LinearPredictor
+from .distributions import ClassLinearPredictor, FactorProduct, LinearPredictor
 
 _VIEW_FUNCS = {"squeeze", "unsqueeze", "reshape", "view", "transpose", "t", "permute", "expand",
                "expand_as", "flatten", "contiguous", "__getitem__", "movedim", "swapaxes", "detach_",
                "mT", "T", "narrow", "select", "unflatten"}
-_MATMUL_FUNCS = {"matmul", "__matmul__", "__rmatmul__", "mm", "mv", "linear", "inner"}
+_MATMUL_FUNCS = {"matmul", "__matmul__", "__rmatmul__", "mm", "mv", "linear", "inner", "bmm"}
 _CLASS_MATMUL_FUNCS = {"matmul", "__matmul__", "__rmatmul__", "mm"}
+_FACTOR_MATMUL_FUNCS = {"matmul", "__matmul__", "__rmatmul__", "bmm"}
+# device types on which a product of two site values stays lazy: the fused Poisson kernel is CUDA only (the CPU
+# tests widen this to check the lazy semantics without a GPU)
+_FACTOR_DEVICE_TYPES = ("cuda",)
 _ADD_FUNCS = {"add", "__add__", "__radd__", "__iadd__", "add_"}
 _CHEAP_TRUE = {"eq", "__eq__", "isfinite"}
 _CHEAP_FALSE = {"ne", "__ne__", "isnan", "isinf"}
@@ -136,6 +145,10 @@ def _try_lazy_matmul(name, args):
     a, b = args
     if name == "__rmatmul__":
         a, b = b, a
+    if isinstance(a, SiteValue) and isinstance(b, SiteValue):
+        return _try_factor_product(name, a, b)
+    if name == "bmm":
+        return None
     if isinstance(a, SiteValue) and _is_data(b):
         # w_view [..., D] @ X^T [D, N]
         rm = _row_major(b)
@@ -161,6 +174,22 @@ def _try_lazy_matmul(name, args):
     return None
 
 
+def _try_factor_product(name, a, b):
+    """``z [N, K] @ w [K, J]`` or ``z [P, N, K] @ w [P, K, J]`` of two site values: a lazy rate, or None."""
+    if name not in _FACTOR_MATMUL_FUNCS or a.dtype != torch.float32 or b.dtype != torch.float32:
+        return None
+    if a.device != b.device or a.device.type not in _FACTOR_DEVICE_TYPES:
+        return None
+    if a.dim() == 2 and b.dim() == 2 and name != "bmm":
+        pass
+    elif not (a.dim() == 3 and b.dim() == 3 and a.shape[0] == b.shape[0]):
+        return None
+    K = a.shape[-1]
+    if b.shape[-2] != K or not 1 <= K <= 16:
+        return None
+    return LinearPredictorTensor(FactorProduct(a, b, bmm=name == "bmm"))
+
+
 def _class_weights_of(W, X):
     """A site value usable as class weights for the data matrix X: [K, D] or [P, K, D], same dtype/device."""
     return (W.dim() in (2, 3) and W.shape[-1] == X.shape[1] and W.shape[-2] >= 1 and W.dtype == X.dtype
@@ -184,7 +213,8 @@ def _make(X, w, b):
 
 class LinearPredictorTensor(torch.Tensor):
     """``X @ w^T + b`` not yet computed: metadata of a ``[P, N]`` / ``[N]`` tensor, no storage.  Wrapping a
-    :class:`ClassLinearPredictor` it stands for ``[N, K]`` / ``[P, N, K]`` class logits."""
+    :class:`ClassLinearPredictor` it stands for ``[N, K]`` / ``[P, N, K]`` class logits, wrapping a
+    :class:`FactorProduct` for an ``[N, J]`` / ``[P, N, J]`` product of two latent factors."""
 
     @staticmethod
     def __new__(cls, lazy):
@@ -208,6 +238,8 @@ class LinearPredictorTensor(torch.Tensor):
 
     def _with_bias(self, b):
         lz = self._lazy
+        if isinstance(lz, FactorProduct):
+            return None
         if isinstance(lz, ClassLinearPredictor):
             if isinstance(b, LinearPredictorTensor):
                 return None
