@@ -264,7 +264,7 @@ int b2_elbo_combine(const void* const* terms, const double* coeffs, int n, int d
  * X and y are read from HBM exactly once for value AND gradient.  Replaces the chain
  * matmul -> Bernoulli(logits).log_prob -> sum -> backward (pyro/poutine/trace_struct.py:264-278
  * applied to the model of tests/infer/mcmc/test_hmc.py:189-198).
- * X: [N,D] row-major fp32 (16-byte aligned), D in {4, 8, 16, 32}; W: [P,D]; b: [P] (nullable);
+ * X: [N,D] row-major fp32 (16-byte aligned), 1 <= D <= 128; W: [P,D]; b: [P] (nullable);
  * y: [N] fp32.
  * out_total (nullable): scalar, (=|+=) sum_coeff * scale * SUM_p sum_p[p].
  * For D == 32 and N >= 8192 the two contractions run on the tensor cores (wgmma) out of TMA-staged
@@ -273,10 +273,15 @@ int b2_elbo_combine(const void* const* terms, const double* coeffs, int n, int d
  * the same way and survives the N-term sums); X and g = y - sigmoid are rounded to nearest TF32
  * (incoherent, averages as 1/sqrt(N)): sum_p, dW, db agree with an fp64 evaluation to ~1e-6 / ~1e-5
  * relative at N = 1e6.  Below 65536 rows, and at any N with B2_FLAG_GLM_3XTF32, X is split as well
- * (every logit fp32-exact).  All other calls run the fp32 SIMT kernel: D != 32, N < 8192 without
- * B2_FLAG_GLM_3XTF32, B2_FLAG_GLM_FP32, a y that is not 16-byte aligned (the tensor-core kernel loads
- * y with TMA) and N >= 2^31.  Flag bits 8, 16 and 64 selected variants removed in version 101 and are
- * ignored.
+ * (every logit fp32-exact).  All other calls with D in {4, 8, 16, 32} run the fp32 SIMT kernel: D != 32,
+ * N < 8192 without B2_FLAG_GLM_3XTF32, B2_FLAG_GLM_FP32, a y that is not 16-byte aligned (the tensor-core
+ * kernel loads y with TMA) and N >= 2^31.
+ * Every other D in 1..128 runs on the tensor cores at any N (glm_flat_tc.cu: each 64-row tile arrives by
+ * one 1-D bulk copy, D is padded to a multiple of 32 in shared memory) with the same precision policy.
+ * It needs a 16-byte aligned y and N < 2^31 (B2_ERR_BAD_SHAPE / B2_ERR_TOO_LARGE otherwise) and has no
+ * fp32 SIMT kernel: B2_FLAG_GLM_FP32 with such a D returns B2_ERR_BAD_SHAPE, as does any D outside
+ * 1..128.  All of this is checked before any CUDA call.  Flag bits 8, 16 and 64 selected variants removed
+ * in version 101 and are ignored.
  * workspace: b2_glm_workspace() bytes, zero-initialised ONCE by the caller (its first 256 bytes
  * hold a ticket counter that the library leaves zeroed).  Two launches: the streaming kernel
  * and a finish kernel that sums the CTA partials in a fixed order (deterministic).

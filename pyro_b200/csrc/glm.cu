@@ -7,8 +7,8 @@
 // N=1e6, D=32), instead of materialising the [P,N] logits / log_prob / grad tensors that the
 // reference chain (matmul -> Bernoulli.log_prob -> sum -> backward) writes and re-reads.
 //
-// fp32 SIMT kernel (D != 32, N < 8192 rows, B2_FLAG_GLM_FP32, and operands the wgmma kernel of
-// glm_tc.cu cannot load): CTA = 256 threads = 4 row groups x 64 particles.  Each thread
+// fp32 SIMT kernel (D in {4, 8, 16}; at D = 32: N < 8192 rows, B2_FLAG_GLM_FP32, and operands the wgmma
+// kernel of glm_tc.cu cannot load; every other D in 1..128 takes the wgmma kernel of glm_flat_tc.cu): CTA = 256 threads = 4 row groups x 64 particles.  Each thread
 // keeps W[p,:] and its dW[p,:] accumulator in registers; X tiles are staged through shared memory
 // with cp.async double buffering and read back as warp-wide broadcasts (every lane of a warp has a
 // different particle but the same row, so an LDS.128 serves 4 FMAs x 2 uses for all 32 lanes).
@@ -190,6 +190,9 @@ __global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict
 int glm_tc_grid_x(int64_t N);
 int launch_glm_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int P,
                   float* partials, int gx, bool split_x, cudaStream_t s);
+// wgmma variant for the other feature counts, 1 <= D <= 128 (glm_flat_tc.cu)
+void launch_glm_flat_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
+                        float* partials, int gx, bool split_x, cudaStream_t s);
 
 inline int glm_grid_x(int64_t N) {
   const int64_t ntiles = (N + kGlmTileRows - 1) / kGlmTileRows;
@@ -217,6 +220,13 @@ extern "C" int b2_glm_bernoulli_logits(const float* X, const float* y, const flo
   if (!X || !y || !W) return B2_ERR_NULL;
   if (N <= 0 || P <= 0) return B2_ERR_BAD_SHAPE;
   if (reinterpret_cast<uintptr_t>(X) % 16 != 0) return B2_ERR_BAD_SHAPE;
+  if (D < 1 || D > 128) return B2_ERR_BAD_SHAPE;
+  // D in {4, 8, 16, 32} keep their kernels; every other D takes the wgmma kernel of glm_flat_tc.cu, which
+  // has no fp32 SIMT counterpart and loads y by 16-byte bulk copies with 32-bit row counts
+  const bool flat = !(D == 4 || D == 8 || D == 16 || D == 32);
+  if (flat && (flags & B2_FLAG_GLM_FP32)) return B2_ERR_BAD_SHAPE;
+  if (flat && reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
+  if (flat && N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
   if (!workspace || workspace_bytes < b2_glm_workspace(N, D, P)) return B2_ERR_WORKSPACE;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   // below 8 Ki rows the single-pass TF32 gradient contraction has not averaged its operand rounding
@@ -225,13 +235,15 @@ extern "C" int b2_glm_bernoulli_logits(const float* X, const float* y, const flo
   // 16-byte aligned y and 32-bit row coordinates; other operands take the SIMT kernel as well.
   const bool use_tc = (D == 32) && !(flags & B2_FLAG_GLM_FP32) && reinterpret_cast<uintptr_t>(y) % 16 == 0 &&
                       N < ((int64_t)1 << 31) && (N >= 8192 || (flags & B2_FLAG_GLM_3XTF32));
-  const int gx = use_tc ? glm_tc_grid_x(N) : glm_grid_x(N);
+  const int gx = (use_tc || flat) ? glm_tc_grid_x(N) : glm_grid_x(N);
   dim3 grid((unsigned)gx, (unsigned)((P + kGlmParticles - 1) / kGlmParticles), 1);
   unsigned int* ticket = reinterpret_cast<unsigned int*>(workspace);
   float* partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  if (use_tc) {
-    // default: W split; below 64 Ki rows the incoherent X rounding has not averaged out yet -> full 3xTF32
-    const bool split_x = (flags & B2_FLAG_GLM_3XTF32) || N < 65536;
+  // default: W split; below 64 Ki rows the incoherent X rounding has not averaged out yet -> full 3xTF32
+  const bool split_x = (flags & B2_FLAG_GLM_3XTF32) || N < 65536;
+  if (flat) {
+    launch_glm_flat_tc(X, y, W, b, N, D, P, partials, gx, split_x, s);
+  } else if (use_tc) {
     const int rc = launch_glm_tc(X, y, W, b, N, P, partials, gx, split_x, s);
     if (rc != 0) return rc;
   } else

@@ -1,0 +1,415 @@
+// glm_flat_tc.cu -- Hopper fused logistic-regression likelihood kernel for any feature count D in 1..128
+// (every D without a fused kernel of its own: glm_tc.cu takes D = 32, glm.cu's SIMT kernel D in {4, 8, 16}).
+//
+// Same contract as glm_bernoulli_tc_kernel (glm_tc.cu): ONE pass over X[N,D] and y[N] gives, for up to 64
+// weight vectors (particles) per CTA slab, sum_n log Bernoulli(y_n | logits = x_n.w_p + b_p), dW and db, as
+// CTA partials [gridDim.x][P][D + 2] that glm_finish_kernel adds in a fixed order.
+//
+// D is padded to DC = ceil(D / 32) swizzle atoms of 32 columns (KD = 32 DC).  A 2-D TMA load needs a row
+// stride that is a multiple of 16 bytes, which 4 D mostly is not; but the 64 rows of a tile are one
+// contiguous block of 256 D bytes, 16-byte aligned when X is.  So each tile arrives by ONE 1-D bulk copy
+// (cp.async.bulk, completing on an mbarrier) into an unswizzled [64][D] landing buffer, and its y the same
+// way.  The last tile's byte count need not be a multiple of 16: the thread that issues the copies writes
+// its last (< 4) floats, and the y of rows past N as zeros, with ordinary loads and stores first, so nothing
+// is read past the end of X or y.
+//
+// Per 64-row tile (persistent CTAs, tiles round-robin over CTAs and inside a CTA over its warpgroups):
+//
+//   split    the warpgroup reads the landing buffer and writes the padded SWIZZLE_128B GEMM 1 operand
+//            (X rounded to nearest TF32, or X_hi / X_lo under SPLIT_X) and the transposed X^T (rows kt_pos
+//            permuted like glm_tc.cu, plus 8 rows of ones) that is GEMM 2's B operand.  Columns d >= D and
+//            rows past N are written as exact zeros: a landing buffer that was never written, or that holds
+//            another tile, may hold NaN bit patterns, and 0 * NaN = NaN.  Then the landing buffer is refilled
+//            with the warpgroup's next tile, which arrives while this tile is contracted.
+//   GEMM 1   D1^T[p, n] = sum_d W[p, d] X[n, d] + b[p]    wgmma m64n64k8 over 4 DC k-steps, W split hi + lo.
+//   epilogue the one of glm_tc.cu (glm_tc_common.cuh): lp sums and g = y - sigmoid rounded to TF32, in
+//            registers; only the last, partial tile masks rows.
+//   GEMM 2   [dW | db][p, :] += sum_n g[p, n] [X | 1][n, :]   wgmma m64n(KD + 8)k8, A = g from registers;
+//            db is accumulator column KD.  Committed and left running while the next tile is waited for.
+//
+// Precision policy of glm_tc.cu: W always split, X split under SPLIT_X, g rounded to nearest TF32.
+//
+// Budget: at DC = 4 one warpgroup holds W hi + lo (64 KB), X hi + lo (64 KB), X^T (34 KB) and a landing tile
+// (32 KB), and its GEMM 2 accumulator alone takes 68 registers.  So DC = 1 runs four warpgroups per CTA (the
+// 128-register cap of glm_tc.cu), DC = 2 two and DC >= 3 one, each with a single landing stage.
+//
+// Determinism: every CTA writes its partials once (warpgroups summed in a fixed order); no float atomics.
+#include <cuda.h>
+#include <stdlib.h>
+
+#include "b2_common.cuh"
+#include "glm_tc_common.cuh"
+
+namespace b2 {
+namespace tcf {
+
+using namespace tc;
+
+constexpr int kRows = 64;                       // rows per tile = M of one wgmma
+constexpr int kP = 64;
+
+template <int DC>
+struct Cfg {
+  static constexpr int kKD = 32 * DC;                          // padded feature count
+  static constexpr int kN2 = kKD + 8;                          // GEMM 2 width: dW columns, db, 7 unused
+  static constexpr int kWG = DC == 1 ? 4 : DC == 2 ? 2 : 1;    // warpgroups per CTA
+  static constexpr int kThreads = 128 * kWG;
+  static constexpr uint32_t kOp = DC * 8192u;                  // [DC atoms][64 rows][32] fp32, SW128
+  static constexpr uint32_t kXtBlock = kN2 * 128u;             // X^T k-block: KD + 8 rows of 32 n
+  // per-warpgroup region
+  static constexpr uint32_t WG_XOP = 0;                        // GEMM 1 operand: rounded X or X_hi
+  static constexpr uint32_t WG_XLO = WG_XOP + kOp;             // X_lo (SPLIT_X)
+  static constexpr uint32_t WG_XT = WG_XLO + kOp;              // X^T [kb 2][c KD + 8][32 n], n permuted (kt_pos)
+  static constexpr uint32_t WG_LAND = WG_XT + 2 * kXtBlock;    // landing buffer [64][D], unswizzled
+  static constexpr uint32_t WG_Y = WG_LAND + kOp;              // y [64]
+  static constexpr uint32_t kWGBytes = WG_Y + 1024;
+  // CTA layout (operand regions 1024-byte aligned: the 128-byte swizzle pattern is taken from address bits)
+  static constexpr uint32_t OFF_WHI = 0;                       // [DC][p 64][32] SW128
+  static constexpr uint32_t OFF_WLO = OFF_WHI + kOp;
+  static constexpr uint32_t OFF_WG = OFF_WLO + kOp;
+  static constexpr uint32_t OFF_BAR = OFF_WG + kWG * kWGBytes;
+  static constexpr uint32_t kSmemBytes = OFF_BAR + 64 + 1024;  // + slack for the 1024-byte alignment
+  // the final reduction reuses the warpgroup regions: [kWG][64 p][KD + 1] + [kWG][64 p] floats
+  static constexpr int kRS = kKD + 1;
+  static_assert(kSmemBytes <= 232448, "shared memory budget");
+  static_assert(kXtBlock % 1024 == 0 && kWGBytes % 1024 == 0, "operand alignment");
+  static_assert((kWG * kP * kRS + kWG * kP) * 4 <= kWG * kWGBytes, "reduction scratch");
+};
+
+// one 1-D bulk copy global -> shared, completing `bytes` (a non-zero multiple of 16) on the mbarrier
+__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
+               : "memory");
+}
+
+// GEMM 2: D[64 x N] = A[64 x 8] B[N x 8]^T (+ D when acc != 0), TF32, A from registers (layout of
+// wgmma_n40_tf32_ra), B K-major SWIZZLE_128B in shared memory
+template <int N>
+__device__ __forceinline__ void wgmma_tf32_ra(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b, int acc);
+template <>
+__device__ __forceinline__ void wgmma_tf32_ra<40>(float (&d)[20], const uint32_t (&a)[4], uint64_t b, int acc) {
+  wgmma_n40_tf32_ra(d, a, b, acc);
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32_ra<72>(float (&d)[36], const uint32_t (&a)[4], uint64_t b, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %41, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n72k8.f32.tf32.tf32 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20,"
+      "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35"
+      "}, {%36, %37, %38, %39}, %40, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32_ra<104>(float (&d)[52], const uint32_t (&a)[4], uint64_t b, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %57, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n104k8.f32.tf32.tf32 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20,"
+      "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39,"
+      "%40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51"
+      "}, {%52, %53, %54, %55}, %56, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
+      : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32_ra<136>(float (&d)[68], const uint32_t (&a)[4], uint64_t b, int acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %73, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n136k8.f32.tf32.tf32 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20,"
+      "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39,"
+      "%40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58,"
+      "%59, %60, %61, %62, %63, %64, %65, %66, %67"
+      "}, {%68, %69, %70, %71}, %72, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
+      : "memory");
+}
+
+
+// wgmma accumulator fragment (m64nN, f32): thread (warp w4 of the warpgroup, lane = 4 gid + t4) holds
+// d[4j + 2h + e] = D[16 w4 + gid + 8h][8j + 2 t4 + e].
+template <int DC, bool SPLIT_X>
+__global__ void __launch_bounds__(Cfg<DC>::kThreads, 1)
+glm_bernoulli_flat_tc_kernel(const float* __restrict__ X, const float* __restrict__ y, const float* __restrict__ W,
+                             const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials) {
+  using C = Cfg<DC>;
+  constexpr int kKD = C::kKD, kWG = C::kWG;
+  pdl_enter();   // lets glm_finish_kernel be resident (blocked in its griddepcontrol.wait) before this kernel ends
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;
+  uint8_t* sm = smem_raw + (base - raw);
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int slab = blockIdx.y;
+  const int64_t ntiles = (N + kRows - 1) / kRows;
+  // tiles handled by this CTA: blockIdx.x, blockIdx.x + gridDim.x, ...
+  const int nt = (int)((ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x);
+
+  // ---- one-time setup --------------------------------------------------------------------------------
+  if (tid == 0) {
+    for (int s = 0; s < kWG; ++s) mbar_init(base + C::OFF_BAR + 8u * (uint32_t)s, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  {
+    // weight tiles, zero in the padding columns d >= D (generic-proxy writes, made visible to the tensor cores)
+    float* whi = reinterpret_cast<float*>(sm + C::OFF_WHI);
+    float* wlo = reinterpret_cast<float*>(sm + C::OFF_WLO);
+    for (int e = tid; e < kP * kKD; e += C::kThreads) {
+      const int p = e / kKD, d = e - p * kKD;
+      const int gp = slab * kP + p;
+      const float w = (gp < P && d < D) ? W[(int64_t)gp * D + d] : 0.f;
+      const float hi = tf32_trunc(w);
+      const int off = (d >> 5) * 2048 + sw128(p, d & 31);
+      whi[off] = hi;
+      wlo[off] = w - hi;
+    }
+    // rows KD..KD+7 of every X^T k-block are ones: GEMM 2 then yields db in column KD of its accumulator
+    for (int e = tid; e < kWG * 2 * 256; e += C::kThreads) {
+      const int g = e >> 9, kb = (e >> 8) & 1, w = e & 255;
+      reinterpret_cast<float*>(sm + C::OFF_WG + g * C::kWGBytes + C::WG_XT + kb * C::kXtBlock + kKD * 128)[w] = 1.f;
+    }
+  }
+  fence_proxy_async();
+  __syncthreads();
+
+  float lpa[2] = {0.f, 0.f};                   // lp sums of the thread's two particles
+  // GEMM 2 accumulator [p][c]: dW in c < D, db in c = KD.  Started by the warpgroup's first GEMM 2 k-step
+  // with scale-d = 0, never written by ordinary instructions before the tile loop (C7515, see glm_tc.cu).
+  float acc2[C::kN2 / 2];
+  // warp-uniform by construction (a shuffle result), so the tile loop is not a divergent branch to ptxas
+  const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0), w4 = warp & 3, t = tid & 127;
+  const int gid = lane >> 2, t4 = lane & 3;
+
+  {
+    uint8_t* my = sm + C::OFF_WG + wg * C::kWGBytes;
+    const uint32_t my_s = base + C::OFF_WG + wg * C::kWGBytes;
+    const uint32_t bar = base + C::OFF_BAR + 8u * (uint32_t)wg;
+    float* land = reinterpret_cast<float*>(my + C::WG_LAND);
+    float* ys = reinterpret_cast<float*>(my + C::WG_Y);
+    float bias[2];                             // of particles 16 w4 + gid + 8h
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int gp = slab * kP + 16 * w4 + gid + 8 * h;
+      bias[h] = (bvec != nullptr && gp < P) ? bvec[gp] : 0.f;
+    }
+    // tile it -> landing buffer; one thread of the warpgroup issues the loads
+    auto load = [&](int it) {
+      const int64_t row0 = (blockIdx.x + (int64_t)it * gridDim.x) * kRows;
+      const int rows = (int)(N - row0 < kRows ? N - row0 : kRows);
+      const uint32_t xb = (uint32_t)(rows * D) * 4u, yb = (uint32_t)rows * 4u;
+      const uint32_t xbulk = xb & ~15u, ybulk = yb & ~15u;
+      if (rows < kRows || xbulk != xb) {       // the last tile: its remainder and zeros for y past N
+        const float* xsrc = X + row0 * D;
+        for (uint32_t i = xbulk / 4; i < xb / 4; ++i) land[i] = xsrc[i];
+        for (int i = (int)(ybulk / 4); i < kRows; ++i) ys[i] = (i < rows) ? y[row0 + i] : 0.f;
+      }
+      // the arrive releases the ordinary stores above to the warpgroup's mbar_wait
+      mbar_expect_tx(bar, xbulk + ybulk);
+      if (xbulk) bulk_load(my_s + C::WG_LAND, X + row0 * D, xbulk, bar);
+      if (ybulk) bulk_load(my_s + C::WG_Y, y + row0, ybulk, bar);
+    };
+    if (t == 0 && wg < nt) load(wg);
+    for (int k = 0, it = wg; it < nt; ++k, it += kWG) {
+      const int64_t row0 = (blockIdx.x + (int64_t)it * gridDim.x) * kRows;
+      const int rows = (int)(N - row0 < kRows ? N - row0 : kRows);
+      mbar_wait(bar, (uint32_t)k & 1u);
+      // GEMM 2 of this warpgroup's previous tile has finished reading X^T and the g registers
+      wgmma_wait0();
+      fence_regs(acc2);
+      // ---- split / transposition pass (thread mapping of glm_tc.cu, once per 32-column atom) ------------
+      // Thread t owns the 16-byte chunk c (d = 32 a + 4c .. +3) of the four rows n = 8 q8 + 2i + e, which
+      // kt_pos puts at the consecutive k = 8 q8 + 4e + i: after a 4x4 transpose in registers each d is one
+      // 16-byte store into X^T.
+      {
+        const int lam = t & 7, mu = t >> 3;
+        const int e = lam & 1, q8 = ((mu >> 3) << 2) | (lam >> 1);
+        const int c = (((lam & 1) << 2) | (lam >> 1)) ^ (mu & 7);
+        const int kc = 2 * (q8 & 3) + e;
+        float4* xs = reinterpret_cast<float4*>(my + C::WG_XOP);
+        float4* xl = reinterpret_cast<float4*>(my + C::WG_XLO);
+        float4* xt = reinterpret_cast<float4*>(my + C::WG_XT + (q8 >> 2) * C::kXtBlock);
+#pragma unroll
+        for (int a = 0; a < DC; ++a) {
+          float xr[4][4];                      // [i][q] = X[8 q8 + 2i + e][32 a + 4c + q] rounded to nearest TF32
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int r = 8 * q8 + 2 * i + e;
+            const int idx = a * 512 + r * 8 + (c ^ (r & 7));   // 16-byte chunk of the SW128 operand
+            float x[4];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              const int d = 32 * a + 4 * c + q;
+              const float v = land[r * D + min(d, D - 1)];
+              x[q] = (d < D && r < rows) ? v : 0.f;
+              xr[i][q] = tf32_rn(x[q]);
+            }
+            if (SPLIT_X) {
+              float h[4];
+#pragma unroll
+              for (int q = 0; q < 4; ++q) h[q] = tf32_trunc(x[q]);
+              xs[idx] = make_float4(h[0], h[1], h[2], h[3]);
+              xl[idx] = make_float4(x[0] - h[0], x[1] - h[1], x[2] - h[2], x[3] - h[3]);
+            } else {
+              xs[idx] = make_float4(xr[i][0], xr[i][1], xr[i][2], xr[i][3]);
+            }
+          }
+          // X^T[d][k]: k-block k >> 5, 16-byte chunk ((k & 31) >> 2) ^ (d & 7), element k & 3 (= i here)
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const int d = 32 * a + 4 * c + q;
+            xt[d * 8 + (kc ^ (d & 7))] = make_float4(xr[0][q], xr[1][q], xr[2][q], xr[3][q]);
+          }
+        }
+      }
+      float2 yr[8];                            // y of the thread's rows n = 8j + 2 t4 + e, read before the refill
+#pragma unroll
+      for (int j = 0; j < 8; ++j) yr[j] = reinterpret_cast<const float2*>(ys)[4 * j + t4];
+      fence_proxy_async();
+      wg_bar(1 + wg);
+      // the landing buffer is free: the warpgroup's next tile arrives while this one is contracted
+      if (t == 0 && it + kWG < nt) load(it + kWG);
+      // ---- GEMM 1: logits D1^T[p, n] = W X^T + b, accumulator initialised with the bias ---------------
+      float acc1[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc1[i] = bias[(i >> 1) & 1];
+      wgmma_fence();
+#pragma unroll
+      for (int a = 0; a < DC; ++a) {
+        const uint64_t d_whi = desc_sw128(base + C::OFF_WHI + a * 8192), d_wlo = desc_sw128(base + C::OFF_WLO + a * 8192);
+        const uint64_t d_x = desc_sw128(my_s + C::WG_XOP + a * 8192), d_xlo = desc_sw128(my_s + C::WG_XLO + a * 8192);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          wgmma_n64_tf32(acc1, d_whi + 2 * k, d_x + 2 * k);
+          wgmma_n64_tf32(acc1, d_wlo + 2 * k, d_x + 2 * k);
+          if (SPLIT_X) wgmma_n64_tf32(acc1, d_whi + 2 * k, d_xlo + 2 * k);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait0();
+      fence_regs(acc1);
+      // ---- epilogue: lp sums and g, both in registers; the row mask only in the last, partial tile ------
+      uint32_t g[32];                          // indexed like acc1
+      float lin[2], prod[2];
+      if (rows < kRows)
+        epilogue<true>(acc1, yr, row0, N, t4, lin, prod, g);
+      else
+        epilogue<false>(acc1, yr, row0, N, t4, lin, prod, g);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) lpa[h] += fmaf(lg2f(prod[h]), -0.6931471805599453f, lin[h]);
+      // ---- GEMM 2: [dW | db] += g [X | 1], g from registers, left running while the next tile is waited for
+      fence_regs(g);
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const uint32_t a[4] = {g[4 * j], g[4 * j + 2], g[4 * j + 1], g[4 * j + 3]};
+        wgmma_tf32_ra<C::kN2>(acc2, a, desc_sw128(my_s + C::WG_XT + (j >> 2) * C::kXtBlock) + 2 * (j & 3),
+                              it != wg || j != 0);
+      }
+      wgmma_commit();
+    }
+    wgmma_wait0();
+    fence_regs(acc2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float v = lpa[h];
+      v += __shfl_xor_sync(0xffffffffu, v, 1);
+      v += __shfl_xor_sync(0xffffffffu, v, 2);
+      lpa[h] = v;
+    }
+  }
+  // ---- CTA results through shared memory (the warpgroup regions are idle now), fixed summation order -----
+  __syncthreads();
+  float* red2 = reinterpret_cast<float*>(sm + C::OFF_WG);   // [kWG][64 p][KD + 1]
+  float* redlp = red2 + kWG * kP * C::kRS;                  // [kWG][64 p]
+  {
+#pragma unroll
+    for (int j = 0; j < C::kN2 / 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int p = 16 * w4 + gid + 8 * h, c = 8 * j + 2 * t4 + e;
+          if (c < D || c == kKD) red2[(wg * kP + p) * C::kRS + c] = acc2[4 * j + 2 * h + e];
+        }
+    if (t4 == 0) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) redlp[wg * kP + 16 * w4 + gid + 8 * h] = lpa[h];
+    }
+  }
+  __syncthreads();
+  if (tid < kP) {
+    const int gp = slab * kP + tid;
+    if (gp < P) {
+      float* o = partials + ((int64_t)blockIdx.x * P + gp) * (D + 2);
+      for (int c = 0; c <= D; ++c) {           // dW[0..D-1], then db from accumulator column KD
+        const int col = c < D ? c : kKD;
+        float v = 0.f;
+        for (int g = 0; g < kWG && g < nt; ++g) v += red2[(g * kP + tid) * C::kRS + col];
+        o[c] = v;
+      }
+      float v = 0.f;
+      for (int g = 0; g < kWG && g < nt; ++g) v += redlp[g * kP + tid];
+      o[D + 1] = v;
+    }
+  }
+}
+
+template <int DC, bool SPLIT_X>
+void launch_one(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
+                float* partials, int gx, cudaStream_t s) {
+  using C = Cfg<DC>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaFuncSetAttribute(glm_bernoulli_flat_tc_kernel<DC, SPLIT_X>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)C::kSmemBytes);
+    attr_set = true;
+  }
+  dim3 grid((unsigned)gx, (unsigned)((P + kP - 1) / kP), 1);
+  launch_pdl(glm_bernoulli_flat_tc_kernel<DC, SPLIT_X>, grid, dim3(C::kThreads), (size_t)C::kSmemBytes, s,
+             X, y, W, b, N, D, P, partials);
+}
+
+}  // namespace tcf
+
+// ---- host side -------------------------------------------------------------------------------------------
+// The caller (b2_glm_bernoulli_logits) has checked 1 <= D <= 128, N < 2^31 and 16-byte aligned X and y.
+void launch_glm_flat_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
+                        float* partials, int gx, bool split_x, cudaStream_t s) {
+  using namespace tcf;
+  switch ((D + 31) / 32) {
+    case 1: (split_x ? launch_one<1, true> : launch_one<1, false>)(X, y, W, b, N, D, P, partials, gx, s); break;
+    case 2: (split_x ? launch_one<2, true> : launch_one<2, false>)(X, y, W, b, N, D, P, partials, gx, s); break;
+    case 3: (split_x ? launch_one<3, true> : launch_one<3, false>)(X, y, W, b, N, D, P, partials, gx, s); break;
+    default: (split_x ? launch_one<4, true> : launch_one<4, false>)(X, y, W, b, N, D, P, partials, gx, s); break;
+  }
+}
+
+}  // namespace b2

@@ -82,82 +82,6 @@ static_assert(kWGBytes % 1024 == 0 && kXtBlock % 1024 == 0, "operand alignment")
 // the final reduction reuses the X ring: [kWG][64 p][33] + [kWG][64 p] floats
 static_assert((kWG * kP * 33 + kWG * kP) * 4 <= kStages * kTile, "reduction scratch");
 
-constexpr int kEpiBatch = 4;                    // logits of one particle per epilogue batch (8 fits, no faster)
-
-// lp = y*l - softplus(l) = y*l - max(l, 0) - ln(1 + e^-|l|).  The epilogue sums the linear part per tile and
-// multiplies the denominators den = 1 + e^-|l| instead of taking a logarithm of each: den is in (1, 2], so
-// the product of a thread's 16 rows of one particle is at most 2^16, and one lg2 per particle and tile
-// replaces 16.  Rounding: each of the 15 products adds at most 2^-24 relative, at most 15 * 2^-24 = 9e-7
-// nats per 16 logits, no worse than the sixteen lg2.approx results it replaces (about 1e-7 nats each).
-//
-// One batch of B logits of one particle, stage by stage: each MUFU result is consumed a stage (>= B
-// instructions) after it was issued, and the four warps per scheduler cover the rest of the MUFU latency.
-// Returns the sum of y*l - max(l, 0) over the batch, multiplies the batch's den into prod and writes
-// g = y - sigmoid(l) rounded to nearest TF32.  MASK weights the linear part and g with vw (0 for rows past
-// N) and gives a masked row the factor 1 exactly.
-template <bool MASK, int B>
-__device__ __forceinline__ float epi_batch(const float* lr, const float* y, const float* vw, float& prod,
-                                           uint32_t* g) {
-  float e[B], den[B], inv[B], f[B], lp[B];
-#pragma unroll
-  for (int j = 0; j < B; ++j) e[j] = ex2f(-1.4426950408889634f * fabsf(lr[j]));
-#pragma unroll
-  for (int j = 0; j < B; ++j) den[j] = 1.f + e[j];
-#pragma unroll
-  for (int j = 0; j < B; ++j) inv[j] = rcpf(den[j]);
-#pragma unroll
-  for (int j = 0; j < B; ++j) f[j] = MASK ? fmaf(vw[j], e[j], 1.f) : den[j];
-#pragma unroll
-  for (int j = 0; j < B; ++j) {
-    const float l = lr[j];
-    lp[j] = fmaf(y[j], l, -fmaxf(l, 0.f));
-    const float sg = (l >= 0.f) ? inv[j] : e[j] * inv[j];
-    float gg = y[j] - sg;
-    if (MASK) {
-      lp[j] *= vw[j];
-      gg *= vw[j];
-    }
-    g[j] = __float_as_uint(tf32_rn(gg));
-  }
-#pragma unroll
-  for (int w = 1; w < B; w *= 2)
-#pragma unroll
-    for (int j = 0; j < B; j += 2 * w) {
-      lp[j] += lp[j + w];
-      f[j] *= f[j + w];
-    }
-  prod *= f[0];
-  return lp[0];
-}
-
-// The epilogue of one tile: the linear lp sums lin[h] and den products prod[h] of the thread's two particles
-// (16 rows each), and g indexed like acc1.  MASK (the last, partial tile only) zeroes rows past N.
-template <bool MASK>
-__device__ __forceinline__ void epilogue(const float (&acc1)[32], const float2 (&yr)[8], int64_t row0, int64_t N,
-                                         int t4, float (&lin)[2], float (&prod)[2], uint32_t (&g)[32]) {
-  constexpr int B = kEpiBatch;
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    prod[h] = 1.f;
-#pragma unroll
-    for (int q = 0; q < 16 / B; ++q) {         // k-blocks j = B/2 q .. B/2 q + B/2 - 1
-      float l[B], yy[B], vw[B];
-      uint32_t gb[B];
-#pragma unroll
-      for (int i = 0; i < B; ++i) {
-        const int j = B / 2 * q + (i >> 1), e = i & 1;
-        l[i] = acc1[4 * j + 2 * h + e];
-        yy[i] = e ? yr[j].y : yr[j].x;
-        vw[i] = MASK ? ((row0 + 8 * j + 2 * t4 + e < N) ? 1.f : 0.f) : 1.f;
-      }
-      const float s = epi_batch<MASK, B>(l, yy, vw, prod[h], gb);
-      lin[h] = q ? lin[h] + s : s;
-#pragma unroll
-      for (int i = 0; i < B; ++i) g[4 * (B / 2 * q + (i >> 1)) + 2 * h + (i & 1)] = gb[i];
-    }
-  }
-}
-
 // SPLIT_X = false (default): W split hi/lo, X rounded to nearest.  SPLIT_X = true: full 3xTF32, X split
 // hi/lo as well.
 //

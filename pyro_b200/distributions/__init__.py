@@ -1101,15 +1101,21 @@ class _BernoulliLinear(Bernoulli):
         lz = self._lazy
         X = lz.X
         D = X.shape[-1]
-        ok = (mask is None and X.dtype == torch.float32 and X.is_contiguous() and D in (4, 8, 16, 32)
+        tc = getattr(lz, "tensor_cores", True)
+        # D in {4, 8, 16, 32} have their own kernels; every other D up to 128 takes the wgmma kernel of
+        # glm_flat_tc.cu, from 8192 rows (below that its TF32 gradient has not averaged its rounding down to
+        # fp32 accuracy yet, and there is no fp32 kernel for these D)
+        flat = D not in (4, 8, 16, 32)
+        ok = (mask is None and X.dtype == torch.float32 and X.is_contiguous()
+              and (not flat or (1 <= D <= 128 and tc and X.shape[0] >= 8192))
               and isinstance(value, torch.Tensor) and value.numel() == X.shape[0]
               and tuple(self.batch_shape) == tuple(lz.shape) and X.data_ptr() % 16 == 0)
-        if not ok:
+        y = value.reshape(-1).to(torch.float32).contiguous() if ok else None
+        if not ok or (flat and y.data_ptr() % 16 != 0):
             return super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
-        y = value.reshape(-1).to(torch.float32).contiguous()
         W = lz.w.reshape(lz.P, D)
         b = lz.b.reshape(lz.P) if lz.b is not None else None
-        flags = 0 if getattr(lz, "tensor_cores", True) else N.B2_FLAG_GLM_FP32
+        flags = 0 if tc else N.B2_FLAG_GLM_FP32
         return _GlmBernoulliFn.apply((scale, weight, sum_coeff, unit, flags), X, y, W, b)
 
 
