@@ -305,7 +305,8 @@ size_t b2_glm_workspace(int64_t N, int D, int P);
  * read); the other particles are unaffected.
  * out_total (nullable): scalar, (=|+=) sum_coeff * scale * SUM_p sum_p[p] (B2_FLAG_ACCUMULATE_SUM).
  * out_sum_p, out_dW, out_db are nullable; dW and db are scaled by weight * scale.
- * Both contractions run on the tensor cores (wgmma, glm_categorical_tc.cu) with the precision policy of
+ * Both contractions run on the tensor cores (wgmma, glm_categorical_tc.cu on the D = 32 tile pipeline of
+ * the Bernoulli kernel, glm_tc_common.cuh) with the precision policy of
  * b2_glm_bernoulli_logits: W is split hi + lo and X rounded to nearest TF32 (incoherent error, averages
  * as 1/sqrt(N)); below 65536 rows, and at any N with B2_FLAG_GLM_3XTF32, X is split as well (every
  * logit fp32-exact).  g is rounded to nearest TF32 for the gradient contraction.

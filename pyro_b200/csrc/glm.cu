@@ -8,7 +8,9 @@
 // reference chain (matmul -> Bernoulli.log_prob -> sum -> backward) writes and re-reads.
 //
 // fp32 SIMT kernel (D in {4, 8, 16}; at D = 32: N < 8192 rows, B2_FLAG_GLM_FP32, and operands the wgmma
-// kernel of glm_tc.cu cannot load; every other D in 1..128 takes the wgmma kernel of glm_flat_tc.cu): CTA = 256 threads = 4 row groups x 64 particles.  Each thread
+// kernel of glm_tc.cu cannot load; every other D in 1..128 takes the wgmma kernel of glm_flat_tc.cu).
+// glm_finish_kernel below is the second launch of every GLM likelihood call, Bernoulli and softmax
+// (b2_glm_categorical_logits).  CTA = 256 threads = 4 row groups x 64 particles.  Each thread
 // keeps W[p,:] and its dW[p,:] accumulator in registers; X tiles are staged through shared memory
 // with cp.async double buffering and read back as warp-wide broadcasts (every lane of a warp has a
 // different particle but the same row, so an LDS.128 serves 4 FMAs x 2 uses for all 32 lanes).
@@ -134,11 +136,12 @@ __global__ void __launch_bounds__(256) glm_bernoulli_kernel(const float* __restr
   }
 }
 
-// second stage: fixed-order sum over the CTAs' partials; applies weight / scale.
-// One WARP per entry of the [P, D+2] table: lanes stride over the CTAs (L2-resident partials),
+// second stage: fixed-order sum over the CTAs' partials [nblocks][P][K (D + 1) + 1] (per class dW[0..D-1]
+// and db, then the particle's lp sum; K = 1 for Bernoulli); applies weight / scale.
+// One WARP per entry of the [P, K (D + 1) + 1] table: lanes stride over the CTAs (L2-resident partials),
 // then a shuffle tree (a thread-per-entry loop is a chain of ~300 dependent loads).
 __global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict__ partials,
-                                                         int nblocks, int P, int D, double scale,
+                                                         int nblocks, int P, int K, int D, double scale,
                                                          double weight, float* __restrict__ sum_p,
                                                          float* __restrict__ out_dW,
                                                          float* __restrict__ out_db,
@@ -146,20 +149,24 @@ __global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict
                                                          float* __restrict__ out_total,
                                                          unsigned int* __restrict__ ticket) {
   pdl_enter();
-  const int total = P * (D + 2);
+  const int S = K * (D + 1) + 1;
+  const int total = P * S;
   const int e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (e >= total) return;
   double s = 0.0;
   for (int bl = lane; bl < nblocks; bl += 32) s += (double)partials[(int64_t)bl * total + e];
   s = warp_sum(s);
-  const int p = e / (D + 2), d = e - p * (D + 2);
-  if (d < D) {
-    if (lane == 0 && out_dW) out_dW[(int64_t)p * D + d] = (float)(weight * scale * s);
-    return;
-  }
-  if (d == D) {
-    if (lane == 0 && out_db) out_db[p] = (float)(weight * scale * s);
+  const int p = e / S, r = e - p * S;
+  if (r < K * (D + 1)) {
+    const int k = r / (D + 1), c = r - k * (D + 1);
+    if (lane == 0) {
+      if (c < D) {
+        if (out_dW) out_dW[((int64_t)p * K + k) * D + c] = (float)(weight * scale * s);
+      } else if (out_db) {
+        out_db[(int64_t)p * K + k] = (float)(weight * scale * s);
+      }
+    }
     return;
   }
   // per-particle sum; the LAST of the P warps to get here also totals them (fixed order), with
@@ -184,6 +191,17 @@ __global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict
     *out_total = (flags & B2_FLAG_ACCUMULATE_SUM) ? (float)((double)*out_total + v) : (float)v;
     *ticket = 0u;
   }
+}
+
+// The second launch of b2_glm_bernoulli_logits and b2_glm_categorical_logits.  The per-particle sums go to
+// out_sum_p, or without one to the [P] row of the workspace after the partials.
+void launch_glm_finish(const float* partials, unsigned int* ticket, int gx, int P, int K, int D, double scale,
+                       double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
+                       float* out_dW, float* out_db, cudaStream_t s) {
+  const int total = P * (K * (D + 1) + 1);
+  float* sum_p = out_sum_p ? out_sum_p : const_cast<float*>(partials) + (size_t)gx * total;
+  launch_pdl(glm_finish_kernel, dim3((total + 7) / 8), dim3(256), 0, s, partials, gx, P, K, D, scale, weight, sum_p,
+             out_dW, out_db, sum_coeff, flags, out_total, ticket);
 }
 
 // wgmma + TMA variant (glm_tc.cu)
@@ -254,11 +272,8 @@ extern "C" int b2_glm_bernoulli_logits(const float* X, const float* y, const flo
     case 32: glm_bernoulli_kernel<32><<<grid, 256, 0, s>>>(X, y, W, b, N, P, partials); break;
     default: return B2_ERR_BAD_SHAPE;
   }
-  float* sum_p = out_sum_p ? out_sum_p : partials + (size_t)gx * P * (D + 2);
-  const int total = P * (D + 2);
-  launch_pdl(glm_finish_kernel, dim3((total + 7) / 8), dim3(256), 0, s,
-             partials, gx, P, D, scale, weight, sum_p, out_dW, out_db, sum_coeff, flags, out_total, ticket);
-  const int nl = 2;
-  count_launch(nl);
+  launch_glm_finish(partials, ticket, gx, P, 1, D, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW,
+                    out_db, s);
+  count_launch(2);
   return check_launch();
 }

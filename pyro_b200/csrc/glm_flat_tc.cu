@@ -45,9 +45,6 @@ namespace tcf {
 
 using namespace tc;
 
-constexpr int kRows = 64;                       // rows per tile = M of one wgmma
-constexpr int kP = 64;
-
 template <int DC>
 struct Cfg {
   static constexpr int kKD = 32 * DC;                          // padded feature count
@@ -73,7 +70,7 @@ struct Cfg {
   static constexpr int kRS = kKD + 1;
   static_assert(kSmemBytes <= 232448, "shared memory budget");
   static_assert(kXtBlock % 1024 == 0 && kWGBytes % 1024 == 0, "operand alignment");
-  static_assert((kWG * kP * kRS + kWG * kP) * 4 <= kWG * kWGBytes, "reduction scratch");
+  static_assert((kWG * kM * kRS + kWG * kM) * 4 <= kWG * kWGBytes, "reduction scratch");
 };
 
 // one 1-D bulk copy global -> shared, completing `bytes` (a non-zero multiple of 16) on the mbarrier
@@ -82,76 +79,6 @@ __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
-
-// GEMM 2: D[64 x N] = A[64 x 8] B[N x 8]^T (+ D when acc != 0), TF32, A from registers (layout of
-// wgmma_n40_tf32_ra), B K-major SWIZZLE_128B in shared memory
-template <int N>
-__device__ __forceinline__ void wgmma_tf32_ra(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b, int acc);
-template <>
-__device__ __forceinline__ void wgmma_tf32_ra<40>(float (&d)[20], const uint32_t (&a)[4], uint64_t b, int acc) {
-  wgmma_n40_tf32_ra(d, a, b, acc);
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32_ra<72>(float (&d)[36], const uint32_t (&a)[4], uint64_t b, int acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %41, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n72k8.f32.tf32.tf32 "
-      "{"
-      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20,"
-      "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35"
-      "}, {%36, %37, %38, %39}, %40, p, 1, 1;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
-      : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32_ra<104>(float (&d)[52], const uint32_t (&a)[4], uint64_t b, int acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %57, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n104k8.f32.tf32.tf32 "
-      "{"
-      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20,"
-      "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39,"
-      "%40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51"
-      "}, {%52, %53, %54, %55}, %56, p, 1, 1;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
-      : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32_ra<136>(float (&d)[68], const uint32_t (&a)[4], uint64_t b, int acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %73, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n136k8.f32.tf32.tf32 "
-      "{"
-      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20,"
-      "%21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39,"
-      "%40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58,"
-      "%59, %60, %61, %62, %63, %64, %65, %66, %67"
-      "}, {%68, %69, %70, %71}, %72, p, 1, 1;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
-        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc)
-      : "memory");
-}
-
 
 // wgmma accumulator fragment (m64nN, f32): thread (warp w4 of the warpgroup, lane = 4 gid + t4) holds
 // d[4j + 2h + e] = D[16 w4 + gid + 8h][8j + 2 t4 + e].
@@ -178,25 +105,10 @@ glm_bernoulli_flat_tc_kernel(const float* __restrict__ X, const float* __restric
     for (int s = 0; s < kWG; ++s) mbar_init(base + C::OFF_BAR + 8u * (uint32_t)s, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  {
-    // weight tiles, zero in the padding columns d >= D (generic-proxy writes, made visible to the tensor cores)
-    float* whi = reinterpret_cast<float*>(sm + C::OFF_WHI);
-    float* wlo = reinterpret_cast<float*>(sm + C::OFF_WLO);
-    for (int e = tid; e < kP * kKD; e += C::kThreads) {
-      const int p = e / kKD, d = e - p * kKD;
-      const int gp = slab * kP + p;
-      const float w = (gp < P && d < D) ? W[(int64_t)gp * D + d] : 0.f;
-      const float hi = tf32_trunc(w);
-      const int off = (d >> 5) * 2048 + sw128(p, d & 31);
-      whi[off] = hi;
-      wlo[off] = w - hi;
-    }
-    // rows KD..KD+7 of every X^T k-block are ones: GEMM 2 then yields db in column KD of its accumulator
-    for (int e = tid; e < kWG * 2 * 256; e += C::kThreads) {
-      const int g = e >> 9, kb = (e >> 8) & 1, w = e & 255;
-      reinterpret_cast<float*>(sm + C::OFF_WG + g * C::kWGBytes + C::WG_XT + kb * C::kXtBlock + kKD * 128)[w] = 1.f;
-    }
-  }
+  // weight tiles, zero in the padding columns d >= D, and the ones rows of X^T
+  stage_w_and_ones<1, kKD, C::kThreads>(reinterpret_cast<float*>(sm + C::OFF_WHI),
+                                        reinterpret_cast<float*>(sm + C::OFF_WLO), sm + C::OFF_WG + C::WG_XT,
+                                        C::kWGBytes, W, slab, P, 1, D);
   fence_proxy_async();
   __syncthreads();
 
@@ -217,7 +129,7 @@ glm_bernoulli_flat_tc_kernel(const float* __restrict__ X, const float* __restric
     float bias[2];                             // of particles 16 w4 + gid + 8h
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int gp = slab * kP + 16 * w4 + gid + 8 * h;
+      const int gp = slab * kM + 16 * w4 + gid + 8 * h;
       bias[h] = (bvec != nullptr && gp < P) ? bvec[gp] : 0.f;
     }
     // tile it -> landing buffer; one thread of the warpgroup issues the loads
@@ -244,10 +156,8 @@ glm_bernoulli_flat_tc_kernel(const float* __restrict__ X, const float* __restric
       // GEMM 2 of this warpgroup's previous tile has finished reading X^T and the g registers
       wgmma_wait0();
       fence_regs(acc2);
-      // ---- split / transposition pass (thread mapping of glm_tc.cu, once per 32-column atom) ------------
-      // Thread t owns the 16-byte chunk c (d = 32 a + 4c .. +3) of the four rows n = 8 q8 + 2i + e, which
-      // kt_pos puts at the consecutive k = 8 q8 + 4e + i: after a 4x4 transpose in registers each d is one
-      // 16-byte store into X^T.
+      // ---- split pass, once per 32-column atom, with the thread mapping of the D = 32 pipeline
+      // (glm_tc_common.cuh): columns d >= D and rows past N are exact zeros --------------------------------
       {
         const int lam = t & 7, mu = t >> 3;
         const int e = lam & 1, q8 = ((mu >> 3) << 2) | (lam >> 1);
@@ -258,11 +168,11 @@ glm_bernoulli_flat_tc_kernel(const float* __restrict__ X, const float* __restric
         float4* xt = reinterpret_cast<float4*>(my + C::WG_XT + (q8 >> 2) * C::kXtBlock);
 #pragma unroll
         for (int a = 0; a < DC; ++a) {
-          float xr[4][4];                      // [i][q] = X[8 q8 + 2i + e][32 a + 4c + q] rounded to nearest TF32
+          float xr[4][4];                      // [i][q] = X[8 q8 + 2i + e][32 a + 4c + q] rounded to TF32
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             const int r = 8 * q8 + 2 * i + e;
-            const int idx = a * 512 + r * 8 + (c ^ (r & 7));   // 16-byte chunk of the SW128 operand
+            const int idx = a * 512 + r * 8 + (c ^ (r & 7));
             float x[4];
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
@@ -296,44 +206,12 @@ glm_bernoulli_flat_tc_kernel(const float* __restrict__ X, const float* __restric
       wg_bar(1 + wg);
       // the landing buffer is free: the warpgroup's next tile arrives while this one is contracted
       if (t == 0 && it + kWG < nt) load(it + kWG);
-      // ---- GEMM 1: logits D1^T[p, n] = W X^T + b, accumulator initialised with the bias ---------------
       float acc1[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) acc1[i] = bias[(i >> 1) & 1];
-      wgmma_fence();
-#pragma unroll
-      for (int a = 0; a < DC; ++a) {
-        const uint64_t d_whi = desc_sw128(base + C::OFF_WHI + a * 8192), d_wlo = desc_sw128(base + C::OFF_WLO + a * 8192);
-        const uint64_t d_x = desc_sw128(my_s + C::WG_XOP + a * 8192), d_xlo = desc_sw128(my_s + C::WG_XLO + a * 8192);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          wgmma_n64_tf32(acc1, d_whi + 2 * k, d_x + 2 * k);
-          wgmma_n64_tf32(acc1, d_wlo + 2 * k, d_x + 2 * k);
-          if (SPLIT_X) wgmma_n64_tf32(acc1, d_whi + 2 * k, d_xlo + 2 * k);
-        }
-      }
-      wgmma_commit();
-      wgmma_wait0();
-      fence_regs(acc1);
-      // ---- epilogue: lp sums and g, both in registers; the row mask only in the last, partial tile ------
+      gemm1<DC, SPLIT_X>(acc1, bias, base + C::OFF_WHI, base + C::OFF_WLO, my_s + C::WG_XOP, my_s + C::WG_XLO);
       uint32_t g[32];                          // indexed like acc1
-      float lin[2], prod[2];
-      if (rows < kRows)
-        epilogue<true>(acc1, yr, row0, N, t4, lin, prod, g);
-      else
-        epilogue<false>(acc1, yr, row0, N, t4, lin, prod, g);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) lpa[h] += fmaf(lg2f(prod[h]), -0.6931471805599453f, lin[h]);
-      // ---- GEMM 2: [dW | db] += g [X | 1], g from registers, left running while the next tile is waited for
-      fence_regs(g);
-      wgmma_fence();
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const uint32_t a[4] = {g[4 * j], g[4 * j + 2], g[4 * j + 1], g[4 * j + 3]};
-        wgmma_tf32_ra<C::kN2>(acc2, a, desc_sw128(my_s + C::WG_XT + (j >> 2) * C::kXtBlock) + 2 * (j & 3),
-                              it != wg || j != 0);
-      }
-      wgmma_commit();
+      bernoulli_epilogue(acc1, yr, row0, N, t4, rows < kRows, lpa, g);
+      // left running while the next tile is waited for
+      gemm2<C::kN2>(acc2, g, my_s + C::WG_XT, it == wg);
     }
     wgmma_wait0();
     fence_regs(acc2);
@@ -345,41 +223,9 @@ glm_bernoulli_flat_tc_kernel(const float* __restrict__ X, const float* __restric
       lpa[h] = v;
     }
   }
-  // ---- CTA results through shared memory (the warpgroup regions are idle now), fixed summation order -----
-  __syncthreads();
-  float* red2 = reinterpret_cast<float*>(sm + C::OFF_WG);   // [kWG][64 p][KD + 1]
-  float* redlp = red2 + kWG * kP * C::kRS;                  // [kWG][64 p]
-  {
-#pragma unroll
-    for (int j = 0; j < C::kN2 / 8; ++j)
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int p = 16 * w4 + gid + 8 * h, c = 8 * j + 2 * t4 + e;
-          if (c < D || c == kKD) red2[(wg * kP + p) * C::kRS + c] = acc2[4 * j + 2 * h + e];
-        }
-    if (t4 == 0) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) redlp[wg * kP + 16 * w4 + gid + 8 * h] = lpa[h];
-    }
-  }
-  __syncthreads();
-  if (tid < kP) {
-    const int gp = slab * kP + tid;
-    if (gp < P) {
-      float* o = partials + ((int64_t)blockIdx.x * P + gp) * (D + 2);
-      for (int c = 0; c <= D; ++c) {           // dW[0..D-1], then db from accumulator column KD
-        const int col = c < D ? c : kKD;
-        float v = 0.f;
-        for (int g = 0; g < kWG && g < nt; ++g) v += red2[(g * kP + tid) * C::kRS + col];
-        o[c] = v;
-      }
-      float v = 0.f;
-      for (int g = 0; g < kWG && g < nt; ++g) v += redlp[g * kP + tid];
-      o[D + 1] = v;
-    }
-  }
+  // CTA results through the warpgroup regions, idle now
+  cta_partials<1, C::kN2, C::kThreads>(reinterpret_cast<float*>(sm + C::OFF_WG), acc2, lpa, wg, nt, slab, P, 1, D,
+                                       partials);
 }
 
 template <int DC, bool SPLIT_X>
@@ -392,7 +238,7 @@ void launch_one(const float* X, const float* y, const float* W, const float* b, 
                          (int)C::kSmemBytes);
     attr_set = true;
   }
-  dim3 grid((unsigned)gx, (unsigned)((P + kP - 1) / kP), 1);
+  dim3 grid((unsigned)gx, (unsigned)((P + kM - 1) / kM), 1);
   launch_pdl(glm_bernoulli_flat_tc_kernel<DC, SPLIT_X>, grid, dim3(C::kThreads), (size_t)C::kSmemBytes, s,
              X, y, W, b, N, D, P, partials);
 }

@@ -4,7 +4,8 @@
 //   grad[c] = dU / dz[c]                                           (in z's layout)
 //
 // The likelihood and its gradient come from the fused GLM kernels (glm.cu / glm_tc.cu for Bernoulli,
-// glm_categorical_tc.cu for Categorical) with their particle axis set to the chains, so X is read once per
+// glm_categorical_tc.cu for Categorical, the D = 32 ones on the tile pipeline of glm_tc_common.cuh, and
+// glm_finish_kernel of glm.cu for both) with their particle axis set to the chains, so X is read once per
 // evaluation for every chain together.  One evaluation is a fixed launch sequence with no host sync (CUDA
 // graph capturable):
 //   1. glm_potential_pack_kernel    z's weight / bias columns -> the contiguous [C, K*D] / [C, K] operands

@@ -202,9 +202,9 @@ poisson_product_tc_kernel(const float* __restrict__ A, const float* __restrict__
         const uint32_t b[4] = {glo[4 * i], glo[4 * i + 2], glo[4 * i + 1], glo[4 * i + 3]};
         const uint64_t d_hi = desc_sw128(base + OFF_AT + (i >> 2) * 2048) + 2 * (i & 3);
         const uint64_t d_lo = desc_sw128(base + OFF_AT + (2 + (i >> 2)) * 2048) + 2 * (i & 3);
-        wgmma_n16_tf32_ra(accB, a, d_hi, t != 0 || i != 0);
-        wgmma_n16_tf32_ra(accB, a, d_lo, 1);
-        wgmma_n16_tf32_ra(accB, b, d_hi, 1);
+        wgmma_tf32_ra<16>(accB, a, d_hi, t != 0 || i != 0);
+        wgmma_tf32_ra<16>(accB, a, d_lo, 1);
+        wgmma_tf32_ra<16>(accB, b, d_hi, 1);
       }
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
