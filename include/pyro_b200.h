@@ -322,6 +322,34 @@ int b2_glm_categorical_logits(const float* X, const int64_t* y, const float* W, 
 size_t b2_glm_categorical_workspace(int64_t N, int D, int K, int P);
 
 /*
+ * b2_glm_poisson_log_rate -- fused Poisson-regression (log link) likelihood term: for P particles,
+ * l[p,n] = <X[n,:], W[p,:]> + b[p] is the log-rate;
+ *   sum_p[p]  = SUM_n ( y[n]*l[p,n] - exp(l[p,n]) - lgamma(y[n] + 1) )        (Poisson log_prob)
+ *   dW[p,:]   = weight * SUM_n (y[n] - exp(l[p,n])) * X[n,:]
+ *   db[p]     = weight * SUM_n (y[n] - exp(l[p,n]))
+ * X and y are read from HBM about once for value AND gradient, and no [P,N] tensor is written; SUM lgamma(y + 1)
+ * is evaluated once per call, not once per particle.  The arguments are those of b2_glm_bernoulli_logits:
+ * X: [N,D] row-major fp32, 1 <= D <= 128; W: [P,D]; b: [P] (nullable); y: [N] fp32 counts.  X and y must be
+ * 16-byte aligned and N < 2^31.  Both contractions run on the tensor cores (glm_poisson_tc.cu: D == 32 on the
+ * TMA tile pipeline of glm_tc.cu, every other D on the bulk-copy tile loop of glm_flat_tc.cu) with their
+ * precision policy: W split hi + lo, X rounded to nearest TF32, split as well below 65536 rows and at any N
+ * with B2_FLAG_GLM_3XTF32; g = y - exp(l) rounded to nearest TF32.  There is no fp32 SIMT kernel:
+ * B2_FLAG_GLM_FP32 returns B2_ERR_BAD_SHAPE.  A null X, y or W returns B2_ERR_NULL; N <= 0, P <= 0, D outside
+ * 1..128 or a misaligned X or y B2_ERR_BAD_SHAPE; N >= 2^31 B2_ERR_TOO_LARGE; all before any CUDA call.
+ * A log-rate above 88.72 overflows exp to +inf: that row's lp and g are -inf, so sum_p is -inf, db is -inf
+ * times weight and dW is non-finite (the materialised log_prob is NaN there for a positive count).
+ * out_total (nullable): scalar, (=|+=) sum_coeff * scale * SUM_p sum_p[p].
+ * workspace: b2_glm_poisson_workspace() bytes, zero-initialised ONCE by the caller (its first 256 bytes hold
+ * a ticket counter that the library leaves zeroed).  Two launches: the streaming kernel and the finish kernel
+ * of b2_glm_bernoulli_logits, which sums the CTA partials in a fixed order (deterministic, no float atomics).
+ */
+int b2_glm_poisson_log_rate(const float* X, const float* y, const float* W, const float* b, int64_t N, int D,
+                            int P, double scale, double weight, double sum_coeff, int flags, float* out_sum_p,
+                            float* out_total, float* out_dW, float* out_db, void* workspace,
+                            size_t workspace_bytes, void* stream);
+size_t b2_glm_poisson_workspace(int64_t N, int D, int P);
+
+/*
  * b2_poisson_product -- fused Poisson matrix-factorisation likelihood term (the bottom layer of the sparse
  * gamma DEF, Gamma-Poisson NMF): for P particles with latent factors A[p] (N x K) and B[p] (K x J) and shared
  * counts x (N x J), rate[p,n,j] = SUM_k A[p,n,k] * B[p,k,j];
@@ -357,18 +385,20 @@ size_t b2_poisson_product_workspace(int64_t N, int K, int64_t J, int P);
 
 /*
  * b2_glm_potential -- HMC / NUTS potential energy and gradient of Bayesian logistic (kind
- * B2_GLM_BERNOULLI) or softmax (B2_GLM_CATEGORICAL) regression for C chains, with the likelihood of
- * every chain computed in one pass over X by the kernels of b2_glm_bernoulli_logits /
- * b2_glm_categorical_logits (the chains are their particles):
+ * B2_GLM_BERNOULLI), softmax (B2_GLM_CATEGORICAL) or Poisson (B2_GLM_POISSON, log link) regression for C
+ * chains, with the likelihood of every chain computed in one pass over X by the kernels of
+ * b2_glm_bernoulli_logits / b2_glm_categorical_logits / b2_glm_poisson_log_rate (the chains are their
+ * particles):
  *   U[c]       = -( SUM_n log p(y[n] | logits[c,n]) + SUM_i log Normal(w[c,i]; 0, s_w)
  *                   + SUM_k log Normal(b[c,k]; 0, s_b) )
  *   grad[c,:]  = dU / dz[c,:]
- * logits[c,n] = <X[n,:], w[c,:]> + b[c] (Bernoulli, K == 1) or logits[c,n,k] = <X[n,:], W[c,k,:]> + b[c,k]
- * (Categorical).  z: [C, Dz] fp32 row-major chain state; the weights (K*D values, W row-major [K, D])
+ * logits[c,n] = <X[n,:], w[c,:]> + b[c] (Bernoulli, and Poisson's log-rate, K == 1) or logits[c,n,k] =
+ * <X[n,:], W[c,k,:]> + b[c,k] (Categorical).  z: [C, Dz] fp32 row-major chain state; the weights (K*D values, W row-major [K, D])
  * start at column w_off, the bias (K values, only if has_bias) at column b_off, and Dz == K*D + (has_bias ? K
  * : 0).  grad has z's layout.  X: [N, D] fp32 row-major, 16-byte aligned; y: [N] fp32 0/1 (Bernoulli) or
- * int64 labels, 16-byte aligned (Categorical).
- * Scope: Bernoulli with K == 1 and D in {4, 8, 16, 32}; Categorical with D == 32 and 2 <= K <= 16;
+ * int64 labels, 16-byte aligned (Categorical), or fp32 counts, 16-byte aligned (Poisson).
+ * Scope: Bernoulli with K == 1 and D in {4, 8, 16, 32}; Categorical with D == 32 and 2 <= K <= 16; Poisson
+ * with K == 1 and 1 <= D <= 128;
  * s_w > 0 and (with a bias) s_b > 0; anything else returns B2_ERR_BAD_SHAPE.
  * The GLM kernels always run with B2_FLAG_GLM_3XTF32 (every logit fp32-exact).  The prior and the totals
  * are accumulated in fp64 in a fixed order: results are deterministic.
@@ -378,6 +408,7 @@ size_t b2_poisson_product_workspace(int64_t N, int K, int64_t J, int P);
  */
 #define B2_GLM_BERNOULLI 0
 #define B2_GLM_CATEGORICAL 1
+#define B2_GLM_POISSON 2
 int b2_glm_potential(int kind, const float* X, const void* y, int64_t N, int D, int K, int has_bias,
                      const float* z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, double s_w,
                      double s_b, float* U, float* grad, void* workspace, size_t workspace_bytes,

@@ -35,7 +35,7 @@ EMULATE_RSAMPLE = False   # tests/cpu_emulation.py flips this to exercise the fu
 SITE_SMALL_N = 8192   # B2_SITE_SMALL_N: one-CTA kernel with fused stored-shape gradient reductions
 DIRICHLET, CATEGORICAL, MVN_TRIL = 32, 33, 34
 MODEL_HIER_NORMAL, MODEL_LOGISTIC = 0, 1
-GLM_BERNOULLI, GLM_CATEGORICAL = 0, 1
+GLM_BERNOULLI, GLM_CATEGORICAL, GLM_POISSON = 0, 1, 2
 NUTS_SMALL_MAX_D = 64
 
 
@@ -116,6 +116,9 @@ SIGNATURES = {
     "b2_glm_categorical_logits": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _f64,
                                          _i32, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2_glm_categorical_workspace": (_sz, [_i64, _i32, _i32, _i32]),
+    "b2_glm_poisson_log_rate": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _f64, _f64, _f64, _i32,
+                                       _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "b2_glm_poisson_workspace": (_sz, [_i64, _i32, _i32]),
     "b2_poisson_product": (_i32, [_vp, _vp, _vp, _i64, _i32, _i64, _i32, _f64, _f64, _f64, _i32, _vp, _vp, _vp,
                                   _vp, _vp, _sz, _vp]),
     "b2_poisson_product_workspace": (_sz, [_i64, _i32, _i64, _i32]),

@@ -9,9 +9,9 @@
 //
 // fp32 SIMT kernel (D in {4, 8, 16}; at D = 32: N < 8192 rows, B2_FLAG_GLM_FP32, and operands the wgmma
 // kernel of glm_tc.cu cannot load; every other D in 1..128 takes the wgmma kernel of glm_flat_tc.cu).
-// glm_finish_kernel below is the second launch of every GLM likelihood call, Bernoulli and softmax
-// (b2_glm_categorical_logits).  CTA = 256 threads = 4 row groups x 64 particles.  Each thread
-// keeps W[p,:] and its dW[p,:] accumulator in registers; X tiles are staged through shared memory
+// glm_finish_kernel below is the second launch of every GLM likelihood call, Bernoulli, softmax
+// (b2_glm_categorical_logits) and Poisson (b2_glm_poisson_log_rate).  CTA = 256 threads = 4 row groups x 64
+// particles.  Each thread keeps W[p,:] and its dW[p,:] accumulator in registers; X tiles are staged through shared memory
 // with cp.async double buffering and read back as warp-wide broadcasts (every lane of a warp has a
 // different particle but the same row, so an LDS.128 serves 4 FMAs x 2 uses for all 32 lanes).
 // FLOPs = 4*N*D*P; at P=64, D=32 the FMA pipe, not HBM, bounds this kernel (see DESIGN.md).
@@ -137,7 +137,8 @@ __global__ void __launch_bounds__(256) glm_bernoulli_kernel(const float* __restr
 }
 
 // second stage: fixed-order sum over the CTAs' partials [nblocks][P][K (D + 1) + 1] (per class dW[0..D-1]
-// and db, then the particle's lp sum; K = 1 for Bernoulli); applies weight / scale.
+// and db, then the particle's lp sum; K = 1 for Bernoulli and Poisson); applies weight / scale.  lg (Poisson
+// only, else null) holds one more partial per CTA, of a term every particle's sum subtracts: SUM lgamma(y + 1).
 // One WARP per entry of the [P, K (D + 1) + 1] table: lanes stride over the CTAs (L2-resident partials),
 // then a shuffle tree (a thread-per-entry loop is a chain of ~300 dependent loads).
 __global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict__ partials,
@@ -147,7 +148,8 @@ __global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict
                                                          float* __restrict__ out_db,
                                                          double sum_coeff, int flags,
                                                          float* __restrict__ out_total,
-                                                         unsigned int* __restrict__ ticket) {
+                                                         unsigned int* __restrict__ ticket,
+                                                         const float* __restrict__ lg) {
   pdl_enter();
   const int S = K * (D + 1) + 1;
   const int total = P * S;
@@ -168,6 +170,11 @@ __global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict
       }
     }
     return;
+  }
+  if (lg != nullptr) {
+    double l = 0.0;
+    for (int bl = lane; bl < nblocks; bl += 32) l += (double)lg[bl];
+    s -= warp_sum(l);
   }
   // per-particle sum; the LAST of the P warps to get here also totals them (fixed order), with
   // the ELBO coefficient -- a ticket instead of a third launch
@@ -193,15 +200,15 @@ __global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict
   }
 }
 
-// The second launch of b2_glm_bernoulli_logits and b2_glm_categorical_logits.  The per-particle sums go to
-// out_sum_p, or without one to the [P] row of the workspace after the partials.
+// The second launch of b2_glm_bernoulli_logits, b2_glm_categorical_logits and b2_glm_poisson_log_rate.  The
+// per-particle sums go to out_sum_p, or without one to the [P] row of the workspace after the partials.
 void launch_glm_finish(const float* partials, unsigned int* ticket, int gx, int P, int K, int D, double scale,
                        double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
-                       float* out_dW, float* out_db, cudaStream_t s) {
+                       float* out_dW, float* out_db, const float* lg, cudaStream_t s) {
   const int total = P * (K * (D + 1) + 1);
   float* sum_p = out_sum_p ? out_sum_p : const_cast<float*>(partials) + (size_t)gx * total;
   launch_pdl(glm_finish_kernel, dim3((total + 7) / 8), dim3(256), 0, s, partials, gx, P, K, D, scale, weight, sum_p,
-             out_dW, out_db, sum_coeff, flags, out_total, ticket);
+             out_dW, out_db, sum_coeff, flags, out_total, ticket, lg);
 }
 
 // wgmma + TMA variant (glm_tc.cu)
@@ -273,7 +280,7 @@ extern "C" int b2_glm_bernoulli_logits(const float* X, const float* y, const flo
     default: return B2_ERR_BAD_SHAPE;
   }
   launch_glm_finish(partials, ticket, gx, P, 1, D, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW,
-                    out_db, s);
+                    out_db, nullptr, s);
   count_launch(2);
   return check_launch();
 }

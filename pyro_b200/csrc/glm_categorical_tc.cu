@@ -39,7 +39,7 @@ namespace b2 {
 // launches glm_finish_kernel (glm.cu) over the partials [gx][P][K (D + 1) + 1]
 void launch_glm_finish(const float* partials, unsigned int* ticket, int gx, int P, int K, int D, double scale,
                        double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
-                       float* out_dW, float* out_db, cudaStream_t s);
+                       float* out_dW, float* out_db, const float* lg, cudaStream_t s);
 
 namespace tcc {
 
@@ -67,6 +67,7 @@ __device__ __forceinline__ float class_sum(float v) {
 template <int KP>
 struct Softmax {
   static_assert(KP == 2 || KP == 4 || KP == 8 || KP == 16, "class padding");
+  static constexpr bool kBiasInEpilogue = false;
   static constexpr int kKP = KP;
   static constexpr uint32_t kYBytes = kRows * 8;  // 512 B of int64 labels
   static constexpr CUtensorMapDataType kYType = CU_TENSOR_MAP_DATA_TYPE_INT64;
@@ -217,7 +218,7 @@ extern "C" int b2_glm_categorical_logits(const float* X, const int64_t* y, const
   else
     launch_split<false>(class_pad(K), mx, my, W, b, N, P, K, partials, gx, s);
   launch_glm_finish(partials, ticket, gx, P, K, kD, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW,
-                    out_db, s);
+                    out_db, nullptr, s);
   count_launch(2);
   return check_launch();
 }

@@ -1,11 +1,12 @@
-// glm_potential.cu -- HMC / NUTS potential energy of Bayesian logistic and softmax regression for C chains.
+// glm_potential.cu -- HMC / NUTS potential energy of Bayesian logistic, softmax and Poisson regression for C
+// chains.
 //
 //   U[c]    = -( SUM_n log p(y_n | logits_cn) + SUM log Normal(w; 0, s_w) + SUM log Normal(b; 0, s_b) )
 //   grad[c] = dU / dz[c]                                           (in z's layout)
 //
 // The likelihood and its gradient come from the fused GLM kernels (glm.cu / glm_tc.cu for Bernoulli,
-// glm_categorical_tc.cu for Categorical, the D = 32 ones on the tile pipeline of glm_tc_common.cuh, and
-// glm_finish_kernel of glm.cu for both) with their particle axis set to the chains, so X is read once per
+// glm_categorical_tc.cu for Categorical, glm_poisson_tc.cu for Poisson, the D = 32 ones on the tile pipeline
+// of glm_tc_common.cuh, and glm_finish_kernel of glm.cu for all three) with their particle axis set to the chains, so X is read once per
 // evaluation for every chain together.  One evaluation is a fixed launch sequence with no host sync (CUDA
 // graph capturable):
 //   1. glm_potential_pack_kernel    z's weight / bias columns -> the contiguous [C, K*D] / [C, K] operands
@@ -78,6 +79,7 @@ inline GlmPotentialLayout glm_potential_layout(int kind, int64_t N, int D, int K
   const size_t KD = (size_t)K * D, c = (size_t)C;
   L.glm = 0;
   size_t off = round256(kind == B2_GLM_BERNOULLI ? b2_glm_workspace(N, D, (int)C)
+                        : kind == B2_GLM_POISSON ? b2_glm_poisson_workspace(N, D, (int)C)
                                                  : b2_glm_categorical_workspace(N, D, K, (int)C));
   L.wp = off; off += round256(c * KD * sizeof(float));
   L.bp = off; off += round256(c * K * sizeof(float));
@@ -92,6 +94,7 @@ inline bool glm_potential_in_scope(int kind, int64_t N, int D, int K, int64_t C)
   if (N < 1 || C < 1 || C >= ((int64_t)1 << 31)) return false;
   if (kind == B2_GLM_BERNOULLI) return K == 1 && (D == 4 || D == 8 || D == 16 || D == 32);
   if (kind == B2_GLM_CATEGORICAL) return D == 32 && K >= 2 && K <= 16;
+  if (kind == B2_GLM_POISSON) return K == 1 && D >= 1 && D <= 128;
   return false;
 }
 
@@ -134,6 +137,9 @@ extern "C" int b2_glm_potential(int kind, const float* X, const void* y, int64_t
   const size_t glm_bytes = L.wp - L.glm;
   if (kind == B2_GLM_BERNOULLI)
     rc = b2_glm_bernoulli_logits(X, static_cast<const float*>(y), Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
+                                 B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws + L.glm, glm_bytes, stream);
+  else if (kind == B2_GLM_POISSON)
+    rc = b2_glm_poisson_log_rate(X, static_cast<const float*>(y), Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
                                  B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws + L.glm, glm_bytes, stream);
   else
     rc = b2_glm_categorical_logits(X, static_cast<const int64_t*>(y), Wp, bp, N, D, K, (int)C, 1.0, -1.0, 1.0,

@@ -47,7 +47,7 @@
 // adds the CTA partials in a fixed order.
 //
 // The tile loop is glm_tile_pipeline (glm_tc_common.cuh), which the softmax kernel of glm_categorical_tc.cu
-// runs as well; this file gives its Bernoulli family: fp32 labels and the epilogue above.
+// runs as well, with the Bernoulli family of glm_tc_common.cuh: fp32 labels and the epilogue above.
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -58,24 +58,6 @@ namespace b2 {
 namespace tc {
 
 using namespace tile32;
-
-// the Bernoulli family of the D = 32 tile pipeline: one GEMM 1 row per particle, fp32 labels y
-struct Bernoulli {
-  static constexpr int kKP = 1;
-  static constexpr uint32_t kYBytes = kRows * 4;  // 256 B of y
-  static constexpr CUtensorMapDataType kYType = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-  using Labels = float2[8];                       // y of the thread's rows n = 8j + 2 t4 + e
-  static __device__ __forceinline__ void read_labels(const uint8_t* ys, int t4, int, Labels& y) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) y[j] = reinterpret_cast<const float2*>(ys)[4 * j + t4];
-  }
-  // lp sums and g, both in registers; the row mask only in the last, partial tile
-  static __device__ __forceinline__ void epilogue(const float (&acc1)[32], const Labels& y, const int (&)[2], int,
-                                                  int64_t row0, int64_t N, int t4, float (&lpa)[2],
-                                                  uint32_t (&g)[32]) {
-    bernoulli_epilogue(acc1, y, row0, N, t4, row0 + kRows > N, lpa, g);
-  }
-};
 
 // SPLIT_X = false (default): W split hi/lo, X rounded to nearest.  SPLIT_X = true: full 3xTF32, X split
 // hi/lo as well.

@@ -1,7 +1,8 @@
 // glm_tc_common.cuh -- device helpers shared by the Hopper wgmma kernels (glm_tc.cu, glm_flat_tc.cu,
-// glm_categorical_tc.cu, poisson_product_tc.cu): mbarriers, TMA tile loads, SWIZZLE_128B operand
-// descriptors, the TF32 wgmma wrappers, MUFU wrappers and TF32 rounding, the Bernoulli epilogue, the stages
-// of the GLM tile pipeline and the D = 32 pipeline itself, and the host-side tensor-map encoders.
+// glm_categorical_tc.cu, glm_poisson_tc.cu, poisson_product_tc.cu): mbarriers, TMA tile loads, SWIZZLE_128B
+// operand descriptors, the TF32 wgmma wrappers, MUFU wrappers and TF32 rounding, the Bernoulli and Poisson
+// epilogues and families, the stages of the GLM tile pipeline and the D = 32 pipeline itself, and the
+// host-side tensor-map encoders.
 #pragma once
 #include <cuda.h>
 
@@ -223,6 +224,9 @@ __device__ __forceinline__ float tf32_rn(float x) {
 // that order, so g never leaves the registers.
 __device__ __forceinline__ int kt_pos(int n) { return (n & ~7) | ((n & 7) >> 1) | ((n & 1) << 2); }
 
+constexpr int kRows = 64;                       // rows per tile = N of GEMM 1 = K of GEMM 2
+constexpr int kM = 64;                          // GEMM 1 rows per slab
+
 // ---- Bernoulli epilogue of the logistic-regression kernels (glm_tc.cu, glm_flat_tc.cu) ----------------------
 constexpr int kEpiBatch = 4;                    // logits of one particle per epilogue batch (8 fits, no faster)
 
@@ -314,6 +318,94 @@ __device__ __forceinline__ void bernoulli_epilogue(const float (&acc1)[32], cons
   for (int h = 0; h < 2; ++h) lpa[h] += fmaf(lg2f(prod[h]), -0.6931471805599453f, lin[h]);
 }
 
+// ---- Poisson epilogue of the log-link regression kernels (glm_poisson_tc.cu) -------------------------------
+// lp = y*l - e^l (the parameter-free -lgamma(y + 1) is summed once per call, not here) and g = y - e^l rounded
+// to nearest TF32: ONE MUFU op (ex2) per logit.  MASK (the last, partial tile only) zeroes rows past N.
+// Above l = 88.72 e^l is +inf: lp and g are then -inf, never NaN.
+// The bias is added here, rounded to nearest, not carried by GEMM 1's accumulator: the tensor cores truncate
+// each fp32 accumulation, and from an accumulator of |b| (a log-rate of a few units) every k-step shifts l
+// toward zero by about half an ulp of b.  That shift enters the sum as SUM (y - e^l) dl, which does not cancel
+// for a particle away from the data's optimum: at counts of mean 100 and b off by 0.05 it cost 2.3e-5 of
+// sum_p at D = 100 (48 accumulation steps), against 7.5e-6 at D = 32 (12 steps).
+template <bool MASK>
+__device__ __forceinline__ void poisson_epilogue(const float (&acc1)[32], const float (&bias)[2],
+                                                 const float2 (&yr)[8], int64_t row0, int64_t N, int t4,
+                                                 float (&lpa)[2], uint32_t (&g)[32]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float s[2] = {0.f, 0.f};                    // two chains of adds (k-blocks j even / odd)
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int i = 4 * j + 2 * h + e;
+        const float l = acc1[i] + bias[h], yy = e ? yr[j].y : yr[j].x;
+        const float ex = ex2f(1.4426950408889634f * l);
+        float lp = fmaf(yy, l, -ex), gg = yy - ex;
+        if (MASK) {
+          const bool v = row0 + 8 * j + 2 * t4 + e < N;
+          lp = v ? lp : 0.f;
+          gg = v ? gg : 0.f;
+        }
+        s[j & 1] += lp;
+        g[i] = __float_as_uint(tf32_rn(gg));
+      }
+    lpa[h] += s[0] + s[1];
+  }
+}
+
+// ---- likelihood families of the GLM tile pipelines ----------------------------------------------------------
+// Fam is the likelihood family: kBiasInEpilogue (the bias is added by the epilogue, which then takes it after
+// acc1, instead of starting GEMM 1's accumulator), kKP (GEMM 1 rows per particle), kYBytes (labels of one
+// tile), kYType (their TMA type), Labels (a thread's labels of one tile), read_labels(stage, t4, K, labels) and epilogue(acc1, labels,
+// cls, K, row0, N, t4, lpa, g), which writes g (indexed like acc1, rounded to TF32) and adds the tile's lp sums
+// of the thread's two rows to lpa; the any-D tile loop (glm_flat_tc.cuh) calls tile_epilogue(acc1, labels,
+// row0, N, t4, last, lpa, g) instead.
+
+// logistic regression: one GEMM 1 row per particle, fp32 labels y
+struct Bernoulli {
+  static constexpr bool kBiasInEpilogue = false;  // GEMM 1's accumulator starts at the bias
+  static constexpr int kKP = 1;
+  static constexpr uint32_t kYBytes = kRows * 4;  // 256 B of y
+  static constexpr CUtensorMapDataType kYType = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  using Labels = float2[8];                       // y of the thread's rows n = 8j + 2 t4 + e
+  static __device__ __forceinline__ void read_labels(const uint8_t* ys, int t4, int, Labels& y) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) y[j] = reinterpret_cast<const float2*>(ys)[4 * j + t4];
+  }
+  // lp sums and g, both in registers; the row mask only in the last, partial tile
+  static __device__ __forceinline__ void epilogue(const float (&acc1)[32], const Labels& y, const int (&)[2], int,
+                                                  int64_t row0, int64_t N, int t4, float (&lpa)[2],
+                                                  uint32_t (&g)[32]) {
+    bernoulli_epilogue(acc1, y, row0, N, t4, row0 + kRows > N, lpa, g);
+  }
+  // the same for the any-D tile loop (glm_flat_tc.cuh), which knows whether its tile is the last
+  static __device__ __forceinline__ void tile_epilogue(const float (&acc1)[32], const Labels& y, int64_t row0,
+                                                       int64_t N, int t4, bool last, float (&lpa)[2],
+                                                       uint32_t (&g)[32]) {
+    bernoulli_epilogue(acc1, y, row0, N, t4, last, lpa, g);
+  }
+};
+
+// Poisson regression (log link): the labels of Bernoulli, fp32 counts y
+// (GEMM 1 starts from zero and the epilogue adds the bias, see poisson_epilogue)
+struct Poisson : Bernoulli {
+  static constexpr bool kBiasInEpilogue = true;
+  static __device__ __forceinline__ void tile_epilogue(const float (&acc1)[32], const float (&bias)[2],
+                                                       const Labels& y, int64_t row0, int64_t N, int t4, bool last,
+                                                       float (&lpa)[2], uint32_t (&g)[32]) {
+    if (last)
+      poisson_epilogue<true>(acc1, bias, y, row0, N, t4, lpa, g);
+    else
+      poisson_epilogue<false>(acc1, bias, y, row0, N, t4, lpa, g);
+  }
+  static __device__ __forceinline__ void epilogue(const float (&acc1)[32], const float (&bias)[2], const Labels& y,
+                                                  const int (&)[2], int, int64_t row0, int64_t N, int t4,
+                                                  float (&lpa)[2], uint32_t (&g)[32]) {
+    tile_epilogue(acc1, bias, y, row0, N, t4, row0 + kRows > N, lpa, g);
+  }
+};
+
 // ---- stages of the GLM tile pipeline (glm_tc.cu, glm_categorical_tc.cu, glm_flat_tc.cu) ---------------------
 //
 // GEMM 1's M = 64 rows of a CTA slab are particles (KP = 1) or (particle, class) pairs: each particle's K
@@ -321,8 +413,6 @@ __device__ __forceinline__ void bernoulli_epilogue(const float (&acc1)[32], cons
 //
 // wgmma accumulator fragment (m64nN, f32): thread (warp w4 of the warpgroup, lane = 4 gid + t4) holds
 // d[4j + 2h + e] = D[16 w4 + gid + 8h][8j + 2 t4 + e].
-constexpr int kRows = 64;                       // rows per tile = N of GEMM 1 = K of GEMM 2
-constexpr int kM = 64;                          // GEMM 1 rows per slab
 
 // W hi / lo, the A operands of GEMM 1: [KD / 32 atoms][m 64][32] SW128, zero for a particle past P, a class
 // past K and a column past D (generic-proxy writes; the caller makes them visible to the tensor cores).  And
@@ -464,10 +554,7 @@ struct Smem32 {
   static_assert((kWG * kM * 33 + kWG * kM) * 4 <= kStages * kTile, "reduction scratch");
 };
 
-// Fam is the likelihood family: kKP (GEMM 1 rows per particle), kYBytes (labels of one tile), Labels (a
-// thread's labels of one tile), read_labels(stage, t4, K, labels) and epilogue(acc1, labels, cls, K, row0, N,
-// t4, lpa, g), which writes g (indexed like acc1, rounded to TF32) and adds the tile's lp sums of the thread's
-// two rows to lpa.
+// Fam is the likelihood family (Bernoulli, Poisson above, Softmax of glm_categorical_tc.cu).
 template <class Fam, bool SPLIT_X>
 __device__ __forceinline__ void glm_tile_pipeline(const CUtensorMap& map_x, const CUtensorMap& map_y,
                                                   const float* W, const float* bvec, int64_t N, int P, int K,
@@ -583,12 +670,21 @@ __device__ __forceinline__ void glm_tile_pipeline(const CUtensorMap& map_x, cons
       fence_proxy_async();
       wg_bar(1 + wg);
       float acc1[32];
-      gemm1<1, SPLIT_X>(acc1, bias, base + L::OFF_WHI, base + L::OFF_WLO, base + L::OFF_X + s * kTile,
-                        my_s + WG_XLO);
+      if constexpr (Fam::kBiasInEpilogue) {
+        const float zero[2] = {0.f, 0.f};
+        gemm1<1, SPLIT_X>(acc1, zero, base + L::OFF_WHI, base + L::OFF_WLO, base + L::OFF_X + s * kTile,
+                          my_s + WG_XLO);
+      } else {
+        gemm1<1, SPLIT_X>(acc1, bias, base + L::OFF_WHI, base + L::OFF_WLO, base + L::OFF_X + s * kTile,
+                          my_s + WG_XLO);
+      }
       // GEMM 1 has read the X stage and the labels are in registers: refill the stage with tile it + 2 kWG
       if (t == 0 && it + 2 * kWG < nt) load(it + 2 * kWG, s);
       uint32_t g[32];
-      Fam::epilogue(acc1, lab, cls, K, row0, N, t4, lpa, g);
+      if constexpr (Fam::kBiasInEpilogue)
+        Fam::epilogue(acc1, bias, lab, cls, K, row0, N, t4, lpa, g);
+      else
+        Fam::epilogue(acc1, lab, cls, K, row0, N, t4, lpa, g);
       // left running while the next tile is waited for
       gemm2<kD + 8>(acc2, g, my_s + WG_XT, it == wg);
     }

@@ -1034,6 +1034,20 @@ def linear_predictor(X, w, b=None, tensor_cores=True):
     return LinearPredictor(X, w, b, tensor_cores)
 
 
+class ExpLinearPredictor:
+    """Lazy ``exp(X @ w^T + b)`` of a :class:`LinearPredictor` ``lp``: behaves like the ``[P, N]`` (or ``[N]``)
+    rate tensor when handed to ``Poisson(rate)``, which then scores the site with ONE kernel that reads X and the
+    counts once and emits sum, dW and db (``b2_glm_poisson_log_rate``).  ``eager`` (optional) computes the
+    log-rate the way the model wrote it, so that :meth:`dense` is ``torch.exp`` of the eager value bit for bit."""
+
+    def __init__(self, lp, eager=None):
+        self.lp, self._eager = lp, eager
+        self.shape, self.dtype, self.device = lp.shape, lp.dtype, lp.device
+
+    def dense(self):
+        return torch.exp(self._eager() if self._eager is not None else self.lp.dense())
+
+
 class _GlmBernoulliFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, meta, X, y, W, b):
@@ -1393,16 +1407,102 @@ class _PoissonProduct(Poisson):
         return _PoissonProductFn.apply((scale, weight, sum_coeff, unit), lz.A, lz.B, x)
 
 
+# ---------------------------------------------------------------------------------------------
+# fused Poisson regression: Poisson(rate = exp(X @ w + b))
+# ---------------------------------------------------------------------------------------------
+class _GlmPoissonFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, meta, X, y, W, b):
+        scale, weight, coeff, unit = meta
+        N.require_cuda(X, "fused Poisson-regression likelihood")
+        P, D = W.shape
+        n = X.shape[0]
+        dev = X.device
+        Wc = W.contiguous()
+        bc = b.contiguous() if b is not None else None
+        total = torch.empty((), dtype=torch.float32, device=dev)
+        dW = torch.empty(P, D, dtype=torch.float32, device=dev)
+        db = torch.empty(P, dtype=torch.float32, device=dev)
+        need = int(N.lib().b2_glm_poisson_workspace(n, D, P))
+        ws = N.workspace(dev, need, tag="glm")
+        N.check(N.lib().b2_glm_poisson_log_rate(
+            X.data_ptr(), y.data_ptr(), Wc.data_ptr(), bc.data_ptr() if bc is not None else None,
+            n, D, P, float(scale), float(weight), float(coeff), 0, None, total.data_ptr(),
+            dW.data_ptr(), db.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(dev)),
+            "b2_glm_poisson_log_rate")
+        ctx.grads = (dW, db if b is not None else None)
+        ctx.unit = unit
+        return total
+
+    @staticmethod
+    def backward(ctx, gout):
+        dW, db = ctx.grads
+        if not ctx.unit:
+            dW = dW * gout
+            db = db * gout if db is not None else None
+        return None, None, None, dW, db
+
+
+def _exp_lazy_of(rate):
+    if isinstance(rate, ExpLinearPredictor):
+        return rate
+    lz = getattr(rate, "_lazy", None) if isinstance(rate, torch.Tensor) else None
+    return lz if isinstance(lz, ExpLinearPredictor) else None
+
+
+class _PoissonLinear(Poisson):
+    """Poisson whose rate is an ExpLinearPredictor (built by ``Poisson(lazy)`` when an unchanged model's
+    ``torch.exp(X @ w + b)`` was kept lazy by pyro_b200/lazy.py).  ``rate``, ``log_prob`` and every other use
+    materialise the rate; the ELBO's site sum takes the fused kernel."""
+
+    def __init__(self, rate, validate_args=None, is_sparse=False):
+        lazy = _exp_lazy_of(rate)
+        self._lazy = lazy
+        self._dense = None
+        Distribution.__init__(self, lazy.shape)
+
+    @property
+    def _params(self):
+        if self._dense is None:
+            self._dense = self._lazy.dense()
+        return [self._dense]
+
+    @property
+    def rate(self):
+        return self._params[0]
+
+    def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
+        lp = self._lazy.lp
+        X = lp.X
+        D = X.shape[-1]
+        # the scope of the any-D logistic-regression kernel: tensor cores asked for, 1 <= D <= 128, from 8192
+        # rows (below that the TF32 gradient has not averaged its rounding down to fp32 accuracy yet), fp32,
+        # contiguous 16-byte aligned X and y, no mask
+        ok = (mask is None and X.dtype == torch.float32 and X.is_contiguous() and X.data_ptr() % 16 == 0
+              and 1 <= D <= 128 and getattr(lp, "tensor_cores", True) and X.shape[0] >= 8192
+              and isinstance(value, torch.Tensor) and value.numel() == X.shape[0]
+              and tuple(self.batch_shape) == tuple(lp.shape))
+        y = value.reshape(-1).to(torch.float32).contiguous() if ok else None
+        if not ok or y.data_ptr() % 16 != 0:
+            return super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
+        W = lp.w.reshape(lp.P, D)
+        b = lp.b.reshape(lp.P) if lp.b is not None else None
+        return _GlmPoissonFn.apply((scale, weight, sum_coeff, unit), X, y, W, b)
+
+
 def _poisson_new(cls, rate=None, validate_args=None, is_sparse=False):
-    # ``Poisson(FactorProduct)`` builds the fused factorisation subclass
+    # ``Poisson(FactorProduct)`` builds the fused factorisation subclass, ``Poisson(ExpLinearPredictor)`` the
+    # fused Poisson-regression one
     if cls is Poisson and _factor_lazy_of(rate) is not None:
         return object.__new__(_PoissonProduct)
+    if cls is Poisson and _exp_lazy_of(rate) is not None:
+        return object.__new__(_PoissonLinear)
     return object.__new__(cls)
 
 
 Poisson.__new__ = staticmethod(_poisson_new)
-__all__ += ["LinearPredictor", "linear_predictor", "ClassLinearPredictor", "class_linear_predictor", "FactorProduct",
-            "constant"]
+__all__ += ["LinearPredictor", "linear_predictor", "ExpLinearPredictor", "ClassLinearPredictor",
+            "class_linear_predictor", "FactorProduct", "constant"]
 
 from .hmm import GaussianHMM  # noqa: E402,F401
 __all__ += ["GaussianHMM"]

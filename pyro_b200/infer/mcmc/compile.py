@@ -182,16 +182,19 @@ def _try_logistic(poutine, model, args, kwargs, latent, observed):
 
 
 def _try_glm(poutine, model, args, kwargs, latent, observed):
-    """Logistic regression with an intercept, or softmax regression with or without one, in fp32, within
-    the GLM kernels' scope: Bernoulli D in {4, 8, 16, 32}; Categorical D == 32, 2 <= K <= 16."""
+    """Logistic regression with an intercept, or softmax or Poisson (log link) regression with or without one,
+    in fp32, within the GLM kernels' scope: Bernoulli D in {4, 8, 16, 32}; Categorical D == 32, 2 <= K <= 16;
+    Poisson 1 <= D <= 128."""
     from .potential import GlmPotential
     if len(observed) != 1 or len(latent) not in (1, 2):
         return None
     (obs_name, obs), = observed.items()
     _, kind = _base(obs["fn"])
     # lazy linear-predictor logits build _BernoulliLinear / _CategoricalLinear (pyro_b200/distributions)
-    kind = {"BernoulliLinear": "Bernoulli", "CategoricalLinear": "Categorical"}.get(kind, kind)
-    if kind not in ("Bernoulli", "Categorical") or not _plain_site(obs):
+    # (and _PoissonLinear for a lazy exp of one)
+    kind = {"BernoulliLinear": "Bernoulli", "CategoricalLinear": "Categorical",
+            "PoissonLinear": "Poisson"}.get(kind, kind)
+    if kind not in ("Bernoulli", "Categorical", "Poisson") or not _plain_site(obs):
         return None
     y = obs["value"]
     if not isinstance(y, torch.Tensor) or y.dim() != 1:
@@ -221,6 +224,11 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
         wshapes, bshapes = [(D,)], [(), (1,)]
         if D not in (4, 8, 16, 32) or y.dtype != torch.float32:
             return None
+    elif kind == "Poisson":
+        K = 1
+        wshapes, bshapes = [(D,)], [(), (1,)]
+        if not 1 <= D <= 128 or y.dtype != torch.float32:
+            return None
     else:
         wmat = [s for s in shapes.values() if len(s) == 2]
         K = wmat[0][0] if len(wmat) == 1 else 0
@@ -234,16 +242,22 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
     weight, bias = weight[0], (bias[0] if bias else None)
     if kind == "Bernoulli" and bias is None:
         return None   # intercept-free logistic regression keeps LogisticPotential's route
-    # ---- functional probe: logits == X @ w + b  /  log_softmax(logits) == log_softmax(X @ W.mT + b) --------
+    # ---- functional probe: logits == X @ w + b  /  log_softmax(logits) == log_softmax(X @ W.mT + b)  /
+    # log(rate) == X @ w + b ----------------------------------------------------------------------------------
     gen = torch.Generator(device="cpu").manual_seed(20240302)
     for _ in range(3):
         wv = torch.randn(shapes[weight], generator=gen).to(X)
+        if kind == "Poisson":
+            wv = wv / D ** 0.5            # log-rates of a few units: exp neither overflows nor underflows
         bv = torch.randn(shapes[bias], generator=gen).to(X) if bias is not None else None
         data = {weight: wv} if bias is None else {weight: wv, bias: bv}
-        logits = _probe(poutine, model, args, kwargs, data, obs_name).logits
+        pfn = _probe(poutine, model, args, kwargs, data, obs_name)
+        logits = torch.log(pfn.rate) if kind == "Poisson" else pfn.logits
         if hasattr(logits, "dense"):
             logits = logits.dense()
-        if kind == "Bernoulli":
+        if kind == "Poisson":
+            want = X @ wv + (bv.reshape(()) if bv is not None else 0.0)
+        elif kind == "Bernoulli":
             want = X @ wv + bv.reshape(())
         else:
             want = X @ wv.mT + (bv if bv is not None else 0.0)

@@ -111,10 +111,11 @@ class LogisticPotential(NativePotential):
 
 
 class GlmPotential:
-    """Bayesian logistic or softmax regression with constant-scale Normal priors:
+    """Bayesian logistic, softmax or Poisson regression with constant-scale Normal priors:
     ``w ~ Normal(0, s_w)[D]``, ``b ~ Normal(0, s_b)``, ``y ~ Bernoulli(logits = X @ w + b)``, or
     ``W ~ Normal(0, s_w)[K, D]``, ``b ~ Normal(0, s_b)[K]`` (optional),
-    ``y ~ Categorical(logits = X @ W.mT + b)``.
+    ``y ~ Categorical(logits = X @ W.mT + b)``, or
+    ``w ~ Normal(0, s_w)[D]``, ``b ~ Normal(0, s_b)`` (optional), ``y ~ Poisson(rate = exp(X @ w + b))``.
 
     ``value_and_grad`` is ``b2_glm_potential``: the likelihood of all chains comes from one pass of the
     fused GLM kernel over X, the chains being its particles.  ``sites`` maps each site name to
@@ -127,14 +128,14 @@ class GlmPotential:
         if X.dtype != torch.float32 or X.dim() != 2:
             raise ValueError("GlmPotential needs fp32 X of shape [N, D]")
         self.X = X.contiguous()
-        self.kind = N.GLM_BERNOULLI if kind == "Bernoulli" else N.GLM_CATEGORICAL
+        self.kind = {"Bernoulli": N.GLM_BERNOULLI, "Categorical": N.GLM_CATEGORICAL, "Poisson": N.GLM_POISSON}[kind]
         # private contiguous copies: the kernels load y with TMA (16-byte aligned)
-        self.y = (y.to(torch.float32) if self.kind == N.GLM_BERNOULLI else y.to(torch.int64)).clone()
+        self.y = (y.to(torch.int64) if self.kind == N.GLM_CATEGORICAL else y.to(torch.float32)).clone()
         self.sites = dict(sites)
         self.weight, self.bias = weight, bias
         self.n, self.Dx = self.X.shape
         wshape = self.sites[weight][2]
-        self.K = 1 if self.kind == N.GLM_BERNOULLI else int(wshape[0])
+        self.K = int(wshape[0]) if self.kind == N.GLM_CATEGORICAL else 1
         self.w_off = self.sites[weight][0].start
         self.b_off = self.sites[bias][0].start if bias is not None else 0
         self.has_bias = bias is not None

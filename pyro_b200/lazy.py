@@ -19,6 +19,11 @@ Softmax regression has the same seam: ``X @ W.mT`` (``W.transpose(-1, -2)``, ``t
 kept as a :class:`ClassLinearPredictor`; a bias ``[K]`` or ``[P, 1, K]`` keeps them lazy, and
 ``Categorical(logits=lazy)`` scores the site with ``b2_glm_categorical_logits``.
 
+Poisson regression has one more: ``torch.exp(t)`` or ``t.exp()`` of a lazy ``X @ w + b`` (a
+:class:`LinearPredictor`) gives an :class:`ExpLinearPredictor`, and ``Poisson(lazy)`` scores the site with
+``b2_glm_poisson_log_rate``; any other use, ``+ offset`` and ``* c`` included, materialises ``exp`` of the
+eager expression, bit for bit.
+
 Poisson matrix factorisation (the bottom layer of the sparse gamma DEF) has one more: ``torch.matmul(z, w)``,
 ``z @ w`` or ``torch.bmm(z, w)`` of TWO site values ``z[N, K] @ w[K, J]`` or ``z[P, N, K] @ w[P, K, J]``
 (fp32, one CUDA device, 1 <= K <= 16) gives a :class:`FactorProduct`, and ``Poisson(lazy)`` scores the site with
@@ -30,7 +35,7 @@ guide value of pyro/poutine/replay_messenger.py:50-61); nothing in the model is 
 import torch
 
 from ._lazyparam import LazyExpParam
-from .distributions import ClassLinearPredictor, FactorProduct, LinearPredictor
+from .distributions import ClassLinearPredictor, ExpLinearPredictor, FactorProduct, LinearPredictor
 
 _VIEW_FUNCS = {"squeeze", "unsqueeze", "reshape", "view", "transpose", "t", "permute", "expand",
                "expand_as", "flatten", "contiguous", "__getitem__", "movedim", "swapaxes", "detach_",
@@ -109,6 +114,8 @@ class SiteValue(torch.Tensor):
         if name in _MATMUL_FUNCS and not kwargs:
             lazy = _try_lazy_matmul(name, args)
             if lazy is not None:
+                if isinstance(lazy, LinearPredictorTensor) and isinstance(lazy.lazy, LinearPredictor):
+                    lazy._eager = _eager_call(func, args, kwargs)   # read by exp (ExpLinearPredictor)
                 return lazy
         if any(isinstance(a, LinearPredictorTensor) for a in args):
             return LinearPredictorTensor.__torch_function__(func, types, args, kwargs)
@@ -117,6 +124,22 @@ class SiteValue(torch.Tensor):
         if name in _VIEW_FUNCS and isinstance(out, torch.Tensor) and not isinstance(out, SiteValue):
             return out.as_subclass(SiteValue)
         return out
+
+
+def _eager_args(x):
+    if isinstance(x, LinearPredictorTensor):
+        return x.eager()
+    if isinstance(x, (list, tuple)):
+        return type(x)(_eager_args(v) for v in x)
+    return _plain(x)
+
+
+def _eager_call(func, args, kwargs):
+    """The expression as the model wrote it, run on plain tensors when called."""
+    def run():
+        with torch._C.DisableTorchFunctionSubclass():
+            return func(*_eager_args(args), **{k: _eager_args(v) for k, v in kwargs.items()})
+    return run
 
 
 def _try_lazy_matmul(name, args):
@@ -222,6 +245,7 @@ class LinearPredictorTensor(torch.Tensor):
                                                 requires_grad=False)
         t._lazy = lazy
         t._dense = None
+        t._eager = None
         return t
 
     def __init__(self, lazy):
@@ -236,9 +260,14 @@ class LinearPredictorTensor(torch.Tensor):
             self._dense = self._lazy.dense()
         return self._dense
 
+    def eager(self):
+        """The value of the expression the model wrote, computed as it wrote it (``dense`` may contract in
+        another order)."""
+        return self._eager() if self._eager is not None else self.dense()
+
     def _with_bias(self, b):
         lz = self._lazy
-        if isinstance(lz, FactorProduct):
+        if isinstance(lz, (FactorProduct, ExpLinearPredictor)):
             return None
         if isinstance(lz, ClassLinearPredictor):
             if isinstance(b, LinearPredictorTensor):
@@ -286,7 +315,15 @@ class LinearPredictorTensor(torch.Tensor):
                 other = args[1] if args[0] is self else args[0]
                 out = self._with_bias(other)
                 if out is not None:
+                    if isinstance(out.lazy, LinearPredictor):
+                        out._eager = _eager_call(func, args, kwargs)
                     return out
+            if name == "exp" and len(args) == 1 and not kwargs and isinstance(self._lazy, LinearPredictor):
+                return LinearPredictorTensor(ExpLinearPredictor(self._lazy, self.eager))
+            # Poisson's rate check (constraints.nonnegative: rate >= 0) answered from the operation: exp >= 0
+            if name in ("ge", "__ge__") and isinstance(self._lazy, ExpLinearPredictor) and len(args) == 2 \
+                    and args[0] is self and isinstance(args[1], (int, float)) and args[1] <= 0 and not kwargs:
+                return torch.ones((), dtype=torch.bool, device=self.device).expand(self.shape)
             if name in ("expand", "broadcast_to") and len(args) >= 2:
                 shape = args[1] if isinstance(args[1], (tuple, list, torch.Size)) else args[1:]
                 if tuple(shape) == tuple(self.shape):
@@ -301,7 +338,9 @@ class LinearPredictorTensor(torch.Tensor):
                 return self
             # distribution-argument validation (constraints.real.check): an affine image of finite
             # operands; a NaN would surface in the ELBO itself (warn_if_nan)
-            if name in _CHEAP_TRUE or name in _CHEAP_FALSE:
+            # (not for exp(...): its value may be 0 or inf, so those answers are not constants; every use but the
+            # rate check above materialises it)
+            if (name in _CHEAP_TRUE or name in _CHEAP_FALSE) and not isinstance(self._lazy, ExpLinearPredictor):
                 flag = torch.ones((), dtype=torch.bool, device=self.device) if name in _CHEAP_TRUE \
                     else torch.zeros((), dtype=torch.bool, device=self.device)
                 return flag.expand(self.shape)
