@@ -197,7 +197,8 @@ int b2_gamma_rsample(const b2_tensor* conc, const b2_tensor* rate, int ndim, con
  * their autograd backward, including the accumulation of the two gradients that reach z.
  * A job is one site (<= B2_RSAMPLE_MAX_N elements); one CTA per job, so the sites of a step share a launch.
  *   b2_latent_normal_draw      z, eps [shape] contiguous out; out0 = 0-d SUM log Normal(z | loc, scale);
- *                              noise from Philox(seed, stream = job << 32 | element, launch counter)
+ *                              noise of job k from Philox(seed, stream = element, counter + k), the same as k
+ *                              one-job launches; rng_state = {seed, counter, ticket (zero)}, counter += n_jobs
  *   b2_latent_normal_prior     out0 = 0-d SUM log Normal(z | prior_loc, prior_scale), value only
  *   b2_latent_normal_backward  g = gz + prior_weight * d log p(z)/dz;  out0 = d/dloc = g,
  *                              out1 = d/dscale = g*eps - c/scale  (or d/dlog_scale = g*eps*scale - c), each summed
@@ -291,6 +292,19 @@ int b2_glm_bernoulli_logits(const float* X, const float* y, const float* W, cons
                             int flags, float* out_sum_p, float* out_total, float* out_dW,
                             float* out_db, void* workspace, size_t workspace_bytes, void* stream);
 size_t b2_glm_workspace(int64_t N, int D, int P);
+/* b2_glm_bernoulli_logits that also writes the step's loss, as b2_latent_normal_prior_combine would (bit for
+ * bit), with no launch of its own: the finish kernel scores the value-only Normal priors of the fp32 jobs and adds
+ *   *loss = SUM_j job_coeffs[j] * SUM log Normal(z_j | prior_j)  +  SUM_t term_coeffs[t] * *terms[t]
+ * where a NULL term stands for this call's own *out_total (required).  warp_sums: device scratch of
+ * b2_glm_elbo_workspace() bytes, not shared with a call in flight. */
+int b2_glm_bernoulli_logits_elbo(const float* X, const float* y, const float* W, const float* b,
+                                 int64_t N, int D, int P, double scale, double weight, double sum_coeff,
+                                 int flags, float* out_sum_p, float* out_total, float* out_dW,
+                                 float* out_db, void* workspace, size_t workspace_bytes,
+                                 const b2_latent_job* jobs, int n_jobs, const double* job_coeffs,
+                                 const void* const* terms, const double* term_coeffs, int n_terms, void* loss,
+                                 void* warp_sums, size_t warp_sums_bytes, void* stream);
+size_t b2_glm_elbo_workspace(void);
 
 /*
  * b2_glm_categorical_logits -- fused softmax-regression (multiclass logistic) likelihood term: for P

@@ -112,6 +112,10 @@ SIGNATURES = {
     "b2_elbo_combine": (_i32, [_vp, _vp, _i32, _i32, _vp, _vp]),
     "b2_glm_bernoulli_logits": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _f64, _f64, _f64, _i32,
                                        _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "b2_glm_bernoulli_logits_elbo": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _f64, _f64, _f64, _i32,
+                                            _vp, _vp, _vp, _vp, _vp, _sz, _vp, _i32, _vp, _vp, _vp, _i32, _vp,
+                                            _vp, _sz, _vp]),
+    "b2_glm_elbo_workspace": (_sz, []),
     "b2_glm_workspace": (_sz, [_i64, _i32, _i32]),
     "b2_glm_categorical_logits": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _f64, _f64, _f64,
                                          _i32, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
@@ -223,7 +227,14 @@ def capturing():
     return torch.cuda.is_available() and torch.cuda.is_current_stream_capturing()
 
 
+# set by distributions/_ops.py to launch the pending (deferred) draws: every native launch asks for its stream
+# here first, so no kernel can read a site value whose draw has not run
+before_launch = None
+
+
 def stream_ptr(device=None):
+    if before_launch is not None:
+        before_launch()
     return torch.cuda.current_stream(device).cuda_stream
 
 

@@ -32,6 +32,17 @@ __device__ __forceinline__ void pdl_enter() {
   asm volatile("griddepcontrol.wait;" ::: "memory");
 #endif
 }
+// The two halves of pdl_enter, for a kernel that does work which no predecessor can affect before it waits.
+__device__ __forceinline__ void pdl_launch_dependents() {
+#if __CUDA_ARCH__ >= 900
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+#endif
+}
+__device__ __forceinline__ void pdl_wait() {
+#if __CUDA_ARCH__ >= 900
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+#endif
+}
 inline bool pdl_enabled() {
   static const bool on = [] {
     const char* e = getenv("B2_PDL");

@@ -19,6 +19,7 @@
 
 #include "b2_common.cuh"
 #include "b2_math.cuh"
+#include "latent.cuh"
 
 namespace b2 {
 
@@ -136,79 +137,153 @@ __global__ void __launch_bounds__(256) glm_bernoulli_kernel(const float* __restr
   }
 }
 
+// Loss assembly in the finish (b2_glm_bernoulli_logits_elbo): the value-only Normal priors of the step's latent
+// sites and the other 0-d terms of the ELBO, so that the likelihood call also writes the step's loss
+//   *out = SUM_j job_coeff[j] * SUM log Normal(z_j | prior_j)  +  SUM_t term_coeff[t] * *term[t]
+// with the arithmetic of latent_prior_combine_kernel (latent.cu), bit for bit: that kernel's CTA of nwarps warps
+// is replayed by nwarps warps per job here (warp w adds the elements w*32 + lane + k*nwarps*32 in fp64, then the
+// same shuffle tree), and the last warp to arrive sums the nwarps per-warp values of each job with the shuffle
+// tree of block_sum and adds the jobs, then the terms, in order, in fp64.  A null term is this call's own total.
+struct GlmElbo {
+  LatentJob job[B2_LATENT_MAX_JOBS];   // z (fp32, contiguous), ploc / pscale with their strides
+  double job_coeff[B2_LATENT_MAX_JOBS];
+  const float* term[B2_LATENT_MAX_TERMS];
+  double term_coeff[B2_LATENT_MAX_TERMS];
+  int n_jobs, n_terms, nwarps;
+  double* warp_sums;                   // [n_jobs][32]
+  float* out;
+};
+
 // second stage: fixed-order sum over the CTAs' partials [nblocks][P][K (D + 1) + 1] (per class dW[0..D-1]
 // and db, then the particle's lp sum; K = 1 for Bernoulli and Poisson); applies weight / scale.  lg (Poisson
 // only, else null) holds one more partial per CTA, of a term every particle's sum subtracts: SUM lgamma(y + 1).
 // One WARP per entry of the [P, K (D + 1) + 1] table: lanes stride over the CTAs (L2-resident partials),
-// then a shuffle tree (a thread-per-entry loop is a chain of ~300 dependent loads).
-__global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict__ partials,
-                                                         int nblocks, int P, int K, int D, double scale,
-                                                         double weight, float* __restrict__ sum_p,
-                                                         float* __restrict__ out_dW,
-                                                         float* __restrict__ out_db,
-                                                         double sum_coeff, int flags,
-                                                         float* __restrict__ out_total,
-                                                         unsigned int* __restrict__ ticket,
-                                                         const float* __restrict__ lg) {
+// then a shuffle tree (a thread-per-entry loop is a chain of ~300 dependent loads).  With E, E->n_jobs *
+// E->nwarps more warps score the priors, and the ticket counts them too.
+__device__ __forceinline__ void glm_finish_body(const float* __restrict__ partials, int nblocks, int P, int K, int D,
+                                                double scale, double weight, float* __restrict__ sum_p,
+                                                float* __restrict__ out_dW, float* __restrict__ out_db,
+                                                double sum_coeff, int flags, float* __restrict__ out_total,
+                                                unsigned int* __restrict__ ticket, const float* __restrict__ lg,
+                                                const GlmElbo* E) {
   pdl_enter();
   const int S = K * (D + 1) + 1;
   const int total = P * S;
+  const int n_prior = E ? E->n_jobs * E->nwarps : 0;
   const int e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
-  if (e >= total) return;
-  double s = 0.0;
-  for (int bl = lane; bl < nblocks; bl += 32) s += (double)partials[(int64_t)bl * total + e];
-  s = warp_sum(s);
-  const int p = e / S, r = e - p * S;
-  if (r < K * (D + 1)) {
-    const int k = r / (D + 1), c = r - k * (D + 1);
-    if (lane == 0) {
-      if (c < D) {
-        if (out_dW) out_dW[((int64_t)p * K + k) * D + c] = (float)(weight * scale * s);
-      } else if (out_db) {
-        out_db[(int64_t)p * K + k] = (float)(weight * scale * s);
-      }
-    }
-    return;
-  }
-  if (lg != nullptr) {
-    double l = 0.0;
-    for (int bl = lane; bl < nblocks; bl += 32) l += (double)lg[bl];
-    s -= warp_sum(l);
-  }
-  // per-particle sum; the LAST of the P warps to get here also totals them (fixed order), with
-  // the ELBO coefficient -- a ticket instead of a third launch
+  if (e >= total + n_prior) return;
   unsigned int t = 0;
-  if (lane == 0) {
-    sum_p[p] = (float)(scale * s);
-    if (out_total) {
+  if (e >= total) {
+    const int k = (e - total) / E->nwarps, w = (e - total) - k * E->nwarps;
+    const LatentJob& j = E->job[k];
+    double acc = 0.0;
+    for (unsigned i = (unsigned)(w * 32 + lane); i < j.n; i += (unsigned)(E->nwarps * 32)) {
+      int ol, os, opl, ops;
+      unravel(j, i, ol, os, opl, ops);
+      float p[2] = {reinterpret_cast<const float*>(j.ploc)[opl], reinterpret_cast<const float*>(j.pscale)[ops]};
+      ElemOut<float> o;
+      Eval<kNormal, float, false>::run(reinterpret_cast<const float*>(j.z)[i], p, o);
+      acc += (double)o.lp;
+    }
+    acc = warp_sum(acc);
+    if (lane == 0) {
+      E->warp_sums[k * 32 + w] = acc;
       __threadfence();
       t = atomicAdd(ticket, 1u);
     }
+  } else {
+    double s = 0.0;
+    for (int bl = lane; bl < nblocks; bl += 32) s += (double)partials[(int64_t)bl * total + e];
+    s = warp_sum(s);
+    const int p = e / S, r = e - p * S;
+    if (r < K * (D + 1)) {
+      const int k = r / (D + 1), c = r - k * (D + 1);
+      if (lane == 0) {
+        if (c < D) {
+          if (out_dW) out_dW[((int64_t)p * K + k) * D + c] = (float)(weight * scale * s);
+        } else if (out_db) {
+          out_db[(int64_t)p * K + k] = (float)(weight * scale * s);
+        }
+      }
+      return;
+    }
+    if (lg != nullptr) {
+      double l = 0.0;
+      for (int bl = lane; bl < nblocks; bl += 32) l += (double)lg[bl];
+      s -= warp_sum(l);
+    }
+    // per-particle sum; the LAST of the P warps (and prior warps) to get here also totals them (fixed order),
+    // with the ELBO coefficient -- a ticket instead of a third launch
+    if (lane == 0) {
+      sum_p[p] = (float)(scale * s);
+      if (out_total) {
+        __threadfence();
+        t = atomicAdd(ticket, 1u);
+      }
+    }
+    if (!out_total) return;
   }
-  if (!out_total) return;
   t = __shfl_sync(0xffffffffu, t, 0);
-  if (t != (unsigned)(P - 1)) return;
+  if (t != (unsigned)(P + n_prior - 1)) return;
   __threadfence();
   double acc = 0.0;
   for (int q = lane; q < P; q += 32) acc += (double)__ldcg(sum_p + q);
   acc = warp_sum(acc);
+  float own = 0.f;
   if (lane == 0) {
     const double v = sum_coeff * acc;
-    *out_total = (flags & B2_FLAG_ACCUMULATE_SUM) ? (float)((double)*out_total + v) : (float)v;
+    own = (flags & B2_FLAG_ACCUMULATE_SUM) ? (float)((double)*out_total + v) : (float)v;
+    *out_total = own;
     *ticket = 0u;
   }
+  if (!E) return;
+  double loss = 0.0;
+  for (int k = 0; k < E->n_jobs; ++k) {
+    double w = lane < E->nwarps ? __ldcg(E->warp_sums + k * 32 + lane) : 0.0;
+    w = warp_sum(w);
+    loss += E->job_coeff[k] * w;
+  }
+  if (lane == 0) {
+    for (int q = 0; q < E->n_terms; ++q)
+      loss += E->term_coeff[q] * (double)(E->term[q] ? __ldcg(E->term[q]) : own);
+    *E->out = (float)loss;
+  }
+}
+
+__global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict__ partials, int nblocks, int P,
+                                                         int K, int D, double scale, double weight,
+                                                         float* __restrict__ sum_p, float* __restrict__ out_dW,
+                                                         float* __restrict__ out_db, double sum_coeff, int flags,
+                                                         float* __restrict__ out_total,
+                                                         unsigned int* __restrict__ ticket,
+                                                         const float* __restrict__ lg) {
+  glm_finish_body(partials, nblocks, P, K, D, scale, weight, sum_p, out_dW, out_db, sum_coeff, flags, out_total,
+                  ticket, lg, nullptr);
+}
+
+__global__ void __launch_bounds__(256) glm_finish_elbo_kernel(const float* __restrict__ partials, int nblocks, int P,
+                                                              int K, int D, double scale, double weight,
+                                                              float* __restrict__ sum_p, float* __restrict__ out_dW,
+                                                              float* __restrict__ out_db, double sum_coeff,
+                                                              int flags, float* __restrict__ out_total,
+                                                              unsigned int* __restrict__ ticket, const GlmElbo E) {
+  glm_finish_body(partials, nblocks, P, K, D, scale, weight, sum_p, out_dW, out_db, sum_coeff, flags, out_total,
+                  ticket, nullptr, &E);
 }
 
 // The second launch of b2_glm_bernoulli_logits, b2_glm_categorical_logits and b2_glm_poisson_log_rate.  The
 // per-particle sums go to out_sum_p, or without one to the [P] row of the workspace after the partials.
+static float* glm_sum_p(const float* partials, float* out_sum_p, int gx, int total) {
+  return out_sum_p ? out_sum_p : const_cast<float*>(partials) + (size_t)gx * total;
+}
+
 void launch_glm_finish(const float* partials, unsigned int* ticket, int gx, int P, int K, int D, double scale,
                        double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
                        float* out_dW, float* out_db, const float* lg, cudaStream_t s) {
   const int total = P * (K * (D + 1) + 1);
-  float* sum_p = out_sum_p ? out_sum_p : const_cast<float*>(partials) + (size_t)gx * total;
-  launch_pdl(glm_finish_kernel, dim3((total + 7) / 8), dim3(256), 0, s, partials, gx, P, K, D, scale, weight, sum_p,
-             out_dW, out_db, sum_coeff, flags, out_total, ticket, lg);
+  launch_pdl(glm_finish_kernel, dim3((total + 7) / 8), dim3(256), 0, s, partials, gx, P, K, D, scale, weight,
+             glm_sum_p(partials, out_sum_p, gx, total), out_dW, out_db, sum_coeff, flags, out_total, ticket, lg);
 }
 
 // wgmma + TMA variant (glm_tc.cu)
@@ -231,17 +306,17 @@ inline int glm_grid_x(int64_t N) {
 
 using namespace b2;
 
+extern "C" size_t b2_glm_elbo_workspace(void) { return (size_t)B2_LATENT_MAX_JOBS * 32 * sizeof(double); }
+
 extern "C" size_t b2_glm_workspace(int64_t N, int D, int P) {
   // [ticket, 256 B] + CTA partials + one [P] row for the per-particle sums
   return 256 + ((size_t)glm_grid_x(N) * (size_t)P * (size_t)(D + 2) + (size_t)P) * sizeof(float);
 }
 
-extern "C" int b2_glm_bernoulli_logits(const float* X, const float* y, const float* W,
-                                       const float* b, int64_t N, int D, int P, double scale,
-                                       double weight, double sum_coeff, int flags,
-                                       float* out_sum_p, float* out_total, float* out_dW,
-                                       float* out_db, void* workspace, size_t workspace_bytes,
-                                       void* stream) {
+static int glm_bernoulli(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
+                         double scale, double weight, double sum_coeff, int flags, float* out_sum_p,
+                         float* out_total, float* out_dW, float* out_db, void* workspace, size_t workspace_bytes,
+                         cudaStream_t s, const GlmElbo* E) {
   if (!X || !y || !W) return B2_ERR_NULL;
   if (N <= 0 || P <= 0) return B2_ERR_BAD_SHAPE;
   if (reinterpret_cast<uintptr_t>(X) % 16 != 0) return B2_ERR_BAD_SHAPE;
@@ -253,7 +328,6 @@ extern "C" int b2_glm_bernoulli_logits(const float* X, const float* y, const flo
   if (flat && reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
   if (flat && N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
   if (!workspace || workspace_bytes < b2_glm_workspace(N, D, P)) return B2_ERR_WORKSPACE;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   // below 8 Ki rows the single-pass TF32 gradient contraction has not averaged its operand rounding
   // (2^-12 relative per term) below the fp32 tolerance yet: those sizes take the exact fp32 SIMT kernel
   // unless the tensor-core kernel is asked for explicitly (B2_FLAG_GLM_3XTF32).  The TMA loads need a
@@ -279,8 +353,61 @@ extern "C" int b2_glm_bernoulli_logits(const float* X, const float* y, const flo
     case 32: glm_bernoulli_kernel<32><<<grid, 256, 0, s>>>(X, y, W, b, N, P, partials); break;
     default: return B2_ERR_BAD_SHAPE;
   }
-  launch_glm_finish(partials, ticket, gx, P, 1, D, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW,
-                    out_db, nullptr, s);
+  if (E) {
+    const int total = P * (D + 2);
+    launch_pdl(glm_finish_elbo_kernel, dim3((total + E->n_jobs * E->nwarps + 7) / 8), dim3(256), 0, s, partials, gx,
+               P, 1, D, scale, weight, glm_sum_p(partials, out_sum_p, gx, total), out_dW, out_db, sum_coeff, flags,
+               out_total, ticket, *E);
+  } else {
+    launch_glm_finish(partials, ticket, gx, P, 1, D, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW,
+                      out_db, nullptr, s);
+  }
   count_launch(2);
   return check_launch();
+}
+
+extern "C" int b2_glm_bernoulli_logits(const float* X, const float* y, const float* W,
+                                       const float* b, int64_t N, int D, int P, double scale,
+                                       double weight, double sum_coeff, int flags,
+                                       float* out_sum_p, float* out_total, float* out_dW,
+                                       float* out_db, void* workspace, size_t workspace_bytes,
+                                       void* stream) {
+  return glm_bernoulli(X, y, W, b, N, D, P, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW, out_db,
+                       workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), nullptr);
+}
+
+extern "C" int b2_glm_bernoulli_logits_elbo(const float* X, const float* y, const float* W,
+                                            const float* b, int64_t N, int D, int P, double scale,
+                                            double weight, double sum_coeff, int flags,
+                                            float* out_sum_p, float* out_total, float* out_dW,
+                                            float* out_db, void* workspace, size_t workspace_bytes,
+                                            const b2_latent_job* jobs, int n_jobs, const double* job_coeffs,
+                                            const void* const* terms, const double* term_coeffs, int n_terms,
+                                            void* loss, void* warp_sums, size_t warp_sums_bytes, void* stream) {
+  if (!out_total || !loss || !job_coeffs || (n_terms > 0 && (!terms || !term_coeffs))) return B2_ERR_NULL;
+  if (n_terms < 0 || n_terms > B2_LATENT_MAX_TERMS) return B2_ERR_TOO_LARGE;
+  if (!warp_sums || warp_sums_bytes < b2_glm_elbo_workspace()) return B2_ERR_WORKSPACE;
+  LatentArgs a;
+  int dtype;
+  unsigned nmax;
+  const int code = fill_args(a, jobs, n_jobs, dtype, nmax);
+  if (code != B2_OK) return code;
+  if (dtype != B2_F32) return B2_ERR_BAD_DTYPE;
+  GlmElbo E;
+  for (int k = 0; k < n_jobs; ++k) {
+    if (!a.job[k].ploc || !a.job[k].pscale || !a.job[k].z) return B2_ERR_NULL;
+    E.job[k] = a.job[k];
+    E.job_coeff[k] = job_coeffs[k];
+  }
+  for (int t = 0; t < n_terms; ++t) {
+    E.term[t] = static_cast<const float*>(terms[t]);   // null: this call's own total
+    E.term_coeff[t] = term_coeffs[t];
+  }
+  E.n_jobs = n_jobs;
+  E.n_terms = n_terms;
+  E.nwarps = threads_for(nmax) / 32;
+  E.warp_sums = static_cast<double*>(warp_sums);
+  E.out = static_cast<float*>(loss);
+  return glm_bernoulli(X, y, W, b, N, D, P, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW, out_db,
+                       workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream), &E);
 }

@@ -562,7 +562,7 @@ __device__ __forceinline__ void glm_tile_pipeline(const CUtensorMap& map_x, cons
   using L = Smem32<Fam::kYBytes>;
   constexpr int KP = Fam::kKP;
   constexpr uint32_t kYBytes = Fam::kYBytes;
-  pdl_enter();   // lets glm_finish_kernel be resident (blocked in its griddepcontrol.wait) before this kernel ends
+  pdl_launch_dependents();   // lets glm_finish_kernel be resident (blocked in its griddepcontrol.wait) early
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
@@ -581,6 +581,24 @@ __device__ __forceinline__ void glm_tile_pipeline(const CUtensorMap& map_x, cons
     for (int s = 0; s < kStages; ++s) mbar_init(bar_full(s), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
+  __syncthreads();
+  // warp-uniform by construction (a shuffle result), so the tile loop is not a divergent branch to ptxas
+  const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0), w4 = warp & 3, t = tid & 127;
+  // tile it -> X / label stage; one thread of the warpgroup issues the loads
+  auto load = [&](int it, int s) {
+    const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
+    mbar_expect_tx(bar_full(s), kTile + kYBytes);
+    tma_load_2d(base + L::OFF_X + s * kTile, &map_x, 0, (int)(tile * kRows), bar_full(s));
+    tma_load_1d(base + L::OFF_Y + s * kYBytes, &map_y, (int)(tile * kRows), bar_full(s));
+  };
+  // Each warpgroup's first two X / label tiles are requested BEFORE griddepcontrol.wait, so they stream while the
+  // predecessor (the step's draw kernel, on a CTA or two) finishes.  Sound because no native kernel that can
+  // precede a GLM launch writes X or the labels: the draws write site values, the pack kernels of glm_potential.cu
+  // write W and b only, and a predecessor launched without PDL never lets this kernel start early.  W, the bias
+  // and everything else a predecessor may write are read after the wait.
+  if (t == 0)
+    for (int k = 0; k < 2 && wg + k * kWG < nt; ++k) load(wg + k * kWG, 2 * wg + k);
+  pdl_wait();
   stage_w_and_ones<KP, kD, kThreads>(reinterpret_cast<float*>(sm + L::OFF_WHI),
                                      reinterpret_cast<float*>(sm + L::OFF_WLO), sm + L::OFF_WG + WG_XT, kWGBytes,
                                      W, slab, P, K, kD);
@@ -592,8 +610,6 @@ __device__ __forceinline__ void glm_tile_pipeline(const CUtensorMap& map_x, cons
   // the tile loop (C7515): the warpgroup's first GEMM 2 k-step starts it with scale-d = 0, and a warpgroup
   // without a tile is left out of the CTA reduction.
   float acc2[20];
-  // warp-uniform by construction (a shuffle result), so the tile loop is not a divergent branch to ptxas
-  const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0), w4 = warp & 3, t = tid & 127;
   const int gid = lane >> 2, t4 = lane & 3;
   // the thread's two rows m = 16 w4 + gid + 8h: class (gid + 8h) % KP of particle slab * 64 / KP + m / KP
   int cls[2];
@@ -609,15 +625,6 @@ __device__ __forceinline__ void glm_tile_pipeline(const CUtensorMap& map_x, cons
   {
     uint8_t* my = sm + L::OFF_WG + wg * kWGBytes;
     const uint32_t my_s = base + L::OFF_WG + wg * kWGBytes;
-    // tile it -> X / label stage; one thread of the warpgroup issues the loads
-    auto load = [&](int it, int s) {
-      const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
-      mbar_expect_tx(bar_full(s), kTile + kYBytes);
-      tma_load_2d(base + L::OFF_X + s * kTile, &map_x, 0, (int)(tile * kRows), bar_full(s));
-      tma_load_1d(base + L::OFF_Y + s * kYBytes, &map_y, (int)(tile * kRows), bar_full(s));
-    };
-    if (t == 0)
-      for (int k = 0; k < 2 && wg + k * kWG < nt; ++k) load(wg + k * kWG, 2 * wg + k);
     for (int k = 0, it = wg; it < nt; ++k, it += kWG) {
       const int s = 2 * wg + (k & 1);
       const int64_t row0 = (blockIdx.x + (int64_t)it * gridDim.x) * kRows;

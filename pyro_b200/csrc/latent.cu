@@ -21,46 +21,10 @@
 
 #include "b2_common.cuh"
 #include "b2_math.cuh"
+#include "latent.cuh"
 #include "nuts_core.cuh"
 
 namespace b2 {
-
-struct LatentJob {
-  int ndim;
-  unsigned n;
-  unsigned shape[kMaxD];
-  int st_loc[kMaxD], st_scale[kMaxD], st_ploc[kMaxD], st_pscale[kMaxD];
-  int flags;
-  const void* loc;
-  const void* scale;    // scale, or log(scale) with B2_LATENT_LOG_SCALE
-  const void* ploc;     // prior (may be null)
-  const void* pscale;
-  void* z;              // [shape] contiguous (draw: out; prior / backward: in)
-  void* eps;            // [shape] contiguous (draw: out; backward: in)
-  const void* gz;       // backward: dL/dz [shape] contiguous, may be null (= 0)
-  void* out0;           // draw: sum log q (0-d); prior: sum log p (0-d); backward: d/dloc (stored shape)
-  void* out1;           // backward: d/dscale or d/dlog_scale (stored shape)
-  double c, pw;         // backward: coefficient of d(sum log q)/d(.), weight of the prior's d log p/dz
-};
-struct LatentArgs {
-  LatentJob job[B2_LATENT_MAX_JOBS];
-  unsigned long long* state;
-};
-
-__device__ __forceinline__ void unravel(const LatentJob& j, unsigned i, int& ol, int& os, int& opl, int& ops) {
-  unsigned rem = i;
-  ol = os = opl = ops = 0;
-  for (int d = j.ndim - 1; d >= 0; --d) {
-    const unsigned sd = j.shape[d];
-    const unsigned q = rem / sd;
-    const int idx = (int)(rem - q * sd);
-    rem = q;
-    ol += idx * j.st_loc[d];
-    os += idx * j.st_scale[d];
-    opl += idx * j.st_ploc[d];
-    ops += idx * j.st_pscale[d];
-  }
-}
 
 template <typename T>
 __global__ void __launch_bounds__(1024) latent_draw_kernel(const LatentArgs a) {
@@ -73,7 +37,7 @@ __global__ void __launch_bounds__(1024) latent_draw_kernel(const LatentArgs a) {
     int ol, os, opl, ops;
     unravel(j, i, ol, os, opl, ops);
     Philox rng;
-    rng.init(seed, ((uint64_t)blockIdx.x << 32) | (uint64_t)i, ctr);
+    rng.init(seed, (uint64_t)i, ctr + blockIdx.x);
     const T e = rng.template normal<T>();
     const T loc = reinterpret_cast<const T*>(j.loc)[ol];
     const T sv = reinterpret_cast<const T*>(j.scale)[os];
@@ -89,13 +53,19 @@ __global__ void __launch_bounds__(1024) latent_draw_kernel(const LatentArgs a) {
   __shared__ double smem[32];
   double v[1] = {acc};
   block_sum<1>(v, smem);
-  if (threadIdx.x == 0) *reinterpret_cast<T*>(j.out0) = (T)v[0];
-  // the launch counter advances once per launch: a one-CTA launch does it here (every thread read it before the
-  // block_sum barriers); a multi-job launch is followed by latent_advance_kernel (b2_latent_normal_draw)
-  if (gridDim.x == 1 && threadIdx.x == 0) a.state[1] = ctr + 1ull;
+  // job k draws what the k-th of n_jobs one-job launches would (counter ctr + k), and the counter advances by
+  // n_jobs.  Every thread of a CTA read it before the block_sum barriers; the last CTA to take a ticket (state[2])
+  // advances it, so no CTA can read the advanced value
+  if (threadIdx.x == 0) {
+    *reinterpret_cast<T*>(j.out0) = (T)v[0];
+    if (gridDim.x == 1) {
+      a.state[1] = ctr + 1ull;
+    } else if (atomicAdd(a.state + 2, 1ull) == (unsigned long long)(gridDim.x - 1)) {
+      a.state[1] = ctr + gridDim.x;
+      a.state[2] = 0ull;
+    }
+  }
 }
-
-__global__ void latent_advance_kernel(unsigned long long* state) { state[1] += 1ull; }
 
 template <typename T>
 __global__ void __launch_bounds__(1024) latent_prior_kernel(const LatentArgs a) {
@@ -228,64 +198,6 @@ __global__ void __launch_bounds__(1024) latent_backward_kernel(const LatentArgs 
   latent_reduce<T, 1>(j, j.st_scale, j.out1, logs, (j.flags & B2_LATENT_ACC_OUT1) != 0);
 }
 
-static int fill_job(LatentJob& j, const b2_latent_job& h, int dtype) {
-  if (h.ndim < 0 || h.ndim > kMaxD) return B2_ERR_BAD_SHAPE;
-  j.ndim = h.ndim;
-  int64_t n = 1;
-  for (int d = 0; d < kMaxD; ++d) {
-    j.shape[d] = 1;
-    j.st_loc[d] = j.st_scale[d] = j.st_ploc[d] = j.st_pscale[d] = 0;
-  }
-  for (int d = 0; d < h.ndim; ++d) {
-    if (h.shape[d] <= 0) return B2_ERR_BAD_SHAPE;
-    // offsets are 32-bit in the kernels (a site has <= 65 536 elements, but an operand may be a strided view)
-    const int64_t lim = INT32_MAX / B2_RSAMPLE_MAX_N;
-    if (h.loc_stride[d] > lim || h.loc_stride[d] < -lim || h.scale_stride[d] > lim || h.scale_stride[d] < -lim ||
-        h.prior_loc_stride[d] > lim || h.prior_loc_stride[d] < -lim || h.prior_scale_stride[d] > lim ||
-        h.prior_scale_stride[d] < -lim)
-      return B2_ERR_TOO_LARGE;
-    j.shape[d] = (unsigned)h.shape[d];
-    n *= h.shape[d];
-    j.st_loc[d] = (int)h.loc_stride[d];
-    j.st_scale[d] = (int)h.scale_stride[d];
-    j.st_ploc[d] = (int)h.prior_loc_stride[d];
-    j.st_pscale[d] = (int)h.prior_scale_stride[d];
-  }
-  if (n <= 0 || n > B2_RSAMPLE_MAX_N) return B2_ERR_TOO_LARGE;
-  if (h.dtype != dtype) return B2_ERR_BAD_DTYPE;
-  j.n = (unsigned)n;
-  j.flags = h.flags;
-  j.loc = h.loc;
-  j.scale = h.scale;
-  j.ploc = h.prior_loc;
-  j.pscale = h.prior_scale;
-  j.z = h.z;
-  j.eps = h.eps;
-  j.gz = h.gz;
-  j.out0 = h.out0;
-  j.out1 = h.out1;
-  j.c = h.c;
-  j.pw = h.prior_weight;
-  return B2_OK;
-}
-
-static int fill_args(LatentArgs& a, const b2_latent_job* jobs, int n_jobs, int& dtype, unsigned& nmax) {
-  if (!jobs) return B2_ERR_NULL;
-  if (n_jobs < 1 || n_jobs > B2_LATENT_MAX_JOBS) return B2_ERR_BAD_SHAPE;
-  dtype = jobs[0].dtype;
-  if (dtype != B2_F32 && dtype != B2_F64) return B2_ERR_BAD_DTYPE;
-  nmax = 0;
-  for (int k = 0; k < n_jobs; ++k) {
-    const int code = fill_job(a.job[k], jobs[k], dtype);
-    if (code != B2_OK) return code;
-    if (a.job[k].n > nmax) nmax = a.job[k].n;
-  }
-  a.state = nullptr;
-  return B2_OK;
-}
-
-static int threads_for(unsigned nmax) { return nmax >= 1024 ? 1024 : (int)((nmax + 31) / 32 * 32); }
-
 }  // namespace b2
 
 using namespace b2;
@@ -304,14 +216,7 @@ extern "C" int b2_latent_normal_draw(const b2_latent_job* jobs, int n_jobs, void
   if (dtype == B2_F32) launch_pdl(latent_draw_kernel<float>, dim3(n_jobs), dim3(threads_for(nmax)), 0, s, a);
   else launch_pdl(latent_draw_kernel<double>, dim3(n_jobs), dim3(threads_for(nmax)), 0, s, a);
   count_launch();
-  int rc = check_launch();
-  if (rc == B2_OK && n_jobs > 1) {
-    // several CTAs read the launch counter: it is advanced by a stream-ordered follow-up instead
-    latent_advance_kernel<<<1, 1, 0, s>>>(a.state);
-    count_launch();
-    rc = check_launch();
-  }
-  return rc;
+  return check_launch();
 }
 
 extern "C" int b2_latent_normal_prior(const b2_latent_job* jobs, int n_jobs, void* stream) {

@@ -302,6 +302,9 @@ class Normal(_Elementwise):
                 z, lq = _NormalRsampleFn.apply(coeff, loc, self._log_scale, None, torch.Size(shape), True)
             else:
                 z, lq = _NormalRsampleFn.apply(coeff, loc, densify(self.scale), None, torch.Size(shape), False)
+            if N.LATENT_BLOCK:
+                # a deferred draw (_ops.defer_latent_draw): reading z or lq launches it first
+                z, lq = z.as_subclass(_ops.DeferredDraw), lq.as_subclass(_ops.DeferredDraw)
             z._b2_rsample = _RsampleTag(self.loc, self.scale, lq, coeff)
             return z
         eps = torch.randn(shape, dtype=loc.dtype, device=loc.device)
@@ -350,7 +353,7 @@ class _NormalRsampleFn(torch.autograd.Function):
     def forward(ctx, coeff, loc, scale, eps, shape, log_scale=False):
         if eps is None:
             if N.LATENT_BLOCK:
-                z, lq, eps = _ops.latent_draw(loc, scale, log_scale, shape)
+                z, lq, eps = _ops.defer_latent_draw(loc, scale, log_scale, shape)
             else:
                 z, lq, eps = _ops.normal_rsample_philox(loc, scale.exp() if log_scale else scale, shape)
         else:
@@ -1011,9 +1014,9 @@ class LinearPredictor:
     def __init__(self, X, w, b=None, tensor_cores=True):
         # latent values may arrive as lazy-aware SiteValue tensors (pyro_b200/lazy.py): score plain ones
         if type(w).__name__ == "SiteValue":
-            w = w.as_subclass(torch.Tensor)
+            w = _ops.plain_value(w)
         if type(b).__name__ == "SiteValue":
-            b = b.as_subclass(torch.Tensor)
+            b = _ops.plain_value(b)
         self.X, self.w, self.b = X, w, b
         self.tensor_cores = tensor_cores  # False: fp32 SIMT contractions (B2_FLAG_GLM_FP32)
         D = X.shape[-1]
@@ -1064,11 +1067,21 @@ class _GlmBernoulliFn(torch.autograd.Function):
         db = torch.empty(P, dtype=torch.float32, device=dev)
         need = int(N.lib().b2_glm_workspace(n, D, P))
         ws = N.workspace(dev, need, tag="glm")
-        N.check(N.lib().b2_glm_bernoulli_logits(
-            X.data_ptr(), y.data_ptr(), Wc.data_ptr(), bc.data_ptr() if bc is not None else None,
-            n, D, P, float(scale), float(weight), float(coeff), int(flags), None, total.data_ptr(),
-            dW.data_ptr(), db.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(dev)),
-            "b2_glm_bernoulli_logits")
+        args = (X.data_ptr(), y.data_ptr(), Wc.data_ptr(), bc.data_ptr() if bc is not None else None,
+                n, D, P, float(scale), float(weight), float(coeff), int(flags), None, total.data_ptr(),
+                dW.data_ptr(), db.data_ptr(), ws.data_ptr(), ws.numel())
+        asm = _ops.take_elbo_assembly(dev)
+        if asm is None:
+            N.check(N.lib().b2_glm_bernoulli_logits(*args, N.stream_ptr(dev)), "b2_glm_bernoulli_logits")
+        else:
+            # the step's loss comes out of this call's finish kernel (the priors' sums and the other ELBO terms)
+            asm, jobs, n_jobs, jc, ptrs, tc, n_terms, _keep = asm
+            loss = torch.empty((), dtype=torch.float32, device=dev)
+            sc = N.workspace(dev, int(N.lib().b2_glm_elbo_workspace()), tag="glm_elbo")
+            N.check(N.lib().b2_glm_bernoulli_logits_elbo(*args, jobs, n_jobs, jc, ptrs, tc, n_terms, loss.data_ptr(),
+                                                         sc.data_ptr(), sc.numel(), N.stream_ptr(dev)),
+                    "b2_glm_bernoulli_logits_elbo")
+            asm.loss, asm.total = loss, total
         ctx.grads = (dW, db if b is not None else None)
         ctx.unit = unit
         return total
@@ -1159,9 +1172,9 @@ class ClassLinearPredictor:
 
     def __init__(self, X, Wt, b=None, linear=False, linear_bias=False):
         if type(Wt).__name__ == "SiteValue":
-            Wt = Wt.as_subclass(torch.Tensor)
+            Wt = _ops.plain_value(Wt)
         if type(b).__name__ == "SiteValue":
-            b = b.as_subclass(torch.Tensor)
+            b = _ops.plain_value(b)
         self.X, self.Wt, self.b = X, Wt, b
         self.linear, self.linear_bias = linear, linear_bias
         self.vectorised = Wt.dim() == 3
@@ -1206,7 +1219,7 @@ def class_linear_predictor(X, W, b=None):
     lp = ClassLinearPredictor(X, W.mT)
     if b is None:
         return lp
-    out = lp.with_bias(b.as_subclass(torch.Tensor) if type(b).__name__ == "SiteValue" else b)
+    out = lp.with_bias(_ops.plain_value(b) if type(b).__name__ == "SiteValue" else b)
     if out is None:
         raise ValueError("class_linear_predictor: the bias must be [K]%s of X's dtype and device, got %s"
                          % (" or [P, 1, K]" if lp.vectorised else "", tuple(getattr(b, "shape", ()))))
@@ -1312,9 +1325,9 @@ class FactorProduct:
 
     def __init__(self, A, B, bmm=False):
         if type(A).__name__ == "SiteValue":
-            A = A.as_subclass(torch.Tensor)
+            A = _ops.plain_value(A)
         if type(B).__name__ == "SiteValue":
-            B = B.as_subclass(torch.Tensor)
+            B = _ops.plain_value(B)
         if not (isinstance(A, torch.Tensor) and isinstance(B, torch.Tensor) and A.dim() == B.dim()
                 and A.dim() in (2, 3) and B.shape[-2] == A.shape[-1] and A.shape[:-2] == B.shape[:-2]
                 and A.dtype == B.dtype and A.device == B.device):

@@ -366,13 +366,13 @@ _RNG_STATE = {}
 
 
 def rng_state(device):
-    """Per-device {seed, launch counter} of the in-kernel Philox draws, seeded from torch's current seed
+    """Per-device {seed, launch counter, ticket} of the in-kernel Philox draws, seeded from torch's current seed
     on first use (``pyro_b200.set_rng_seed`` / ``torch.manual_seed`` before the first draw selects the
-    stream).  The kernels advance the counter themselves."""
+    stream).  The kernels advance the counter themselves (the ticket is the draw kernel's, left zero)."""
     key = (device.type, device.index)
     st = _RNG_STATE.get(key)
     if st is None:
-        st = torch.tensor([torch.initial_seed() & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64, device=device)
+        st = torch.tensor([torch.initial_seed() & 0x7FFFFFFFFFFFFFFF, 0, 0], dtype=torch.int64, device=device)
         _RNG_STATE[key] = st
     return st
 
@@ -380,7 +380,7 @@ def rng_state(device):
 def reseed(seed):
     """Restart the in-kernel Philox streams (called by ``pyro_b200.set_rng_seed``)."""
     for st in _RNG_STATE.values():
-        st.copy_(torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF, 0], dtype=torch.int64))
+        st.copy_(torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF, 0, 0], dtype=torch.int64))
 
 
 def normal_rsample_philox(loc, scale, shape):
@@ -469,17 +469,93 @@ def _latent_job(shape, dtype, loc=None, scale=None, log_scale=False, prior=None,
 
 def latent_draw(loc, scale, log_scale, shape):
     """(z, lq, eps) of ONE Normal site: ``z = loc + eps*s`` with ``s = scale`` or ``exp(scale)`` (``log_scale``),
-    eps from the in-kernel Philox stream, and the 0-d ``sum log Normal(z | loc, s)`` (b2_latent_normal_draw)."""
+    eps from the in-kernel Philox stream, and the 0-d ``sum log Normal(z | loc, s)`` (b2_latent_normal_draw),
+    launched at once (with any draws still pending before it)."""
+    out = defer_latent_draw(loc, scale, log_scale, shape)
+    flush_draws()
+    return out
+
+
+def defer_latent_draw(loc, scale, log_scale, shape):
+    """:func:`latent_draw`, DEFERRED: the site joins the pending draws, which run as ONE launch (per 8 sites) at
+    :func:`flush_draws`.  The returned tensors are not written yet; the caller hands z and lq out only as
+    :class:`DeferredDraw` tensors, whose first read flushes, and eps is read by the draw's backward only."""
     shape = tuple(int(s) for s in shape)
     dev, dtype = loc.device, loc.dtype
     z = torch.empty(shape, dtype=dtype, device=dev)
     eps = torch.empty(shape, dtype=dtype, device=dev)
     lq = torch.empty((), dtype=dtype, device=dev)
-    jobs = (N.b2_latent_job * 1)(_latent_job(shape, dtype, loc=loc, scale=scale, log_scale=log_scale, z=z,
-                                             eps=eps, out0=lq))
-    N.check(N.lib().b2_latent_normal_draw(jobs, 1, rng_state(dev).data_ptr(), N.stream_ptr(dev)),
-            "b2_latent_normal_draw")
+    # the operands are read through pointers at the flush: building the job reads loc and scale through torch,
+    # which flushes any pending draw they come from first
+    job = _latent_job(shape, dtype, loc=loc, scale=scale, log_scale=log_scale, z=z, eps=eps, out0=lq)
+    _PENDING_DRAWS.append((job, (loc, scale, z, eps, lq), dev))
     return z, lq, eps
+
+
+# Draws registered by latent_draw and not launched yet: (job, tensors its pointers refer to, device).
+_PENDING_DRAWS = []
+
+
+def flush_draws():
+    """Launch every pending draw: one b2_latent_normal_draw per run of up to 8 sites of one device and dtype, in
+    the order they were drawn.  Job k of a launch uses the Philox counter the k-th one-job launch would have, so
+    the values equal those of separate launches bit for bit."""
+    global _PENDING_DRAWS
+    if not _PENDING_DRAWS:
+        return
+    pending, _PENDING_DRAWS = _PENDING_DRAWS, []
+    i = 0
+    while i < len(pending):
+        dev, dt = pending[i][2], pending[i][0].dtype
+        j = i
+        while j < len(pending) and j - i < N.LATENT_MAX_JOBS and pending[j][2] == dev and pending[j][0].dtype == dt:
+            j += 1
+        chunk = pending[i:j]
+        jobs = (N.b2_latent_job * len(chunk))(*[jb for jb, _, _ in chunk])
+        N.check(N.lib().b2_latent_normal_draw(jobs, len(chunk), rng_state(dev).data_ptr(), N.stream_ptr(dev)),
+                "b2_latent_normal_draw")
+        i = j
+
+
+# tensor queries that read no element: they leave the pending draws pending
+_NO_READ = {"size", "dim", "ndimension", "numel", "nelement", "__len__", "is_floating_point", "is_complex",
+            "element_size", "get_device", "is_contiguous", "stride", "storage_offset", "as_subclass", "shape",
+            "dtype", "device", "ndim", "layout", "is_cuda", "requires_grad", "grad_fn", "is_leaf", "names",
+            "requires_grad_"}
+
+
+def _func_name(func):
+    name = getattr(func, "__name__", None) or str(func)
+    if name == "__get__":
+        name = getattr(getattr(func, "__self__", None), "__name__", name)
+    return name
+
+
+def flush_before(func):
+    """Flush the pending draws unless ``func`` only asks for metadata."""
+    if _PENDING_DRAWS and _func_name(func) not in _NO_READ:
+        flush_draws()
+
+
+N.before_launch = flush_draws
+
+
+def plain_value(t):
+    """``t`` (a site value of a lazy-aware subclass) as a plain tensor, its pending draw launched first: the plain
+    alias no longer guards its reads."""
+    flush_draws()
+    return t.as_subclass(torch.Tensor)
+
+
+class DeferredDraw(torch.Tensor):
+    """The value (or 0-d score) of a deferred draw: any torch operation that can read it launches the pending
+    draws first, so an unwritten value can never be read; the result is a plain tensor."""
+
+    @classmethod
+    def __torch_function__(cls, func, types, args=(), kwargs=None):
+        flush_before(func)
+        with torch._C.DisableTorchFunctionSubclass():
+            return func(*args, **(kwargs or {}))
 
 
 def latent_prior(items):
@@ -520,6 +596,57 @@ def latent_prior_combine(items, item_coeffs, terms, term_coeffs):
     N.check(N.lib().b2_latent_normal_prior_combine(jobs, len(items), jc, ptrs, tc, n, out.data_ptr(),
                                                    N.stream_ptr(ref.device)), "b2_latent_normal_prior_combine")
     return out
+
+
+# Loss assembly handed to the likelihood call of a step's LAST model site: the fused Bernoulli GLM call computes
+# what latent_prior_combine(items, item_coeffs, terms + [its own total], term_coeffs + [own_coeff]) would, in its
+# finish kernel (b2_glm_bernoulli_logits_elbo), which saves that launch.  Trace_ELBO opens it around the site's
+# scoring; the first GLM call inside takes it and sets ``loss``; if none does, ``loss`` stays None.
+_ELBO_ASSEMBLY = None
+
+
+class elbo_assembly:
+    def __init__(self, items, item_coeffs, terms, term_coeffs, own_coeff):
+        self.items, self.item_coeffs = items, item_coeffs
+        self.terms, self.term_coeffs, self.own_coeff = terms, term_coeffs, own_coeff
+        self.loss = self.total = None
+
+    def __enter__(self):
+        global _ELBO_ASSEMBLY
+        self._prev, _ELBO_ASSEMBLY = _ELBO_ASSEMBLY, self
+        return self
+
+    def __exit__(self, *exc):
+        global _ELBO_ASSEMBLY
+        _ELBO_ASSEMBLY = self._prev
+        return False
+
+
+def take_elbo_assembly(device):
+    """The open assembly as the ctypes arguments of b2_glm_bernoulli_logits_elbo, ``(asm, jobs, n_jobs, job_coeffs,
+    terms, term_coeffs, n_terms, keep)``, or None when there is none or it does not fit one finish kernel (the
+    limits of latent_prior_combine, fp32 on ``device``).  Taking it closes it for any later call."""
+    global _ELBO_ASSEMBLY
+    asm, _ELBO_ASSEMBLY = _ELBO_ASSEMBLY, None
+    if asm is None:
+        return None
+    items, terms = asm.items, asm.terms
+    if (not items or len(items) > N.LATENT_MAX_JOBS or len(terms) + 1 > N.LATENT_MAX_TERMS
+            or sum(z.numel() for z, _, _ in items) > N.LATENT_COMBINE_MAX_N
+            or any(z.dtype != torch.float32 or z.device != device for z, _, _ in items)
+            or any(t.dtype != torch.float32 or t.device != device for t in terms)):
+        return None
+    jobs = (N.b2_latent_job * len(items))()
+    keep = []
+    for k, (z, ploc, pscale) in enumerate(items):
+        zc = z if z.is_contiguous() else z.contiguous()
+        keep.append(zc)
+        jobs[k] = _latent_job(tuple(z.shape), z.dtype, prior=(ploc, pscale), z=zc)
+    jc = (ctypes.c_double * len(items))(*[float(c) for c in asm.item_coeffs])
+    n = len(terms) + 1
+    ptrs = (ctypes.c_void_p * n)(*([t.data_ptr() for t in terms] + [None]))
+    tc = (ctypes.c_double * n)(*([float(c) for c in asm.term_coeffs] + [float(asm.own_coeff)]))
+    return asm, jobs, len(items), jc, ptrs, tc, n, keep
 
 
 # Deferred draw-backwards: inside `deferred_latent_backward()` (Trace_ELBO wraps its autograd.backward call in it)

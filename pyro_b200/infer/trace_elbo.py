@@ -142,24 +142,36 @@ class Trace_ELBO(ELBO):
         for name, site in guide_trace.nodes.items():
             if site["type"] == "sample":
                 add_site(site, -1.0)
-        priors, prior_coeffs = [], []
-        for name, site in model_trace.nodes.items():
-            if site["type"] == "sample":
-                job = None
-                if (not site["is_observed"] and (site["mask"] is None or site["mask"] is True)
-                        and not site["args"] and not site["kwargs"]
-                        and not isinstance(site["scale"], torch.Tensor)):
-                    # Normal prior on a fused draw: value-only scoring now (batched below), its d/dz inside
-                    # the draw's backward kernel
-                    from ..distributions import claim_rsample_prior
-                    sc = float(site["scale"])
-                    job = claim_rsample_prior(site["fn"], site["value"], -sc / P)
-                    if job is not None:
-                        priors.append(job)
-                        prior_coeffs.append(sc)
-                if job is None:
-                    add_site(site, 1.0)
         from ..distributions import _ops
+        priors, prior_coeffs = [], []
+        model_sites = [site for site in model_trace.nodes.values() if site["type"] == "sample"]
+        for i, site in enumerate(model_sites):
+            job = None
+            if (not site["is_observed"] and (site["mask"] is None or site["mask"] is True)
+                    and not site["args"] and not site["kwargs"]
+                    and not isinstance(site["scale"], torch.Tensor)):
+                # Normal prior on a fused draw: value-only scoring now (batched below), its d/dz inside
+                # the draw's backward kernel
+                from ..distributions import claim_rsample_prior
+                sc = float(site["scale"])
+                job = claim_rsample_prior(site["fn"], site["value"], -sc / P)
+                if job is not None:
+                    priors.append(job)
+                    prior_coeffs.append(sc)
+            if job is None:
+                if priors and i == len(model_sites) - 1:
+                    # the last site to score: a fused likelihood call can assemble the loss in its own
+                    # finish kernel (the priors' sums, the parts so far, then its own term)
+                    with _ops.elbo_assembly(priors, [-c / P for c in prior_coeffs], list(parts),
+                                            [-c / P for c in coeffs], -1.0 / P) as asm:
+                        add_site(site, 1.0)
+                    # the assembly's last term is the GLM call's own total with coefficient -1/P: valid only when
+                    # that total is the part this site added, with coefficient 1, which is checked here
+                    if (asm.loss is not None and coeffs and coeffs[-1] == 1.0
+                            and parts[-1].data_ptr() == asm.total.data_ptr()):
+                        return asm.loss, terms
+                else:
+                    add_site(site, 1.0)
         if priors:
             # the priors' value-only sums and the assembly of the loss in one launch when the sites are small
             loss = _ops.latent_prior_combine(priors, [-c / P for c in prior_coeffs], parts, [-c / P for c in coeffs])
@@ -183,11 +195,12 @@ class Trace_ELBO(ELBO):
                         for site in trace.nodes.values())
         if _all_reparam(guide_trace):
             loss_particle, terms = self._fused_particle(model_trace, guide_trace)
+            from ..distributions import _ops as _o
+            _o.flush_draws()    # a draw nothing has read yet still runs inside this step
             if trainable and terms:
                 # every term's upstream gradient is exactly 1 (contract of the fused nodes);
                 # pass one cached ones-scalar instead of letting autograd fill a new one per term
                 ones = [_one_like(t) for t in terms]
-                from ..distributions import _ops as _o
                 with _o.deferred_latent_backward():
                     torch.autograd.backward(terms, ones, retain_graph=self.retain_graph)
             return loss_particle

@@ -35,7 +35,7 @@ guide value of pyro/poutine/replay_messenger.py:50-61); nothing in the model is 
 import torch
 
 from ._lazyparam import LazyExpParam
-from .distributions import ClassLinearPredictor, ExpLinearPredictor, FactorProduct, LinearPredictor
+from .distributions import ClassLinearPredictor, ExpLinearPredictor, FactorProduct, LinearPredictor, _ops
 
 _VIEW_FUNCS = {"squeeze", "unsqueeze", "reshape", "view", "transpose", "t", "permute", "expand",
                "expand_as", "flatten", "contiguous", "__getitem__", "movedim", "swapaxes", "detach_",
@@ -62,6 +62,7 @@ def _plain(x):
     if isinstance(x, (LinearPredictorTensor, LazyExpParam)):
         return x.dense()
     if isinstance(x, SiteValue):
+        # inside SiteValue.__torch_function__: a reading operation has flushed the pending draws already
         return x.as_subclass(torch.Tensor)
     if isinstance(x, (list, tuple)):
         return type(x)(_plain(v) for v in x)
@@ -107,6 +108,7 @@ class SiteValue(torch.Tensor):
     @classmethod
     def __torch_function__(cls, func, types, args=(), kwargs=None):
         kwargs = kwargs or {}
+        _ops.flush_before(func)     # a site value may be a deferred draw (distributions/_ops.py)
         name = _name(func)
         if name == "__get__":
             # a property such as ``W.mT``: name it after the attribute, so a transposed view stays a SiteValue
@@ -229,8 +231,8 @@ def _make_class(X, Wt, b, linear=False):
 
 
 def _make(X, w, b):
-    wp = w.as_subclass(torch.Tensor) if isinstance(w, SiteValue) else w
-    bp = b.as_subclass(torch.Tensor) if isinstance(b, SiteValue) else b
+    wp = _ops.plain_value(w) if isinstance(w, SiteValue) else w
+    bp = _ops.plain_value(b) if isinstance(b, SiteValue) else b
     return LinearPredictorTensor(LinearPredictor(X, wp, bp))
 
 
@@ -272,7 +274,7 @@ class LinearPredictorTensor(torch.Tensor):
         if isinstance(lz, ClassLinearPredictor):
             if isinstance(b, LinearPredictorTensor):
                 return None
-            out = lz.with_bias(b.as_subclass(torch.Tensor) if isinstance(b, SiteValue) else b)
+            out = lz.with_bias(_ops.plain_value(b) if isinstance(b, SiteValue) else b)
             return None if out is None else LinearPredictorTensor(out)
         if lz.b is not None:
             return None
@@ -280,7 +282,7 @@ class LinearPredictorTensor(torch.Tensor):
             return None
         if not isinstance(b, torch.Tensor) or isinstance(b, LinearPredictorTensor):
             return None
-        bp = b.as_subclass(torch.Tensor) if isinstance(b, SiteValue) else b
+        bp = _ops.plain_value(b) if isinstance(b, SiteValue) else b
         # per-particle scalar: [], [1], [P], [P, 1]
         ok = bp.numel() == 1 or (lz.vectorised and bp.numel() == lz.P and
                                  tuple(bp.shape) in ((lz.P,), (lz.P, 1)) and
@@ -369,7 +371,7 @@ def unwrap_site_values(*traces):
                 v = site.get("value")
                 if isinstance(v, SiteValue):
                     plain = getattr(v, "_b2_plain", None)
-                    site["value"] = plain if plain is not None else v.as_subclass(torch.Tensor)
+                    site["value"] = plain if plain is not None else _ops.plain_value(v)
 
 
 def lazy_of(logits):
