@@ -364,6 +364,35 @@ int b2_glm_poisson_log_rate(const float* X, const float* y, const float* W, cons
 size_t b2_glm_poisson_workspace(int64_t N, int D, int P);
 
 /*
+ * b2_glm_normal_loc -- fused linear-regression (Gaussian likelihood) term: for P particles,
+ * l[p,n] = <X[n,:], W[p,:]> + b[p] is the mean, sigma[p * sigma_stride] the noise scale, r = y - l:
+ *   sum_p[p]  = SUM_n log Normal(y[n] | l[p,n], sigma_p)
+ *             = -S_p / (2 sigma_p^2) - N (log sigma_p + log(2 pi) / 2),     S_p = SUM_n r[p,n]^2
+ *   dW[p,:]   = weight * SUM_n r[p,n] X[n,:] / sigma_p^2,   db[p] = weight * SUM_n r[p,n] / sigma_p^2
+ *   dsigma[p] = weight * (S_p / sigma_p^3 - N / sigma_p)
+ * (scale multiplies every output, as for b2_glm_bernoulli_logits).  X and y are read from HBM about once for value
+ * AND gradient, and no [P,N] tensor is written.  X: [N,D] row-major fp32, 1 <= D <= 128; W: [P,D]; b: [P]
+ * (nullable); y: [N] fp32; sigma: device pointer to 1 (sigma_stride 0) or P (sigma_stride 1) positive fp32
+ * values.  X and y must be 16-byte aligned and N < 2^31.  The tile kernel (glm_normal_tc.cu: D == 32 on the TMA
+ * tile pipeline of glm_tc.cu, every other D on the bulk-copy tile loop of glm_flat_tc.cu) accumulates S and
+ * SUM r [x | 1] with W AND X split hi + lo (every mean fp32-exact up to the tensor cores' accumulation; g = r
+ * rounded to nearest TF32 for the gradient contraction), so B2_FLAG_GLM_3XTF32 changes nothing; the finish kernel
+ * applies sigma in fp64.  There is no fp32 SIMT kernel: B2_FLAG_GLM_FP32 returns B2_ERR_BAD_SHAPE.  A null X, y, W
+ * or sigma returns B2_ERR_NULL; N <= 0, P <= 0, D outside 1..128, a sigma_stride other than 0 or 1 or a
+ * misaligned X or y B2_ERR_BAD_SHAPE; N >= 2^31 B2_ERR_TOO_LARGE; all before any CUDA call.
+ * out_sum_p, out_dW, out_db, out_dsigma ([P]) and out_total are nullable; out_total: scalar, (=|+=) sum_coeff *
+ * SUM_p sum_p[p].
+ * workspace: b2_glm_normal_workspace() bytes, zero-initialised ONCE by the caller (its first 256 bytes hold a
+ * ticket counter that the library leaves zeroed).  Two launches: the streaming kernel and the finish kernel of
+ * b2_glm_bernoulli_logits, which sums the CTA partials in a fixed order (deterministic, no float atomics).
+ */
+int b2_glm_normal_loc(const float* X, const float* y, const float* W, const float* b, const float* sigma,
+                      int sigma_stride, int64_t N, int D, int P, double scale, double weight, double sum_coeff,
+                      int flags, float* out_sum_p, float* out_total, float* out_dW, float* out_db,
+                      float* out_dsigma, void* workspace, size_t workspace_bytes, void* stream);
+size_t b2_glm_normal_workspace(int64_t N, int D, int P);
+
+/*
  * b2_poisson_product -- fused Poisson matrix-factorisation likelihood term (the bottom layer of the sparse
  * gamma DEF, Gamma-Poisson NMF): for P particles with latent factors A[p] (N x K) and B[p] (K x J) and shared
  * counts x (N x J), rate[p,n,j] = SUM_k A[p,n,k] * B[p,k,j];
@@ -427,6 +456,31 @@ int b2_glm_potential(int kind, const float* X, const void* y, int64_t N, int D, 
                      const float* z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, double s_w,
                      double s_b, float* U, float* grad, void* workspace, size_t workspace_bytes,
                      void* stream);
+
+/*
+ * b2_glm_normal_potential -- HMC / NUTS potential energy and gradient of Bayesian linear regression for C chains,
+ * with the likelihood of every chain from one pass of b2_glm_normal_loc over X (the chains are its particles):
+ *   U[c] = -( SUM_n log Normal(y[n] | <X[n,:], w[c,:]> + b[c], sigma_c) + SUM_i log Normal(w[c,i]; 0, s_w)
+ *             + log Normal(b[c]; 0, s_b) + log p(sigma_c) + t_c ),       sigma_c = exp(t_c),  t_c = z[c, s_off]
+ *   grad[c,:] = dU / dz[c,:]
+ * z: [C, Dz] fp32 row-major chain state; w at columns w_off .. w_off + D - 1, b at b_off (only if has_bias), and
+ * for a latent noise scale its log at s_off (s_off < 0: the constant noise scale `sigma`, no column), Dz == D +
+ * has_bias + (s_off >= 0).  The prior of a latent sigma is s_prior: B2_SIGMA_HALFNORMAL (sp0 = scale),
+ * B2_SIGMA_HALFCAUCHY (sp0 = scale), B2_SIGMA_EXPONENTIAL (sp0 = rate) or B2_SIGMA_LOGNORMAL (sp0 = loc, sp1 =
+ * scale).  X: [N, D] fp32 row-major, 1 <= D <= 128; y: [N] fp32; both 16-byte aligned.  Any other shape, a
+ * non-positive scale or an unknown prior returns B2_ERR_BAD_SHAPE before any CUDA call.  Three launches (pack,
+ * kernel + finish of b2_glm_normal_loc, potential finish), no host sync; the prior terms and totals are fp64 in a
+ * fixed order.  workspace: b2_glm_normal_potential_workspace() bytes, zero-initialised once.
+ */
+#define B2_SIGMA_HALFNORMAL 1
+#define B2_SIGMA_HALFCAUCHY 2
+#define B2_SIGMA_EXPONENTIAL 3
+#define B2_SIGMA_LOGNORMAL 4
+int b2_glm_normal_potential(const float* X, const float* y, int64_t N, int D, int has_bias, const float* z,
+                            int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int64_t s_off, double s_w,
+                            double s_b, int s_prior, double sp0, double sp1, double sigma, float* U, float* grad,
+                            void* workspace, size_t workspace_bytes, void* stream);
+size_t b2_glm_normal_potential_workspace(int64_t N, int D, int64_t C);
 size_t b2_glm_potential_workspace(int kind, int64_t N, int D, int K, int64_t C);
 
 /* ---- optimisers --------------------------------------------------------------------------

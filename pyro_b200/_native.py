@@ -36,6 +36,7 @@ SITE_SMALL_N = 8192   # B2_SITE_SMALL_N: one-CTA kernel with fused stored-shape 
 DIRICHLET, CATEGORICAL, MVN_TRIL = 32, 33, 34
 MODEL_HIER_NORMAL, MODEL_LOGISTIC = 0, 1
 GLM_BERNOULLI, GLM_CATEGORICAL, GLM_POISSON = 0, 1, 2
+SIGMA_CONST, SIGMA_HALFNORMAL, SIGMA_HALFCAUCHY, SIGMA_EXPONENTIAL, SIGMA_LOGNORMAL = 0, 1, 2, 3, 4
 NUTS_SMALL_MAX_D = 64
 
 
@@ -123,6 +124,12 @@ SIGNATURES = {
     "b2_glm_poisson_log_rate": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _f64, _f64, _f64, _i32,
                                        _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2_glm_poisson_workspace": (_sz, [_i64, _i32, _i32]),
+    "b2_glm_normal_loc": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _f64, _f64, _f64, _i32,
+                                 _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "b2_glm_normal_workspace": (_sz, [_i64, _i32, _i32]),
+    "b2_glm_normal_potential": (_i32, [_vp, _vp, _i64, _i32, _i32, _vp, _i64, _i64, _i64, _i64, _i64, _f64, _f64,
+                                       _i32, _f64, _f64, _f64, _vp, _vp, _vp, _sz, _vp]),
+    "b2_glm_normal_potential_workspace": (_sz, [_i64, _i32, _i64]),
     "b2_poisson_product": (_i32, [_vp, _vp, _vp, _i64, _i32, _i64, _i32, _f64, _f64, _f64, _i32, _vp, _vp, _vp,
                                   _vp, _vp, _sz, _vp]),
     "b2_poisson_product_workspace": (_sz, [_i64, _i32, _i64, _i32]),

@@ -10,7 +10,7 @@
 // fp32 SIMT kernel (D in {4, 8, 16}; at D = 32: N < 8192 rows, B2_FLAG_GLM_FP32, and operands the wgmma
 // kernel of glm_tc.cu cannot load; every other D in 1..128 takes the wgmma kernel of glm_flat_tc.cu).
 // glm_finish_kernel below is the second launch of every GLM likelihood call, Bernoulli, softmax
-// (b2_glm_categorical_logits) and Poisson (b2_glm_poisson_log_rate).  CTA = 256 threads = 4 row groups x 64
+// (b2_glm_categorical_logits), Poisson (b2_glm_poisson_log_rate) and Normal (b2_glm_normal_loc).  CTA = 256 threads = 4 row groups x 64
 // particles.  Each thread keeps W[p,:] and its dW[p,:] accumulator in registers; X tiles are staged through shared memory
 // with cp.async double buffering and read back as warp-wide broadcasts (every lane of a warp has a
 // different particle but the same row, so an LDS.128 serves 4 FMAs x 2 uses for all 32 lanes).
@@ -155,8 +155,11 @@ struct GlmElbo {
 };
 
 // second stage: fixed-order sum over the CTAs' partials [nblocks][P][K (D + 1) + 1] (per class dW[0..D-1]
-// and db, then the particle's lp sum; K = 1 for Bernoulli and Poisson); applies weight / scale.  lg (Poisson
-// only, else null) holds one more partial per CTA, of a term every particle's sum subtracts: SUM lgamma(y + 1).
+// and db, then the particle's lp sum; K = 1 for Bernoulli, Poisson and Normal); applies weight / scale.  lg
+// (Poisson only, else null) holds one more partial per CTA, of a term every particle's sum subtracts: SUM
+// lgamma(y + 1).  sigma (Normal only, else null; sigma[p * sigma_stride] for particle p) turns the sufficient
+// statistics of the Normal tile kernel into the lp sum and gradients: the lp slot holds S = SUM (y - l)^2 and
+// dW / db hold SUM (y - l) [x | 1]; the warp of sum_p[p] also writes out_dsigma[p] (nullable), n is N.
 // One WARP per entry of the [P, K (D + 1) + 1] table: lanes stride over the CTAs (L2-resident partials),
 // then a shuffle tree (a thread-per-entry loop is a chain of ~300 dependent loads).  With E, E->n_jobs *
 // E->nwarps more warps score the priors, and the ticket counts them too.
@@ -165,7 +168,8 @@ __device__ __forceinline__ void glm_finish_body(const float* __restrict__ partia
                                                 float* __restrict__ out_dW, float* __restrict__ out_db,
                                                 double sum_coeff, int flags, float* __restrict__ out_total,
                                                 unsigned int* __restrict__ ticket, const float* __restrict__ lg,
-                                                const GlmElbo* E) {
+                                                const float* __restrict__ sigma, int sigma_stride, int64_t n,
+                                                float* __restrict__ out_dsigma, const GlmElbo* E) {
   pdl_enter();
   const int S = K * (D + 1) + 1;
   const int total = P * S;
@@ -200,6 +204,10 @@ __device__ __forceinline__ void glm_finish_body(const float* __restrict__ partia
     if (r < K * (D + 1)) {
       const int k = r / (D + 1), c = r - k * (D + 1);
       if (lane == 0) {
+        if (sigma) {                           // Normal: SUM r x / sigma^2
+          const double sg = (double)sigma[(int64_t)p * sigma_stride];
+          s *= 1.0 / (sg * sg);
+        }
         if (c < D) {
           if (out_dW) out_dW[((int64_t)p * K + k) * D + c] = (float)(weight * scale * s);
         } else if (out_db) {
@@ -212,6 +220,13 @@ __device__ __forceinline__ void glm_finish_body(const float* __restrict__ partia
       double l = 0.0;
       for (int bl = lane; bl < nblocks; bl += 32) l += (double)lg[bl];
       s -= warp_sum(l);
+    }
+    if (sigma) {
+      // Normal: s is S = SUM (y - l)^2; lp sum = -S / (2 sigma^2) - n (log sigma + log(2 pi) / 2) and
+      // d/dsigma = S / sigma^3 - n / sigma, all in fp64
+      const double sg = (double)sigma[(int64_t)p * sigma_stride], S = s, nn = (double)n;
+      s = -S / (2.0 * sg * sg) - nn * (log(sg) + 0.91893853320467274178);
+      if (lane == 0 && out_dsigma) out_dsigma[p] = (float)(weight * scale * (S / (sg * sg * sg) - nn / sg));
     }
     // per-particle sum; the LAST of the P warps (and prior warps) to get here also totals them (fixed order),
     // with the ELBO coefficient -- a ticket instead of a third launch
@@ -257,9 +272,11 @@ __global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict
                                                          float* __restrict__ out_db, double sum_coeff, int flags,
                                                          float* __restrict__ out_total,
                                                          unsigned int* __restrict__ ticket,
-                                                         const float* __restrict__ lg) {
+                                                         const float* __restrict__ lg,
+                                                         const float* __restrict__ sigma, int sigma_stride,
+                                                         int64_t n, float* __restrict__ out_dsigma) {
   glm_finish_body(partials, nblocks, P, K, D, scale, weight, sum_p, out_dW, out_db, sum_coeff, flags, out_total,
-                  ticket, lg, nullptr);
+                  ticket, lg, sigma, sigma_stride, n, out_dsigma, nullptr);
 }
 
 __global__ void __launch_bounds__(256) glm_finish_elbo_kernel(const float* __restrict__ partials, int nblocks, int P,
@@ -269,7 +286,7 @@ __global__ void __launch_bounds__(256) glm_finish_elbo_kernel(const float* __res
                                                               int flags, float* __restrict__ out_total,
                                                               unsigned int* __restrict__ ticket, const GlmElbo E) {
   glm_finish_body(partials, nblocks, P, K, D, scale, weight, sum_p, out_dW, out_db, sum_coeff, flags, out_total,
-                  ticket, nullptr, &E);
+                  ticket, nullptr, nullptr, 0, 0, nullptr, &E);
 }
 
 // The second launch of b2_glm_bernoulli_logits, b2_glm_categorical_logits and b2_glm_poisson_log_rate.  The
@@ -283,7 +300,20 @@ void launch_glm_finish(const float* partials, unsigned int* ticket, int gx, int 
                        float* out_dW, float* out_db, const float* lg, cudaStream_t s) {
   const int total = P * (K * (D + 1) + 1);
   launch_pdl(glm_finish_kernel, dim3((total + 7) / 8), dim3(256), 0, s, partials, gx, P, K, D, scale, weight,
-             glm_sum_p(partials, out_sum_p, gx, total), out_dW, out_db, sum_coeff, flags, out_total, ticket, lg);
+             glm_sum_p(partials, out_sum_p, gx, total), out_dW, out_db, sum_coeff, flags, out_total, ticket, lg,
+             nullptr, 0, (int64_t)0, nullptr);
+}
+
+// The second launch of b2_glm_normal_loc: the finish above with the noise scale sigma[p * sigma_stride] of
+// every particle applied to the sufficient statistics of the tile kernel (glm_normal_tc.cu).
+void launch_glm_normal_finish(const float* partials, unsigned int* ticket, int gx, int P, int D, int64_t N,
+                              double scale, double weight, double sum_coeff, int flags, float* out_sum_p,
+                              float* out_total, float* out_dW, float* out_db, const float* sigma,
+                              int sigma_stride, float* out_dsigma, cudaStream_t s) {
+  const int total = P * (D + 2);
+  launch_pdl(glm_finish_kernel, dim3((total + 7) / 8), dim3(256), 0, s, partials, gx, P, 1, D, scale, weight,
+             glm_sum_p(partials, out_sum_p, gx, total), out_dW, out_db, sum_coeff, flags, out_total, ticket,
+             (const float*)nullptr, sigma, sigma_stride, N, out_dsigma);
 }
 
 // wgmma + TMA variant (glm_tc.cu)

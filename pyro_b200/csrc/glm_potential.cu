@@ -1,5 +1,5 @@
-// glm_potential.cu -- HMC / NUTS potential energy of Bayesian logistic, softmax and Poisson regression for C
-// chains.
+// glm_potential.cu -- HMC / NUTS potential energy of Bayesian logistic, softmax, Poisson and linear regression
+// for C chains.
 //
 //   U[c]    = -( SUM_n log p(y_n | logits_cn) + SUM log Normal(w; 0, s_w) + SUM log Normal(b; 0, s_b) )
 //   grad[c] = dU / dz[c]                                           (in z's layout)
@@ -16,18 +16,25 @@
 //                                   accumulation in a fixed order, and writes U and grad
 // The GLM kernels always run with B2_FLAG_GLM_3XTF32 here: every logit is fp32-exact, so the sampler
 // targets the posterior of the data as given, not of X rounded to TF32.
+// Linear regression (b2_glm_normal_potential) runs the same three launches around b2_glm_normal_loc: the pack also
+// writes each chain's noise scale sigma_c = exp(z[c, s_off]) (or the constant), and the finish adds sigma's prior
+// and the Jacobian of sigma = e^t in fp64.
 #include <math.h>
 
 #include "b2_common.cuh"
 
 namespace b2 {
 
+// sig (linear regression only, else null): sig[c] = exp(z[c, s_off]) for a latent noise scale (z holds its log),
+// the constant s_const when s_off < 0
 __global__ void __launch_bounds__(256) glm_potential_pack_kernel(const float* __restrict__ z, int64_t C,
                                                                  int64_t Dz, int64_t w_off, int64_t b_off,
                                                                  int KD, int Kb, float* __restrict__ Wp,
-                                                                 float* __restrict__ bp) {
+                                                                 float* __restrict__ bp, int64_t s_off,
+                                                                 float s_const, float* __restrict__ sig) {
   const int64_t per = KD + Kb;
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (sig != nullptr && i < C) sig[i] = s_off >= 0 ? expf(z[i * Dz + s_off]) : s_const;
   if (i >= C * per) return;
   const int64_t c = i / per;
   const int64_t j = i - c * per;
@@ -38,7 +45,8 @@ __global__ void __launch_bounds__(256) glm_potential_pack_kernel(const float* __
 __global__ void __launch_bounds__(256) glm_potential_finish_kernel(
     const float* __restrict__ z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int KD, int Kb, double s_w,
     double s_b, const float* __restrict__ sum_p, const float* __restrict__ dW, const float* __restrict__ db,
-    float* __restrict__ U, float* __restrict__ grad) {
+    float* __restrict__ U, float* __restrict__ grad, const float* __restrict__ sig, const float* __restrict__ dsig,
+    int64_t s_off, int s_prior, double sp0, double sp1) {
   const int64_t c = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (c >= C) return;
@@ -63,6 +71,29 @@ __global__ void __launch_bounds__(256) glm_potential_finish_kernel(
     constexpr double kHalfLog2Pi = 0.91893853320467274178;
     double u = -(double)sum_p[c] + 0.5 * qw + (double)KD * (log(s_w) + kHalfLog2Pi);
     if (Kb) u += 0.5 * qb + (double)Kb * (log(s_b) + kHalfLog2Pi);
+    if (sig != nullptr && s_off >= 0) {
+      // a latent noise scale v = e^t, t = z[c, s_off]: U += -log p(v) - t (the Jacobian of v = e^t), and
+      // dU/dt = v (dU/dv) - 1 with dU/dv = dsig (the likelihood's, already negated) - d log p(v) / dv
+      constexpr double kLog2 = 0.69314718055994531, kLogPi = 1.14472988584940017;
+      const double t = (double)zc[s_off], v = (double)sig[c];
+      double lp = 0.0, dlp = 0.0;
+      if (s_prior == B2_SIGMA_HALFNORMAL) {             // sp0 = scale
+        lp = kLog2 - log(sp0) - kHalfLog2Pi - v * v / (2.0 * sp0 * sp0);
+        dlp = -v / (sp0 * sp0);
+      } else if (s_prior == B2_SIGMA_HALFCAUCHY) {      // sp0 = scale
+        lp = kLog2 - kLogPi - log(sp0) - log1p(v * v / (sp0 * sp0));
+        dlp = -2.0 * v / (sp0 * sp0 + v * v);
+      } else if (s_prior == B2_SIGMA_EXPONENTIAL) {     // sp0 = rate
+        lp = log(sp0) - sp0 * v;
+        dlp = -sp0;
+      } else {                                          // B2_SIGMA_LOGNORMAL: sp0 = loc, sp1 = scale
+        const double lv = log(v), q = (lv - sp0) / sp1;
+        lp = -lv - log(sp1) - kHalfLog2Pi - 0.5 * q * q;
+        dlp = -1.0 / v - q / (sp1 * v);
+      }
+      u += -lp - t;
+      gc[s_off] = (float)(v * ((double)dsig[c] - dlp) - 1.0);
+    }
     U[c] = (float)u;
   }
 }
@@ -130,7 +161,8 @@ extern "C" int b2_glm_potential(int kind, const float* X, const void* y, int64_t
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
 
   const int64_t npack = C * (KD + Kb);
-  glm_potential_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, Wp, bp);
+  glm_potential_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, Wp, bp,
+                                                                             (int64_t)-1, 0.f, nullptr);
   count_launch(1);
   int rc = check_launch();
   if (rc != 0) return rc;
@@ -146,7 +178,85 @@ extern "C" int b2_glm_potential(int kind, const float* X, const void* y, int64_t
                                    B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws + L.glm, glm_bytes, stream);
   if (rc != 0) return rc;
   glm_potential_finish_kernel<<<(unsigned)((C * 32 + 255) / 256), 256, 0, s>>>(
-      z, C, Dz, w_off, b_off, KD, Kb, s_w, s_b, sum_p, dW, db, U, grad);
+      z, C, Dz, w_off, b_off, KD, Kb, s_w, s_b, sum_p, dW, db, U, grad, nullptr, nullptr, (int64_t)-1, 0, 0.0, 0.0);
+  count_launch(1);
+  return check_launch();
+}
+
+// ---- linear regression: Normal(X @ w + b, sigma), sigma constant or latent with a positive-support prior ----
+// workspace areas, each 256-byte aligned: [b2_glm_normal_loc workspace][Wp][bp][dW][db][sum_p][sig][dsig]
+struct GlmNormalPotentialLayout {
+  size_t wp, bp, dw, db, sum_p, sig, dsig, total;
+};
+
+inline GlmNormalPotentialLayout glm_normal_potential_layout(int64_t N, int D, int64_t C) {
+  GlmNormalPotentialLayout L;
+  const size_t c = (size_t)C;
+  size_t off = round256(b2_glm_normal_workspace(N, D, (int)C));
+  L.wp = off; off += round256(c * D * sizeof(float));
+  L.bp = off; off += round256(c * sizeof(float));
+  L.dw = off; off += round256(c * D * sizeof(float));
+  L.db = off; off += round256(c * sizeof(float));
+  L.sum_p = off; off += round256(c * sizeof(float));
+  L.sig = off; off += round256(c * sizeof(float));
+  L.dsig = off; off += round256(c * sizeof(float));
+  L.total = off;
+  return L;
+}
+
+extern "C" size_t b2_glm_normal_potential_workspace(int64_t N, int D, int64_t C) {
+  if (N < 1 || D < 1 || D > 128 || C < 1 || C >= ((int64_t)1 << 31)) return 256;
+  return glm_normal_potential_layout(N, D, C).total;
+}
+
+extern "C" int b2_glm_normal_potential(const float* X, const float* y, int64_t N, int D, int has_bias,
+                                       const float* z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off,
+                                       int64_t s_off, double s_w, double s_b, int s_prior, double sp0, double sp1,
+                                       double sigma, float* U, float* grad, void* workspace, size_t workspace_bytes,
+                                       void* stream) {
+  if (!X || !y || !z || !U || !grad) return B2_ERR_NULL;
+  if (N < 1 || D < 1 || D > 128 || C < 1 || C >= ((int64_t)1 << 31)) return B2_ERR_BAD_SHAPE;
+  const int Kb = has_bias ? 1 : 0, Ks = s_off >= 0 ? 1 : 0;
+  // z's row is exactly the weight block, the bias and log sigma, none overlapping another or out of the row
+  if (Dz != (int64_t)D + Kb + Ks || w_off < 0 || w_off + D > Dz) return B2_ERR_BAD_SHAPE;
+  if (has_bias && (b_off < 0 || b_off >= Dz || (b_off >= w_off && b_off < w_off + D))) return B2_ERR_BAD_SHAPE;
+  if (Ks && (s_off >= Dz || (s_off >= w_off && s_off < w_off + D) || (has_bias && s_off == b_off)))
+    return B2_ERR_BAD_SHAPE;
+  if (!(s_w > 0.0) || (has_bias && !(s_b > 0.0))) return B2_ERR_BAD_SHAPE;
+  if (Ks) {
+    if (s_prior == B2_SIGMA_LOGNORMAL ? !(sp1 > 0.0) || !(fabs(sp0) < INFINITY)
+        : (s_prior < B2_SIGMA_HALFNORMAL || s_prior > B2_SIGMA_EXPONENTIAL || !(sp0 > 0.0)))
+      return B2_ERR_BAD_SHAPE;
+  } else if (!(sigma > 0.0) || !((float)sigma > 0.f)) {
+    return B2_ERR_BAD_SHAPE;
+  }
+  if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
+  const GlmNormalPotentialLayout L = glm_normal_potential_layout(N, D, C);
+  if (!workspace || workspace_bytes < L.total) return B2_ERR_WORKSPACE;
+  char* ws = reinterpret_cast<char*>(workspace);
+  float* Wp = reinterpret_cast<float*>(ws + L.wp);
+  float* bp = has_bias ? reinterpret_cast<float*>(ws + L.bp) : nullptr;
+  float* dW = reinterpret_cast<float*>(ws + L.dw);
+  float* db = has_bias ? reinterpret_cast<float*>(ws + L.db) : nullptr;
+  float* sum_p = reinterpret_cast<float*>(ws + L.sum_p);
+  float* sig = reinterpret_cast<float*>(ws + L.sig);
+  float* dsig = reinterpret_cast<float*>(ws + L.dsig);
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+
+  const int64_t npack = C * (D + Kb);
+  glm_potential_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(z, C, Dz, w_off, b_off, D, Kb, Wp, bp,
+                                                                             Ks ? s_off : (int64_t)-1,
+                                                                             (float)sigma, sig);
+  count_launch(1);
+  int rc = check_launch();
+  if (rc != 0) return rc;
+  // weight = -1: dW, db and dsig are derivatives of -loglik; X is always split (every mean fp32-exact)
+  rc = b2_glm_normal_loc(X, y, Wp, bp, sig, 1, N, D, (int)C, 1.0, -1.0, 1.0, 0, sum_p, nullptr, dW, db,
+                         Ks ? dsig : nullptr, ws, L.wp, stream);
+  if (rc != 0) return rc;
+  glm_potential_finish_kernel<<<(unsigned)((C * 32 + 255) / 256), 256, 0, s>>>(
+      z, C, Dz, w_off, b_off, D, Kb, s_w, s_b, sum_p, dW, db, U, grad, sig, dsig, Ks ? s_off : (int64_t)-1, s_prior,
+      sp0, sp1);
   count_launch(1);
   return check_launch();
 }

@@ -1,7 +1,7 @@
 // glm_tc_common.cuh -- device helpers shared by the Hopper wgmma kernels (glm_tc.cu, glm_flat_tc.cu,
-// glm_categorical_tc.cu, glm_poisson_tc.cu, poisson_product_tc.cu): mbarriers, TMA tile loads, SWIZZLE_128B
-// operand descriptors, the TF32 wgmma wrappers, MUFU wrappers and TF32 rounding, the Bernoulli and Poisson
-// epilogues and families, the stages of the GLM tile pipeline and the D = 32 pipeline itself, and the
+// glm_categorical_tc.cu, glm_poisson_tc.cu, glm_normal_tc.cu, poisson_product_tc.cu): mbarriers, TMA tile
+// loads, SWIZZLE_128B operand descriptors, the TF32 wgmma wrappers, MUFU wrappers and TF32 rounding, the
+// Bernoulli, Poisson and Normal epilogues and families, the stages of the GLM tile pipeline and the D = 32 pipeline itself, and the
 // host-side tensor-map encoders.
 #pragma once
 #include <cuda.h>
@@ -354,6 +354,33 @@ __device__ __forceinline__ void poisson_epilogue(const float (&acc1)[32], const 
   }
 }
 
+// ---- Normal epilogue of the linear-regression kernels (glm_normal_tc.cu) -----------------------------------
+// The residual r = y - l with l = acc1 + b (the bias added here, rounded to nearest, as in poisson_epilogue):
+// lpa accumulates the sufficient statistic S = SUM r^2 and g = r, rounded to nearest TF32, is GEMM 2's register
+// operand.  sigma never enters the tile loop: glm_finish_kernel applies it per particle in fp64, so the epilogue
+// takes no MUFU op at all.  MASK (the last, partial tile only) zeroes rows past N.
+template <bool MASK>
+__device__ __forceinline__ void normal_epilogue(const float (&acc1)[32], const float (&bias)[2],
+                                                const float2 (&yr)[8], int64_t row0, int64_t N, int t4,
+                                                float (&lpa)[2], uint32_t (&g)[32]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float s[2] = {0.f, 0.f};                    // two chains of adds (k-blocks j even / odd)
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int i = 4 * j + 2 * h + e;
+        const float yy = e ? yr[j].y : yr[j].x;
+        float r = yy - (acc1[i] + bias[h]);
+        if (MASK) r = (row0 + 8 * j + 2 * t4 + e < N) ? r : 0.f;
+        s[j & 1] = fmaf(r, r, s[j & 1]);
+        g[i] = __float_as_uint(tf32_rn(r));
+      }
+    lpa[h] += s[0] + s[1];
+  }
+}
+
 // ---- likelihood families of the GLM tile pipelines ----------------------------------------------------------
 // Fam is the likelihood family: kBiasInEpilogue (the bias is added by the epilogue, which then takes it after
 // acc1, instead of starting GEMM 1's accumulator), kKP (GEMM 1 rows per particle), kYBytes (labels of one
@@ -398,6 +425,25 @@ struct Poisson : Bernoulli {
       poisson_epilogue<true>(acc1, bias, y, row0, N, t4, lpa, g);
     else
       poisson_epilogue<false>(acc1, bias, y, row0, N, t4, lpa, g);
+  }
+  static __device__ __forceinline__ void epilogue(const float (&acc1)[32], const float (&bias)[2], const Labels& y,
+                                                  const int (&)[2], int, int64_t row0, int64_t N, int t4,
+                                                  float (&lpa)[2], uint32_t (&g)[32]) {
+    tile_epilogue(acc1, bias, y, row0, N, t4, row0 + kRows > N, lpa, g);
+  }
+};
+
+// linear regression (Gaussian likelihood): the labels of Bernoulli, fp32 y; lpa holds SUM (y - l)^2, not lp
+// (GEMM 1 starts from zero and the epilogue adds the bias, see normal_epilogue)
+struct Normal : Bernoulli {
+  static constexpr bool kBiasInEpilogue = true;
+  static __device__ __forceinline__ void tile_epilogue(const float (&acc1)[32], const float (&bias)[2],
+                                                       const Labels& y, int64_t row0, int64_t N, int t4, bool last,
+                                                       float (&lpa)[2], uint32_t (&g)[32]) {
+    if (last)
+      normal_epilogue<true>(acc1, bias, y, row0, N, t4, lpa, g);
+    else
+      normal_epilogue<false>(acc1, bias, y, row0, N, t4, lpa, g);
   }
   static __device__ __forceinline__ void epilogue(const float (&acc1)[32], const float (&bias)[2], const Labels& y,
                                                   const int (&)[2], int, int64_t row0, int64_t N, int t4,

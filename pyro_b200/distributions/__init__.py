@@ -1514,6 +1514,145 @@ def _poisson_new(cls, rate=None, validate_args=None, is_sparse=False):
 
 
 Poisson.__new__ = staticmethod(_poisson_new)
+
+
+# ---------------------------------------------------------------------------------------------
+# fused linear regression: Normal(loc = X @ w + b, scale = sigma)
+# ---------------------------------------------------------------------------------------------
+class _GlmNormalFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, meta, X, y, W, b, sigma):
+        scale, weight, coeff, unit, stride = meta
+        N.require_cuda(X, "fused linear-regression likelihood")
+        P, D = W.shape
+        n = X.shape[0]
+        dev = X.device
+        Wc = W.contiguous()
+        bc = b.contiguous() if b is not None else None
+        sc = sigma.contiguous()
+        total = torch.empty((), dtype=torch.float32, device=dev)
+        dW = torch.empty(P, D, dtype=torch.float32, device=dev)
+        db = torch.empty(P, dtype=torch.float32, device=dev)
+        dsig = torch.empty(P, dtype=torch.float32, device=dev) if sigma.requires_grad else None
+        need = int(N.lib().b2_glm_normal_workspace(n, D, P))
+        ws = N.workspace(dev, need, tag="glm")
+        N.check(N.lib().b2_glm_normal_loc(
+            X.data_ptr(), y.data_ptr(), Wc.data_ptr(), bc.data_ptr() if bc is not None else None, sc.data_ptr(),
+            stride, n, D, P, float(scale), float(weight), float(coeff), 0, None, total.data_ptr(), dW.data_ptr(),
+            db.data_ptr(), dsig.data_ptr() if dsig is not None else None, ws.data_ptr(), ws.numel(),
+            N.stream_ptr(dev)), "b2_glm_normal_loc")
+        if dsig is not None and stride == 0:
+            dsig = dsig.sum().reshape(sigma.shape)      # one sigma shared by every particle
+        ctx.grads = (dW, db if b is not None else None, dsig)
+        ctx.unit = unit
+        return total
+
+    @staticmethod
+    def backward(ctx, gout):
+        dW, db, dsig = ctx.grads
+        if not ctx.unit:
+            dW = dW * gout
+            db = db * gout if db is not None else None
+            dsig = dsig * gout if dsig is not None else None
+        return None, None, None, dW, db, dsig
+
+
+def _linear_loc_of(loc):
+    """The LinearPredictorTensor behind a Normal loc (a lazy ``X @ w + b``), or None."""
+    if type(loc).__name__ != "LinearPredictorTensor":
+        return None
+    return loc if isinstance(getattr(loc, "_lazy", None), LinearPredictor) else None
+
+
+def _per_particle_sigma(scale, lp):
+    """``(sigma, stride)``: the stored tensor of a Normal scale that is one value per particle -- a number,
+    ``[]``, ``[1]``, ``[P, 1]`` or a stride-0 expansion of one of these along N (as ``broadcast_all`` leaves it) --
+    flattened to 1 (stride 0) or P (stride 1) values; None for any other scale.  An expansion is replaced by its
+    base, never sliced: the backward of a slice would write a ``[P, N]`` zero tensor."""
+    s = densify(scale)
+    if type(s).__name__ == "SiteValue":
+        s = _ops.plain_value(s)
+    if not isinstance(s, torch.Tensor) or s.dtype != torch.float32 or s.device != lp.X.device:
+        return None
+    if s.dim() >= 1 and s.shape[-1] > 1 and s.stride(-1) == 0:
+        # the lazy broadcast_tensors of pyro_b200/lazy.py remembers what it expanded
+        # (or, for an expand of a tensor that is not itself a view, the autograd base); anything else, such as an
+        # expansion of a slice, whose base is the sliced tensor, is not one value per particle here
+        base = getattr(s, "_b2_unexpanded", None)
+        base = s._base if base is None else base
+        if base is None or base.dim() > s.dim() or base.data_ptr() != s.data_ptr():
+            return None
+        try:
+            if torch.broadcast_shapes(base.shape, s.shape) != s.shape:
+                return None
+        except RuntimeError:
+            return None
+        if base.expand(s.shape).stride() != s.stride():
+            return None
+        s = base
+    if s.numel() == 1 and s.dim() <= len(lp.shape):
+        return s.reshape(1), 0
+    if lp.vectorised and tuple(s.shape) == (lp.P, 1) and lp.P > 1:
+        return s.reshape(lp.P), 1
+    return None
+
+
+class _NormalLinear(Normal):
+    """Normal whose loc is a lazy ``X @ w + b`` (built by ``Normal(lazy, scale)`` when an unchanged model's linear
+    predictor was kept lazy by pyro_b200/lazy.py).  ``loc``, ``log_prob``, ``rsample`` and every other use
+    materialise the loc as the model wrote it, bit for bit; the ELBO's site sum takes the fused kernel
+    (``b2_glm_normal_loc``) when the scale is one value per particle."""
+
+    def __init__(self, loc, scale, validate_args=None):
+        _, sc = _broadcast_params(loc, scale)
+        self._loc_lazy = loc
+        self._scale = sc
+        self._dense = None
+        self._log_scale = sc.log_value if isinstance(sc, LazyExpParam) and sc.dtype == loc.dtype else None
+        Distribution.__init__(self, torch.broadcast_shapes(loc.shape, sc.shape))
+
+    @property
+    def _params(self):
+        if self._dense is None:
+            self._dense = self._loc_lazy.eager()
+        return [self._dense, self._scale]
+
+    @property
+    def loc(self):
+        return self._params[0]
+
+    @property
+    def scale(self):
+        return self._scale
+
+    def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
+        lp = self._loc_lazy.lazy
+        X = lp.X
+        D = X.shape[-1]
+        # the scope of the linear-regression kernel: tensor cores asked for, 1 <= D <= 128, from 8192 rows (below
+        # that the single-pass TF32 gradient has not averaged its rounding down to fp32 accuracy yet), fp32,
+        # contiguous 16-byte aligned X and y, no mask, one noise scale per particle
+        ok = (mask is None and X.dtype == torch.float32 and X.is_contiguous() and X.data_ptr() % 16 == 0
+              and 1 <= D <= 128 and getattr(lp, "tensor_cores", True) and X.shape[0] >= 8192
+              and isinstance(value, torch.Tensor) and value.numel() == X.shape[0]
+              and tuple(self.batch_shape) == tuple(lp.shape))
+        sig = _per_particle_sigma(self._scale, lp) if ok else None
+        y = value.reshape(-1).to(torch.float32).contiguous() if sig is not None else None
+        if sig is None or y.data_ptr() % 16 != 0:
+            return super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
+        W = lp.w.reshape(lp.P, D)
+        b = lp.b.reshape(lp.P) if lp.b is not None else None
+        return _GlmNormalFn.apply((scale, weight, sum_coeff, unit, sig[1]), X, y, W, b, sig[0])
+
+
+def _normal_new(cls, loc=None, scale=None, validate_args=None):
+    # ``Normal(lazy X @ w + b, scale)`` builds the fused linear-regression subclass
+    if cls is Normal and _linear_loc_of(loc) is not None:
+        return object.__new__(_NormalLinear)
+    return object.__new__(cls)
+
+
+Normal.__new__ = staticmethod(_normal_new)
 __all__ += ["LinearPredictor", "linear_predictor", "ExpLinearPredictor", "ClassLinearPredictor",
             "class_linear_predictor", "FactorProduct", "constant"]
 

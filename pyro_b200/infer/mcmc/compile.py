@@ -182,19 +182,44 @@ def _try_logistic(poutine, model, args, kwargs, latent, observed):
 
 
 def _try_glm(poutine, model, args, kwargs, latent, observed):
-    """Logistic regression with an intercept, or softmax or Poisson (log link) regression with or without one,
-    in fp32, within the GLM kernels' scope: Bernoulli D in {4, 8, 16, 32}; Categorical D == 32, 2 <= K <= 16;
-    Poisson 1 <= D <= 128."""
+    """Logistic regression with an intercept, or softmax, Poisson (log link) or linear regression with or without
+    one, in fp32, within the GLM kernels' scope: Bernoulli D in {4, 8, 16, 32}; Categorical D == 32, 2 <= K <= 16;
+    Poisson and Normal 1 <= D <= 128.  Linear regression's noise scale is a constant or one latent scalar site with
+    a constant-parameter HalfNormal, HalfCauchy, Exponential or LogNormal prior."""
     from .potential import GlmPotential
-    if len(observed) != 1 or len(latent) not in (1, 2):
+    if len(observed) != 1 or len(latent) not in (1, 2, 3):
         return None
     (obs_name, obs), = observed.items()
     _, kind = _base(obs["fn"])
     # lazy linear-predictor logits build _BernoulliLinear / _CategoricalLinear (pyro_b200/distributions)
-    # (and _PoissonLinear for a lazy exp of one)
+    # (and _PoissonLinear for a lazy exp of one, _NormalLinear for a lazy loc)
     kind = {"BernoulliLinear": "Bernoulli", "CategoricalLinear": "Categorical",
-            "PoissonLinear": "Poisson"}.get(kind, kind)
-    if kind not in ("Bernoulli", "Categorical", "Poisson") or not _plain_site(obs):
+            "PoissonLinear": "Poisson", "NormalLinear": "Normal"}.get(kind, kind)
+    if kind not in ("Bernoulli", "Categorical", "Poisson", "Normal") or not _plain_site(obs):
+        return None
+    # linear regression: at most one latent noise-scale site, positive support (z holds its log)
+    order = list(latent)                   # TracePotential's site order
+    sigma_site, sigma_prior, shapes_sigma = None, None, None
+    if kind == "Normal":
+        for name, site in latent.items():
+            fn, cls = _base(site["fn"])
+            if cls not in ("HalfNormal", "HalfCauchy", "Exponential", "LogNormal"):
+                continue
+            v = site["value"]
+            if sigma_site is not None or not _plain_site(site) or not isinstance(v, torch.Tensor) \
+                    or v.dtype != torch.float32 or v.numel() != 1:
+                return None
+            if cls == "LogNormal":
+                p0, p1 = _const(fn.loc), _const(fn.scale)
+            else:
+                p0, p1 = _const(fn.rate if cls == "Exponential" else fn.scale), 1.0
+            if p0 is None or p1 is None or not p1 > 0.0 or (cls != "LogNormal" and not p0 > 0.0):
+                return None
+            sigma_site, sigma_prior, shapes_sigma = name, (cls, p0, p1), tuple(v.shape)
+        latent = {k: v for k, v in latent.items() if k != sigma_site}
+        if len(latent) not in (1, 2):
+            return None
+    elif len(latent) == 3:
         return None
     y = obs["value"]
     if not isinstance(y, torch.Tensor) or y.dim() != 1:
@@ -224,7 +249,7 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
         wshapes, bshapes = [(D,)], [(), (1,)]
         if D not in (4, 8, 16, 32) or y.dtype != torch.float32:
             return None
-    elif kind == "Poisson":
+    elif kind in ("Poisson", "Normal"):
         K = 1
         wshapes, bshapes = [(D,)], [(), (1,)]
         if not 1 <= D <= 128 or y.dtype != torch.float32:
@@ -245,17 +270,34 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
     # ---- functional probe: logits == X @ w + b  /  log_softmax(logits) == log_softmax(X @ W.mT + b)  /
     # log(rate) == X @ w + b ----------------------------------------------------------------------------------
     gen = torch.Generator(device="cpu").manual_seed(20240302)
+    sigma_const = None
     for _ in range(3):
         wv = torch.randn(shapes[weight], generator=gen).to(X)
         if kind == "Poisson":
             wv = wv / D ** 0.5            # log-rates of a few units: exp neither overflows nor underflows
         bv = torch.randn(shapes[bias], generator=gen).to(X) if bias is not None else None
         data = {weight: wv} if bias is None else {weight: wv, bias: bv}
+        if sigma_site is not None:
+            sv = torch.exp(0.5 * torch.randn((), generator=gen)).to(X)
+            data[sigma_site] = sv.reshape(shapes_sigma)
         pfn = _probe(poutine, model, args, kwargs, data, obs_name)
-        logits = torch.log(pfn.rate) if kind == "Poisson" else pfn.logits
+        if kind == "Normal":
+            # scale: the latent sigma as drawn, or one constant that does not move with the weights
+            sc = pfn.scale
+            if sigma_site is not None:
+                if not isinstance(sc, torch.Tensor) or not _close(sc, sv, X.dtype):
+                    return None
+            else:
+                c = _const(sc)
+                if c is None or not c > 0.0 or (sigma_const is not None and c != sigma_const):
+                    return None
+                sigma_const = c
+            logits = pfn.loc
+        else:
+            logits = torch.log(pfn.rate) if kind == "Poisson" else pfn.logits
         if hasattr(logits, "dense"):
             logits = logits.dense()
-        if kind == "Poisson":
+        if kind in ("Poisson", "Normal"):
             want = X @ wv + (bv.reshape(()) if bv is not None else 0.0)
         elif kind == "Bernoulli":
             want = X @ wv + bv.reshape(())
@@ -265,14 +307,20 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
         if tuple(logits.shape) != tuple(want.shape) or not _close(logits, want, X.dtype):
             return None
     off, sites = 0, {}
-    for name in latent:
+    for name in order:
+        if name == sigma_site:
+            sites[name] = (slice(off, off + 1), "exp", shapes_sigma)
+            off += 1
+            continue
         width = 1
         for d in shapes[name]:
             width *= d
         sites[name] = (slice(off, off + width), "identity", shapes[name])
         off += width
     return GlmPotential(X, y.detach(), kind, sites, weight, bias, s_w=scales[weight],
-                        s_b=scales[bias] if bias is not None else 1.0)
+                        s_b=scales[bias] if bias is not None else 1.0,
+                        sigma=sigma_const if sigma_const is not None else 1.0, sigma_site=sigma_site,
+                        sigma_prior=sigma_prior)
 
 
 def recognise(model, args=(), kwargs=None, poutine=None):

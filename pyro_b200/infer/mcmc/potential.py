@@ -115,7 +115,11 @@ class GlmPotential:
     ``w ~ Normal(0, s_w)[D]``, ``b ~ Normal(0, s_b)``, ``y ~ Bernoulli(logits = X @ w + b)``, or
     ``W ~ Normal(0, s_w)[K, D]``, ``b ~ Normal(0, s_b)[K]`` (optional),
     ``y ~ Categorical(logits = X @ W.mT + b)``, or
-    ``w ~ Normal(0, s_w)[D]``, ``b ~ Normal(0, s_b)`` (optional), ``y ~ Poisson(rate = exp(X @ w + b))``.
+    ``w ~ Normal(0, s_w)[D]``, ``b ~ Normal(0, s_b)`` (optional), ``y ~ Poisson(rate = exp(X @ w + b))``, or
+    ``w ~ Normal(0, s_w)[D]``, ``b ~ Normal(0, s_b)`` (optional), ``y ~ Normal(X @ w + b, sigma)`` with a constant
+    ``sigma`` or a latent one (``sigma_site``) whose prior ``sigma_prior = (kind, p0, p1)`` is HalfNormal(p0),
+    HalfCauchy(p0), Exponential(p0) or LogNormal(p0, p1); z then holds ``log sigma`` (transform ``"exp"``) and U
+    carries the Jacobian ``-log sigma``, as ``TracePotential`` gives it (``b2_glm_normal_potential``).
 
     ``value_and_grad`` is ``b2_glm_potential``: the likelihood of all chains comes from one pass of the
     fused GLM kernel over X, the chains being its particles.  ``sites`` maps each site name to
@@ -123,12 +127,24 @@ class GlmPotential:
     model, so samples, ``initial_params`` and ``full_mass`` behave the same on either.  Every chain is
     evaluated; the sampler masks inactive chains, as it does for ``TracePotential``."""
 
-    def __init__(self, X, y, kind, sites, weight, bias=None, s_w=1.0, s_b=1.0):
+    _SIGMA_PRIORS = {"HalfNormal": N.SIGMA_HALFNORMAL, "HalfCauchy": N.SIGMA_HALFCAUCHY,
+                     "Exponential": N.SIGMA_EXPONENTIAL, "LogNormal": N.SIGMA_LOGNORMAL}
+
+    def __init__(self, X, y, kind, sites, weight, bias=None, s_w=1.0, s_b=1.0, sigma=1.0, sigma_site=None,
+                 sigma_prior=None):
         N.require_cuda(X, "GlmPotential")
         if X.dtype != torch.float32 or X.dim() != 2:
             raise ValueError("GlmPotential needs fp32 X of shape [N, D]")
         self.X = X.contiguous()
-        self.kind = {"Bernoulli": N.GLM_BERNOULLI, "Categorical": N.GLM_CATEGORICAL, "Poisson": N.GLM_POISSON}[kind]
+        self.normal = kind == "Normal"
+        self.sigma, self.sigma_site = float(sigma), sigma_site
+        if sigma_site is not None:
+            pk, p0, p1 = sigma_prior
+            self.sigma_prior = (self._SIGMA_PRIORS[pk], float(p0), float(p1))
+        else:
+            self.sigma_prior = (N.SIGMA_CONST, 0.0, 0.0)
+        self.kind = {"Bernoulli": N.GLM_BERNOULLI, "Categorical": N.GLM_CATEGORICAL, "Poisson": N.GLM_POISSON,
+                     "Normal": None}[kind]
         # private contiguous copies: the kernels load y with TMA (16-byte aligned)
         self.y = (y.to(torch.int64) if self.kind == N.GLM_CATEGORICAL else y.to(torch.float32)).clone()
         self.sites = dict(sites)
@@ -155,6 +171,16 @@ class GlmPotential:
         U = torch.empty(C, dtype=torch.float32, device=z.device)
         g = torch.empty_like(z)
         lib = N.lib()
+        if self.normal:
+            need = int(lib.b2_glm_normal_potential_workspace(self.n, self.Dx, C))
+            ws = N.workspace(z.device, need, tag="glm_potential")
+            s_off = self.sites[self.sigma_site][0].start if self.sigma_site is not None else -1
+            pk, p0, p1 = self.sigma_prior
+            N.check(lib.b2_glm_normal_potential(
+                self.X.data_ptr(), self.y.data_ptr(), self.n, self.Dx, int(self.has_bias), z.data_ptr(), C, self.D,
+                self.w_off, self.b_off, s_off, self.s_w, self.s_b, pk, p0, p1, self.sigma, U.data_ptr(),
+                g.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(z.device)), "b2_glm_normal_potential")
+            return U, g
         need = int(lib.b2_glm_potential_workspace(self.kind, self.n, self.Dx, self.K, C))
         ws = N.workspace(z.device, need, tag="glm_potential")
         N.check(lib.b2_glm_potential(
@@ -167,7 +193,9 @@ class GlmPotential:
         return {name: self.unpack_site(name, z[..., sl]) for name, (sl, _, _) in self.sites.items()}
 
     def unpack_site(self, name, u):
-        return u.reshape(u.shape[:-1] + tuple(self.sites[name][2]))
+        _, transform, shape = self.sites[name]
+        v = u.exp() if transform == "exp" else u
+        return v.reshape(u.shape[:-1] + tuple(shape))
 
     def init_uniform(self, num_chains, radius=2.0, generator=None):
         return (torch.rand(num_chains, self.D, dtype=self.dtype, device=self.device,

@@ -24,6 +24,10 @@ Poisson regression has one more: ``torch.exp(t)`` or ``t.exp()`` of a lazy ``X @
 ``b2_glm_poisson_log_rate``; any other use, ``+ offset`` and ``* c`` included, materialises ``exp`` of the
 eager expression, bit for bit.
 
+Linear regression needs no new seam: ``Normal(lazy X @ w + b, sigma)`` with one noise scale per particle (a
+number, ``[]``, ``[1]``, ``[P, 1]``) scores the site with ``b2_glm_normal_loc``; ``broadcast_all(loc, sigma)`` of
+``torch.distributions.Normal`` keeps the loc lazy and expands sigma.
+
 Poisson matrix factorisation (the bottom layer of the sparse gamma DEF) has one more: ``torch.matmul(z, w)``,
 ``z @ w`` or ``torch.bmm(z, w)`` of TWO site values ``z[N, K] @ w[K, J]`` or ``z[P, N, K] @ w[P, K, J]``
 (fp32, one CUDA device, 1 <= K <= 16) gives a :class:`FactorProduct`, and ``Poisson(lazy)`` scores the site with
@@ -336,6 +340,25 @@ class LinearPredictorTensor(torch.Tensor):
                 with torch._C.DisableTorchFunctionSubclass():
                     return tuple(a if isinstance(a, LinearPredictorTensor) else a.expand(self.shape)
                                  for a in args)
+            # torch.distributions.Normal(lazy X @ w + b, scale) calls broadcast_all(loc, scale): a scale that
+            # broadcasts to the loc's shape ([P, 1] per particle, [N], ...) is expanded and the loc stays lazy.  The
+            # expanded view remembers its operand, so the fused Normal site takes the stored scale, not a slice.
+            if name == "broadcast_tensors" and isinstance(self._lazy, LinearPredictor) and not kwargs and all(
+                    a is self or (isinstance(a, torch.Tensor) and not isinstance(a, LinearPredictorTensor)
+                                  and a.dim() <= len(self.shape)
+                                  and torch.broadcast_shapes(a.shape, self.shape) == self.shape)
+                    for a in args):
+                out = []
+                for a in args:
+                    if a is self:
+                        out.append(a)
+                        continue
+                    plain = _plain(a)
+                    with torch._C.DisableTorchFunctionSubclass():
+                        v = plain.expand(self.shape)
+                    v._b2_unexpanded = plain
+                    out.append(v)
+                return tuple(out)
             if name in ("detach", "clone", "contiguous", "float", "to") and len(args) == 1 and not kwargs:
                 return self
             # distribution-argument validation (constraints.real.check): an affine image of finite
