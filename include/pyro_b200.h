@@ -82,7 +82,9 @@ extern "C" {
  *                           shapes of loc / scale)                                              */
 #define B2_NORMAL_RSAMPLE 14
 #define B2_NORMAL_RSAMPLE_BWD 15
-#define B2_NUM_ELEMENTWISE_FAMILIES 16
+#define B2_BINOMIAL_LOGITS 16  /* (total_count, logits)   pyro/distributions/torch.py:83-101 (tol = 0) */
+#define B2_BINOMIAL_PROBS 17   /* (total_count, probs)    the same, logits = probs_to_logits(clamped probs) */
+#define B2_NUM_ELEMENTWISE_FAMILIES 18
 /* Event families (event_dim >= 1), scored by b2_event_score. */
 #define B2_DIRICHLET 32   /* (concentration[...,K])           torch/distributions/dirichlet.py:90-97 */
 #define B2_CATEGORICAL 33 /* (logits[...,K]), int64 value      categorical.py:78,151-157             */
@@ -393,6 +395,35 @@ int b2_glm_normal_loc(const float* X, const float* y, const float* W, const floa
 size_t b2_glm_normal_workspace(int64_t N, int D, int P);
 
 /*
+ * b2_glm_binomial_logits -- fused Binomial-regression (logit link) likelihood term: for P particles,
+ * l[p,n] = <X[n,:], W[p,:]> + b[p] are the logits, y[n] the successes out of m_n trials:
+ *   sum_p[p] = SUM_n ( y[n] l[p,n] - m_n softplus(l[p,n]) - log C(m_n, y[n]) )   (pyro/distributions/torch.py
+ *              Binomial.log_prob with log_binomial at tol = 0)
+ *   dW[p,:]  = weight * SUM_n (y[n] - m_n sigmoid(l[p,n])) X[n,:],   db[p] = weight * SUM_n (y[n] - m_n sigmoid(l))
+ * (scale multiplies every output, as for b2_glm_bernoulli_logits).  X: [N,D] row-major fp32, 1 <= D <= 128;
+ * W: [P,D]; b: [P] (nullable); y: [N] fp32; trials: device pointer to m, the [N] fp32 counts (trials_per_row = 1,
+ * 16-byte aligned, loaded next to y) or ONE fp32 count for every row (trials_per_row = 0, read on the device, so
+ * a count held in a tensor needs no host read and the call can be captured in a CUDA graph).  X and y must be
+ * 16-byte aligned and N < 2^31.  The tile kernel (glm_binomial_tc.cu: D == 32 on the TMA tile pipeline of
+ * glm_tc.cu, every other D on the bulk-copy tile loop of glm_flat_tc.cu) follows the precision policy of
+ * b2_glm_poisson_log_rate: W split hi + lo, X rounded to nearest TF32 from 65536 rows, split below that and at
+ * any N with B2_FLAG_GLM_3XTF32; g = y - m sigmoid(l) rounded to nearest TF32.  SUM log C(m, y) is computed once
+ * per call.  There is no fp32 SIMT kernel: B2_FLAG_GLM_FP32 returns B2_ERR_BAD_SHAPE.  A null X, y, trials or W
+ * returns B2_ERR_NULL; N <= 0, P <= 0, D outside 1..128, trials_per_row other than 0 or 1, a misaligned X or y
+ * (or per-row trials) B2_ERR_BAD_SHAPE; N >= 2^31 B2_ERR_TOO_LARGE; all before any CUDA call.
+ * out_sum_p, out_dW, out_db ([P]) and out_total are nullable; out_total: scalar, (=|+=) sum_coeff * scale *
+ * SUM_p sum_p[p].
+ * workspace: b2_glm_binomial_workspace() bytes, zero-initialised ONCE by the caller (its first 256 bytes hold a
+ * ticket counter that the library leaves zeroed).  Two launches: the streaming kernel and the finish kernel of
+ * b2_glm_bernoulli_logits, which sums the CTA partials in a fixed order (deterministic, no float atomics).
+ */
+int b2_glm_binomial_logits(const float* X, const float* y, const float* trials, int trials_per_row, const float* W,
+                           const float* b, int64_t N, int D, int P, double scale, double weight, double sum_coeff,
+                           int flags, float* out_sum_p, float* out_total, float* out_dW, float* out_db,
+                           void* workspace, size_t workspace_bytes, void* stream);
+size_t b2_glm_binomial_workspace(int64_t N, int D, int P);
+
+/*
  * b2_poisson_product -- fused Poisson matrix-factorisation likelihood term (the bottom layer of the sparse
  * gamma DEF, Gamma-Poisson NMF): for P particles with latent factors A[p] (N x K) and B[p] (K x J) and shared
  * counts x (N x J), rate[p,n,j] = SUM_k A[p,n,k] * B[p,k,j];
@@ -481,6 +512,22 @@ int b2_glm_normal_potential(const float* X, const float* y, int64_t N, int D, in
                             double s_b, int s_prior, double sp0, double sp1, double sigma, float* U, float* grad,
                             void* workspace, size_t workspace_bytes, void* stream);
 size_t b2_glm_normal_potential_workspace(int64_t N, int D, int64_t C);
+
+/*
+ * b2_glm_binomial_potential -- HMC / NUTS potential energy and gradient of Bayesian Binomial regression for C
+ * chains: w ~ Normal(0, s_w)[D], b ~ Normal(0, s_b) (has_bias), y ~ Binomial(m, logits = X @ w + b), with trials
+ * as for b2_glm_binomial_logits (one count or [N] counts, on the device).  z: [C, Dz] fp32 with Dz = D + has_bias,
+ * the weights at w_off and the bias at b_off; U: [C], grad: [C, Dz].  Four launches with no host sync (CUDA graph
+ * capturable): the pack kernel of b2_glm_potential, b2_glm_binomial_logits with weight -1 and B2_FLAG_GLM_3XTF32
+ * (kernel + finish), and the potential finish, which adds the priors in fp64.  Argument checks as for
+ * b2_glm_potential and b2_glm_binomial_logits, all before any CUDA call.
+ * workspace: b2_glm_binomial_potential_workspace() bytes, zero-initialised once.
+ */
+int b2_glm_binomial_potential(const float* X, const float* y, const float* trials, int trials_per_row, int64_t N,
+                              int D, int has_bias, const float* z, int64_t C, int64_t Dz, int64_t w_off,
+                              int64_t b_off, double s_w, double s_b, float* U, float* grad, void* workspace,
+                              size_t workspace_bytes, void* stream);
+size_t b2_glm_binomial_potential_workspace(int64_t N, int D, int64_t C);
 size_t b2_glm_potential_workspace(int kind, int64_t N, int D, int K, int64_t C);
 
 /* ---- optimisers --------------------------------------------------------------------------

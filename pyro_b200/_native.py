@@ -27,7 +27,7 @@ B2_ERR_UNSUPPORTED_REDUCTION = -6
 # family ids (include/pyro_b200.h)
 NORMAL, BERNOULLI_LOGITS, GAMMA, BETA, POISSON, CAUCHY, HALFCAUCHY, EXPONENTIAL, LOGNORMAL, \
     HALFNORMAL, BERNOULLI_PROBS, UNIFORM, KL_NORMAL_NORMAL, KL_GAMMA_GAMMA, NORMAL_RSAMPLE, \
-    NORMAL_RSAMPLE_BWD = range(16)
+    NORMAL_RSAMPLE_BWD, BINOMIAL_LOGITS, BINOMIAL_PROBS = range(18)
 FUSED_DRAW = True         # Normal.rsample draws and scores in one kernel (b2 family 14)
 PHILOX_DRAW = True        # ... and generates its noise in that kernel (b2_normal_rsample) instead of torch.randn
 RSAMPLE_MAX_N = 65536
@@ -127,6 +127,12 @@ SIGNATURES = {
     "b2_glm_normal_loc": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _f64, _f64, _f64, _i32,
                                  _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2_glm_normal_workspace": (_sz, [_i64, _i32, _i32]),
+    "b2_glm_binomial_logits": (_i32, [_vp, _vp, _vp, _i32, _vp, _vp, _i64, _i32, _i32, _f64, _f64, _f64, _i32,
+                                      _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "b2_glm_binomial_workspace": (_sz, [_i64, _i32, _i32]),
+    "b2_glm_binomial_potential": (_i32, [_vp, _vp, _vp, _i32, _i64, _i32, _i32, _vp, _i64, _i64, _i64, _i64, _f64,
+                                         _f64, _vp, _vp, _vp, _sz, _vp]),
+    "b2_glm_binomial_potential_workspace": (_sz, [_i64, _i32, _i64]),
     "b2_glm_normal_potential": (_i32, [_vp, _vp, _i64, _i32, _i32, _vp, _i64, _i64, _i64, _i64, _i64, _f64, _f64,
                                        _i32, _f64, _f64, _f64, _vp, _vp, _vp, _sz, _vp]),
     "b2_glm_normal_potential_workspace": (_sz, [_i64, _i32, _i64]),

@@ -69,6 +69,15 @@ def _cat(fn):
     return b2d.Categorical(probs=fn.probs)
 
 
+def _binom(fn):
+    # a reference Binomial scored with the approximate log binomial coefficient keeps the reference path
+    if getattr(fn, "approx_log_prob_tol", 0.0) != 0.0:
+        return None
+    if "logits" in fn.__dict__:
+        return b2d.Binomial(fn.total_count, logits=fn.__dict__["logits"])
+    return b2d.Binomial(fn.total_count, probs=fn.probs)
+
+
 _SIMPLE = {
     "Normal": lambda fn: b2d.Normal(fn.loc, fn.scale),
     "Cauchy": lambda fn: b2d.Cauchy(fn.loc, fn.scale),
@@ -81,6 +90,7 @@ _SIMPLE = {
     "Beta": lambda fn: b2d.Beta(fn.concentration1, fn.concentration0),
     "Poisson": lambda fn: b2d.Poisson(fn.rate),
     "Bernoulli": _bern,
+    "Binomial": _binom,
     "Dirichlet": lambda fn: b2d.Dirichlet(fn.concentration),
     "Categorical": _cat,
     "MultivariateNormal": lambda fn: b2d.MultivariateNormal(fn.loc, scale_tril=fn._unbroadcasted_scale_tril),

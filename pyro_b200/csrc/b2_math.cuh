@@ -381,7 +381,9 @@ enum : int {
   kKLGammaGamma = 13,
   kNormalRsample = 14,     // reparameterised draw + its own log density (guide sites)
   kNormalRsampleBwd = 15,  // chain rule of that draw back to (loc, scale)
-  kNumElementwise = 16
+  kBinomialLogits = 16,
+  kBinomialProbs = 17,
+  kNumElementwise = 18
 };
 
 template <int FAM>
@@ -408,6 +410,8 @@ B2_TRAITS(kKLNormalNormal, 4, false)
 B2_TRAITS(kKLGammaGamma, 4, false)
 B2_TRAITS(kNormalRsample, 2, true)
 B2_TRAITS(kNormalRsampleBwd, 3, true)
+B2_TRAITS(kBinomialLogits, 2, true)
+B2_TRAITS(kBinomialProbs, 2, true)
 #undef B2_TRAITS
 
 // eval<FAM, T, GRAD>(x, p, out): p[k] are the parameters in the order pyro_b200.h documents.
@@ -617,6 +621,48 @@ struct Eval<kPoisson, T, GRAD> {
   }
   static B2_HD void run(T x, const T* p, ElemOut<T>& o) {
     run_aux(x, ValueAux<kPoisson, T, GRAD>::make(x), p, o);
+  }
+};
+
+// Binomial(total_count n, logits l): pyro/distributions/torch.py:83-101 with log_binomial (pyro/ops/special.py:93-108)
+// at tol = 0
+//   k*l - n*(max(l, 0) + log1p(e^-|l|)) + lgamma(n + 1) - lgamma(k + 1) - lgamma(n - k + 1)
+// The reference evaluates log_binomial under torch.no_grad, so autograd of it gives d/dl = k - n*sigmoid(l),
+// d/dn = -softplus(l) and d/dk = l: the lgamma terms carry no gradient, and these are the gradients here too.
+// lgamma(v + 1) of an integer count below 64 comes from the table of the Poisson family.
+template <typename T>
+B2_HD T lfact(T v) {
+  return ValueAux<kPoisson, T, false>::make(v).lgx;
+}
+template <typename T, bool GRAD>
+B2_HD void binomial_logits_run(T x, T n, T l, ElemOut<T>& o) {
+  T sp, sg;
+  softplus_sigmoid(l, sp, sg);
+  o.lp = x * l - n * sp + (lfact(n) - lfact(x) - lfact(n - x));
+  if (GRAD) {
+    o.dx = l;
+    o.dp[0] = -sp;
+    o.dp[1] = x - n * sg;
+  }
+}
+
+template <typename T, bool GRAD>
+struct Eval<kBinomialLogits, T, GRAD> {
+  static B2_HD void run(T x, const T* p, ElemOut<T>& o) { binomial_logits_run<T, GRAD>(x, p[0], p[1], o); }
+};
+
+// Binomial(total_count n, probs): logits = log(p) - log1p(-p) with p clamped to [eps, 1-eps] (torch's
+// probs_to_logits, as for kBernoulliProbs), then as above; zero probs gradient where the clamp is active
+template <typename T, bool GRAD>
+struct Eval<kBinomialProbs, T, GRAD> {
+  static B2_HD void run(T x, const T* p, ElemOut<T>& o) {
+    const T eps = b2_eps<T>();
+    const T pr = p[1];
+    const bool clamped = (pr < eps) || (pr > (T)1 - eps);
+    const T pc = b2_min(b2_max(pr, eps), (T)1 - eps);
+    const T l = b2_log(pc) - b2_log1p(-pc);
+    binomial_logits_run<T, GRAD>(x, p[0], l, o);
+    if (GRAD) o.dp[1] = clamped ? (T)0 : o.dp[1] / (pc * ((T)1 - pc));
   }
 };
 

@@ -1,0 +1,198 @@
+// glm_binomial_tc.cu -- Hopper fused Binomial-regression (logit link) likelihood kernels: for up to 64 weight
+// vectors (particles) per CTA slab, ONE pass over X[N,D], the successes y[N] and the trial counts m (one count for
+// every row, or m[N]) gives
+//   l_pn    = x_n.w_p + b_p
+//   sum_p   = SUM_n ( y_n l_pn - m_n softplus(l_pn) - log C(m_n, y_n) )    pyro/distributions/torch.py Binomial
+//   dW_p    = weight * SUM_n (y_n - m_n sigmoid(l_pn)) x_n,   db_p = weight * SUM_n (y_n - m_n sigmoid(l_pn))
+// It replaces the model's `X @ w + b`, Binomial(m, logits).log_prob, the site sum and the autograd backward of
+// all of them, which write and re-read the [P, N] logits, log_prob and gradient tensors.  It is the logistic
+// kernel with a weight per row: at m = 1 it scores what b2_glm_bernoulli_logits scores.
+//
+// The tile loops are the GLM ones with the Binomial family of glm_tc_common.cuh: glm_tile_pipeline at D = 32 (TMA
+// tiles, glm_tc.cu) and glm_flat_pipeline at every other D in 1..128 (bulk-copied tiles, glm_flat_tc.cuh; D < 32
+// padded to two atoms, see launch).  Per-row
+// trial counts arrive next to y, on the same mbarrier, straight from the caller's [N] tensor; one count for every
+// row is read once per call from device memory.  The epilogue reads y and m from shared memory and takes ex2, rcp
+// and lg2 per logit (see binomial_epilogue).
+// Precision policy of the Poisson kernels: W always split hi + lo, X split too under SPLIT_X; GEMM 1 starts from
+// zero and the epilogue adds the bias, rounded to nearest (see poisson_epilogue); g rounded to nearest TF32.
+//
+// SUM log C(m, y) = SUM [lgamma(y + 1) + lgamma(m - y + 1) - lgamma(m + 1)] depends on the data alone: after its
+// tile loop each CTA of particle slab 0 sums it over the rows of its own tiles (read again from L2, outside the
+// wgmma pipeline) into one more partial, and glm_finish_kernel subtracts the sum of those partials from every
+// particle's sum.  Every sum has a fixed order; no float atomics, and a call is two launches (kernel + finish).
+#include <cuda.h>
+#include <stdlib.h>
+
+#include "b2_common.cuh"
+#include "b2_math.cuh"
+#include "glm_flat_tc.cuh"
+
+namespace b2 {
+
+// glm.cu / glm_tc.cu
+void launch_glm_finish(const float* partials, unsigned int* ticket, int gx, int P, int K, int D, double scale,
+                       double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
+                       float* out_dW, float* out_db, const float* lg, cudaStream_t s);
+int glm_tc_grid_x(int64_t N);
+
+namespace tcbi {
+
+using namespace tc;
+
+// lgamma(v + 1): the table of integer counts below 64, the shifted Stirling series above
+__device__ __forceinline__ float lgamma1(float v) { return ValueAux<kPoisson, float, false>::make(v).lgx; }
+
+// lg[blockIdx.x] = SUM [lgamma(y_n + 1) + lgamma(m_n - y_n + 1) - lgamma(m_n + 1)] over the rows of the CTA's
+// tiles (blockIdx.x, blockIdx.x + gridDim.x, ...), in a fixed order; called by every thread of a CTA of slab 0
+// after its tile loop
+template <int NT, bool ROW>
+__device__ __forceinline__ void lbinom_partial(const float* __restrict__ y, const float* __restrict__ trials,
+                                               int64_t N, float* __restrict__ lg) {
+  __shared__ float red[NT / 32];
+  const int64_t ntiles = (N + kRows - 1) / kRows;
+  const int nt = (int)((ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x);
+  const float mc = ROW ? 0.f : __ldg(trials);
+  const float lgm = ROW ? 0.f : lgamma1(mc);
+  float s = 0.f;
+  for (int64_t i = threadIdx.x; i < (int64_t)nt * kRows; i += NT) {
+    const int64_t n = (blockIdx.x + (i / kRows) * (int64_t)gridDim.x) * kRows + i % kRows;
+    if (n < N) {
+      const float yv = __ldg(y + n), m = ROW ? __ldg(trials + n) : mc;
+      s += (lgamma1(yv) + lgamma1(m - yv)) - (ROW ? lgamma1(m) : lgm);
+    }
+  }
+  s = warp_sum(s);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float v = 0.f;
+    for (int w = 0; w < NT / 32; ++w) v += red[w];
+    lg[blockIdx.x] = v;
+  }
+}
+
+// D = 32.  SPLIT_X = false (default): W split hi/lo, X rounded to nearest.  SPLIT_X = true: X split as well.
+// ROW: per-row trial counts (map_m); else the one count trials[0].
+template <bool ROW, bool SPLIT_X>
+__global__ void __launch_bounds__(tile32::kThreads, 1)
+glm_binomial_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_y,
+                       const __grid_constant__ CUtensorMap map_m, const float* __restrict__ y,
+                       const float* __restrict__ trials, const float* __restrict__ W,
+                       const float* __restrict__ bvec, int64_t N, int P, float* __restrict__ partials,
+                       float* __restrict__ lg) {
+  tile32::glm_tile_pipeline<Binomial<ROW>, SPLIT_X>(map_x, map_y, W, bvec, N, P, 1, partials, &map_m, trials);
+  if (blockIdx.y == 0) lbinom_partial<tile32::kThreads, ROW>(y, trials, N, lg);
+}
+
+// every other D in 1..128, padded to DC atoms of 32 columns
+template <bool ROW, int DC, bool SPLIT_X>
+__global__ void __launch_bounds__(tcf::Cfg<DC>::kThreads, 1)
+glm_binomial_flat_tc_kernel(const float* __restrict__ X, const float* __restrict__ y,
+                            const float* __restrict__ trials, const float* __restrict__ W,
+                            const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
+                            float* __restrict__ lg) {
+  tcf::glm_flat_pipeline<Binomial<ROW>, DC, SPLIT_X>(X, y, W, bvec, N, D, P, partials, trials);
+  if (blockIdx.y == 0) lbinom_partial<tcf::Cfg<DC>::kThreads, ROW>(y, trials, N, lg);
+}
+
+template <bool ROW, bool SPLIT_X>
+int launch_32(const float* X, const float* y, const float* m, const float* W, const float* b, int64_t N, int P,
+              float* partials, float* lg, int gx, cudaStream_t s) {
+  using namespace tile32;
+  using Fam = Binomial<ROW>;
+  CUtensorMap mx, my, mm;
+  if (!encode_x_map(&mx, X, N) || !encode_label_map(&my, y, N, Fam::kYType)) return B2_ERR_LAUNCH;
+  if (ROW ? !encode_label_map(&mm, m, N, Fam::kYType) : false) return B2_ERR_LAUNCH;
+  if (!ROW) mm = my;                           // not read
+  constexpr uint32_t kSmemBytes = Smem32<Fam::kYBytes>::kBytes;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaFuncSetAttribute(glm_binomial_tc_kernel<ROW, SPLIT_X>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)kSmemBytes);
+    attr_set = true;
+  }
+  dim3 grid((unsigned)gx, (unsigned)((P + kM - 1) / kM), 1);
+  launch_pdl(glm_binomial_tc_kernel<ROW, SPLIT_X>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, mm, y, m,
+             W, b, N, P, partials, lg);
+  return 0;
+}
+
+template <bool ROW, int DC, bool SPLIT_X>
+int launch_flat(const float* X, const float* y, const float* m, const float* W, const float* b, int64_t N, int D,
+                int P, float* partials, float* lg, int gx, cudaStream_t s) {
+  using C = tcf::Cfg<DC>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaFuncSetAttribute(glm_binomial_flat_tc_kernel<ROW, DC, SPLIT_X>,
+                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::kSmemBytes);
+    attr_set = true;
+  }
+  dim3 grid((unsigned)gx, (unsigned)((P + kM - 1) / kM), 1);
+  launch_pdl(glm_binomial_flat_tc_kernel<ROW, DC, SPLIT_X>, grid, dim3(C::kThreads), (size_t)C::kSmemBytes, s, X,
+             y, m, W, b, N, D, P, partials, lg);
+  return 0;
+}
+
+template <bool ROW, bool SPLIT_X>
+int launch(const float* X, const float* y, const float* m, const float* W, const float* b, int64_t N, int D,
+           int P, float* partials, float* lg, int gx, cudaStream_t s) {
+  if (D == 32) return launch_32<ROW, SPLIT_X>(X, y, m, W, b, N, P, partials, lg, gx, s);
+  // D < 32 runs the two-atom loop (two warpgroups, 255 registers): with one atom and four warpgroups the
+  // 128-register cap made this epilogue spill
+  switch ((D + 31) / 32) {
+    case 1:
+    case 2: return launch_flat<ROW, 2, SPLIT_X>(X, y, m, W, b, N, D, P, partials, lg, gx, s);
+    case 3: return launch_flat<ROW, 3, SPLIT_X>(X, y, m, W, b, N, D, P, partials, lg, gx, s);
+    default: return launch_flat<ROW, 4, SPLIT_X>(X, y, m, W, b, N, D, P, partials, lg, gx, s);
+  }
+}
+
+}  // namespace tcbi
+}  // namespace b2
+
+using namespace b2;
+
+extern "C" size_t b2_glm_binomial_workspace(int64_t N, int D, int P) {
+  // [ticket, 256 B] + CTA partials [gx][P][D + 2] + one [P] row for the per-particle sums + log C partials [gx]
+  if (N < 1 || D < 1 || D > 128 || P < 1) return 256;
+  const size_t gx = (size_t)glm_tc_grid_x(N);
+  return 256 + (gx * (size_t)P * (size_t)(D + 2) + (size_t)P + gx) * sizeof(float);
+}
+
+extern "C" int b2_glm_binomial_logits(const float* X, const float* y, const float* trials, int trials_per_row,
+                                      const float* W, const float* b, int64_t N, int D, int P, double scale,
+                                      double weight, double sum_coeff, int flags, float* out_sum_p,
+                                      float* out_total, float* out_dW, float* out_db, void* workspace,
+                                      size_t workspace_bytes, void* stream) {
+  if (!X || !y || !trials || !W) return B2_ERR_NULL;
+  if (N <= 0 || P <= 0 || D < 1 || D > 128) return B2_ERR_BAD_SHAPE;
+  if (trials_per_row != 0 && trials_per_row != 1) return B2_ERR_BAD_SHAPE;
+  // the tiles arrive by TMA / bulk copies (16-byte aligned sources, 32-bit row coordinates); there is no fp32
+  // SIMT kernel for this family
+  if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
+  if (trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0) return B2_ERR_BAD_SHAPE;
+  if (flags & B2_FLAG_GLM_FP32) return B2_ERR_BAD_SHAPE;
+  if (N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
+  if (!workspace || workspace_bytes < b2_glm_binomial_workspace(N, D, P)) return B2_ERR_WORKSPACE;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const int gx = glm_tc_grid_x(N);
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(workspace);
+  float* partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
+  float* lg = partials + (size_t)gx * P * (D + 2) + P;
+  // the precision policy of b2_glm_bernoulli_logits: below 64 Ki rows the incoherent X rounding has not
+  // averaged out yet -> X split as well
+  const bool split_x = (flags & B2_FLAG_GLM_3XTF32) || N < 65536;
+  int rc;
+  if (trials_per_row)
+    rc = split_x ? tcbi::launch<true, true>(X, y, trials, W, b, N, D, P, partials, lg, gx, s)
+                 : tcbi::launch<true, false>(X, y, trials, W, b, N, D, P, partials, lg, gx, s);
+  else
+    rc = split_x ? tcbi::launch<false, true>(X, y, trials, W, b, N, D, P, partials, lg, gx, s)
+                 : tcbi::launch<false, false>(X, y, trials, W, b, N, D, P, partials, lg, gx, s);
+  if (rc != 0) return rc;
+  launch_glm_finish(partials, ticket, gx, P, 1, D, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW,
+                    out_db, lg, s);
+  count_launch(2);
+  return check_launch();
+}

@@ -67,6 +67,7 @@ __device__ __forceinline__ float class_sum(float v) {
 template <int KP>
 struct Softmax {
   static_assert(KP == 2 || KP == 4 || KP == 8 || KP == 16, "class padding");
+  static constexpr int kTrials = kNoTrials;
   static constexpr bool kBiasInEpilogue = false;
   static constexpr int kKP = KP;
   static constexpr uint32_t kYBytes = kRows * 8;  // 512 B of int64 labels

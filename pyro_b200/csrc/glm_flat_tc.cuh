@@ -1,6 +1,6 @@
 // glm_flat_tc.cuh -- the any-D tile loop of the Hopper GLM likelihood kernels: glm_flat_pipeline<Fam, DC,
 // SPLIT_X> runs one likelihood family (glm_tc_common.cuh: Bernoulli for glm_flat_tc.cu, Poisson for
-// glm_poisson_tc.cu) for any feature count D in 1..128.
+// glm_poisson_tc.cu, Normal for glm_normal_tc.cu, Binomial for glm_binomial_tc.cu) for any feature count D in 1..128.
 //
 // Same contract as the D = 32 tile pipeline (glm_tc_common.cuh): ONE pass over X[N,D] and y[N] gives, for up
 // to 64 weight vectors (particles) per CTA slab, sum_n lp(y_n | l_n = x_n.w_p + b_p), dW and db, as CTA
@@ -83,10 +83,13 @@ __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_
 
 // wgmma accumulator fragment (m64nN, f32): thread (warp w4 of the warpgroup, lane = 4 gid + t4) holds
 // d[4j + 2h + e] = D[16 w4 + gid + 8h][8j + 2 t4 + e].
+// Binomial only (glm_tc_common.cuh): trials are the per-row counts [N] (kRowTrials, bulk-copied behind y) or
+// the one count of every row (kConstTrials).
 template <class Fam, int DC, bool SPLIT_X>
 __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, const float* __restrict__ y,
                                                   const float* __restrict__ W, const float* __restrict__ bvec,
-                                                  int64_t N, int D, int P, float* __restrict__ partials) {
+                                                  int64_t N, int D, int P, float* __restrict__ partials,
+                                                  const float* __restrict__ trials = nullptr) {
   using C = Cfg<DC>;
   constexpr int kKD = C::kKD, kWG = C::kWG;
   pdl_enter();   // lets glm_finish_kernel be resident (blocked in its griddepcontrol.wait) before this kernel ends
@@ -133,21 +136,31 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
       const int gp = slab * kM + 16 * w4 + gid + 8 * h;
       bias[h] = (bvec != nullptr && gp < P) ? bvec[gp] : 0.f;
     }
+    // Binomial keeps the labels of two tiles, slot k & 1 of y [64] + trials [64] each, because its epilogue reads
+    // them from shared memory while the next tile lands
+    constexpr bool kRowM = Fam::kTrials == kRowTrials;
+    float mconst = 0.f;                        // the one trial count (kConstTrials)
+    if constexpr (Fam::kTrials == kConstTrials) mconst = *trials;
     // tile it -> landing buffer; one thread of the warpgroup issues the loads
     auto load = [&](int it) {
       const int64_t row0 = (blockIdx.x + (int64_t)it * gridDim.x) * kRows;
       const int rows = (int)(N - row0 < kRows ? N - row0 : kRows);
       const uint32_t xb = (uint32_t)(rows * D) * 4u, yb = (uint32_t)rows * 4u;
       const uint32_t xbulk = xb & ~15u, ybulk = yb & ~15u;
+      const int yo = Fam::kTrials != kNoTrials ? (((it - wg) / kWG) & 1) * 2 * kRows : 0;
       if (rows < kRows || xbulk != xb) {       // the last tile: its remainder and zeros for y past N
         const float* xsrc = X + row0 * D;
         for (uint32_t i = xbulk / 4; i < xb / 4; ++i) land[i] = xsrc[i];
-        for (int i = (int)(ybulk / 4); i < kRows; ++i) ys[i] = (i < rows) ? y[row0 + i] : 0.f;
+        for (int i = (int)(ybulk / 4); i < kRows; ++i) ys[yo + i] = (i < rows) ? y[row0 + i] : 0.f;
+        if constexpr (kRowM)
+          for (int i = (int)(ybulk / 4); i < kRows; ++i) ys[yo + kRows + i] = (i < rows) ? trials[row0 + i] : 0.f;
       }
       // the arrive releases the ordinary stores above to the warpgroup's mbar_wait
-      mbar_expect_tx(bar, xbulk + ybulk);
+      mbar_expect_tx(bar, xbulk + (kRowM ? 2 : 1) * ybulk);
       if (xbulk) bulk_load(my_s + C::WG_LAND, X + row0 * D, xbulk, bar);
-      if (ybulk) bulk_load(my_s + C::WG_Y, y + row0, ybulk, bar);
+      if (ybulk) bulk_load(my_s + C::WG_Y + 4 * yo, y + row0, ybulk, bar);
+      if constexpr (kRowM)
+        if (ybulk) bulk_load(my_s + C::WG_Y + 4 * (yo + kRows), trials + row0, ybulk, bar);
     };
     if (t == 0 && wg < nt) load(wg);
     for (int k = 0, it = wg; it < nt; ++k, it += kWG) {
@@ -201,7 +214,13 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
         }
       }
       typename Fam::Labels yr;                 // read before the refill
-      Fam::read_labels(reinterpret_cast<const uint8_t*>(ys), t4, 1, yr);
+      if constexpr (Fam::kTrials != kNoTrials) {
+        const float* slot = ys + (k & 1) * 2 * kRows;
+        Fam::read_labels(reinterpret_cast<const uint8_t*>(slot), t4, 1, yr);
+        Fam::read_trials(reinterpret_cast<const uint8_t*>(slot + kRows), t4, mconst, yr);
+      } else {
+        Fam::read_labels(reinterpret_cast<const uint8_t*>(ys), t4, 1, yr);
+      }
       fence_proxy_async();
       wg_bar(1 + wg);
       // the landing buffer is free: the warpgroup's next tile arrives while this one is contracted

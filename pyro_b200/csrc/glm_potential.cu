@@ -1,5 +1,5 @@
-// glm_potential.cu -- HMC / NUTS potential energy of Bayesian logistic, softmax, Poisson and linear regression
-// for C chains.
+// glm_potential.cu -- HMC / NUTS potential energy of Bayesian logistic, softmax, Poisson, Binomial and linear
+// regression for C chains.
 //
 //   U[c]    = -( SUM_n log p(y_n | logits_cn) + SUM log Normal(w; 0, s_w) + SUM log Normal(b; 0, s_b) )
 //   grad[c] = dU / dz[c]                                           (in z's layout)
@@ -18,7 +18,8 @@
 // targets the posterior of the data as given, not of X rounded to TF32.
 // Linear regression (b2_glm_normal_potential) runs the same three launches around b2_glm_normal_loc: the pack also
 // writes each chain's noise scale sigma_c = exp(z[c, s_off]) (or the constant), and the finish adds sigma's prior
-// and the Jacobian of sigma = e^t in fp64.
+// and the Jacobian of sigma = e^t in fp64.  Binomial regression (b2_glm_binomial_potential) runs the same three
+// launches around b2_glm_binomial_logits (kernel + finish: four in all) with the trial counts as a fixed operand.
 #include <math.h>
 
 #include "b2_common.cuh"
@@ -257,6 +258,67 @@ extern "C" int b2_glm_normal_potential(const float* X, const float* y, int64_t N
   glm_potential_finish_kernel<<<(unsigned)((C * 32 + 255) / 256), 256, 0, s>>>(
       z, C, Dz, w_off, b_off, D, Kb, s_w, s_b, sum_p, dW, db, U, grad, sig, dsig, Ks ? s_off : (int64_t)-1, s_prior,
       sp0, sp1);
+  count_launch(1);
+  return check_launch();
+}
+
+// ---- Binomial regression: Binomial(m, logits = X @ w + b), m one count for every row or one per row ------------
+// workspace areas, each 256-byte aligned: [b2_glm_binomial_logits workspace][Wp][bp][dW][db][sum_p]
+inline GlmPotentialLayout glm_binomial_potential_layout(int64_t N, int D, int64_t C) {
+  GlmPotentialLayout L;
+  const size_t c = (size_t)C;
+  L.glm = 0;
+  size_t off = round256(b2_glm_binomial_workspace(N, D, (int)C));
+  L.wp = off; off += round256(c * D * sizeof(float));
+  L.bp = off; off += round256(c * sizeof(float));
+  L.dw = off; off += round256(c * D * sizeof(float));
+  L.db = off; off += round256(c * sizeof(float));
+  L.sum_p = off; off += round256(c * sizeof(float));
+  L.total = off;
+  return L;
+}
+
+extern "C" size_t b2_glm_binomial_potential_workspace(int64_t N, int D, int64_t C) {
+  if (N < 1 || D < 1 || D > 128 || C < 1 || C >= ((int64_t)1 << 31)) return 256;
+  return glm_binomial_potential_layout(N, D, C).total;
+}
+
+extern "C" int b2_glm_binomial_potential(const float* X, const float* y, const float* trials, int trials_per_row,
+                                         int64_t N, int D, int has_bias, const float* z, int64_t C, int64_t Dz,
+                                         int64_t w_off, int64_t b_off, double s_w, double s_b, float* U,
+                                         float* grad, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!X || !y || !trials || !z || !U || !grad) return B2_ERR_NULL;
+  if (N < 1 || D < 1 || D > 128 || C < 1 || C >= ((int64_t)1 << 31)) return B2_ERR_BAD_SHAPE;
+  if (trials_per_row != 0 && trials_per_row != 1) return B2_ERR_BAD_SHAPE;
+  const int Kb = has_bias ? 1 : 0;
+  // z's row is exactly the weight block and the bias, neither overlapping the other or out of the row
+  if (Dz != (int64_t)D + Kb || w_off < 0 || w_off + D > Dz) return B2_ERR_BAD_SHAPE;
+  if (has_bias && (b_off < 0 || b_off >= Dz || (b_off >= w_off && b_off < w_off + D))) return B2_ERR_BAD_SHAPE;
+  if (!(s_w > 0.0) || (has_bias && !(s_b > 0.0))) return B2_ERR_BAD_SHAPE;
+  if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
+  if (trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0) return B2_ERR_BAD_SHAPE;
+  const GlmPotentialLayout L = glm_binomial_potential_layout(N, D, C);
+  if (!workspace || workspace_bytes < L.total) return B2_ERR_WORKSPACE;
+  char* ws = reinterpret_cast<char*>(workspace);
+  float* Wp = reinterpret_cast<float*>(ws + L.wp);
+  float* bp = has_bias ? reinterpret_cast<float*>(ws + L.bp) : nullptr;
+  float* dW = reinterpret_cast<float*>(ws + L.dw);
+  float* db = has_bias ? reinterpret_cast<float*>(ws + L.db) : nullptr;
+  float* sum_p = reinterpret_cast<float*>(ws + L.sum_p);
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+
+  const int64_t npack = C * (D + Kb);
+  glm_potential_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(z, C, Dz, w_off, b_off, D, Kb, Wp, bp,
+                                                                             (int64_t)-1, 0.f, nullptr);
+  count_launch(1);
+  int rc = check_launch();
+  if (rc != 0) return rc;
+  // weight = -1: dW and db are derivatives of -loglik; every logit fp32-exact (X split)
+  rc = b2_glm_binomial_logits(X, y, trials, trials_per_row, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
+                              B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws + L.glm, L.wp - L.glm, stream);
+  if (rc != 0) return rc;
+  glm_potential_finish_kernel<<<(unsigned)((C * 32 + 255) / 256), 256, 0, s>>>(
+      z, C, Dz, w_off, b_off, D, Kb, s_w, s_b, sum_p, dW, db, U, grad, nullptr, nullptr, (int64_t)-1, 0, 0.0, 0.0);
   count_launch(1);
   return check_launch();
 }

@@ -1,7 +1,7 @@
 // glm_tc_common.cuh -- device helpers shared by the Hopper wgmma kernels (glm_tc.cu, glm_flat_tc.cu,
-// glm_categorical_tc.cu, glm_poisson_tc.cu, glm_normal_tc.cu, poisson_product_tc.cu): mbarriers, TMA tile
-// loads, SWIZZLE_128B operand descriptors, the TF32 wgmma wrappers, MUFU wrappers and TF32 rounding, the
-// Bernoulli, Poisson and Normal epilogues and families, the stages of the GLM tile pipeline and the D = 32 pipeline itself, and the
+// glm_categorical_tc.cu, glm_poisson_tc.cu, glm_normal_tc.cu, glm_binomial_tc.cu, poisson_product_tc.cu): mbarriers,
+// TMA tile loads, SWIZZLE_128B operand descriptors, the TF32 wgmma wrappers, MUFU wrappers and TF32 rounding, the
+// Bernoulli, Poisson, Normal and Binomial epilogues and families, the stages of the GLM tile pipeline and the D = 32 pipeline itself, and the
 // host-side tensor-map encoders.
 #pragma once
 #include <cuda.h>
@@ -381,16 +381,61 @@ __device__ __forceinline__ void normal_epilogue(const float (&acc1)[32], const f
   }
 }
 
+// ---- Binomial epilogue of the aggregated logistic-regression kernels (glm_binomial_tc.cu) -------------------
+// lp = y*l - m*softplus(l) (the parameter-free log binomial coefficient is summed once per call, not here) and
+// g = y - m*sigmoid(l) rounded to nearest TF32, for y successes out of m trials: ex2, rcp and lg2 per logit.  The
+// linear part is y*l for l < 0 and (y - m)*l otherwise, exact for integer counts.  y and m are read from shared
+// memory here (ROW: one m per row, else the count mc of every row).  The bias is added here, as in
+// poisson_epilogue.  MASK (the last, partial tile only) zeroes rows past N.
+// (The running product of epi_batch, one lg2 per particle and tile for one count of every row, made the 128-register
+// kernels spill.)
+template <bool MASK, bool ROW>
+__device__ __forceinline__ void binomial_epilogue(const float (&acc1)[32], const float (&bias)[2],
+                                                  const float2* yr, const float2* mr, float mc, int64_t row0,
+                                                  int64_t N, int t4, float (&lpa)[2], uint32_t (&g)[32]) {
+  // k-block outermost: the labels of a k-block serve both particles of the thread and are dead after it
+  float s[2] = {0.f, 0.f};
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float2 y2 = yr[4 * j], m2 = ROW ? mr[4 * j] : make_float2(mc, mc);
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int i = 4 * j + 2 * h + e;
+        const float l = acc1[i] + bias[h], yy = e ? y2.y : y2.x, m = e ? m2.y : m2.x;
+        const float ex = ex2f(-1.4426950408889634f * fabsf(l));
+        const float den = 1.f + ex, inv = rcpf(den);
+        const float sg = (l >= 0.f) ? inv : ex * inv;
+        float lp = fmaf(-0.6931471805599453f * m, lg2f(den), (l >= 0.f ? yy - m : yy) * l);
+        float gg = fmaf(-m, sg, yy);
+        if (MASK) {
+          const bool v = row0 + 8 * j + 2 * t4 + e < N;
+          lp = v ? lp : 0.f;
+          gg = v ? gg : 0.f;
+        }
+        s[h] += lp;
+        g[i] = __float_as_uint(tf32_rn(gg));
+      }
+  }
+  lpa[0] += s[0];
+  lpa[1] += s[1];
+}
+
 // ---- likelihood families of the GLM tile pipelines ----------------------------------------------------------
 // Fam is the likelihood family: kBiasInEpilogue (the bias is added by the epilogue, which then takes it after
 // acc1, instead of starting GEMM 1's accumulator), kKP (GEMM 1 rows per particle), kYBytes (labels of one
 // tile), kYType (their TMA type), Labels (a thread's labels of one tile), read_labels(stage, t4, K, labels) and epilogue(acc1, labels,
 // cls, K, row0, N, t4, lpa, g), which writes g (indexed like acc1, rounded to TF32) and adds the tile's lp sums
 // of the thread's two rows to lpa; the any-D tile loop (glm_flat_tc.cuh) calls tile_epilogue(acc1, labels,
-// row0, N, t4, last, lpa, g) instead.
+// row0, N, t4, last, lpa, g) instead.  kTrials (Binomial only) adds a second label operand, the trial counts:
+// one device value for every row (kConstTrials) or one per row (kRowTrials, loaded next to y on the same
+// mbarrier); read_trials(stage + 256, t4, m, labels) then completes the labels.
+enum : int { kNoTrials = 0, kConstTrials = 1, kRowTrials = 2 };
 
 // logistic regression: one GEMM 1 row per particle, fp32 labels y
 struct Bernoulli {
+  static constexpr int kTrials = kNoTrials;
   static constexpr bool kBiasInEpilogue = false;  // GEMM 1's accumulator starts at the bias
   static constexpr int kKP = 1;
   static constexpr uint32_t kYBytes = kRows * 4;  // 256 B of y
@@ -449,6 +494,45 @@ struct Normal : Bernoulli {
                                                   const int (&)[2], int, int64_t row0, int64_t N, int t4,
                                                   float (&lpa)[2], uint32_t (&g)[32]) {
     tile_epilogue(acc1, bias, y, row0, N, t4, row0 + kRows > N, lpa, g);
+  }
+};
+
+// Binomial regression (logit link): fp32 successes y and trial counts m, one for every row (ROW = false, a
+// device value read once per call) or one per row (ROW: [N] fp32, loaded next to y).  GEMM 1 starts from zero
+// and the epilogue adds the bias, see binomial_epilogue.
+template <bool ROW>
+struct Binomial : Bernoulli {
+  static constexpr int kTrials = ROW ? kRowTrials : kConstTrials;
+  static constexpr bool kBiasInEpilogue = true;
+  static constexpr uint32_t kYBytes = (ROW ? 2 : 1) * kRows * 4;   // y, then the trials of the tile
+  // The labels stay in shared memory until the epilogue reads them (y and m of the thread's rows n = 8j + 2 t4 + e
+  // at y[4j], m[4j]): held in registers across GEMM 1 they made the 128-register kernels spill.  So the tile
+  // pipelines keep a tile's labels in place until its epilogue is done: glm_tile_pipeline refills a stage one
+  // tile later, glm_flat_pipeline alternates two label slots.
+  struct Labels {
+    const float2* y;
+    const float2* m;                            // ROW only
+    float mc;                                   // the trial count of every row (ROW = false)
+  };
+  static __device__ __forceinline__ void read_labels(const uint8_t* ys, int t4, int, Labels& lab) {
+    lab.y = reinterpret_cast<const float2*>(ys) + t4;
+  }
+  static __device__ __forceinline__ void read_trials(const uint8_t* ms, int t4, float mc, Labels& lab) {
+    lab.m = reinterpret_cast<const float2*>(ms) + t4;
+    lab.mc = mc;
+  }
+  static __device__ __forceinline__ void tile_epilogue(const float (&acc1)[32], const float (&bias)[2],
+                                                       const Labels& lab, int64_t row0, int64_t N, int t4,
+                                                       bool last, float (&lpa)[2], uint32_t (&g)[32]) {
+    if (last)
+      binomial_epilogue<true, ROW>(acc1, bias, lab.y, lab.m, lab.mc, row0, N, t4, lpa, g);
+    else
+      binomial_epilogue<false, ROW>(acc1, bias, lab.y, lab.m, lab.mc, row0, N, t4, lpa, g);
+  }
+  static __device__ __forceinline__ void epilogue(const float (&acc1)[32], const float (&bias)[2],
+                                                  const Labels& lab, const int (&)[2], int, int64_t row0,
+                                                  int64_t N, int t4, float (&lpa)[2], uint32_t (&g)[32]) {
+    tile_epilogue(acc1, bias, lab, row0, N, t4, row0 + kRows > N, lpa, g);
   }
 };
 
@@ -600,11 +684,13 @@ struct Smem32 {
   static_assert((kWG * kM * 33 + kWG * kM) * 4 <= kStages * kTile, "reduction scratch");
 };
 
-// Fam is the likelihood family (Bernoulli, Poisson above, Softmax of glm_categorical_tc.cu).
+// Fam is the likelihood family (Bernoulli, Poisson, Normal, Binomial above, Softmax of glm_categorical_tc.cu).
+// Binomial only: map_m is the trials' label map (kRowTrials), trials the one device count (kConstTrials).
 template <class Fam, bool SPLIT_X>
 __device__ __forceinline__ void glm_tile_pipeline(const CUtensorMap& map_x, const CUtensorMap& map_y,
                                                   const float* W, const float* bvec, int64_t N, int P, int K,
-                                                  float* partials) {
+                                                  float* partials, const CUtensorMap* map_m = nullptr,
+                                                  const float* trials = nullptr) {
   using L = Smem32<Fam::kYBytes>;
   constexpr int KP = Fam::kKP;
   constexpr uint32_t kYBytes = Fam::kYBytes;
@@ -636,6 +722,8 @@ __device__ __forceinline__ void glm_tile_pipeline(const CUtensorMap& map_x, cons
     mbar_expect_tx(bar_full(s), kTile + kYBytes);
     tma_load_2d(base + L::OFF_X + s * kTile, &map_x, 0, (int)(tile * kRows), bar_full(s));
     tma_load_1d(base + L::OFF_Y + s * kYBytes, &map_y, (int)(tile * kRows), bar_full(s));
+    if constexpr (Fam::kTrials == kRowTrials)
+      tma_load_1d(base + L::OFF_Y + s * kYBytes + kRows * 4, map_m, (int)(tile * kRows), bar_full(s));
   };
   // Each warpgroup's first two X / label tiles are requested BEFORE griddepcontrol.wait, so they stream while the
   // predecessor (the step's draw kernel, on a CTA or two) finishes.  Sound because no native kernel that can
@@ -667,6 +755,8 @@ __device__ __forceinline__ void glm_tile_pipeline(const CUtensorMap& map_x, cons
     cls[h] = m % KP;
     bias[h] = (bvec != nullptr && gp < P && cls[h] < K) ? bvec[(int64_t)gp * K + cls[h]] : 0.f;
   }
+  float mconst = 0.f;                          // Binomial with one trial count for every row
+  if constexpr (Fam::kTrials == kConstTrials) mconst = *trials;
 
   {
     uint8_t* my = sm + L::OFF_WG + wg * kWGBytes;
@@ -720,8 +810,14 @@ __device__ __forceinline__ void glm_tile_pipeline(const CUtensorMap& map_x, cons
       }
       typename Fam::Labels lab;                // read before the refill
       Fam::read_labels(sm + L::OFF_Y + s * kYBytes, t4, K, lab);
+      if constexpr (Fam::kTrials != kNoTrials)
+        Fam::read_trials(sm + L::OFF_Y + s * kYBytes + kRows * 4, t4, mconst, lab);
       fence_proxy_async();
       wg_bar(1 + wg);
+      // Binomial reads its labels from the stage in the epilogue: the stage of the previous tile, whose epilogue
+      // every thread of the warpgroup has now finished, is refilled here instead of after GEMM 1
+      if constexpr (Fam::kTrials != kNoTrials)
+        if (t == 0 && k > 0 && it + kWG < nt) load(it + kWG, s ^ 1);
       float acc1[32];
       if constexpr (Fam::kBiasInEpilogue) {
         const float zero[2] = {0.f, 0.f};
@@ -732,7 +828,8 @@ __device__ __forceinline__ void glm_tile_pipeline(const CUtensorMap& map_x, cons
                           my_s + WG_XLO);
       }
       // GEMM 1 has read the X stage and the labels are in registers: refill the stage with tile it + 2 kWG
-      if (t == 0 && it + 2 * kWG < nt) load(it + 2 * kWG, s);
+      if constexpr (Fam::kTrials == kNoTrials)
+        if (t == 0 && it + 2 * kWG < nt) load(it + 2 * kWG, s);
       uint32_t g[32];
       if constexpr (Fam::kBiasInEpilogue)
         Fam::epilogue(acc1, bias, lab, cls, K, row0, N, t4, lpa, g);

@@ -39,6 +39,8 @@ int eval_t(int family, int grad, int64_t n, const T* x, const T* const* p, T* lp
       B2H_CASE(kKLGammaGamma)
       B2H_CASE(kNormalRsample)
       B2H_CASE(kNormalRsampleBwd)
+      B2H_CASE(kBinomialLogits)
+      B2H_CASE(kBinomialProbs)
       default:
         return -3;
     }

@@ -33,10 +33,11 @@ int dispatch_site(int family, int dtype, bool grad, const SiteArgs& a, int kind,
   if (family < 0 || family >= kNumElementwise) return B2_ERR_BAD_FAMILY;
   if (family <= kPoisson) return dispatch_site_a(family, dtype, grad, a, kind, s);
   if (family <= kHalfNormal) return dispatch_site_b(family, dtype, grad, a, kind, s);
-  return dispatch_site_c(family, dtype, grad, a, kind, s);
+  if (family <= kNormalRsampleBwd) return dispatch_site_c(family, dtype, grad, a, kind, s);
+  return dispatch_site_d(family, dtype, grad, a, kind, s);
 }
 
-static const int kFamilyNumParams[kNumElementwise] = {2, 1, 2, 2, 1, 2, 1, 1, 2, 1, 1, 2, 4, 4, 2, 3};
+static const int kFamilyNumParams[kNumElementwise] = {2, 1, 2, 2, 1, 2, 1, 1, 2, 1, 1, 2, 4, 4, 2, 3, 2, 2};
 
 }  // namespace b2
 

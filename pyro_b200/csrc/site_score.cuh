@@ -282,7 +282,8 @@ struct VecBody {
 // Poisson) are bound by instruction issue, not by loads in flight: 2 vectors (4 would only cost registers).
 template <int FAM, typename T, bool GRAD>
 struct VecUnroll {
-  static constexpr bool kHeavy = (FAM == kGamma || FAM == kBeta || FAM == kPoisson);
+  static constexpr bool kHeavy =
+      (FAM == kGamma || FAM == kBeta || FAM == kPoisson || FAM == kBinomialLogits || FAM == kBinomialProbs);
   static constexpr int U = (sizeof(T) == 4 && !GRAD && !kHeavy) ? 4 : 2;
   static constexpr int kMinBlocks = (sizeof(T) == 8 && GRAD) ? 2 : 3;
 };
@@ -576,6 +577,7 @@ int launch_site(const SiteArgs& a, int kind, cudaStream_t stream) {
 int dispatch_site_a(int family, int dtype, bool grad, const SiteArgs& a, int kind, cudaStream_t s);
 int dispatch_site_b(int family, int dtype, bool grad, const SiteArgs& a, int kind, cudaStream_t s);
 int dispatch_site_c(int family, int dtype, bool grad, const SiteArgs& a, int kind, cudaStream_t s);
+int dispatch_site_d(int family, int dtype, bool grad, const SiteArgs& a, int kind, cudaStream_t s);
 
 #define B2_DISPATCH_CASE(FAM)                                                         \
   case FAM:                                                                           \

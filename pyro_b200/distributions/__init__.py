@@ -617,6 +617,47 @@ class Bernoulli(_Elementwise):
         return self._torch().sample(sample_shape)
 
 
+class Binomial(_Elementwise):
+    """Binomial(total_count, probs | logits) of pyro/distributions/torch.py:83-101 with ``approx_log_prob_tol = 0``
+    (the exact log binomial coefficient).  Gradients are those autograd gives for the reference expression, whose
+    ``log_binomial`` is gradient-free: d/dlogits = k - n sigmoid(logits), d/dtotal_count = -softplus(logits)."""
+    arg_constraints = {"total_count": constraints.nonnegative_integer, "probs": constraints.unit_interval,
+                       "logits": constraints.real}
+    has_rsample = False
+
+    def __init__(self, total_count=1, probs=None, logits=None, validate_args=None):
+        if (probs is None) == (logits is None):
+            raise ValueError("Either `probs` or `logits` must be specified, but not both.")
+        param = logits if logits is not None else probs
+        param, total_count = _broadcast_params(param, total_count)
+        if not total_count.is_floating_point() or total_count.dtype != param.dtype:
+            total_count = total_count.to(param.dtype)
+        if logits is not None:
+            self.family = N.BINOMIAL_LOGITS
+            self.param_names = ("total_count", "logits")
+        else:
+            self.family = N.BINOMIAL_PROBS
+            self.param_names = ("total_count", "probs")
+        super().__init__(total_count, param)
+
+    @constraints.dependent_property(is_discrete=True, event_dim=0)
+    def support(self):
+        return constraints.integer_interval(0, self.total_count)
+
+    def _torch(self):
+        n, p = (t.expand(self.batch_shape) if tuple(t.shape) != tuple(self.batch_shape) else t
+                for t in self._params)
+        if self.family == N.BINOMIAL_LOGITS:
+            return torch.distributions.Binomial(n, logits=p, validate_args=False)
+        return torch.distributions.Binomial(n, probs=p, validate_args=False)
+
+    def rsample(self, sample_shape=torch.Size()):
+        raise NotImplementedError("Binomial has no rsample")
+
+    def sample(self, sample_shape=torch.Size()):
+        return self._torch().sample(sample_shape)
+
+
 # ---------------------------------------------------------------------------------------------
 # event families
 # ---------------------------------------------------------------------------------------------
@@ -994,7 +1035,7 @@ def fused_kl_sum(p, q, mask, scale, weight, sum_coeff, unit=True):
                                scale=scale, weight=weight, sum_coeff=sum_coeff, assume_unit_upstream=unit)
 
 
-__all__ = ["Distribution", "Normal", "Bernoulli", "Gamma", "Beta", "Poisson", "Cauchy", "HalfCauchy",
+__all__ = ["Distribution", "Normal", "Bernoulli", "Binomial", "Gamma", "Beta", "Poisson", "Cauchy", "HalfCauchy",
            "HalfNormal", "LogNormal", "Exponential", "Uniform", "Dirichlet", "Categorical",
            "MultivariateNormal", "Delta", "Independent", "MaskedDistribution", "ScoreParts",
            "kl_divergence", "scale_and_mask", "is_identically_zero", "is_identically_one"]
@@ -1653,6 +1694,145 @@ def _normal_new(cls, loc=None, scale=None, validate_args=None):
 
 
 Normal.__new__ = staticmethod(_normal_new)
+
+
+# ---------------------------------------------------------------------------------------------
+# fused Binomial regression: Binomial(total_count, logits = X @ w + b)
+# ---------------------------------------------------------------------------------------------
+class _GlmBinomialFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, meta, X, y, trials, W, b):
+        scale, weight, coeff, unit, per_row = meta
+        N.require_cuda(X, "fused Binomial-regression likelihood")
+        P, D = W.shape
+        n = X.shape[0]
+        dev = X.device
+        Wc = W.contiguous()
+        bc = b.contiguous() if b is not None else None
+        total = torch.empty((), dtype=torch.float32, device=dev)
+        dW = torch.empty(P, D, dtype=torch.float32, device=dev)
+        db = torch.empty(P, dtype=torch.float32, device=dev)
+        need = int(N.lib().b2_glm_binomial_workspace(n, D, P))
+        ws = N.workspace(dev, need, tag="glm")
+        N.check(N.lib().b2_glm_binomial_logits(
+            X.data_ptr(), y.data_ptr(), trials.data_ptr(), per_row, Wc.data_ptr(),
+            bc.data_ptr() if bc is not None else None, n, D, P, float(scale), float(weight), float(coeff), 0, None,
+            total.data_ptr(), dW.data_ptr(), db.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(dev)),
+            "b2_glm_binomial_logits")
+        ctx.grads = (dW, db if b is not None else None)
+        ctx.unit = unit
+        return total
+
+    @staticmethod
+    def backward(ctx, gout):
+        dW, db = ctx.grads
+        if not ctx.unit:
+            dW = dW * gout
+            db = db * gout if db is not None else None
+        return None, None, None, None, dW, db
+
+
+def _unexpanded(t):
+    """The stored tensor behind a stride-0 expansion (``broadcast_all`` of pyro_b200/lazy.py remembers it; an expand
+    of a tensor that is not itself a view has it as its autograd base), ``t`` itself when it is not an expansion,
+    None for anything else, such as an expansion of a slice."""
+    if all(s == 1 or st != 0 for s, st in zip(t.shape, t.stride())):
+        return t
+    base = getattr(t, "_b2_unexpanded", None)
+    base = t._base if base is None else base
+    if base is None or base.dim() > t.dim() or base.data_ptr() != t.data_ptr():
+        return None
+    try:
+        if torch.broadcast_shapes(base.shape, t.shape) != t.shape:
+            return None
+    except RuntimeError:
+        return None
+    return base if base.expand(t.shape).stride() == t.stride() else None
+
+
+def _binomial_trials(total_count, lp):
+    """``(trials, per_row)`` for the fused kernel: ONE count (a number, ``[]``, ``[1]``) as a 1-element device tensor
+    (per_row 0), or the counts of the N rows (``[N]``, contiguous, 16-byte aligned) as stored (per_row 1); None for
+    any other total_count, one that requires grad, or a slice of one."""
+    t = densify(total_count)
+    if type(t).__name__ == "SiteValue":
+        t = _ops.plain_value(t)
+    if not isinstance(t, torch.Tensor) or t.requires_grad or t.dtype != torch.float32 or t.device != lp.X.device:
+        return None
+    t = _unexpanded(t)
+    if t is None:
+        return None
+    n = lp.X.shape[0]
+    if t.numel() == 1 and t.dim() <= len(lp.shape):
+        return t.reshape(1), 0
+    if t.dim() >= 1 and t.shape[-1] == n and t.numel() == n and t.is_contiguous() and t.data_ptr() % 16 == 0:
+        return t.reshape(n), 1
+    return None
+
+
+class _BinomialLinear(Binomial):
+    """Binomial whose logits are a lazy ``X @ w + b`` (built by ``Binomial(total_count, logits=lazy)``, also when an
+    unchanged model's linear predictor was kept lazy by pyro_b200/lazy.py).  ``logits``, ``log_prob``, ``sample`` and
+    every other use materialise the logits as the model wrote them, bit for bit; the ELBO's site sum takes the fused
+    kernel (``b2_glm_binomial_logits``) when total_count is one count or one count per row."""
+
+    def __init__(self, total_count=1, probs=None, logits=None, validate_args=None):
+        lz = _lazy_of(logits)
+        self._lazy, self._logits_src = lz, logits
+        self.family = N.BINOMIAL_LOGITS
+        self.param_names = ("total_count", "logits")
+        tc = total_count
+        if isinstance(tc, Number):
+            tc = _const(tc, lz.dtype, lz.device)
+        elif not tc.is_floating_point() or tc.dtype != lz.dtype:
+            tc = tc.to(lz.dtype)
+        self._total_count = tc
+        self._dense = None
+        Distribution.__init__(self, torch.broadcast_shapes(tc.shape, lz.shape))
+
+    @property
+    def _params(self):
+        if self._dense is None:
+            src = self._logits_src
+            self._dense = src.eager() if hasattr(src, "eager") else self._lazy.dense()
+        return [self._total_count, self._dense]
+
+    @property
+    def total_count(self):
+        return self._total_count
+
+    @property
+    def logits(self):
+        return self._params[1]
+
+    def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
+        lp = self._lazy
+        X = lp.X
+        D = X.shape[-1]
+        # the scope of the any-D logistic-regression kernel: tensor cores asked for, 1 <= D <= 128, from 8192 rows
+        # (below that the TF32 gradient has not averaged its rounding down to fp32 accuracy yet), fp32, contiguous
+        # 16-byte aligned X, y and trials, no mask, one count or one count per row
+        ok = (mask is None and X.dtype == torch.float32 and X.is_contiguous() and X.data_ptr() % 16 == 0
+              and 1 <= D <= 128 and getattr(lp, "tensor_cores", True) and X.shape[0] >= 8192
+              and isinstance(value, torch.Tensor) and value.numel() == X.shape[0]
+              and tuple(self.batch_shape) == tuple(lp.shape))
+        trials = _binomial_trials(self._total_count, lp) if ok else None
+        y = value.reshape(-1).to(torch.float32).contiguous() if trials is not None else None
+        if trials is None or y.data_ptr() % 16 != 0:
+            return super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
+        W = lp.w.reshape(lp.P, D)
+        b = lp.b.reshape(lp.P) if lp.b is not None else None
+        return _GlmBinomialFn.apply((scale, weight, sum_coeff, unit, trials[1]), X, y, trials[0], W, b)
+
+
+def _binomial_new(cls, total_count=1, probs=None, logits=None, validate_args=None):
+    # ``Binomial(total_count, logits=lazy X @ w + b)`` builds the fused Binomial-regression subclass
+    if cls is Binomial and probs is None and _lazy_of(logits) is not None:
+        return object.__new__(_BinomialLinear)
+    return object.__new__(cls)
+
+
+Binomial.__new__ = staticmethod(_binomial_new)
 __all__ += ["LinearPredictor", "linear_predictor", "ExpLinearPredictor", "ClassLinearPredictor",
             "class_linear_predictor", "FactorProduct", "constant"]
 

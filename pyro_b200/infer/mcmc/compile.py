@@ -182,9 +182,10 @@ def _try_logistic(poutine, model, args, kwargs, latent, observed):
 
 
 def _try_glm(poutine, model, args, kwargs, latent, observed):
-    """Logistic regression with an intercept, or softmax, Poisson (log link) or linear regression with or without
-    one, in fp32, within the GLM kernels' scope: Bernoulli D in {4, 8, 16, 32}; Categorical D == 32, 2 <= K <= 16;
-    Poisson and Normal 1 <= D <= 128.  Linear regression's noise scale is a constant or one latent scalar site with
+    """Logistic regression with an intercept, or softmax, Poisson (log link), Binomial (logit link) or linear
+    regression with or without one, in fp32, within the GLM kernels' scope: Bernoulli D in {4, 8, 16, 32};
+    Categorical D == 32, 2 <= K <= 16; Poisson, Binomial and Normal 1 <= D <= 128.  Binomial's total_count is a
+    constant or gradient-free fp32 [N] counts, the same at every probe.  Linear regression's noise scale is a constant or one latent scalar site with
     a constant-parameter HalfNormal, HalfCauchy, Exponential or LogNormal prior."""
     from .potential import GlmPotential
     if len(observed) != 1 or len(latent) not in (1, 2, 3):
@@ -194,8 +195,8 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
     # lazy linear-predictor logits build _BernoulliLinear / _CategoricalLinear (pyro_b200/distributions)
     # (and _PoissonLinear for a lazy exp of one, _NormalLinear for a lazy loc)
     kind = {"BernoulliLinear": "Bernoulli", "CategoricalLinear": "Categorical",
-            "PoissonLinear": "Poisson", "NormalLinear": "Normal"}.get(kind, kind)
-    if kind not in ("Bernoulli", "Categorical", "Poisson", "Normal") or not _plain_site(obs):
+            "PoissonLinear": "Poisson", "NormalLinear": "Normal", "BinomialLinear": "Binomial"}.get(kind, kind)
+    if kind not in ("Bernoulli", "Categorical", "Poisson", "Normal", "Binomial") or not _plain_site(obs):
         return None
     # linear regression: at most one latent noise-scale site, positive support (z holds its log)
     order = list(latent)                   # TracePotential's site order
@@ -249,7 +250,7 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
         wshapes, bshapes = [(D,)], [(), (1,)]
         if D not in (4, 8, 16, 32) or y.dtype != torch.float32:
             return None
-    elif kind in ("Poisson", "Normal"):
+    elif kind in ("Poisson", "Normal", "Binomial"):
         K = 1
         wshapes, bshapes = [(D,)], [(), (1,)]
         if not 1 <= D <= 128 or y.dtype != torch.float32:
@@ -271,6 +272,11 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
     # log(rate) == X @ w + b ----------------------------------------------------------------------------------
     gen = torch.Generator(device="cpu").manual_seed(20240302)
     sigma_const = None
+    trials = None                          # Binomial: the constant count, or the [N] counts of the prototype
+    if kind == "Binomial":
+        trials = _binomial_trials(_base(obs["fn"])[0], n)
+        if trials is None:
+            return None
     for _ in range(3):
         wv = torch.randn(shapes[weight], generator=gen).to(X)
         if kind == "Poisson":
@@ -293,11 +299,19 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
                     return None
                 sigma_const = c
             logits = pfn.loc
+        elif kind == "Binomial":
+            # logits as the model gave them (not probs), and the same trial counts at every probe
+            t = _binomial_trials(pfn, n)
+            if t is None or type(t) is not type(trials) or (
+                    isinstance(t, float) and t != trials) or (
+                    isinstance(t, torch.Tensor) and not torch.equal(t, trials)):
+                return None
+            logits = pfn.logits
         else:
             logits = torch.log(pfn.rate) if kind == "Poisson" else pfn.logits
         if hasattr(logits, "dense"):
             logits = logits.dense()
-        if kind in ("Poisson", "Normal"):
+        if kind in ("Poisson", "Normal", "Binomial"):
             want = X @ wv + (bv.reshape(()) if bv is not None else 0.0)
         elif kind == "Bernoulli":
             want = X @ wv + bv.reshape(())
@@ -320,7 +334,28 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
     return GlmPotential(X, y.detach(), kind, sites, weight, bias, s_w=scales[weight],
                         s_b=scales[bias] if bias is not None else 1.0,
                         sigma=sigma_const if sigma_const is not None else 1.0, sigma_site=sigma_site,
-                        sigma_prior=sigma_prior)
+                        sigma_prior=sigma_prior, trials=trials)
+
+
+def _binomial_trials(fn, n):
+    """The trial counts of a logits-parameterised Binomial with ``n`` rows: a python float when they are one
+    gradient-free value, else the fp32 ``[n]`` counts (no gradient); None for a Binomial given ``probs`` or any other
+    total_count."""
+    if getattr(fn, "family", None) is not None:
+        from ... import _native as N
+        if fn.family != N.BINOMIAL_LOGITS:
+            return None
+    elif "logits" not in fn.__dict__:
+        return None
+    tc = fn.total_count
+    if not isinstance(tc, torch.Tensor) or tc.requires_grad or tc.dtype != torch.float32:
+        return None
+    c = _const(tc)
+    if c is not None:
+        return c
+    if tc.numel() != n:
+        return None
+    return tc.detach().reshape(n)
 
 
 def recognise(model, args=(), kwargs=None, poutine=None):

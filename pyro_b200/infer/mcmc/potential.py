@@ -116,6 +116,8 @@ class GlmPotential:
     ``W ~ Normal(0, s_w)[K, D]``, ``b ~ Normal(0, s_b)[K]`` (optional),
     ``y ~ Categorical(logits = X @ W.mT + b)``, or
     ``w ~ Normal(0, s_w)[D]``, ``b ~ Normal(0, s_b)`` (optional), ``y ~ Poisson(rate = exp(X @ w + b))``, or
+    ``y ~ Binomial(trials, logits = X @ w + b)`` with ``trials`` one count or ``[N]`` counts
+    (``b2_glm_binomial_potential``), or
     ``w ~ Normal(0, s_w)[D]``, ``b ~ Normal(0, s_b)`` (optional), ``y ~ Normal(X @ w + b, sigma)`` with a constant
     ``sigma`` or a latent one (``sigma_site``) whose prior ``sigma_prior = (kind, p0, p1)`` is HalfNormal(p0),
     HalfCauchy(p0), Exponential(p0) or LogNormal(p0, p1); z then holds ``log sigma`` (transform ``"exp"``) and U
@@ -131,7 +133,7 @@ class GlmPotential:
                      "Exponential": N.SIGMA_EXPONENTIAL, "LogNormal": N.SIGMA_LOGNORMAL}
 
     def __init__(self, X, y, kind, sites, weight, bias=None, s_w=1.0, s_b=1.0, sigma=1.0, sigma_site=None,
-                 sigma_prior=None):
+                 sigma_prior=None, trials=None):
         N.require_cuda(X, "GlmPotential")
         if X.dtype != torch.float32 or X.dim() != 2:
             raise ValueError("GlmPotential needs fp32 X of shape [N, D]")
@@ -144,7 +146,15 @@ class GlmPotential:
         else:
             self.sigma_prior = (N.SIGMA_CONST, 0.0, 0.0)
         self.kind = {"Bernoulli": N.GLM_BERNOULLI, "Categorical": N.GLM_CATEGORICAL, "Poisson": N.GLM_POISSON,
-                     "Normal": None}[kind]
+                     "Normal": None, "Binomial": None}[kind]
+        self.binomial = kind == "Binomial"
+        if self.binomial:
+            # one count (on the device, read by the kernel) or the [N] counts, private and 16-byte aligned
+            if isinstance(trials, torch.Tensor):
+                self.trials, self.trials_per_row = trials.detach().to(X.device, torch.float32).reshape(-1).clone(), 1
+            else:
+                self.trials = torch.full((1,), float(trials), dtype=torch.float32, device=X.device)
+                self.trials_per_row = 0
         # private contiguous copies: the kernels load y with TMA (16-byte aligned)
         self.y = (y.to(torch.int64) if self.kind == N.GLM_CATEGORICAL else y.to(torch.float32)).clone()
         self.sites = dict(sites)
@@ -180,6 +190,15 @@ class GlmPotential:
                 self.X.data_ptr(), self.y.data_ptr(), self.n, self.Dx, int(self.has_bias), z.data_ptr(), C, self.D,
                 self.w_off, self.b_off, s_off, self.s_w, self.s_b, pk, p0, p1, self.sigma, U.data_ptr(),
                 g.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(z.device)), "b2_glm_normal_potential")
+            return U, g
+        if self.binomial:
+            need = int(lib.b2_glm_binomial_potential_workspace(self.n, self.Dx, C))
+            ws = N.workspace(z.device, need, tag="glm_potential")
+            N.check(lib.b2_glm_binomial_potential(
+                self.X.data_ptr(), self.y.data_ptr(), self.trials.data_ptr(), self.trials_per_row, self.n, self.Dx,
+                int(self.has_bias), z.data_ptr(), C, self.D, self.w_off, self.b_off, self.s_w, self.s_b,
+                U.data_ptr(), g.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(z.device)),
+                "b2_glm_binomial_potential")
             return U, g
         need = int(lib.b2_glm_potential_workspace(self.kind, self.n, self.Dx, self.K, C))
         ws = N.workspace(z.device, need, tag="glm_potential")

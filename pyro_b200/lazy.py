@@ -24,6 +24,10 @@ Poisson regression has one more: ``torch.exp(t)`` or ``t.exp()`` of a lazy ``X @
 ``b2_glm_poisson_log_rate``; any other use, ``+ offset`` and ``* c`` included, materialises ``exp`` of the
 eager expression, bit for bit.
 
+Binomial regression needs one: ``Binomial(total_count, logits=lazy X @ w + b)`` scores the site with
+``b2_glm_binomial_logits``; torch's constructor calls ``broadcast_all(total_count, logits)``, which keeps the logits
+lazy and expands the count, and ``total_count.type_as(logits)``, which is answered without materialising them.
+
 Linear regression needs no new seam: ``Normal(lazy X @ w + b, sigma)`` with one noise scale per particle (a
 number, ``[]``, ``[1]``, ``[P, 1]``) scores the site with ``b2_glm_normal_loc``; ``broadcast_all(loc, sigma)`` of
 ``torch.distributions.Normal`` keeps the loc lazy and expands sigma.
@@ -359,6 +363,15 @@ class LinearPredictorTensor(torch.Tensor):
                     v._b2_unexpanded = plain
                     out.append(v)
                 return tuple(out)
+            # torch.distributions.Binomial casts the broadcast total_count with ``type_as(logits)``: answered from
+            # the metadata, so the logits stay lazy and the cast count keeps what it expanded
+            if name == "type_as" and len(args) == 2 and args[1] is self and not kwargs \
+                    and isinstance(args[0], torch.Tensor) and not isinstance(args[0], LinearPredictorTensor):
+                a = args[0]
+                if a.dtype == self.dtype and a.device == self.device:
+                    return a
+                with torch._C.DisableTorchFunctionSubclass():
+                    return a.to(dtype=self.dtype, device=self.device)
             if name in ("detach", "clone", "contiguous", "float", "to") and len(args) == 1 and not kwargs:
                 return self
             # distribution-argument validation (constraints.real.check): an affine image of finite
