@@ -161,8 +161,17 @@ struct GlmElbo {
 // statistics of the Normal tile kernel into the lp sum and gradients: the lp slot holds S = SUM (y - l)^2 and
 // dW / db hold SUM (y - l) [x | 1]; the warp of sum_p[p] also writes out_dsigma[p] (nullable), n is N.
 // One WARP per entry of the [P, K (D + 1) + 1] table: lanes stride over the CTAs (L2-resident partials),
-// then a shuffle tree (a thread-per-entry loop is a chain of ~300 dependent loads).  With E, E->n_jobs *
-// E->nwarps more warps score the priors, and the ticket counts them too.
+// then a shuffle tree (a thread-per-entry loop is a chain of ~300 dependent loads).  The 8 warps of a CTA
+// take 8 adjacent entries, whose partials are one 32-byte sector per CTA: the CTA first copies that
+// [nblocks][8] slice to shared memory, every thread's loads issued at once, so the sum of a warp's lane reads
+// no global memory (read directly, a warp's lanes would touch one sector per CTA for 4 useful bytes each).
+// With E, E->n_jobs * E->nwarps more warps score the priors, and the ticket counts them too.
+constexpr int kFinishThreads = 256;
+constexpr int kFinishEntries = kFinishThreads / 32;      // entries (warps) per CTA
+constexpr int kFinishMaxBlocks = 2 * kNumSMs;             // nblocks <= glm_grid_x, glm_tc_grid_x
+constexpr int kFinishLoads = (kFinishMaxBlocks * kFinishEntries + kFinishThreads - 1) / kFinishThreads;
+constexpr int kFinishPitch = kFinishEntries + 1;         // odd row pitch: the lanes of a warp hit 32 banks
+
 __device__ __forceinline__ void glm_finish_body(const float* __restrict__ partials, int nblocks, int P, int K, int D,
                                                 double scale, double weight, float* __restrict__ sum_p,
                                                 float* __restrict__ out_dW, float* __restrict__ out_db,
@@ -174,8 +183,25 @@ __device__ __forceinline__ void glm_finish_body(const float* __restrict__ partia
   const int S = K * (D + 1) + 1;
   const int total = P * S;
   const int n_prior = E ? E->n_jobs * E->nwarps : 0;
-  const int e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int e0 = blockIdx.x * kFinishEntries;
+  const int e = e0 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
+  __shared__ float tile[kFinishMaxBlocks * kFinishPitch];
+  if (e0 < total) {
+    const int ncol = total - e0 < kFinishEntries ? total - e0 : kFinishEntries;
+    float v[kFinishLoads];
+#pragma unroll
+    for (int k = 0; k < kFinishLoads; ++k) {
+      const int i = threadIdx.x + k * kFinishThreads, bl = i / kFinishEntries, c = i % kFinishEntries;
+      v[k] = (bl < nblocks && c < ncol) ? partials[(int64_t)bl * total + e0 + c] : 0.f;
+    }
+#pragma unroll
+    for (int k = 0; k < kFinishLoads; ++k) {
+      const int i = threadIdx.x + k * kFinishThreads, bl = i / kFinishEntries, c = i % kFinishEntries;
+      if (bl < nblocks) tile[bl * kFinishPitch + c] = v[k];
+    }
+    __syncthreads();
+  }
   if (e >= total + n_prior) return;
   unsigned int t = 0;
   if (e >= total) {
@@ -198,7 +224,7 @@ __device__ __forceinline__ void glm_finish_body(const float* __restrict__ partia
     }
   } else {
     double s = 0.0;
-    for (int bl = lane; bl < nblocks; bl += 32) s += (double)partials[(int64_t)bl * total + e];
+    for (int bl = lane; bl < nblocks; bl += 32) s += (double)tile[bl * kFinishPitch + (e - e0)];
     s = warp_sum(s);
     const int p = e / S, r = e - p * S;
     if (r < K * (D + 1)) {
@@ -242,8 +268,18 @@ __device__ __forceinline__ void glm_finish_body(const float* __restrict__ partia
   t = __shfl_sync(0xffffffffu, t, 0);
   if (t != (unsigned)(P + n_prior - 1)) return;
   __threadfence();
+  // every value the rest adds is requested before the first add, not one job or term after another
   double acc = 0.0;
   for (int q = lane; q < P; q += 32) acc += (double)__ldcg(sum_p + q);
+  static_assert(B2_LATENT_MAX_TERMS <= 32, "one term per lane");
+  double ws[B2_LATENT_MAX_JOBS];
+  float tv = 0.f;   // lane q holds term q; a term that is out_total itself reads as own below
+  if (E) {
+#pragma unroll
+    for (int k = 0; k < B2_LATENT_MAX_JOBS; ++k)
+      ws[k] = (k < E->n_jobs && lane < E->nwarps) ? __ldcg(E->warp_sums + k * 32 + lane) : 0.0;
+    if (lane < E->n_terms && E->term[lane] && E->term[lane] != out_total) tv = __ldcg(E->term[lane]);
+  }
   acc = warp_sum(acc);
   float own = 0.f;
   if (lane == 0) {
@@ -254,19 +290,19 @@ __device__ __forceinline__ void glm_finish_body(const float* __restrict__ partia
   }
   if (!E) return;
   double loss = 0.0;
-  for (int k = 0; k < E->n_jobs; ++k) {
-    double w = lane < E->nwarps ? __ldcg(E->warp_sums + k * 32 + lane) : 0.0;
-    w = warp_sum(w);
-    loss += E->job_coeff[k] * w;
+#pragma unroll
+  for (int k = 0; k < B2_LATENT_MAX_JOBS; ++k) {
+    if (k >= E->n_jobs) break;
+    loss += E->job_coeff[k] * warp_sum(ws[k]);
   }
-  if (lane == 0) {
-    for (int q = 0; q < E->n_terms; ++q)
-      loss += E->term_coeff[q] * (double)(E->term[q] ? __ldcg(E->term[q]) : own);
-    *E->out = (float)loss;
+  for (int q = 0; q < E->n_terms; ++q) {
+    const float t = __shfl_sync(0xffffffffu, tv, q);
+    if (lane == 0) loss += E->term_coeff[q] * (double)(E->term[q] && E->term[q] != out_total ? t : own);
   }
+  if (lane == 0) *E->out = (float)loss;
 }
 
-__global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict__ partials, int nblocks, int P,
+__global__ void __launch_bounds__(kFinishThreads) glm_finish_kernel(const float* __restrict__ partials, int nblocks, int P,
                                                          int K, int D, double scale, double weight,
                                                          float* __restrict__ sum_p, float* __restrict__ out_dW,
                                                          float* __restrict__ out_db, double sum_coeff, int flags,
@@ -279,7 +315,7 @@ __global__ void __launch_bounds__(256) glm_finish_kernel(const float* __restrict
                   ticket, lg, sigma, sigma_stride, n, out_dsigma, nullptr);
 }
 
-__global__ void __launch_bounds__(256) glm_finish_elbo_kernel(const float* __restrict__ partials, int nblocks, int P,
+__global__ void __launch_bounds__(kFinishThreads) glm_finish_elbo_kernel(const float* __restrict__ partials, int nblocks, int P,
                                                               int K, int D, double scale, double weight,
                                                               float* __restrict__ sum_p, float* __restrict__ out_dW,
                                                               float* __restrict__ out_db, double sum_coeff,
@@ -299,7 +335,8 @@ void launch_glm_finish(const float* partials, unsigned int* ticket, int gx, int 
                        double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
                        float* out_dW, float* out_db, const float* lg, cudaStream_t s) {
   const int total = P * (K * (D + 1) + 1);
-  launch_pdl(glm_finish_kernel, dim3((total + 7) / 8), dim3(256), 0, s, partials, gx, P, K, D, scale, weight,
+  launch_pdl(glm_finish_kernel, dim3((total + kFinishEntries - 1) / kFinishEntries), dim3(kFinishThreads), 0, s,
+             partials, gx, P, K, D, scale, weight,
              glm_sum_p(partials, out_sum_p, gx, total), out_dW, out_db, sum_coeff, flags, out_total, ticket, lg,
              nullptr, 0, (int64_t)0, nullptr);
 }
@@ -311,7 +348,8 @@ void launch_glm_normal_finish(const float* partials, unsigned int* ticket, int g
                               float* out_total, float* out_dW, float* out_db, const float* sigma,
                               int sigma_stride, float* out_dsigma, cudaStream_t s) {
   const int total = P * (D + 2);
-  launch_pdl(glm_finish_kernel, dim3((total + 7) / 8), dim3(256), 0, s, partials, gx, P, 1, D, scale, weight,
+  launch_pdl(glm_finish_kernel, dim3((total + kFinishEntries - 1) / kFinishEntries), dim3(kFinishThreads), 0, s,
+             partials, gx, P, 1, D, scale, weight,
              glm_sum_p(partials, out_sum_p, gx, total), out_dW, out_db, sum_coeff, flags, out_total, ticket,
              (const float*)nullptr, sigma, sigma_stride, N, out_dsigma);
 }
@@ -385,7 +423,8 @@ static int glm_bernoulli(const float* X, const float* y, const float* W, const f
   }
   if (E) {
     const int total = P * (D + 2);
-    launch_pdl(glm_finish_elbo_kernel, dim3((total + E->n_jobs * E->nwarps + 7) / 8), dim3(256), 0, s, partials, gx,
+    launch_pdl(glm_finish_elbo_kernel, dim3((total + E->n_jobs * E->nwarps + kFinishEntries - 1) / kFinishEntries),
+               dim3(kFinishThreads), 0, s, partials, gx,
                P, 1, D, scale, weight, glm_sum_p(partials, out_sum_p, gx, total), out_dW, out_db, sum_coeff, flags,
                out_total, ticket, *E);
   } else {

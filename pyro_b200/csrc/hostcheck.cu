@@ -157,3 +157,13 @@ extern "C" void b2h_philox(uint64_t seed, uint64_t stream, uint64_t counter, int
   r.init(seed, stream, counter);
   for (int i = 0; i < n; ++i) out[i] = r.next_u32();
 }
+
+#include "latent.cuh"
+// 1 when b2_latent_normal_backward reduces the job's d/dloc and d/dscale in one pass, 0 when in two, or the
+// B2_ERR code with which it rejects the job
+extern "C" int b2h_latent_same_reduction(const b2_latent_job* job) {
+  LatentJob j;
+  const int code = fill_job(j, *job, job->dtype);
+  if (code != B2_OK) return code;
+  return latent_same_reduction(j) ? 1 : 0;
+}

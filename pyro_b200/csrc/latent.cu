@@ -189,11 +189,81 @@ __device__ __forceinline__ void latent_reduce(const LatentJob& j, const int* st,
   }
 }
 
+// Both reductions in one pass, for a job whose loc and scale broadcast over the same positions
+// (kLatentSameReduction, set by the host): each element's d/dloc and d/dscale come from one set of loads and
+// go to two sums, and a lane requests the operands of two elements before adding either.  Every output is summed
+// over the same positions in the same order as latent_reduce.
+template <typename T>
+__device__ __forceinline__ void latent_reduce_both(const LatentJob& j, bool logs) {
+  unsigned cst[kMaxD], m = 1;
+  {
+    unsigned c = 1;
+    for (int d = j.ndim - 1; d >= 0; --d) {
+      cst[d] = c;
+      c *= j.shape[d];
+      if (j.st_loc[d] != 0) m *= j.shape[d];
+    }
+  }
+  const unsigned q = j.n / m;
+  const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  auto flat_of = [&](unsigned t, unsigned base) {
+    for (int d = j.ndim - 1; d >= 0; --d) {
+      if (j.st_loc[d] != 0) continue;
+      const unsigned qq = t / j.shape[d];
+      base += (t - qq * j.shape[d]) * cst[d];
+      t = qq;
+    }
+    return base;
+  };
+  for (unsigned jj = warp; jj < m; jj += nwarps) {
+    unsigned rem = jj, base = 0;
+    int offl = 0, offs = 0;
+    for (int d = j.ndim - 1; d >= 0; --d) {
+      if (j.st_loc[d] == 0) continue;
+      const unsigned qq = rem / j.shape[d];
+      const unsigned idx = rem - qq * j.shape[d];
+      rem = qq;
+      base += idx * cst[d];
+      offl += (int)idx * j.st_loc[d];
+      offs += (int)idx * j.st_scale[d];
+    }
+    double s0 = 0.0, s1 = 0.0;
+    for (unsigned t = lane; t < q; t += 64) {
+      const bool two = t + 32 < q;
+      T gl0, gs0, gl1 = (T)0, gs1 = (T)0;
+      latent_grad_elem<T>(j, flat_of(t, base), logs, gl0, gs0);
+      if (two) latent_grad_elem<T>(j, flat_of(t + 32, base), logs, gl1, gs1);
+      s0 += (double)gl0;
+      s1 += (double)gs0;
+      if (two) {
+        s0 += (double)gl1;
+        s1 += (double)gs1;
+      }
+    }
+    s0 = warp_sum(s0);
+    s1 = warp_sum(s1);
+    if (lane == 0) {
+      if (j.out0) {
+        T* out = reinterpret_cast<T*>(j.out0);
+        out[offl] = (j.flags & B2_LATENT_ACC_OUT0) ? (T)((double)out[offl] + s0) : (T)s0;
+      }
+      if (j.out1) {
+        T* out = reinterpret_cast<T*>(j.out1);
+        out[offs] = (j.flags & B2_LATENT_ACC_OUT1) ? (T)((double)out[offs] + s1) : (T)s1;
+      }
+    }
+  }
+}
+
 template <typename T>
 __global__ void __launch_bounds__(1024) latent_backward_kernel(const LatentArgs a) {
   pdl_enter();
   const LatentJob& j = a.job[blockIdx.x];
   const bool logs = (j.flags & B2_LATENT_LOG_SCALE) != 0;
+  if (j.flags & kLatentSameReduction) {
+    latent_reduce_both<T>(j, logs);
+    return;
+  }
   latent_reduce<T, 0>(j, j.st_loc, j.out0, logs, (j.flags & B2_LATENT_ACC_OUT0) != 0);
   latent_reduce<T, 1>(j, j.st_scale, j.out1, logs, (j.flags & B2_LATENT_ACC_OUT1) != 0);
 }
@@ -274,6 +344,8 @@ extern "C" int b2_latent_normal_backward(const b2_latent_job* jobs, int n_jobs, 
     if (!a.job[k].scale || !a.job[k].eps) return B2_ERR_NULL;
     if ((a.job[k].ploc != nullptr) != (a.job[k].pscale != nullptr)) return B2_ERR_NULL;
     if (a.job[k].ploc && !a.job[k].z) return B2_ERR_NULL;
+    a.job[k].flags &= ~kLatentSameReduction;
+    if (latent_same_reduction(a.job[k])) a.job[k].flags |= kLatentSameReduction;
   }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (dtype == B2_F32) launch_pdl(latent_backward_kernel<float>, dim3(n_jobs), dim3(threads_for(nmax)), 0, s, a);

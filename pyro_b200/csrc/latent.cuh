@@ -101,6 +101,17 @@ static inline int fill_args(LatentArgs& a, const b2_latent_job* jobs, int n_jobs
   return B2_OK;
 }
 
+// Job flag set by the host for the backward (never by a caller): loc and scale are summed over the same broadcast
+// positions, so latent_backward_kernel reduces both in one pass.  That holds when every dim of more than one
+// element is broadcast (stride 0) in both operands or in neither.
+constexpr int kLatentSameReduction = 1 << 16;
+
+static inline bool latent_same_reduction(const LatentJob& j) {
+  for (int d = 0; d < j.ndim; ++d)
+    if (j.shape[d] > 1 && (j.st_loc[d] == 0) != (j.st_scale[d] == 0)) return false;
+  return true;
+}
+
 // threads of a one-CTA-per-job launch whose largest job has nmax elements
 static inline int threads_for(unsigned nmax) { return nmax >= 1024 ? 1024 : (int)((nmax + 31) / 32 * 32); }
 
