@@ -9,8 +9,9 @@
 //
 // fp32 SIMT kernel (D in {4, 8, 16}; at D = 32: N < 8192 rows, B2_FLAG_GLM_FP32, and operands the wgmma
 // kernel of glm_tc.cu cannot load; every other D in 1..128 takes the wgmma kernel of glm_flat_tc.cu).
-// glm_finish_kernel below is the second launch of every GLM likelihood call, Bernoulli, softmax
-// (b2_glm_categorical_logits), Poisson (b2_glm_poisson_log_rate) and Normal (b2_glm_normal_loc).  CTA = 256 threads = 4 row groups x 64
+// glm_finish_kernel below, launched by launch_glm_finish (glm_host.cuh), is the second launch of every GLM likelihood
+// call: Bernoulli, softmax (b2_glm_categorical_logits), Poisson (b2_glm_poisson_log_rate), Normal (b2_glm_normal_loc)
+// and Binomial (b2_glm_binomial_logits).  SIMT kernel: CTA = 256 threads = 4 row groups x 64
 // particles.  Each thread keeps W[p,:] and its dW[p,:] accumulator in registers; X tiles are staged through shared memory
 // with cp.async double buffering and read back as warp-wide broadcasts (every lane of a warp has a
 // different particle but the same row, so an LDS.128 serves 4 FMAs x 2 uses for all 32 lanes).
@@ -19,6 +20,7 @@
 
 #include "b2_common.cuh"
 #include "b2_math.cuh"
+#include "glm_host.cuh"
 #include "latent.cuh"
 
 namespace b2 {
@@ -155,9 +157,9 @@ struct GlmElbo {
 };
 
 // second stage: fixed-order sum over the CTAs' partials [nblocks][P][K (D + 1) + 1] (per class dW[0..D-1]
-// and db, then the particle's lp sum; K = 1 for Bernoulli, Poisson and Normal); applies weight / scale.  lg
-// (Poisson only, else null) holds one more partial per CTA, of a term every particle's sum subtracts: SUM
-// lgamma(y + 1).  sigma (Normal only, else null; sigma[p * sigma_stride] for particle p) turns the sufficient
+// and db, then the particle's lp sum; K = 1 but for softmax); applies weight / scale.  lg (Poisson and
+// Binomial, else null) holds one more partial per CTA, of a data term every particle's sum subtracts: SUM
+// lgamma(y + 1), SUM log C(m, y).  sigma (Normal only, else null; sigma[p * sigma_stride] for particle p) turns the sufficient
 // statistics of the Normal tile kernel into the lp sum and gradients: the lp slot holds S = SUM (y - l)^2 and
 // dW / db hold SUM (y - l) [x | 1]; the warp of sum_p[p] also writes out_dsigma[p] (nullable), n is N.
 // One WARP per entry of the [P, K (D + 1) + 1] table: lanes stride over the CTAs (L2-resident partials),
@@ -325,42 +327,20 @@ __global__ void __launch_bounds__(kFinishThreads) glm_finish_elbo_kernel(const f
                   ticket, nullptr, nullptr, 0, 0, nullptr, &E);
 }
 
-// The second launch of b2_glm_bernoulli_logits, b2_glm_categorical_logits and b2_glm_poisson_log_rate.  The
-// per-particle sums go to out_sum_p, or without one to the [P] row of the workspace after the partials.
+// The per-particle sums go to out_sum_p, or without one to the [P] row of the workspace after the partials.
 static float* glm_sum_p(const float* partials, float* out_sum_p, int gx, int total) {
   return out_sum_p ? out_sum_p : const_cast<float*>(partials) + (size_t)gx * total;
 }
 
 void launch_glm_finish(const float* partials, unsigned int* ticket, int gx, int P, int K, int D, double scale,
                        double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
-                       float* out_dW, float* out_db, const float* lg, cudaStream_t s) {
+                       float* out_dW, float* out_db, const float* lg, cudaStream_t s, const float* sigma,
+                       int sigma_stride, int64_t n, float* out_dsigma) {
   const int total = P * (K * (D + 1) + 1);
   launch_pdl(glm_finish_kernel, dim3((total + kFinishEntries - 1) / kFinishEntries), dim3(kFinishThreads), 0, s,
-             partials, gx, P, K, D, scale, weight,
-             glm_sum_p(partials, out_sum_p, gx, total), out_dW, out_db, sum_coeff, flags, out_total, ticket, lg,
-             nullptr, 0, (int64_t)0, nullptr);
+             partials, gx, P, K, D, scale, weight, glm_sum_p(partials, out_sum_p, gx, total), out_dW, out_db,
+             sum_coeff, flags, out_total, ticket, lg, sigma, sigma_stride, n, out_dsigma);
 }
-
-// The second launch of b2_glm_normal_loc: the finish above with the noise scale sigma[p * sigma_stride] of
-// every particle applied to the sufficient statistics of the tile kernel (glm_normal_tc.cu).
-void launch_glm_normal_finish(const float* partials, unsigned int* ticket, int gx, int P, int D, int64_t N,
-                              double scale, double weight, double sum_coeff, int flags, float* out_sum_p,
-                              float* out_total, float* out_dW, float* out_db, const float* sigma,
-                              int sigma_stride, float* out_dsigma, cudaStream_t s) {
-  const int total = P * (D + 2);
-  launch_pdl(glm_finish_kernel, dim3((total + kFinishEntries - 1) / kFinishEntries), dim3(kFinishThreads), 0, s,
-             partials, gx, P, 1, D, scale, weight,
-             glm_sum_p(partials, out_sum_p, gx, total), out_dW, out_db, sum_coeff, flags, out_total, ticket,
-             (const float*)nullptr, sigma, sigma_stride, N, out_dsigma);
-}
-
-// wgmma + TMA variant (glm_tc.cu)
-int glm_tc_grid_x(int64_t N);
-int launch_glm_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int P,
-                  float* partials, int gx, bool split_x, cudaStream_t s);
-// wgmma variant for the other feature counts, 1 <= D <= 128 (glm_flat_tc.cu)
-void launch_glm_flat_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
-                        float* partials, int gx, bool split_x, cudaStream_t s);
 
 inline int glm_grid_x(int64_t N) {
   const int64_t ntiles = (N + kGlmTileRows - 1) / kGlmTileRows;
@@ -406,12 +386,10 @@ static int glm_bernoulli(const float* X, const float* y, const float* W, const f
   dim3 grid((unsigned)gx, (unsigned)((P + kGlmParticles - 1) / kGlmParticles), 1);
   unsigned int* ticket = reinterpret_cast<unsigned int*>(workspace);
   float* partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  // default: W split; below 64 Ki rows the incoherent X rounding has not averaged out yet -> full 3xTF32
-  const bool split_x = (flags & B2_FLAG_GLM_3XTF32) || N < 65536;
-  if (flat) {
-    launch_glm_flat_tc(X, y, W, b, N, D, P, partials, gx, split_x, s);
-  } else if (use_tc) {
-    const int rc = launch_glm_tc(X, y, W, b, N, P, partials, gx, split_x, s);
+  if (flat || use_tc) {
+    const bool split_x = glm_split_x(flags, N);
+    const int rc = flat ? launch_glm_flat_tc(X, y, W, b, N, D, P, partials, gx, split_x, s)
+                        : launch_glm_tc(X, y, W, b, N, P, partials, gx, split_x, s);
     if (rc != 0) return rc;
   } else
   switch (D) {

@@ -27,14 +27,9 @@
 #include "b2_common.cuh"
 #include "b2_math.cuh"
 #include "glm_flat_tc.cuh"
+#include "glm_host.cuh"
 
 namespace b2 {
-
-// glm.cu / glm_tc.cu
-void launch_glm_finish(const float* partials, unsigned int* ticket, int gx, int P, int K, int D, double scale,
-                       double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
-                       float* out_dW, float* out_db, const float* lg, cudaStream_t s);
-int glm_tc_grid_x(int64_t N);
 
 namespace tcbi {
 
@@ -96,56 +91,30 @@ glm_binomial_flat_tc_kernel(const float* __restrict__ X, const float* __restrict
   if (blockIdx.y == 0) lbinom_partial<tcf::Cfg<DC>::kThreads, ROW>(y, trials, N, lg);
 }
 
-template <bool ROW, bool SPLIT_X>
-int launch_32(const float* X, const float* y, const float* m, const float* W, const float* b, int64_t N, int P,
-              float* partials, float* lg, int gx, cudaStream_t s) {
-  using namespace tile32;
-  using Fam = Binomial<ROW>;
-  CUtensorMap mx, my, mm;
-  if (!encode_x_map(&mx, X, N) || !encode_label_map(&my, y, N, Fam::kYType)) return B2_ERR_LAUNCH;
-  if (ROW ? !encode_label_map(&mm, m, N, Fam::kYType) : false) return B2_ERR_LAUNCH;
-  if (!ROW) mm = my;                           // not read
-  constexpr uint32_t kSmemBytes = Smem32<Fam::kYBytes>::kBytes;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(glm_binomial_tc_kernel<ROW, SPLIT_X>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)kSmemBytes);
-    attr_set = true;
+template <bool ROW>
+int launch(const float* X, const float* y, const float* m, const float* W, const float* b, int64_t N, int D, int P,
+           float* partials, float* lg, int gx, bool split_x, cudaStream_t s) {
+  const dim3 grid = slab_grid(gx, P);
+  if (D == 32) {
+    using namespace tile32;
+    using Fam = Binomial<ROW>;
+    CUtensorMap mx, my, mm;
+    if (!encode_x_map(&mx, X, N) || !encode_label_map(&my, y, N, Fam::kYType)) return B2_ERR_LAUNCH;
+    if (ROW ? !encode_label_map(&mm, m, N, Fam::kYType) : false) return B2_ERR_LAUNCH;
+    if (!ROW) mm = my;                           // not read
+    constexpr uint32_t kSmemBytes = Smem32<Fam::kYBytes>::kBytes;
+    return split_x ? launch_tc(glm_binomial_tc_kernel<ROW, true>, grid, dim3(kThreads), kSmemBytes, s, mx, my, mm, y,
+                               m, W, b, N, P, partials, lg)
+                   : launch_tc(glm_binomial_tc_kernel<ROW, false>, grid, dim3(kThreads), kSmemBytes, s, mx, my, mm, y,
+                               m, W, b, N, P, partials, lg);
   }
-  dim3 grid((unsigned)gx, (unsigned)((P + kM - 1) / kM), 1);
-  launch_pdl(glm_binomial_tc_kernel<ROW, SPLIT_X>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, mm, y, m,
-             W, b, N, P, partials, lg);
-  return 0;
-}
-
-template <bool ROW, int DC, bool SPLIT_X>
-int launch_flat(const float* X, const float* y, const float* m, const float* W, const float* b, int64_t N, int D,
-                int P, float* partials, float* lg, int gx, cudaStream_t s) {
-  using C = tcf::Cfg<DC>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(glm_binomial_flat_tc_kernel<ROW, DC, SPLIT_X>,
-                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::kSmemBytes);
-    attr_set = true;
-  }
-  dim3 grid((unsigned)gx, (unsigned)((P + kM - 1) / kM), 1);
-  launch_pdl(glm_binomial_flat_tc_kernel<ROW, DC, SPLIT_X>, grid, dim3(C::kThreads), (size_t)C::kSmemBytes, s, X,
-             y, m, W, b, N, D, P, partials, lg);
-  return 0;
-}
-
-template <bool ROW, bool SPLIT_X>
-int launch(const float* X, const float* y, const float* m, const float* W, const float* b, int64_t N, int D,
-           int P, float* partials, float* lg, int gx, cudaStream_t s) {
-  if (D == 32) return launch_32<ROW, SPLIT_X>(X, y, m, W, b, N, P, partials, lg, gx, s);
   // D < 32 runs the two-atom loop (two warpgroups, 255 registers): with one atom and four warpgroups the
   // 128-register cap made this epilogue spill
-  switch ((D + 31) / 32) {
-    case 1:
-    case 2: return launch_flat<ROW, 2, SPLIT_X>(X, y, m, W, b, N, D, P, partials, lg, gx, s);
-    case 3: return launch_flat<ROW, 3, SPLIT_X>(X, y, m, W, b, N, D, P, partials, lg, gx, s);
-    default: return launch_flat<ROW, 4, SPLIT_X>(X, y, m, W, b, N, D, P, partials, lg, gx, s);
-  }
+  return glm_dispatch_dc<2>(D, split_x, [&](auto dc, auto sx) {
+    using C = tcf::Cfg<decltype(dc)::value>;
+    return launch_tc(glm_binomial_flat_tc_kernel<ROW, decltype(dc)::value, decltype(sx)::value>, grid,
+                     dim3(C::kThreads), C::kSmemBytes, s, X, y, m, W, b, N, D, P, partials, lg);
+  });
 }
 
 }  // namespace tcbi
@@ -153,46 +122,25 @@ int launch(const float* X, const float* y, const float* m, const float* W, const
 
 using namespace b2;
 
-extern "C" size_t b2_glm_binomial_workspace(int64_t N, int D, int P) {
-  // [ticket, 256 B] + CTA partials [gx][P][D + 2] + one [P] row for the per-particle sums + log C partials [gx]
-  if (N < 1 || D < 1 || D > 128 || P < 1) return 256;
-  const size_t gx = (size_t)glm_tc_grid_x(N);
-  return 256 + (gx * (size_t)P * (size_t)(D + 2) + (size_t)P + gx) * sizeof(float);
-}
+extern "C" size_t b2_glm_binomial_workspace(int64_t N, int D, int P) { return glm_row_workspace(N, D, P, true); }
 
 extern "C" int b2_glm_binomial_logits(const float* X, const float* y, const float* trials, int trials_per_row,
                                       const float* W, const float* b, int64_t N, int D, int P, double scale,
                                       double weight, double sum_coeff, int flags, float* out_sum_p,
                                       float* out_total, float* out_dW, float* out_db, void* workspace,
                                       size_t workspace_bytes, void* stream) {
-  if (!X || !y || !trials || !W) return B2_ERR_NULL;
-  if (N <= 0 || P <= 0 || D < 1 || D > 128) return B2_ERR_BAD_SHAPE;
-  if (trials_per_row != 0 && trials_per_row != 1) return B2_ERR_BAD_SHAPE;
-  // the tiles arrive by TMA / bulk copies (16-byte aligned sources, 32-bit row coordinates); there is no fp32
-  // SIMT kernel for this family
-  if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
-  if (trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0) return B2_ERR_BAD_SHAPE;
-  if (flags & B2_FLAG_GLM_FP32) return B2_ERR_BAD_SHAPE;
-  if (N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
-  if (!workspace || workspace_bytes < b2_glm_binomial_workspace(N, D, P)) return B2_ERR_WORKSPACE;
+  const bool bad_trials = (trials_per_row != 0 && trials_per_row != 1) ||
+                          (trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0);
+  int rc = glm_row_check(X, y, W, !trials, N, D, P, bad_trials, flags, workspace, workspace_bytes, true);
+  if (rc != B2_OK) return rc;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const int gx = glm_tc_grid_x(N);
-  unsigned int* ticket = reinterpret_cast<unsigned int*>(workspace);
-  float* partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  float* lg = partials + (size_t)gx * P * (D + 2) + P;
-  // the precision policy of b2_glm_bernoulli_logits: below 64 Ki rows the incoherent X rounding has not
-  // averaged out yet -> X split as well
-  const bool split_x = (flags & B2_FLAG_GLM_3XTF32) || N < 65536;
-  int rc;
-  if (trials_per_row)
-    rc = split_x ? tcbi::launch<true, true>(X, y, trials, W, b, N, D, P, partials, lg, gx, s)
-                 : tcbi::launch<true, false>(X, y, trials, W, b, N, D, P, partials, lg, gx, s);
-  else
-    rc = split_x ? tcbi::launch<false, true>(X, y, trials, W, b, N, D, P, partials, lg, gx, s)
-                 : tcbi::launch<false, false>(X, y, trials, W, b, N, D, P, partials, lg, gx, s);
+  const GlmRowWorkspace w = glm_row_areas(workspace, N, D, P, true);
+  const bool split_x = glm_split_x(flags, N);
+  rc = trials_per_row ? tcbi::launch<true>(X, y, trials, W, b, N, D, P, w.partials, w.lg, w.gx, split_x, s)
+                      : tcbi::launch<false>(X, y, trials, W, b, N, D, P, w.partials, w.lg, w.gx, split_x, s);
   if (rc != 0) return rc;
-  launch_glm_finish(partials, ticket, gx, P, 1, D, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW,
-                    out_db, lg, s);
+  launch_glm_finish(w.partials, w.ticket, w.gx, P, 1, D, scale, weight, sum_coeff, flags, out_sum_p, out_total,
+                    out_dW, out_db, w.lg, s);
   count_launch(2);
   return check_launch();
 }

@@ -32,14 +32,10 @@
 #include <stdlib.h>
 
 #include "b2_common.cuh"
+#include "glm_host.cuh"
 #include "glm_tc_common.cuh"
 
 namespace b2 {
-
-// launches glm_finish_kernel (glm.cu) over the partials [gx][P][K (D + 1) + 1]
-void launch_glm_finish(const float* partials, unsigned int* ticket, int gx, int P, int K, int D, double scale,
-                       double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
-                       float* out_dW, float* out_db, const float* lg, cudaStream_t s);
 
 namespace tcc {
 
@@ -158,31 +154,16 @@ inline int grid_x(int64_t N, int K, int P) {
   return (int)gx;
 }
 
-template <int KP, bool SPLIT_X>
-void launch(const CUtensorMap& mx, const CUtensorMap& my, const float* W, const float* b, int64_t N, int P, int K,
-            float* partials, int gx, cudaStream_t s) {
+template <int KP>
+int launch(const CUtensorMap& mx, const CUtensorMap& my, const float* W, const float* b, int64_t N, int P, int K,
+           float* partials, int gx, bool split_x, cudaStream_t s) {
   constexpr uint32_t kSmemBytes = Smem32<Softmax<KP>::kYBytes>::kBytes;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(glm_categorical_tc_kernel<KP, SPLIT_X>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)kSmemBytes);
-    attr_set = true;
-  }
   constexpr int PPS = kM / KP;
   dim3 grid((unsigned)gx, (unsigned)((P + PPS - 1) / PPS), 1);
-  launch_pdl(glm_categorical_tc_kernel<KP, SPLIT_X>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, W, b, N,
-             P, K, partials);
-}
-
-template <bool SPLIT_X>
-void launch_split(int KP, const CUtensorMap& mx, const CUtensorMap& my, const float* W, const float* b, int64_t N,
-                  int P, int K, float* partials, int gx, cudaStream_t s) {
-  switch (KP) {
-    case 2: launch<2, SPLIT_X>(mx, my, W, b, N, P, K, partials, gx, s); break;
-    case 4: launch<4, SPLIT_X>(mx, my, W, b, N, P, K, partials, gx, s); break;
-    case 8: launch<8, SPLIT_X>(mx, my, W, b, N, P, K, partials, gx, s); break;
-    default: launch<16, SPLIT_X>(mx, my, W, b, N, P, K, partials, gx, s); break;
-  }
+  return split_x ? launch_tc(glm_categorical_tc_kernel<KP, true>, grid, dim3(kThreads), kSmemBytes, s, mx, my, W, b,
+                             N, P, K, partials)
+                 : launch_tc(glm_categorical_tc_kernel<KP, false>, grid, dim3(kThreads), kSmemBytes, s, mx, my, W, b,
+                             N, P, K, partials);
 }
 
 }  // namespace tcc
@@ -212,12 +193,15 @@ extern "C" int b2_glm_categorical_logits(const float* X, const int64_t* y, const
   const int gx = grid_x(N, K, P);
   unsigned int* ticket = reinterpret_cast<unsigned int*>(workspace);
   float* partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  // same precision policy as b2_glm_bernoulli_logits: below 64 Ki rows X is split hi + lo as well
-  const bool split_x = (flags & B2_FLAG_GLM_3XTF32) || N < 65536;
-  if (split_x)
-    launch_split<true>(class_pad(K), mx, my, W, b, N, P, K, partials, gx, s);
-  else
-    launch_split<false>(class_pad(K), mx, my, W, b, N, P, K, partials, gx, s);
+  const bool split_x = glm_split_x(flags, N);
+  int rc;
+  switch (class_pad(K)) {
+    case 2: rc = launch<2>(mx, my, W, b, N, P, K, partials, gx, split_x, s); break;
+    case 4: rc = launch<4>(mx, my, W, b, N, P, K, partials, gx, split_x, s); break;
+    case 8: rc = launch<8>(mx, my, W, b, N, P, K, partials, gx, split_x, s); break;
+    default: rc = launch<16>(mx, my, W, b, N, P, K, partials, gx, split_x, s); break;
+  }
+  if (rc != 0) return rc;
   launch_glm_finish(partials, ticket, gx, P, K, kD, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW,
                     out_db, nullptr, s);
   count_launch(2);

@@ -11,6 +11,7 @@
 
 #include "b2_common.cuh"
 #include "glm_flat_tc.cuh"
+#include "glm_host.cuh"
 
 namespace b2 {
 namespace tcf {
@@ -22,34 +23,17 @@ glm_bernoulli_flat_tc_kernel(const float* __restrict__ X, const float* __restric
   glm_flat_pipeline<Bernoulli, DC, SPLIT_X>(X, y, W, bvec, N, D, P, partials);
 }
 
-template <int DC, bool SPLIT_X>
-void launch_one(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
-                float* partials, int gx, cudaStream_t s) {
-  using C = Cfg<DC>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(glm_bernoulli_flat_tc_kernel<DC, SPLIT_X>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)C::kSmemBytes);
-    attr_set = true;
-  }
-  dim3 grid((unsigned)gx, (unsigned)((P + kM - 1) / kM), 1);
-  launch_pdl(glm_bernoulli_flat_tc_kernel<DC, SPLIT_X>, grid, dim3(C::kThreads), (size_t)C::kSmemBytes, s,
-             X, y, W, b, N, D, P, partials);
-}
-
 }  // namespace tcf
 
 // ---- host side -------------------------------------------------------------------------------------------
 // The caller (b2_glm_bernoulli_logits) has checked 1 <= D <= 128, N < 2^31 and 16-byte aligned X and y.
-void launch_glm_flat_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
-                        float* partials, int gx, bool split_x, cudaStream_t s) {
-  using namespace tcf;
-  switch ((D + 31) / 32) {
-    case 1: (split_x ? launch_one<1, true> : launch_one<1, false>)(X, y, W, b, N, D, P, partials, gx, s); break;
-    case 2: (split_x ? launch_one<2, true> : launch_one<2, false>)(X, y, W, b, N, D, P, partials, gx, s); break;
-    case 3: (split_x ? launch_one<3, true> : launch_one<3, false>)(X, y, W, b, N, D, P, partials, gx, s); break;
-    default: (split_x ? launch_one<4, true> : launch_one<4, false>)(X, y, W, b, N, D, P, partials, gx, s); break;
-  }
+int launch_glm_flat_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
+                       float* partials, int gx, bool split_x, cudaStream_t s) {
+  return glm_dispatch_dc<1>(D, split_x, [&](auto dc, auto sx) {
+    using C = tcf::Cfg<decltype(dc)::value>;
+    return launch_tc(tcf::glm_bernoulli_flat_tc_kernel<decltype(dc)::value, decltype(sx)::value>,
+                     tc::slab_grid(gx, P), dim3(C::kThreads), C::kSmemBytes, s, X, y, W, b, N, D, P, partials);
+  });
 }
 
 }  // namespace b2

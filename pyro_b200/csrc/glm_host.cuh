@@ -1,0 +1,102 @@
+// glm_host.cuh -- host plumbing shared by the GLM likelihood entry points (glm.cu, glm_tc.cu, glm_flat_tc.cu,
+// glm_categorical_tc.cu, glm_poisson_tc.cu, glm_normal_tc.cu, glm_binomial_tc.cu) and poisson_product_tc.cu: the
+// tensor-core kernel launcher, the dispatch from D to the atom count of glm_flat_pipeline, the precision policy, the
+// finish launch, and the checks and workspace of the per-row entry points (Poisson, Normal, Binomial).
+#pragma once
+#include <type_traits>
+
+#include "b2_common.cuh"
+
+namespace b2 {
+
+// ---- glm.cu ----
+// The second launch of every GLM likelihood call: glm_finish_kernel over the CTA partials [gx][P][K (D + 1) + 1].
+// lg (one more partial per CTA that every particle's sum subtracts) and the Normal noise scale sigma[p *
+// sigma_stride] with n = N rows and out_dsigma are optional.  The per-particle sums go to out_sum_p, or without
+// one to the [P] row of the workspace after the partials.
+void launch_glm_finish(const float* partials, unsigned int* ticket, int gx, int P, int K, int D, double scale,
+                       double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
+                       float* out_dW, float* out_db, const float* lg, cudaStream_t s, const float* sigma = nullptr,
+                       int sigma_stride = 0, int64_t n = 0, float* out_dsigma = nullptr);
+
+// ---- glm_tc.cu ----
+// CTAs per particle slab of the tensor-core tile loops: one per SM, at most one per 64-row tile
+int glm_tc_grid_x(int64_t N);
+// Bernoulli at D = 32 on glm_tile_pipeline; 0 or a negative B2_ERR code
+int launch_glm_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int P,
+                  float* partials, int gx, bool split_x, cudaStream_t s);
+// cudaFuncAttributeMaxDynamicSharedMemorySize = bytes for kernel on the current device, set once per (kernel,
+// device, under a lock; false when CUDA refuses it
+bool set_max_dynamic_smem(const void* kernel, int bytes);
+
+// ---- glm_flat_tc.cu ----
+// Bernoulli at every other D in 1..128 on glm_flat_pipeline
+int launch_glm_flat_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
+                       float* partials, int gx, bool split_x, cudaStream_t s);
+
+// Launch of a kernel that needs more than 48 KB of dynamic shared memory: 0, or B2_ERR_LAUNCH when its
+// shared-memory limit could not be raised.
+template <typename... KArgs, typename... Args>
+int launch_tc(void (*kernel)(KArgs...), dim3 grid, dim3 block, uint32_t smem, cudaStream_t s, Args... args) {
+  if (!set_max_dynamic_smem(reinterpret_cast<const void*>(kernel), (int)smem)) return B2_ERR_LAUNCH;
+  launch_pdl(kernel, grid, block, (size_t)smem, s, args...);
+  return 0;
+}
+
+// Precision policy of the tensor-core tile loops: W is always split hi + lo; below 64 Ki rows the incoherent
+// rounding of X to TF32 has not averaged out yet, so X is split as well (and whenever B2_FLAG_GLM_3XTF32 asks).
+inline bool glm_split_x(int flags, int64_t N) { return (flags & B2_FLAG_GLM_3XTF32) || N < 65536; }
+
+// f(std::integral_constant<int, DC>, std::integral_constant<bool, split_x>) for the glm_flat_pipeline
+// instantiation that holds D: D padded to DC atoms of 32 columns, at least MinDC of them (D <= 128, so DC <= 4).
+// Only DC >= MinDC are instantiated.
+template <int MinDC, int DC = MinDC, class F>
+int glm_dispatch_dc(int D, bool split_x, F&& f) {
+  if constexpr (DC < 4) {
+    if ((D + 31) / 32 > DC) return glm_dispatch_dc<MinDC, DC + 1>(D, split_x, f);
+  }
+  return split_x ? f(std::integral_constant<int, DC>{}, std::true_type{})
+                 : f(std::integral_constant<int, DC>{}, std::false_type{});
+}
+
+// ---- the per-row entry points: b2_glm_poisson_log_rate, b2_glm_normal_loc, b2_glm_binomial_logits ----
+// workspace: [ticket, 256 B][CTA partials gx * P * (D + 2)][one [P] row for the per-particle sums], then with lg
+// the [gx] partials of the data term of the finish (Poisson, Binomial)
+inline size_t glm_row_workspace(int64_t N, int D, int P, bool with_lg) {
+  if (N < 1 || D < 1 || D > 128 || P < 1) return 256;
+  const size_t gx = (size_t)glm_tc_grid_x(N);
+  return 256 + (gx * (size_t)P * (size_t)(D + 2) + (size_t)P + (with_lg ? gx : 0)) * sizeof(float);
+}
+
+struct GlmRowWorkspace {
+  int gx;
+  unsigned int* ticket;
+  float* partials;
+  float* lg;          // null without lg
+};
+
+inline GlmRowWorkspace glm_row_areas(void* workspace, int64_t N, int D, int P, bool with_lg) {
+  GlmRowWorkspace w;
+  w.gx = glm_tc_grid_x(N);
+  w.ticket = reinterpret_cast<unsigned int*>(workspace);
+  w.partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
+  w.lg = with_lg ? w.partials + (size_t)w.gx * P * (D + 2) + P : nullptr;
+  return w;
+}
+
+// The argument checks of the per-row entry points, in order; null_operand and bad_operand are the family's own
+// (a null sigma or trial-count pointer; a bad sigma_stride, trials_per_row or trial-count alignment).  The tiles
+// arrive by TMA / bulk copies (16-byte aligned sources, 32-bit row coordinates), and these families have no fp32
+// SIMT kernel.
+inline int glm_row_check(const float* X, const float* y, const float* W, bool null_operand, int64_t N, int D, int P,
+                         bool bad_operand, int flags, const void* workspace, size_t workspace_bytes, bool with_lg) {
+  if (!X || !y || !W || null_operand) return B2_ERR_NULL;
+  if (N <= 0 || P <= 0 || D < 1 || D > 128 || bad_operand) return B2_ERR_BAD_SHAPE;
+  if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
+  if (flags & B2_FLAG_GLM_FP32) return B2_ERR_BAD_SHAPE;
+  if (N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
+  if (!workspace || workspace_bytes < glm_row_workspace(N, D, P, with_lg)) return B2_ERR_WORKSPACE;
+  return B2_OK;
+}
+
+}  // namespace b2

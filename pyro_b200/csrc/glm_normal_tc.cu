@@ -36,15 +36,9 @@
 
 #include "b2_common.cuh"
 #include "glm_flat_tc.cuh"
+#include "glm_host.cuh"
 
 namespace b2 {
-
-// glm.cu / glm_tc.cu
-void launch_glm_normal_finish(const float* partials, unsigned int* ticket, int gx, int P, int D, int64_t N,
-                              double scale, double weight, double sum_coeff, int flags, float* out_sum_p,
-                              float* out_total, float* out_dW, float* out_db, const float* sigma,
-                              int sigma_stride, float* out_dsigma, cudaStream_t s);
-int glm_tc_grid_x(int64_t N);
 
 namespace tcn {
 
@@ -66,47 +60,22 @@ glm_normal_flat_tc_kernel(const float* __restrict__ X, const float* __restrict__
   tcf::glm_flat_pipeline<Normal, DC, true>(X, y, W, bvec, N, D, P, partials);
 }
 
-int launch_32(const float* X, const float* y, const float* W, const float* b, int64_t N, int P, float* partials,
-              int gx, cudaStream_t s) {
-  using namespace tile32;
-  CUtensorMap mx, my;
-  if (!encode_x_map(&mx, X, N) || !encode_label_map(&my, y, N, Normal::kYType)) return B2_ERR_LAUNCH;
-  constexpr uint32_t kSmemBytes = Smem32<Normal::kYBytes>::kBytes;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(glm_normal_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    attr_set = true;
-  }
-  dim3 grid((unsigned)gx, (unsigned)((P + kM - 1) / kM), 1);
-  launch_pdl(glm_normal_tc_kernel, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, W, b, N, P, partials);
-  return 0;
-}
-
-template <int DC>
-int launch_flat(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
-                float* partials, int gx, cudaStream_t s) {
-  using C = tcf::Cfg<DC>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(glm_normal_flat_tc_kernel<DC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)C::kSmemBytes);
-    attr_set = true;
-  }
-  dim3 grid((unsigned)gx, (unsigned)((P + kM - 1) / kM), 1);
-  launch_pdl(glm_normal_flat_tc_kernel<DC>, grid, dim3(C::kThreads), (size_t)C::kSmemBytes, s, X, y, W, b, N, D,
-             P, partials);
-  return 0;
-}
-
 int launch(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
            float* partials, int gx, cudaStream_t s) {
-  if (D == 32) return launch_32(X, y, W, b, N, P, partials, gx, s);
-  switch ((D + 31) / 32) {
-    case 1: return launch_flat<1>(X, y, W, b, N, D, P, partials, gx, s);
-    case 2: return launch_flat<2>(X, y, W, b, N, D, P, partials, gx, s);
-    case 3: return launch_flat<3>(X, y, W, b, N, D, P, partials, gx, s);
-    default: return launch_flat<4>(X, y, W, b, N, D, P, partials, gx, s);
+  const dim3 grid = slab_grid(gx, P);
+  if (D == 32) {
+    using namespace tile32;
+    CUtensorMap mx, my;
+    if (!encode_x_map(&mx, X, N) || !encode_label_map(&my, y, N, Normal::kYType)) return B2_ERR_LAUNCH;
+    return launch_tc(glm_normal_tc_kernel, grid, dim3(kThreads), Smem32<Normal::kYBytes>::kBytes, s, mx, my, W, b, N,
+                     P, partials);
   }
+  // X is always split: there is one instantiation per DC
+  return glm_dispatch_dc<1>(D, true, [&](auto dc, auto) {
+    using C = tcf::Cfg<decltype(dc)::value>;
+    return launch_tc(glm_normal_flat_tc_kernel<decltype(dc)::value>, grid, dim3(C::kThreads), C::kSmemBytes, s, X, y,
+                     W, b, N, D, P, partials);
+  });
 }
 
 }  // namespace tcn
@@ -114,35 +83,22 @@ int launch(const float* X, const float* y, const float* W, const float* b, int64
 
 using namespace b2;
 
-extern "C" size_t b2_glm_normal_workspace(int64_t N, int D, int P) {
-  // [ticket, 256 B] + CTA partials [gx][P][D + 2] + one [P] row for the per-particle sums
-  if (N < 1 || D < 1 || D > 128 || P < 1) return 256;
-  const size_t gx = (size_t)glm_tc_grid_x(N);
-  return 256 + (gx * (size_t)P * (size_t)(D + 2) + (size_t)P) * sizeof(float);
-}
+extern "C" size_t b2_glm_normal_workspace(int64_t N, int D, int P) { return glm_row_workspace(N, D, P, false); }
 
 extern "C" int b2_glm_normal_loc(const float* X, const float* y, const float* W, const float* b,
                                  const float* sigma, int sigma_stride, int64_t N, int D, int P, double scale,
                                  double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
                                  float* out_dW, float* out_db, float* out_dsigma, void* workspace,
                                  size_t workspace_bytes, void* stream) {
-  if (!X || !y || !W || !sigma) return B2_ERR_NULL;
-  if (N <= 0 || P <= 0 || D < 1 || D > 128) return B2_ERR_BAD_SHAPE;
-  if (sigma_stride != 0 && sigma_stride != 1) return B2_ERR_BAD_SHAPE;
-  // the tiles arrive by TMA / bulk copies (16-byte aligned sources, 32-bit row coordinates); there is no fp32
-  // SIMT kernel for this family
-  if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
-  if (flags & B2_FLAG_GLM_FP32) return B2_ERR_BAD_SHAPE;
-  if (N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
-  if (!workspace || workspace_bytes < b2_glm_normal_workspace(N, D, P)) return B2_ERR_WORKSPACE;
+  int rc = glm_row_check(X, y, W, !sigma, N, D, P, sigma_stride != 0 && sigma_stride != 1, flags, workspace,
+                         workspace_bytes, false);
+  if (rc != B2_OK) return rc;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const int gx = glm_tc_grid_x(N);
-  unsigned int* ticket = reinterpret_cast<unsigned int*>(workspace);
-  float* partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  const int rc = tcn::launch(X, y, W, b, N, D, P, partials, gx, s);
+  const GlmRowWorkspace w = glm_row_areas(workspace, N, D, P, false);
+  rc = tcn::launch(X, y, W, b, N, D, P, w.partials, w.gx, s);
   if (rc != 0) return rc;
-  launch_glm_normal_finish(partials, ticket, gx, P, D, N, scale, weight, sum_coeff, flags, out_sum_p, out_total,
-                           out_dW, out_db, sigma, sigma_stride, out_dsigma, s);
+  launch_glm_finish(w.partials, w.ticket, w.gx, P, 1, D, scale, weight, sum_coeff, flags, out_sum_p, out_total,
+                    out_dW, out_db, nullptr, s, sigma, sigma_stride, N, out_dsigma);
   count_launch(2);
   return check_launch();
 }

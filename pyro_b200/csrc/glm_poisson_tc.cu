@@ -27,14 +27,9 @@
 #include "b2_common.cuh"
 #include "b2_math.cuh"
 #include "glm_flat_tc.cuh"
+#include "glm_host.cuh"
 
 namespace b2 {
-
-// glm.cu / glm_tc.cu
-void launch_glm_finish(const float* partials, unsigned int* ticket, int gx, int P, int K, int D, double scale,
-                       double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
-                       float* out_dW, float* out_db, const float* lg, cudaStream_t s);
-int glm_tc_grid_x(int64_t N);
 
 namespace tcpr {
 
@@ -82,50 +77,24 @@ glm_poisson_flat_tc_kernel(const float* __restrict__ X, const float* __restrict_
   if (blockIdx.y == 0) lgamma_partial<tcf::Cfg<DC>::kThreads>(y, N, lg);
 }
 
-template <bool SPLIT_X>
-int launch_32(const float* X, const float* y, const float* W, const float* b, int64_t N, int P, float* partials,
-              float* lg, int gx, cudaStream_t s) {
-  using namespace tile32;
-  CUtensorMap mx, my;
-  if (!encode_x_map(&mx, X, N) || !encode_label_map(&my, y, N, Poisson::kYType)) return B2_ERR_LAUNCH;
-  constexpr uint32_t kSmemBytes = Smem32<Poisson::kYBytes>::kBytes;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(glm_poisson_tc_kernel<SPLIT_X>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)kSmemBytes);
-    attr_set = true;
-  }
-  dim3 grid((unsigned)gx, (unsigned)((P + kM - 1) / kM), 1);
-  launch_pdl(glm_poisson_tc_kernel<SPLIT_X>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, y, W, b, N, P,
-             partials, lg);
-  return 0;
-}
-
-template <int DC, bool SPLIT_X>
-int launch_flat(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
-                float* partials, float* lg, int gx, cudaStream_t s) {
-  using C = tcf::Cfg<DC>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(glm_poisson_flat_tc_kernel<DC, SPLIT_X>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)C::kSmemBytes);
-    attr_set = true;
-  }
-  dim3 grid((unsigned)gx, (unsigned)((P + kM - 1) / kM), 1);
-  launch_pdl(glm_poisson_flat_tc_kernel<DC, SPLIT_X>, grid, dim3(C::kThreads), (size_t)C::kSmemBytes, s, X, y, W,
-             b, N, D, P, partials, lg);
-  return 0;
-}
-
-template <bool SPLIT_X>
 int launch(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
-           float* partials, float* lg, int gx, cudaStream_t s) {
-  switch ((D + 31) / 32) {
-    case 1: return launch_flat<1, SPLIT_X>(X, y, W, b, N, D, P, partials, lg, gx, s);
-    case 2: return launch_flat<2, SPLIT_X>(X, y, W, b, N, D, P, partials, lg, gx, s);
-    case 3: return launch_flat<3, SPLIT_X>(X, y, W, b, N, D, P, partials, lg, gx, s);
-    default: return launch_flat<4, SPLIT_X>(X, y, W, b, N, D, P, partials, lg, gx, s);
+           float* partials, float* lg, int gx, bool split_x, cudaStream_t s) {
+  const dim3 grid = slab_grid(gx, P);
+  if (D == 32) {
+    using namespace tile32;
+    CUtensorMap mx, my;
+    if (!encode_x_map(&mx, X, N) || !encode_label_map(&my, y, N, Poisson::kYType)) return B2_ERR_LAUNCH;
+    constexpr uint32_t kSmemBytes = Smem32<Poisson::kYBytes>::kBytes;
+    return split_x ? launch_tc(glm_poisson_tc_kernel<true>, grid, dim3(kThreads), kSmemBytes, s, mx, my, y, W, b, N,
+                               P, partials, lg)
+                   : launch_tc(glm_poisson_tc_kernel<false>, grid, dim3(kThreads), kSmemBytes, s, mx, my, y, W, b, N,
+                               P, partials, lg);
   }
+  return glm_dispatch_dc<1>(D, split_x, [&](auto dc, auto sx) {
+    using C = tcf::Cfg<decltype(dc)::value>;
+    return launch_tc(glm_poisson_flat_tc_kernel<decltype(dc)::value, decltype(sx)::value>, grid, dim3(C::kThreads),
+                     C::kSmemBytes, s, X, y, W, b, N, D, P, partials, lg);
+  });
 }
 
 }  // namespace tcpr
@@ -133,43 +102,20 @@ int launch(const float* X, const float* y, const float* W, const float* b, int64
 
 using namespace b2;
 
-extern "C" size_t b2_glm_poisson_workspace(int64_t N, int D, int P) {
-  // [ticket, 256 B] + CTA partials [gx][P][D + 2] + one [P] row for the per-particle sums + lgamma partials [gx]
-  if (N < 1 || D < 1 || D > 128 || P < 1) return 256;
-  const size_t gx = (size_t)glm_tc_grid_x(N);
-  return 256 + (gx * (size_t)P * (size_t)(D + 2) + (size_t)P + gx) * sizeof(float);
-}
+extern "C" size_t b2_glm_poisson_workspace(int64_t N, int D, int P) { return glm_row_workspace(N, D, P, true); }
 
 extern "C" int b2_glm_poisson_log_rate(const float* X, const float* y, const float* W, const float* b, int64_t N,
                                        int D, int P, double scale, double weight, double sum_coeff, int flags,
                                        float* out_sum_p, float* out_total, float* out_dW, float* out_db,
                                        void* workspace, size_t workspace_bytes, void* stream) {
-  if (!X || !y || !W) return B2_ERR_NULL;
-  if (N <= 0 || P <= 0 || D < 1 || D > 128) return B2_ERR_BAD_SHAPE;
-  // the tiles arrive by TMA / bulk copies (16-byte aligned sources, 32-bit row coordinates); there is no fp32
-  // SIMT kernel for this family
-  if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
-  if (flags & B2_FLAG_GLM_FP32) return B2_ERR_BAD_SHAPE;
-  if (N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
-  if (!workspace || workspace_bytes < b2_glm_poisson_workspace(N, D, P)) return B2_ERR_WORKSPACE;
+  int rc = glm_row_check(X, y, W, false, N, D, P, false, flags, workspace, workspace_bytes, true);
+  if (rc != B2_OK) return rc;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const int gx = glm_tc_grid_x(N);
-  unsigned int* ticket = reinterpret_cast<unsigned int*>(workspace);
-  float* partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  float* lg = partials + (size_t)gx * P * (D + 2) + P;
-  // the precision policy of b2_glm_bernoulli_logits: below 64 Ki rows the incoherent X rounding has not
-  // averaged out yet -> X split as well
-  const bool split_x = (flags & B2_FLAG_GLM_3XTF32) || N < 65536;
-  int rc;
-  if (D == 32)
-    rc = split_x ? tcpr::launch_32<true>(X, y, W, b, N, P, partials, lg, gx, s)
-                 : tcpr::launch_32<false>(X, y, W, b, N, P, partials, lg, gx, s);
-  else
-    rc = split_x ? tcpr::launch<true>(X, y, W, b, N, D, P, partials, lg, gx, s)
-                 : tcpr::launch<false>(X, y, W, b, N, D, P, partials, lg, gx, s);
+  const GlmRowWorkspace w = glm_row_areas(workspace, N, D, P, true);
+  rc = tcpr::launch(X, y, W, b, N, D, P, w.partials, w.lg, w.gx, glm_split_x(flags, N), s);
   if (rc != 0) return rc;
-  launch_glm_finish(partials, ticket, gx, P, 1, D, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW,
-                    out_db, lg, s);
+  launch_glm_finish(w.partials, w.ticket, w.gx, P, 1, D, scale, weight, sum_coeff, flags, out_sum_p, out_total,
+                    out_dW, out_db, w.lg, s);
   count_launch(2);
   return check_launch();
 }

@@ -4,22 +4,21 @@
 //   U[c]    = -( SUM_n log p(y_n | logits_cn) + SUM log Normal(w; 0, s_w) + SUM log Normal(b; 0, s_b) )
 //   grad[c] = dU / dz[c]                                           (in z's layout)
 //
-// The likelihood and its gradient come from the fused GLM kernels (glm.cu / glm_tc.cu for Bernoulli,
-// glm_categorical_tc.cu for Categorical, glm_poisson_tc.cu for Poisson, the D = 32 ones on the tile pipeline
-// of glm_tc_common.cuh, and glm_finish_kernel of glm.cu for all three) with their particle axis set to the chains, so X is read once per
-// evaluation for every chain together.  One evaluation is a fixed launch sequence with no host sync (CUDA
-// graph capturable):
+// The likelihood and its gradient come from the fused GLM likelihood entry points (b2_glm_bernoulli_logits,
+// b2_glm_categorical_logits, b2_glm_poisson_log_rate, b2_glm_normal_loc, b2_glm_binomial_logits: a tile kernel and
+// glm_finish_kernel each) with their particle axis set to the chains, so X is read once per evaluation for every
+// chain together.  Each entry point checks its own arguments, then glm_potential_run makes the one fixed launch
+// sequence, with no host sync (CUDA graph capturable):
 //   1. glm_potential_pack_kernel    z's weight / bias columns -> the contiguous [C, K*D] / [C, K] operands
 //                                   (z's rows also hold the other site, so their stride is not the kernels')
-//   2. the GLM kernel + its finish  weight = -1: dW, db are d(-loglik)/dW, d(-loglik)/db; sum_p = loglik
+//   2. the likelihood call          weight = -1: dW, db are d(-loglik)/dW, d(-loglik)/db; sum_p = loglik
 //   3. glm_potential_finish_kernel  adds the Normal prior value and gradient, one warp per chain, fp64
 //                                   accumulation in a fixed order, and writes U and grad
-// The GLM kernels always run with B2_FLAG_GLM_3XTF32 here: every logit is fp32-exact, so the sampler
-// targets the posterior of the data as given, not of X rounded to TF32.
-// Linear regression (b2_glm_normal_potential) runs the same three launches around b2_glm_normal_loc: the pack also
-// writes each chain's noise scale sigma_c = exp(z[c, s_off]) (or the constant), and the finish adds sigma's prior
-// and the Jacobian of sigma = e^t in fp64.  Binomial regression (b2_glm_binomial_potential) runs the same three
-// launches around b2_glm_binomial_logits (kernel + finish: four in all) with the trial counts as a fixed operand.
+// The GLM kernels always run with every logit fp32-exact (B2_FLAG_GLM_3XTF32; the Normal kernels always split X),
+// so the sampler targets the posterior of the data as given, not of X rounded to TF32.
+// With a noise scale (linear regression) the pack also writes each chain's sigma_c = exp(z[c, s_off]) (or the
+// constant), and the finish adds sigma's prior and the Jacobian of sigma = e^t in fp64.  Binomial regression passes
+// the trial counts to its likelihood call as a fixed operand.
 #include <math.h>
 
 #include "b2_common.cuh"
@@ -99,27 +98,75 @@ __global__ void __launch_bounds__(256) glm_potential_finish_kernel(
   }
 }
 
-// workspace areas, each 256-byte aligned: [GLM kernel workspace][Wp][bp][dW][db][sum_p]
+// workspace areas, each 256-byte aligned: [likelihood workspace of lik_bytes][Wp][bp][dW][db][sum_p], then with a
+// noise scale [sig][dsig]
 struct GlmPotentialLayout {
-  size_t glm, wp, bp, dw, db, sum_p, total;
+  size_t wp, bp, dw, db, sum_p, sig, dsig, total;
 };
 
 inline size_t round256(size_t b) { return (b + 255) & ~(size_t)255; }
 
-inline GlmPotentialLayout glm_potential_layout(int kind, int64_t N, int D, int K, int64_t C) {
+inline GlmPotentialLayout glm_potential_layout(size_t lik_bytes, int64_t KD, int K, int64_t C, bool with_sigma) {
   GlmPotentialLayout L;
-  const size_t KD = (size_t)K * D, c = (size_t)C;
-  L.glm = 0;
-  size_t off = round256(kind == B2_GLM_BERNOULLI ? b2_glm_workspace(N, D, (int)C)
-                        : kind == B2_GLM_POISSON ? b2_glm_poisson_workspace(N, D, (int)C)
-                                                 : b2_glm_categorical_workspace(N, D, K, (int)C));
-  L.wp = off; off += round256(c * KD * sizeof(float));
+  const size_t kd = (size_t)KD, c = (size_t)C;
+  size_t off = round256(lik_bytes);
+  L.wp = off; off += round256(c * kd * sizeof(float));
   L.bp = off; off += round256(c * K * sizeof(float));
-  L.dw = off; off += round256(c * KD * sizeof(float));
+  L.dw = off; off += round256(c * kd * sizeof(float));
   L.db = off; off += round256(c * K * sizeof(float));
   L.sum_p = off; off += round256(c * sizeof(float));
+  L.sig = L.dsig = 0;
+  if (with_sigma) {
+    L.sig = off; off += round256(c * sizeof(float));
+    L.dsig = off; off += round256(c * sizeof(float));
+  }
   L.total = off;
   return L;
+}
+
+// The noise scale of linear regression: latent when s_off >= 0 (z[c, s_off] holds its log; prior s_prior with
+// parameters sp0, sp1), else the constant s_const.
+struct PotentialSigma {
+  int64_t s_off;
+  float s_const;
+  int s_prior;
+  double sp0, sp1;
+};
+
+// One potential evaluation after the entry point's own checks: pack -> likelihood -> potential finish.
+// lik(Wp, bp, sig, dsig, sum_p, dW, db, ws, ws_bytes) makes the likelihood call on the chains' packed operands
+// with weight -1, writing sum_p, dW, db (and dsig) into the layout's areas, and returns its B2 code.  sg is
+// null without a noise scale.
+template <class Likelihood>
+int glm_potential_run(size_t lik_bytes, const float* z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int KD,
+                      int K, int has_bias, double s_w, double s_b, const PotentialSigma* sg, float* U, float* grad,
+                      void* workspace, size_t workspace_bytes, cudaStream_t s, Likelihood lik) {
+  const GlmPotentialLayout L = glm_potential_layout(lik_bytes, KD, K, C, sg != nullptr);
+  if (!workspace || workspace_bytes < L.total) return B2_ERR_WORKSPACE;
+  const int Kb = has_bias ? K : 0;
+  char* ws = reinterpret_cast<char*>(workspace);
+  float* Wp = reinterpret_cast<float*>(ws + L.wp);
+  float* bp = has_bias ? reinterpret_cast<float*>(ws + L.bp) : nullptr;
+  float* dW = reinterpret_cast<float*>(ws + L.dw);
+  float* db = has_bias ? reinterpret_cast<float*>(ws + L.db) : nullptr;
+  float* sum_p = reinterpret_cast<float*>(ws + L.sum_p);
+  float* sig = sg ? reinterpret_cast<float*>(ws + L.sig) : nullptr;
+  float* dsig = sg ? reinterpret_cast<float*>(ws + L.dsig) : nullptr;
+  const int64_t s_off = sg ? sg->s_off : -1;
+
+  const int64_t npack = C * (KD + Kb);
+  glm_potential_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, Wp, bp,
+                                                                             s_off, sg ? sg->s_const : 0.f, sig);
+  count_launch(1);
+  int rc = check_launch();
+  if (rc != 0) return rc;
+  rc = lik(Wp, bp, sig, dsig, sum_p, dW, db, ws, L.wp);
+  if (rc != 0) return rc;
+  glm_potential_finish_kernel<<<(unsigned)((C * 32 + 255) / 256), 256, 0, s>>>(
+      z, C, Dz, w_off, b_off, KD, Kb, s_w, s_b, sum_p, dW, db, U, grad, sig, dsig, s_off, sg ? sg->s_prior : 0,
+      sg ? sg->sp0 : 0.0, sg ? sg->sp1 : 0.0);
+  count_launch(1);
+  return check_launch();
 }
 
 inline bool glm_potential_in_scope(int kind, int64_t N, int D, int K, int64_t C) {
@@ -130,13 +177,20 @@ inline bool glm_potential_in_scope(int kind, int64_t N, int D, int K, int64_t C)
   return false;
 }
 
+// the likelihood workspace of an in-scope b2_glm_potential kind
+inline size_t glm_potential_lik_bytes(int kind, int64_t N, int D, int K, int64_t C) {
+  return kind == B2_GLM_BERNOULLI ? b2_glm_workspace(N, D, (int)C)
+         : kind == B2_GLM_POISSON ? b2_glm_poisson_workspace(N, D, (int)C)
+                                  : b2_glm_categorical_workspace(N, D, K, (int)C);
+}
+
 }  // namespace b2
 
 using namespace b2;
 
 extern "C" size_t b2_glm_potential_workspace(int kind, int64_t N, int D, int K, int64_t C) {
   if (!glm_potential_in_scope(kind, N, D, K, C)) return 256;
-  return glm_potential_layout(kind, N, D, K, C).total;
+  return glm_potential_layout(glm_potential_lik_bytes(kind, N, D, K, C), (int64_t)K * D, K, C, false).total;
 }
 
 extern "C" int b2_glm_potential(int kind, const float* X, const void* y, int64_t N, int D, int K, int has_bias,
@@ -151,63 +205,26 @@ extern "C" int b2_glm_potential(int kind, const float* X, const void* y, int64_t
   if (has_bias && (b_off < 0 || b_off + Kb > Dz || (b_off < w_off + KD && w_off < b_off + Kb)))
     return B2_ERR_BAD_SHAPE;
   if (!(s_w > 0.0) || (has_bias && !(s_b > 0.0))) return B2_ERR_BAD_SHAPE;
-  const GlmPotentialLayout L = glm_potential_layout(kind, N, D, K, C);
-  if (!workspace || workspace_bytes < L.total) return B2_ERR_WORKSPACE;
-  char* ws = reinterpret_cast<char*>(workspace);
-  float* Wp = reinterpret_cast<float*>(ws + L.wp);
-  float* bp = has_bias ? reinterpret_cast<float*>(ws + L.bp) : nullptr;
-  float* dW = reinterpret_cast<float*>(ws + L.dw);
-  float* db = has_bias ? reinterpret_cast<float*>(ws + L.db) : nullptr;
-  float* sum_p = reinterpret_cast<float*>(ws + L.sum_p);
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-
-  const int64_t npack = C * (KD + Kb);
-  glm_potential_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, Wp, bp,
-                                                                             (int64_t)-1, 0.f, nullptr);
-  count_launch(1);
-  int rc = check_launch();
-  if (rc != 0) return rc;
-  const size_t glm_bytes = L.wp - L.glm;
-  if (kind == B2_GLM_BERNOULLI)
-    rc = b2_glm_bernoulli_logits(X, static_cast<const float*>(y), Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
-                                 B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws + L.glm, glm_bytes, stream);
-  else if (kind == B2_GLM_POISSON)
-    rc = b2_glm_poisson_log_rate(X, static_cast<const float*>(y), Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
-                                 B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws + L.glm, glm_bytes, stream);
-  else
-    rc = b2_glm_categorical_logits(X, static_cast<const int64_t*>(y), Wp, bp, N, D, K, (int)C, 1.0, -1.0, 1.0,
-                                   B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws + L.glm, glm_bytes, stream);
-  if (rc != 0) return rc;
-  glm_potential_finish_kernel<<<(unsigned)((C * 32 + 255) / 256), 256, 0, s>>>(
-      z, C, Dz, w_off, b_off, KD, Kb, s_w, s_b, sum_p, dW, db, U, grad, nullptr, nullptr, (int64_t)-1, 0, 0.0, 0.0);
-  count_launch(1);
-  return check_launch();
+  return glm_potential_run(
+      glm_potential_lik_bytes(kind, N, D, K, C), z, C, Dz, w_off, b_off, KD, K, has_bias, s_w, s_b, nullptr, U, grad,
+      workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
+      [&](const float* Wp, const float* bp, const float*, float*, float* sum_p, float* dW, float* db, void* ws,
+          size_t ws_bytes) {
+        if (kind == B2_GLM_BERNOULLI)
+          return b2_glm_bernoulli_logits(X, static_cast<const float*>(y), Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
+                                         B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, stream);
+        if (kind == B2_GLM_POISSON)
+          return b2_glm_poisson_log_rate(X, static_cast<const float*>(y), Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
+                                         B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, stream);
+        return b2_glm_categorical_logits(X, static_cast<const int64_t*>(y), Wp, bp, N, D, K, (int)C, 1.0, -1.0, 1.0,
+                                         B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, stream);
+      });
 }
 
 // ---- linear regression: Normal(X @ w + b, sigma), sigma constant or latent with a positive-support prior ----
-// workspace areas, each 256-byte aligned: [b2_glm_normal_loc workspace][Wp][bp][dW][db][sum_p][sig][dsig]
-struct GlmNormalPotentialLayout {
-  size_t wp, bp, dw, db, sum_p, sig, dsig, total;
-};
-
-inline GlmNormalPotentialLayout glm_normal_potential_layout(int64_t N, int D, int64_t C) {
-  GlmNormalPotentialLayout L;
-  const size_t c = (size_t)C;
-  size_t off = round256(b2_glm_normal_workspace(N, D, (int)C));
-  L.wp = off; off += round256(c * D * sizeof(float));
-  L.bp = off; off += round256(c * sizeof(float));
-  L.dw = off; off += round256(c * D * sizeof(float));
-  L.db = off; off += round256(c * sizeof(float));
-  L.sum_p = off; off += round256(c * sizeof(float));
-  L.sig = off; off += round256(c * sizeof(float));
-  L.dsig = off; off += round256(c * sizeof(float));
-  L.total = off;
-  return L;
-}
-
 extern "C" size_t b2_glm_normal_potential_workspace(int64_t N, int D, int64_t C) {
   if (N < 1 || D < 1 || D > 128 || C < 1 || C >= ((int64_t)1 << 31)) return 256;
-  return glm_normal_potential_layout(N, D, C).total;
+  return glm_potential_layout(b2_glm_normal_workspace(N, D, (int)C), D, 1, C, true).total;
 }
 
 extern "C" int b2_glm_normal_potential(const float* X, const float* y, int64_t N, int D, int has_bias,
@@ -232,55 +249,22 @@ extern "C" int b2_glm_normal_potential(const float* X, const float* y, int64_t N
     return B2_ERR_BAD_SHAPE;
   }
   if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
-  const GlmNormalPotentialLayout L = glm_normal_potential_layout(N, D, C);
-  if (!workspace || workspace_bytes < L.total) return B2_ERR_WORKSPACE;
-  char* ws = reinterpret_cast<char*>(workspace);
-  float* Wp = reinterpret_cast<float*>(ws + L.wp);
-  float* bp = has_bias ? reinterpret_cast<float*>(ws + L.bp) : nullptr;
-  float* dW = reinterpret_cast<float*>(ws + L.dw);
-  float* db = has_bias ? reinterpret_cast<float*>(ws + L.db) : nullptr;
-  float* sum_p = reinterpret_cast<float*>(ws + L.sum_p);
-  float* sig = reinterpret_cast<float*>(ws + L.sig);
-  float* dsig = reinterpret_cast<float*>(ws + L.dsig);
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-
-  const int64_t npack = C * (D + Kb);
-  glm_potential_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(z, C, Dz, w_off, b_off, D, Kb, Wp, bp,
-                                                                             Ks ? s_off : (int64_t)-1,
-                                                                             (float)sigma, sig);
-  count_launch(1);
-  int rc = check_launch();
-  if (rc != 0) return rc;
+  const PotentialSigma sg = {Ks ? s_off : (int64_t)-1, (float)sigma, s_prior, sp0, sp1};
   // weight = -1: dW, db and dsig are derivatives of -loglik; X is always split (every mean fp32-exact)
-  rc = b2_glm_normal_loc(X, y, Wp, bp, sig, 1, N, D, (int)C, 1.0, -1.0, 1.0, 0, sum_p, nullptr, dW, db,
-                         Ks ? dsig : nullptr, ws, L.wp, stream);
-  if (rc != 0) return rc;
-  glm_potential_finish_kernel<<<(unsigned)((C * 32 + 255) / 256), 256, 0, s>>>(
-      z, C, Dz, w_off, b_off, D, Kb, s_w, s_b, sum_p, dW, db, U, grad, sig, dsig, Ks ? s_off : (int64_t)-1, s_prior,
-      sp0, sp1);
-  count_launch(1);
-  return check_launch();
+  return glm_potential_run(
+      b2_glm_normal_workspace(N, D, (int)C), z, C, Dz, w_off, b_off, D, 1, has_bias, s_w, s_b, &sg, U, grad,
+      workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
+      [&](const float* Wp, const float* bp, const float* sig, float* dsig, float* sum_p, float* dW, float* db,
+          void* ws, size_t ws_bytes) {
+        return b2_glm_normal_loc(X, y, Wp, bp, sig, 1, N, D, (int)C, 1.0, -1.0, 1.0, 0, sum_p, nullptr, dW, db,
+                                 Ks ? dsig : nullptr, ws, ws_bytes, stream);
+      });
 }
 
 // ---- Binomial regression: Binomial(m, logits = X @ w + b), m one count for every row or one per row ------------
-// workspace areas, each 256-byte aligned: [b2_glm_binomial_logits workspace][Wp][bp][dW][db][sum_p]
-inline GlmPotentialLayout glm_binomial_potential_layout(int64_t N, int D, int64_t C) {
-  GlmPotentialLayout L;
-  const size_t c = (size_t)C;
-  L.glm = 0;
-  size_t off = round256(b2_glm_binomial_workspace(N, D, (int)C));
-  L.wp = off; off += round256(c * D * sizeof(float));
-  L.bp = off; off += round256(c * sizeof(float));
-  L.dw = off; off += round256(c * D * sizeof(float));
-  L.db = off; off += round256(c * sizeof(float));
-  L.sum_p = off; off += round256(c * sizeof(float));
-  L.total = off;
-  return L;
-}
-
 extern "C" size_t b2_glm_binomial_potential_workspace(int64_t N, int D, int64_t C) {
   if (N < 1 || D < 1 || D > 128 || C < 1 || C >= ((int64_t)1 << 31)) return 256;
-  return glm_binomial_potential_layout(N, D, C).total;
+  return glm_potential_layout(b2_glm_binomial_workspace(N, D, (int)C), D, 1, C, false).total;
 }
 
 extern "C" int b2_glm_binomial_potential(const float* X, const float* y, const float* trials, int trials_per_row,
@@ -297,28 +281,13 @@ extern "C" int b2_glm_binomial_potential(const float* X, const float* y, const f
   if (!(s_w > 0.0) || (has_bias && !(s_b > 0.0))) return B2_ERR_BAD_SHAPE;
   if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
   if (trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0) return B2_ERR_BAD_SHAPE;
-  const GlmPotentialLayout L = glm_binomial_potential_layout(N, D, C);
-  if (!workspace || workspace_bytes < L.total) return B2_ERR_WORKSPACE;
-  char* ws = reinterpret_cast<char*>(workspace);
-  float* Wp = reinterpret_cast<float*>(ws + L.wp);
-  float* bp = has_bias ? reinterpret_cast<float*>(ws + L.bp) : nullptr;
-  float* dW = reinterpret_cast<float*>(ws + L.dw);
-  float* db = has_bias ? reinterpret_cast<float*>(ws + L.db) : nullptr;
-  float* sum_p = reinterpret_cast<float*>(ws + L.sum_p);
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-
-  const int64_t npack = C * (D + Kb);
-  glm_potential_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(z, C, Dz, w_off, b_off, D, Kb, Wp, bp,
-                                                                             (int64_t)-1, 0.f, nullptr);
-  count_launch(1);
-  int rc = check_launch();
-  if (rc != 0) return rc;
   // weight = -1: dW and db are derivatives of -loglik; every logit fp32-exact (X split)
-  rc = b2_glm_binomial_logits(X, y, trials, trials_per_row, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
-                              B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws + L.glm, L.wp - L.glm, stream);
-  if (rc != 0) return rc;
-  glm_potential_finish_kernel<<<(unsigned)((C * 32 + 255) / 256), 256, 0, s>>>(
-      z, C, Dz, w_off, b_off, D, Kb, s_w, s_b, sum_p, dW, db, U, grad, nullptr, nullptr, (int64_t)-1, 0, 0.0, 0.0);
-  count_launch(1);
-  return check_launch();
+  return glm_potential_run(
+      b2_glm_binomial_workspace(N, D, (int)C), z, C, Dz, w_off, b_off, D, 1, has_bias, s_w, s_b, nullptr, U, grad,
+      workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
+      [&](const float* Wp, const float* bp, const float*, float*, float* sum_p, float* dW, float* db, void* ws,
+          size_t ws_bytes) {
+        return b2_glm_binomial_logits(X, y, trials, trials_per_row, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
+                                      B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, stream);
+      });
 }

@@ -51,7 +51,12 @@
 #include <cuda.h>
 #include <stdlib.h>
 
+#include <mutex>
+#include <set>
+#include <utility>
+
 #include "b2_common.cuh"
+#include "glm_host.cuh"
 #include "glm_tc_common.cuh"
 
 namespace b2 {
@@ -80,6 +85,22 @@ int glm_tc_grid_x(int64_t N) {
   return (int)gx;
 }
 
+// The attribute belongs to the device's context, and several host threads may make their first launch at once.
+bool set_max_dynamic_smem(const void* kernel, int bytes) {
+  static std::mutex mu;
+  static std::set<std::pair<const void*, int>> done;
+  int dev;
+  if (cudaGetDevice(&dev) != cudaSuccess) return false;
+  std::lock_guard<std::mutex> lock(mu);
+  if (done.count({kernel, dev})) return true;
+  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) != cudaSuccess) {
+    (void)cudaGetLastError();   // reported by the return code, not left for the next launch check
+    return false;
+  }
+  done.insert({kernel, dev});
+  return true;
+}
+
 // returns 0 on success, a negative B2_ERR code when the TMA path cannot be used for these operands
 int launch_glm_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int P,
                   float* partials, int gx, bool split_x, cudaStream_t s) {
@@ -90,18 +111,11 @@ int launch_glm_tc(const float* X, const float* y, const float* W, const float* b
   CUtensorMap mx, my;
   if (!encode_x_map(&mx, X, N) || !encode_label_map(&my, y, N, Bernoulli::kYType)) return B2_ERR_LAUNCH;
   constexpr uint32_t kSmemBytes = Smem32<Bernoulli::kYBytes>::kBytes;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    cudaFuncSetAttribute(glm_bernoulli_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    attr_set = true;
-  }
-  dim3 grid((unsigned)gx, (unsigned)((P + kM - 1) / kM), 1);
-  if (split_x)
-    launch_pdl(glm_bernoulli_tc_kernel<true>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, W, b, N, P, partials);
-  else
-    launch_pdl(glm_bernoulli_tc_kernel<false>, grid, dim3(kThreads), (size_t)kSmemBytes, s, mx, my, W, b, N, P, partials);
-  return 0;
+  const dim3 grid = slab_grid(gx, P);
+  return split_x ? launch_tc(glm_bernoulli_tc_kernel<true>, grid, dim3(kThreads), kSmemBytes, s, mx, my, W, b, N, P,
+                             partials)
+                 : launch_tc(glm_bernoulli_tc_kernel<false>, grid, dim3(kThreads), kSmemBytes, s, mx, my, W, b, N, P,
+                             partials);
 }
 
 }  // namespace b2

@@ -900,5 +900,8 @@ inline bool encode_label_map(CUtensorMap* m, const void* y, int64_t N, CUtensorM
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+// gx CTAs for each slab of kM particles
+inline dim3 slab_grid(int gx, int P) { return dim3((unsigned)gx, (unsigned)((P + kM - 1) / kM), 1); }
+
 }  // namespace tc
 }  // namespace b2

@@ -41,6 +41,7 @@
 
 #include "b2_common.cuh"
 #include "b2_math.cuh"
+#include "glm_host.cuh"
 #include "glm_tc_common.cuh"
 
 namespace b2 {
@@ -347,11 +348,6 @@ extern "C" int b2_poisson_product(const float* A, const float* B, const float* x
   if (!poisson_product_shape_ok(N, K, J, P)) return B2_ERR_BAD_SHAPE;
   if (reinterpret_cast<uintptr_t>(x) % 16 != 0) return B2_ERR_BAD_SHAPE;
   if (!workspace || workspace_bytes < b2_poisson_product_workspace(N, K, J, P)) return B2_ERR_WORKSPACE;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(poisson_product_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
-    attr_set = true;
-  }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const int S = blocks_per_cta(J, P), G = cta_groups(J, P);
   unsigned int* ticket = reinterpret_cast<unsigned int*>(workspace);
@@ -360,8 +356,9 @@ extern "C" int b2_poisson_product(const float* A, const float* B, const float* x
   float* part_lg = part_lp + (size_t)P * G;
   float* sum_p = out_sum_p ? out_sum_p : part_lg + G;
   const float gscale = (float)(weight * scale);
-  launch_pdl(poisson_product_tc_kernel, dim3((unsigned)G, (unsigned)P, 1), dim3(kThreads), (size_t)kSmemBytes, s,
-             A, B, x, N, K, J, S, gscale, part_dA, part_lp, part_lg, out_dB);
+  const int rc = launch_tc(poisson_product_tc_kernel, dim3((unsigned)G, (unsigned)P, 1), dim3(kThreads), kSmemBytes,
+                           s, A, B, x, N, K, J, S, gscale, part_dA, part_lp, part_lg, out_dB);
+  if (rc != 0) return rc;
   const int64_t total = (out_dA ? (int64_t)P * N * K : 0) + P;
   launch_pdl(poisson_product_finish_kernel, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, s,
              (const float*)part_dA, (const float*)part_lp, (const float*)part_lg, G, P, N * K, scale, weight, sum_p,

@@ -1092,55 +1092,106 @@ class ExpLinearPredictor:
         return torch.exp(self._eager() if self._eager is not None else self.lp.dense())
 
 
-class _GlmBernoulliFn(torch.autograd.Function):
+class _FusedSumFn(torch.autograd.Function):
+    """The site sum of a fused likelihood kernel as one autograd node.  ``meta`` is ``(scale, weight, sum_coeff,
+    unit, ...)`` with the family's own arguments after ``unit``; ``launch(meta, *operands)`` makes the native call
+    and returns the total and one gradient per operand (None for a data operand).  ``backward`` returns those
+    gradients, times ``gout`` unless ``unit`` (the kernel already applied the caller's coefficient)."""
+
     @staticmethod
-    def forward(ctx, meta, X, y, W, b):
-        import ctypes
-        scale, weight, coeff, unit, flags = meta
-        N.require_cuda(X, "fused GLM likelihood")
-        P, D = W.shape
-        n = X.shape[0]
-        dev = X.device
-        Wc = W.contiguous()
-        bc = b.contiguous() if b is not None else None
-        total = torch.empty((), dtype=torch.float32, device=dev)
-        dW = torch.empty(P, D, dtype=torch.float32, device=dev)
-        db = torch.empty(P, dtype=torch.float32, device=dev)
-        need = int(N.lib().b2_glm_workspace(n, D, P))
-        ws = N.workspace(dev, need, tag="glm")
-        args = (X.data_ptr(), y.data_ptr(), Wc.data_ptr(), bc.data_ptr() if bc is not None else None,
-                n, D, P, float(scale), float(weight), float(coeff), int(flags), None, total.data_ptr(),
-                dW.data_ptr(), db.data_ptr(), ws.data_ptr(), ws.numel())
-        asm = _ops.take_elbo_assembly(dev)
-        if asm is None:
-            N.check(N.lib().b2_glm_bernoulli_logits(*args, N.stream_ptr(dev)), "b2_glm_bernoulli_logits")
-        else:
-            # the step's loss comes out of this call's finish kernel (the priors' sums and the other ELBO terms)
-            asm, jobs, n_jobs, jc, ptrs, tc, n_terms, _keep = asm
-            loss = torch.empty((), dtype=torch.float32, device=dev)
-            sc = N.workspace(dev, int(N.lib().b2_glm_elbo_workspace()), tag="glm_elbo")
-            N.check(N.lib().b2_glm_bernoulli_logits_elbo(*args, jobs, n_jobs, jc, ptrs, tc, n_terms, loss.data_ptr(),
-                                                         sc.data_ptr(), sc.numel(), N.stream_ptr(dev)),
-                    "b2_glm_bernoulli_logits_elbo")
-            asm.loss, asm.total = loss, total
-        ctx.grads = (dW, db if b is not None else None)
-        ctx.unit = unit
+    def forward(ctx, launch, meta, *operands):
+        total, *grads = launch(meta, *operands)
+        ctx.grads, ctx.unit = grads, meta[3]
         return total
 
     @staticmethod
     def backward(ctx, gout):
-        dW, db = ctx.grads
-        if not ctx.unit:
-            dW = dW * gout
-            db = db * gout if db is not None else None
-        return None, None, None, dW, db
+        grads = ctx.grads if ctx.unit else [g * gout if g is not None else None for g in ctx.grads]
+        return (None, None, *grads)
 
 
-def _lazy_of(logits):
-    if isinstance(logits, LinearPredictor):
-        return logits
-    lz = getattr(logits, "_lazy", None) if type(logits).__name__ == "LinearPredictorTensor" else None
-    return lz if isinstance(lz, LinearPredictor) else None
+class _FusedSum:
+    """One family's fused site sum: ``apply(meta, *operands)`` is :class:`_FusedSumFn` with the family's launch.
+    Every fused call of the family goes through ``apply`` of this one object, so a test or profile can count or
+    intercept a family's calls by replacing it."""
+
+    def __init__(self, launch):
+        self.launch = launch
+
+    def apply(self, meta, *operands):
+        return _FusedSumFn.apply(self.launch, meta, *operands)
+
+
+def _ptr(t):
+    return t.data_ptr() if t is not None else None
+
+
+def _glm_outputs(X, W, need):
+    """The total, dW (W's shape) and db (W's shape without D) of a GLM likelihood call on X's device, and its
+    ``"glm"`` workspace of ``need`` bytes."""
+    dev = X.device
+    total = torch.empty((), dtype=torch.float32, device=dev)
+    dW = torch.empty(W.shape, dtype=torch.float32, device=dev)
+    db = torch.empty(W.shape[:-1], dtype=torch.float32, device=dev)
+    return total, dW, db, N.workspace(dev, need, tag="glm")
+
+
+def _glm_bernoulli(meta, X, y, W, b):
+    scale, weight, coeff, _, flags = meta
+    N.require_cuda(X, "fused GLM likelihood")
+    P, D = W.shape
+    n = X.shape[0]
+    dev = X.device
+    total, dW, db, ws = _glm_outputs(X, W, int(N.lib().b2_glm_workspace(n, D, P)))
+    Wc, bc = W.contiguous(), b.contiguous() if b is not None else None
+    args = (X.data_ptr(), y.data_ptr(), Wc.data_ptr(), _ptr(bc), n, D, P, float(scale), float(weight),
+            float(coeff), int(flags), None, total.data_ptr(), dW.data_ptr(), db.data_ptr(), ws.data_ptr(), ws.numel())
+    asm = _ops.take_elbo_assembly(dev)
+    if asm is None:
+        N.check(N.lib().b2_glm_bernoulli_logits(*args, N.stream_ptr(dev)), "b2_glm_bernoulli_logits")
+    else:
+        # the step's loss comes out of this call's finish kernel (the priors' sums and the other ELBO terms)
+        asm, jobs, n_jobs, jc, ptrs, tc, n_terms, _keep = asm
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        sc = N.workspace(dev, int(N.lib().b2_glm_elbo_workspace()), tag="glm_elbo")
+        N.check(N.lib().b2_glm_bernoulli_logits_elbo(*args, jobs, n_jobs, jc, ptrs, tc, n_terms, loss.data_ptr(),
+                                                     sc.data_ptr(), sc.numel(), N.stream_ptr(dev)),
+                "b2_glm_bernoulli_logits_elbo")
+        asm.loss, asm.total = loss, total
+    return total, None, None, dW, db if b is not None else None
+
+
+_GlmBernoulliFn = _FusedSum(_glm_bernoulli)
+
+
+def _lazy_as(x, cls):
+    """The lazy object of type ``cls`` that ``x`` is or stands for (a LinearPredictorTensor wrapping it), or None."""
+    if isinstance(x, cls):
+        return x
+    lz = getattr(x, "_lazy", None) if isinstance(x, torch.Tensor) else None
+    return lz if isinstance(lz, cls) else None
+
+
+def _weights(lp):
+    """``(W [P, D], b [P] or None)`` of a LinearPredictor."""
+    return lp.w.reshape(lp.P, lp.X.shape[-1]), lp.b.reshape(lp.P) if lp.b is not None else None
+
+
+def _per_row_scope(lp, value, mask, batch_shape):
+    """``(X, y, W, b)`` for the tensor-core kernels of the per-row GLM families (Bernoulli, Poisson, Normal,
+    Binomial) at any D in 1..128, or None outside their scope.  They take tensor cores asked for, fp32, contiguous
+    16-byte aligned X and y, no mask, one value per row and the predictor's batch shape, from 8192 rows: below that
+    the single-pass TF32 gradient has not averaged its rounding down to fp32 accuracy yet, and these kernels have no
+    fp32 counterpart."""
+    X = lp.X
+    ok = (mask is None and X.dtype == torch.float32 and X.is_contiguous() and X.data_ptr() % 16 == 0
+          and 1 <= X.shape[-1] <= 128 and getattr(lp, "tensor_cores", True) and X.shape[0] >= 8192
+          and isinstance(value, torch.Tensor) and value.numel() == X.shape[0]
+          and tuple(batch_shape) == tuple(lp.shape))
+    y = value.reshape(-1).to(torch.float32).contiguous() if ok else None
+    if not ok or y.data_ptr() % 16 != 0:
+        return None
+    return (X, y) + _weights(lp)
 
 
 class _BernoulliLinear(Bernoulli):
@@ -1148,7 +1199,7 @@ class _BernoulliLinear(Bernoulli):
     unchanged model whose ``w @ X.T + b`` was kept lazy by pyro_b200/lazy.py)."""
 
     def __init__(self, probs=None, logits=None, validate_args=None):
-        lazy = _lazy_of(logits)
+        lazy = _lazy_as(logits, LinearPredictor)
         self._lazy = lazy
         self.family = N.BERNOULLI_LOGITS
         self.param_names = ("logits",)
@@ -1168,28 +1219,23 @@ class _BernoulliLinear(Bernoulli):
     def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
         lz = self._lazy
         X = lz.X
-        D = X.shape[-1]
         tc = getattr(lz, "tensor_cores", True)
-        # D in {4, 8, 16, 32} have their own kernels; every other D up to 128 takes the wgmma kernel of
-        # glm_flat_tc.cu, from 8192 rows (below that its TF32 gradient has not averaged its rounding down to
-        # fp32 accuracy yet, and there is no fp32 kernel for these D)
-        flat = D not in (4, 8, 16, 32)
-        ok = (mask is None and X.dtype == torch.float32 and X.is_contiguous()
-              and (not flat or (1 <= D <= 128 and tc and X.shape[0] >= 8192))
-              and isinstance(value, torch.Tensor) and value.numel() == X.shape[0]
-              and tuple(self.batch_shape) == tuple(lz.shape) and X.data_ptr() % 16 == 0)
-        y = value.reshape(-1).to(torch.float32).contiguous() if ok else None
-        if not ok or (flat and y.data_ptr() % 16 != 0):
+        if X.shape[-1] in (4, 8, 16, 32):
+            # these D also have the fp32 SIMT kernel of glm.cu: any N, with or without tensor cores, any y
+            ok = (mask is None and X.dtype == torch.float32 and X.is_contiguous()
+                  and isinstance(value, torch.Tensor) and value.numel() == X.shape[0]
+                  and tuple(self.batch_shape) == tuple(lz.shape) and X.data_ptr() % 16 == 0)
+            args = (X, value.reshape(-1).to(torch.float32).contiguous()) + _weights(lz) if ok else None
+        else:
+            args = _per_row_scope(lz, value, mask, self.batch_shape)
+        if args is None:
             return super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
-        W = lz.w.reshape(lz.P, D)
-        b = lz.b.reshape(lz.P) if lz.b is not None else None
-        flags = 0 if tc else N.B2_FLAG_GLM_FP32
-        return _GlmBernoulliFn.apply((scale, weight, sum_coeff, unit, flags), X, y, W, b)
+        return _GlmBernoulliFn.apply((scale, weight, sum_coeff, unit, 0 if tc else N.B2_FLAG_GLM_FP32), *args)
 
 
 def _bernoulli_new(cls, probs=None, logits=None, validate_args=None):
     # ``Bernoulli(logits=LinearPredictor)`` builds the fused-GLM subclass
-    if cls is Bernoulli and _lazy_of(logits) is not None:
+    if cls is Bernoulli and _lazy_as(logits, LinearPredictor) is not None:
         return object.__new__(_BernoulliLinear)
     return object.__new__(cls)
 
@@ -1267,44 +1313,21 @@ def class_linear_predictor(X, W, b=None):
     return out
 
 
-class _GlmCategoricalFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, meta, X, y, W, b):
-        scale, weight, coeff, unit, flags = meta
-        N.require_cuda(X, "fused softmax-regression likelihood")
-        P, K, D = W.shape
-        n = X.shape[0]
-        dev = X.device
-        Wc = W.contiguous()
-        bc = b.contiguous() if b is not None else None
-        total = torch.empty((), dtype=torch.float32, device=dev)
-        dW = torch.empty(P, K, D, dtype=torch.float32, device=dev)
-        db = torch.empty(P, K, dtype=torch.float32, device=dev)
-        need = int(N.lib().b2_glm_categorical_workspace(n, D, K, P))
-        ws = N.workspace(dev, need, tag="glm")
-        N.check(N.lib().b2_glm_categorical_logits(
-            X.data_ptr(), y.data_ptr(), Wc.data_ptr(), bc.data_ptr() if bc is not None else None,
-            n, D, K, P, float(scale), float(weight), float(coeff), int(flags), None, total.data_ptr(),
-            dW.data_ptr(), db.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(dev)),
-            "b2_glm_categorical_logits")
-        ctx.grads = (dW, db if b is not None else None)
-        ctx.unit = unit
-        return total
-
-    @staticmethod
-    def backward(ctx, gout):
-        dW, db = ctx.grads
-        if not ctx.unit:
-            dW = dW * gout
-            db = db * gout if db is not None else None
-        return None, None, None, dW, db
+def _glm_categorical(meta, X, y, W, b):
+    scale, weight, coeff, _ = meta
+    N.require_cuda(X, "fused softmax-regression likelihood")
+    P, K, D = W.shape
+    n = X.shape[0]
+    total, dW, db, ws = _glm_outputs(X, W, int(N.lib().b2_glm_categorical_workspace(n, D, K, P)))
+    Wc, bc = W.contiguous(), b.contiguous() if b is not None else None
+    N.check(N.lib().b2_glm_categorical_logits(
+        X.data_ptr(), y.data_ptr(), Wc.data_ptr(), _ptr(bc), n, D, K, P, float(scale), float(weight),
+        float(coeff), 0, None, total.data_ptr(), dW.data_ptr(), db.data_ptr(), ws.data_ptr(), ws.numel(),
+        N.stream_ptr(X.device)), "b2_glm_categorical_logits")
+    return total, None, None, dW, db if b is not None else None
 
 
-def _class_lazy_of(logits):
-    if isinstance(logits, ClassLinearPredictor):
-        return logits
-    lz = getattr(logits, "_lazy", None) if isinstance(logits, torch.Tensor) else None
-    return lz if isinstance(lz, ClassLinearPredictor) else None
+_GlmCategoricalFn = _FusedSum(_glm_categorical)
 
 
 class _CategoricalLinear(Categorical):
@@ -1313,7 +1336,7 @@ class _CategoricalLinear(Categorical):
     and ``probs`` materialise the logits; the ELBO's site sum takes the fused kernel."""
 
     def __init__(self, probs=None, logits=None, validate_args=None):
-        lazy = _class_lazy_of(logits)
+        lazy = _lazy_as(logits, ClassLinearPredictor)
         self._lazy = lazy
         self._dense = None
         self._num_events = lazy.K
@@ -1340,12 +1363,12 @@ class _CategoricalLinear(Categorical):
         if y.data_ptr() % 16 != 0:
             y = y.clone()
         W = lz.W.reshape(lz.P, lz.K, D)
-        return _GlmCategoricalFn.apply((scale, weight, sum_coeff, unit, 0), X, y, W, lz.bias_pk())
+        return _GlmCategoricalFn.apply((scale, weight, sum_coeff, unit), X, y, W, lz.bias_pk())
 
 
 def _categorical_new(cls, probs=None, logits=None, validate_args=None):
     # ``Categorical(logits=ClassLinearPredictor)`` builds the fused softmax-regression subclass
-    if cls is Categorical and probs is None and _class_lazy_of(logits) is not None:
+    if cls is Categorical and probs is None and _lazy_as(logits, ClassLinearPredictor) is not None:
         return object.__new__(_CategoricalLinear)
     return object.__new__(cls)
 
@@ -1386,42 +1409,27 @@ class FactorProduct:
         return torch.bmm(self.A, self.B) if self.bmm else torch.matmul(self.A, self.B)
 
 
-class _PoissonProductFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, meta, A, B, x):
-        scale, weight, coeff, unit = meta
-        N.require_cuda(A, "fused Poisson factorisation likelihood")
-        Ac, Bc = A.contiguous(), B.contiguous()
-        n, K = A.shape[-2:]
-        J = B.shape[-1]
-        P = A.shape[0] if A.dim() == 3 else 1
-        dev = A.device
-        total = torch.empty((), dtype=torch.float32, device=dev)
-        dA = torch.empty(Ac.shape, dtype=torch.float32, device=dev)
-        dB = torch.empty(Bc.shape, dtype=torch.float32, device=dev)
-        need = int(N.lib().b2_poisson_product_workspace(n, K, J, P))
-        ws = N.workspace(dev, need, tag="glm")
-        N.check(N.lib().b2_poisson_product(
-            Ac.data_ptr(), Bc.data_ptr(), x.data_ptr(), n, K, J, P, float(scale), float(weight), float(coeff), 0,
-            None, total.data_ptr(), dA.data_ptr(), dB.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(dev)),
-            "b2_poisson_product")
-        ctx.grads = (dA, dB)
-        ctx.unit = unit
-        return total
-
-    @staticmethod
-    def backward(ctx, gout):
-        dA, dB = ctx.grads
-        if not ctx.unit:
-            dA, dB = dA * gout, dB * gout
-        return None, dA, dB, None
+def _poisson_product(meta, A, B, x):
+    scale, weight, coeff, _ = meta
+    N.require_cuda(A, "fused Poisson factorisation likelihood")
+    Ac, Bc = A.contiguous(), B.contiguous()
+    n, K = A.shape[-2:]
+    J = B.shape[-1]
+    P = A.shape[0] if A.dim() == 3 else 1
+    dev = A.device
+    total = torch.empty((), dtype=torch.float32, device=dev)
+    dA = torch.empty(Ac.shape, dtype=torch.float32, device=dev)
+    dB = torch.empty(Bc.shape, dtype=torch.float32, device=dev)
+    need = int(N.lib().b2_poisson_product_workspace(n, K, J, P))
+    ws = N.workspace(dev, need, tag="glm")
+    N.check(N.lib().b2_poisson_product(
+        Ac.data_ptr(), Bc.data_ptr(), x.data_ptr(), n, K, J, P, float(scale), float(weight), float(coeff), 0,
+        None, total.data_ptr(), dA.data_ptr(), dB.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(dev)),
+        "b2_poisson_product")
+    return total, dA, dB, None
 
 
-def _factor_lazy_of(rate):
-    if isinstance(rate, FactorProduct):
-        return rate
-    lz = getattr(rate, "_lazy", None) if isinstance(rate, torch.Tensor) else None
-    return lz if isinstance(lz, FactorProduct) else None
+_PoissonProductFn = _FusedSum(_poisson_product)
 
 
 class _PoissonProduct(Poisson):
@@ -1430,7 +1438,7 @@ class _PoissonProduct(Poisson):
     ``mean`` and every other use materialise the rate; the ELBO's site sum takes the fused kernel."""
 
     def __init__(self, rate, validate_args=None, is_sparse=False):
-        lazy = _factor_lazy_of(rate)
+        lazy = _lazy_as(rate, FactorProduct)
         self._lazy = lazy
         self._dense = None
         Distribution.__init__(self, lazy.shape)
@@ -1464,44 +1472,21 @@ class _PoissonProduct(Poisson):
 # ---------------------------------------------------------------------------------------------
 # fused Poisson regression: Poisson(rate = exp(X @ w + b))
 # ---------------------------------------------------------------------------------------------
-class _GlmPoissonFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, meta, X, y, W, b):
-        scale, weight, coeff, unit = meta
-        N.require_cuda(X, "fused Poisson-regression likelihood")
-        P, D = W.shape
-        n = X.shape[0]
-        dev = X.device
-        Wc = W.contiguous()
-        bc = b.contiguous() if b is not None else None
-        total = torch.empty((), dtype=torch.float32, device=dev)
-        dW = torch.empty(P, D, dtype=torch.float32, device=dev)
-        db = torch.empty(P, dtype=torch.float32, device=dev)
-        need = int(N.lib().b2_glm_poisson_workspace(n, D, P))
-        ws = N.workspace(dev, need, tag="glm")
-        N.check(N.lib().b2_glm_poisson_log_rate(
-            X.data_ptr(), y.data_ptr(), Wc.data_ptr(), bc.data_ptr() if bc is not None else None,
-            n, D, P, float(scale), float(weight), float(coeff), 0, None, total.data_ptr(),
-            dW.data_ptr(), db.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(dev)),
-            "b2_glm_poisson_log_rate")
-        ctx.grads = (dW, db if b is not None else None)
-        ctx.unit = unit
-        return total
-
-    @staticmethod
-    def backward(ctx, gout):
-        dW, db = ctx.grads
-        if not ctx.unit:
-            dW = dW * gout
-            db = db * gout if db is not None else None
-        return None, None, None, dW, db
+def _glm_poisson(meta, X, y, W, b):
+    scale, weight, coeff, _ = meta
+    N.require_cuda(X, "fused Poisson-regression likelihood")
+    P, D = W.shape
+    n = X.shape[0]
+    total, dW, db, ws = _glm_outputs(X, W, int(N.lib().b2_glm_poisson_workspace(n, D, P)))
+    Wc, bc = W.contiguous(), b.contiguous() if b is not None else None
+    N.check(N.lib().b2_glm_poisson_log_rate(
+        X.data_ptr(), y.data_ptr(), Wc.data_ptr(), _ptr(bc), n, D, P, float(scale), float(weight),
+        float(coeff), 0, None, total.data_ptr(), dW.data_ptr(), db.data_ptr(), ws.data_ptr(), ws.numel(),
+        N.stream_ptr(X.device)), "b2_glm_poisson_log_rate")
+    return total, None, None, dW, db if b is not None else None
 
 
-def _exp_lazy_of(rate):
-    if isinstance(rate, ExpLinearPredictor):
-        return rate
-    lz = getattr(rate, "_lazy", None) if isinstance(rate, torch.Tensor) else None
-    return lz if isinstance(lz, ExpLinearPredictor) else None
+_GlmPoissonFn = _FusedSum(_glm_poisson)
 
 
 class _PoissonLinear(Poisson):
@@ -1510,7 +1495,7 @@ class _PoissonLinear(Poisson):
     materialise the rate; the ELBO's site sum takes the fused kernel."""
 
     def __init__(self, rate, validate_args=None, is_sparse=False):
-        lazy = _exp_lazy_of(rate)
+        lazy = _lazy_as(rate, ExpLinearPredictor)
         self._lazy = lazy
         self._dense = None
         Distribution.__init__(self, lazy.shape)
@@ -1526,30 +1511,18 @@ class _PoissonLinear(Poisson):
         return self._params[0]
 
     def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
-        lp = self._lazy.lp
-        X = lp.X
-        D = X.shape[-1]
-        # the scope of the any-D logistic-regression kernel: tensor cores asked for, 1 <= D <= 128, from 8192
-        # rows (below that the TF32 gradient has not averaged its rounding down to fp32 accuracy yet), fp32,
-        # contiguous 16-byte aligned X and y, no mask
-        ok = (mask is None and X.dtype == torch.float32 and X.is_contiguous() and X.data_ptr() % 16 == 0
-              and 1 <= D <= 128 and getattr(lp, "tensor_cores", True) and X.shape[0] >= 8192
-              and isinstance(value, torch.Tensor) and value.numel() == X.shape[0]
-              and tuple(self.batch_shape) == tuple(lp.shape))
-        y = value.reshape(-1).to(torch.float32).contiguous() if ok else None
-        if not ok or y.data_ptr() % 16 != 0:
+        args = _per_row_scope(self._lazy.lp, value, mask, self.batch_shape)
+        if args is None:
             return super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
-        W = lp.w.reshape(lp.P, D)
-        b = lp.b.reshape(lp.P) if lp.b is not None else None
-        return _GlmPoissonFn.apply((scale, weight, sum_coeff, unit), X, y, W, b)
+        return _GlmPoissonFn.apply((scale, weight, sum_coeff, unit), *args)
 
 
 def _poisson_new(cls, rate=None, validate_args=None, is_sparse=False):
     # ``Poisson(FactorProduct)`` builds the fused factorisation subclass, ``Poisson(ExpLinearPredictor)`` the
     # fused Poisson-regression one
-    if cls is Poisson and _factor_lazy_of(rate) is not None:
+    if cls is Poisson and _lazy_as(rate, FactorProduct) is not None:
         return object.__new__(_PoissonProduct)
-    if cls is Poisson and _exp_lazy_of(rate) is not None:
+    if cls is Poisson and _lazy_as(rate, ExpLinearPredictor) is not None:
         return object.__new__(_PoissonLinear)
     return object.__new__(cls)
 
@@ -1560,49 +1533,29 @@ Poisson.__new__ = staticmethod(_poisson_new)
 # ---------------------------------------------------------------------------------------------
 # fused linear regression: Normal(loc = X @ w + b, scale = sigma)
 # ---------------------------------------------------------------------------------------------
-class _GlmNormalFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, meta, X, y, W, b, sigma):
-        scale, weight, coeff, unit, stride = meta
-        N.require_cuda(X, "fused linear-regression likelihood")
-        P, D = W.shape
-        n = X.shape[0]
-        dev = X.device
-        Wc = W.contiguous()
-        bc = b.contiguous() if b is not None else None
-        sc = sigma.contiguous()
-        total = torch.empty((), dtype=torch.float32, device=dev)
-        dW = torch.empty(P, D, dtype=torch.float32, device=dev)
-        db = torch.empty(P, dtype=torch.float32, device=dev)
-        dsig = torch.empty(P, dtype=torch.float32, device=dev) if sigma.requires_grad else None
-        need = int(N.lib().b2_glm_normal_workspace(n, D, P))
-        ws = N.workspace(dev, need, tag="glm")
-        N.check(N.lib().b2_glm_normal_loc(
-            X.data_ptr(), y.data_ptr(), Wc.data_ptr(), bc.data_ptr() if bc is not None else None, sc.data_ptr(),
-            stride, n, D, P, float(scale), float(weight), float(coeff), 0, None, total.data_ptr(), dW.data_ptr(),
-            db.data_ptr(), dsig.data_ptr() if dsig is not None else None, ws.data_ptr(), ws.numel(),
-            N.stream_ptr(dev)), "b2_glm_normal_loc")
-        if dsig is not None and stride == 0:
-            dsig = dsig.sum().reshape(sigma.shape)      # one sigma shared by every particle
-        ctx.grads = (dW, db if b is not None else None, dsig)
-        ctx.unit = unit
-        return total
+def _glm_normal(meta, X, y, W, b, sigma):
+    scale, weight, coeff, _, stride = meta
+    N.require_cuda(X, "fused linear-regression likelihood")
+    P, D = W.shape
+    n = X.shape[0]
+    total, dW, db, ws = _glm_outputs(X, W, int(N.lib().b2_glm_normal_workspace(n, D, P)))
+    dsig = torch.empty(P, dtype=torch.float32, device=X.device) if sigma.requires_grad else None
+    Wc, bc, sc = W.contiguous(), b.contiguous() if b is not None else None, sigma.contiguous()
+    N.check(N.lib().b2_glm_normal_loc(
+        X.data_ptr(), y.data_ptr(), Wc.data_ptr(), _ptr(bc), sc.data_ptr(), stride, n, D,
+        P, float(scale), float(weight), float(coeff), 0, None, total.data_ptr(), dW.data_ptr(), db.data_ptr(),
+        _ptr(dsig), ws.data_ptr(), ws.numel(), N.stream_ptr(X.device)), "b2_glm_normal_loc")
+    if dsig is not None and stride == 0:
+        dsig = dsig.sum().reshape(sigma.shape)      # one sigma shared by every particle
+    return total, None, None, dW, db if b is not None else None, dsig
 
-    @staticmethod
-    def backward(ctx, gout):
-        dW, db, dsig = ctx.grads
-        if not ctx.unit:
-            dW = dW * gout
-            db = db * gout if db is not None else None
-            dsig = dsig * gout if dsig is not None else None
-        return None, None, None, dW, db, dsig
+
+_GlmNormalFn = _FusedSum(_glm_normal)
 
 
 def _linear_loc_of(loc):
     """The LinearPredictorTensor behind a Normal loc (a lazy ``X @ w + b``), or None."""
-    if type(loc).__name__ != "LinearPredictorTensor":
-        return None
-    return loc if isinstance(getattr(loc, "_lazy", None), LinearPredictor) else None
+    return loc if isinstance(loc, torch.Tensor) and _lazy_as(loc, LinearPredictor) is not None else None
 
 
 def _per_particle_sigma(scale, lp):
@@ -1616,21 +1569,10 @@ def _per_particle_sigma(scale, lp):
     if not isinstance(s, torch.Tensor) or s.dtype != torch.float32 or s.device != lp.X.device:
         return None
     if s.dim() >= 1 and s.shape[-1] > 1 and s.stride(-1) == 0:
-        # the lazy broadcast_tensors of pyro_b200/lazy.py remembers what it expanded
-        # (or, for an expand of a tensor that is not itself a view, the autograd base); anything else, such as an
-        # expansion of a slice, whose base is the sliced tensor, is not one value per particle here
-        base = getattr(s, "_b2_unexpanded", None)
-        base = s._base if base is None else base
-        if base is None or base.dim() > s.dim() or base.data_ptr() != s.data_ptr():
+        # only an expansion along N is looked through (a [P, 1] scale expanded along P is taken as it is)
+        s = _unexpanded(s)
+        if s is None:
             return None
-        try:
-            if torch.broadcast_shapes(base.shape, s.shape) != s.shape:
-                return None
-        except RuntimeError:
-            return None
-        if base.expand(s.shape).stride() != s.stride():
-            return None
-        s = base
     if s.numel() == 1 and s.dim() <= len(lp.shape):
         return s.reshape(1), 0
     if lp.vectorised and tuple(s.shape) == (lp.P, 1) and lp.P > 1:
@@ -1668,22 +1610,11 @@ class _NormalLinear(Normal):
 
     def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
         lp = self._loc_lazy.lazy
-        X = lp.X
-        D = X.shape[-1]
-        # the scope of the linear-regression kernel: tensor cores asked for, 1 <= D <= 128, from 8192 rows (below
-        # that the single-pass TF32 gradient has not averaged its rounding down to fp32 accuracy yet), fp32,
-        # contiguous 16-byte aligned X and y, no mask, one noise scale per particle
-        ok = (mask is None and X.dtype == torch.float32 and X.is_contiguous() and X.data_ptr() % 16 == 0
-              and 1 <= D <= 128 and getattr(lp, "tensor_cores", True) and X.shape[0] >= 8192
-              and isinstance(value, torch.Tensor) and value.numel() == X.shape[0]
-              and tuple(self.batch_shape) == tuple(lp.shape))
-        sig = _per_particle_sigma(self._scale, lp) if ok else None
-        y = value.reshape(-1).to(torch.float32).contiguous() if sig is not None else None
-        if sig is None or y.data_ptr() % 16 != 0:
+        args = _per_row_scope(lp, value, mask, self.batch_shape)
+        sig = _per_particle_sigma(self._scale, lp) if args is not None else None     # one noise scale per particle
+        if sig is None:
             return super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
-        W = lp.w.reshape(lp.P, D)
-        b = lp.b.reshape(lp.P) if lp.b is not None else None
-        return _GlmNormalFn.apply((scale, weight, sum_coeff, unit, sig[1]), X, y, W, b, sig[0])
+        return _GlmNormalFn.apply((scale, weight, sum_coeff, unit, sig[1]), *args, sig[0])
 
 
 def _normal_new(cls, loc=None, scale=None, validate_args=None):
@@ -1699,37 +1630,21 @@ Normal.__new__ = staticmethod(_normal_new)
 # ---------------------------------------------------------------------------------------------
 # fused Binomial regression: Binomial(total_count, logits = X @ w + b)
 # ---------------------------------------------------------------------------------------------
-class _GlmBinomialFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, meta, X, y, trials, W, b):
-        scale, weight, coeff, unit, per_row = meta
-        N.require_cuda(X, "fused Binomial-regression likelihood")
-        P, D = W.shape
-        n = X.shape[0]
-        dev = X.device
-        Wc = W.contiguous()
-        bc = b.contiguous() if b is not None else None
-        total = torch.empty((), dtype=torch.float32, device=dev)
-        dW = torch.empty(P, D, dtype=torch.float32, device=dev)
-        db = torch.empty(P, dtype=torch.float32, device=dev)
-        need = int(N.lib().b2_glm_binomial_workspace(n, D, P))
-        ws = N.workspace(dev, need, tag="glm")
-        N.check(N.lib().b2_glm_binomial_logits(
-            X.data_ptr(), y.data_ptr(), trials.data_ptr(), per_row, Wc.data_ptr(),
-            bc.data_ptr() if bc is not None else None, n, D, P, float(scale), float(weight), float(coeff), 0, None,
-            total.data_ptr(), dW.data_ptr(), db.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(dev)),
-            "b2_glm_binomial_logits")
-        ctx.grads = (dW, db if b is not None else None)
-        ctx.unit = unit
-        return total
+def _glm_binomial(meta, X, y, W, b):
+    scale, weight, coeff, _, trials, per_row = meta
+    N.require_cuda(X, "fused Binomial-regression likelihood")
+    P, D = W.shape
+    n = X.shape[0]
+    total, dW, db, ws = _glm_outputs(X, W, int(N.lib().b2_glm_binomial_workspace(n, D, P)))
+    Wc, bc = W.contiguous(), b.contiguous() if b is not None else None
+    N.check(N.lib().b2_glm_binomial_logits(
+        X.data_ptr(), y.data_ptr(), trials.data_ptr(), per_row, Wc.data_ptr(), _ptr(bc), n, D, P,
+        float(scale), float(weight), float(coeff), 0, None, total.data_ptr(), dW.data_ptr(), db.data_ptr(),
+        ws.data_ptr(), ws.numel(), N.stream_ptr(X.device)), "b2_glm_binomial_logits")
+    return total, None, None, dW, db if b is not None else None
 
-    @staticmethod
-    def backward(ctx, gout):
-        dW, db = ctx.grads
-        if not ctx.unit:
-            dW = dW * gout
-            db = db * gout if db is not None else None
-        return None, None, None, None, dW, db
+
+_GlmBinomialFn = _FusedSum(_glm_binomial)
 
 
 def _unexpanded(t):
@@ -1777,7 +1692,7 @@ class _BinomialLinear(Binomial):
     kernel (``b2_glm_binomial_logits``) when total_count is one count or one count per row."""
 
     def __init__(self, total_count=1, probs=None, logits=None, validate_args=None):
-        lz = _lazy_of(logits)
+        lz = _lazy_as(logits, LinearPredictor)
         self._lazy, self._logits_src = lz, logits
         self.family = N.BINOMIAL_LOGITS
         self.param_names = ("total_count", "logits")
@@ -1806,28 +1721,17 @@ class _BinomialLinear(Binomial):
         return self._params[1]
 
     def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
-        lp = self._lazy
-        X = lp.X
-        D = X.shape[-1]
-        # the scope of the any-D logistic-regression kernel: tensor cores asked for, 1 <= D <= 128, from 8192 rows
-        # (below that the TF32 gradient has not averaged its rounding down to fp32 accuracy yet), fp32, contiguous
-        # 16-byte aligned X, y and trials, no mask, one count or one count per row
-        ok = (mask is None and X.dtype == torch.float32 and X.is_contiguous() and X.data_ptr() % 16 == 0
-              and 1 <= D <= 128 and getattr(lp, "tensor_cores", True) and X.shape[0] >= 8192
-              and isinstance(value, torch.Tensor) and value.numel() == X.shape[0]
-              and tuple(self.batch_shape) == tuple(lp.shape))
-        trials = _binomial_trials(self._total_count, lp) if ok else None
-        y = value.reshape(-1).to(torch.float32).contiguous() if trials is not None else None
-        if trials is None or y.data_ptr() % 16 != 0:
+        args = _per_row_scope(self._lazy, value, mask, self.batch_shape)
+        # the counts as the kernel reads them, passed in meta: they are data, never differentiated
+        trials = _binomial_trials(self._total_count, self._lazy) if args is not None else None
+        if trials is None:
             return super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
-        W = lp.w.reshape(lp.P, D)
-        b = lp.b.reshape(lp.P) if lp.b is not None else None
-        return _GlmBinomialFn.apply((scale, weight, sum_coeff, unit, trials[1]), X, y, trials[0], W, b)
+        return _GlmBinomialFn.apply((scale, weight, sum_coeff, unit) + trials, *args)
 
 
 def _binomial_new(cls, total_count=1, probs=None, logits=None, validate_args=None):
     # ``Binomial(total_count, logits=lazy X @ w + b)`` builds the fused Binomial-regression subclass
-    if cls is Binomial and probs is None and _lazy_of(logits) is not None:
+    if cls is Binomial and probs is None and _lazy_as(logits, LinearPredictor) is not None:
         return object.__new__(_BinomialLinear)
     return object.__new__(cls)
 
