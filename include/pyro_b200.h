@@ -530,6 +530,41 @@ int b2_glm_binomial_potential(const float* X, const float* y, const float* trial
 size_t b2_glm_binomial_potential_workspace(int64_t N, int D, int64_t C);
 size_t b2_glm_potential_workspace(int kind, int64_t N, int D, int K, int64_t C);
 
+/*
+ * b2_glm_scaled_potential -- HMC / NUTS potential energy and gradient of the regressions above with a LATENT
+ * weight scale: the hierarchical (w ~ Normal(0, tau)), ARD (w ~ Normal(0, lam)) and horseshoe
+ * (w ~ Normal(0, tau * lam)) weight priors, for C chains.  U is the potential of pyro/infer/mcmc/util.py:275-286:
+ *   U[c] = -( loglik + SUM_j log Normal(w_j; 0, tau lam_j) + log Normal(b; 0, s_b) + log p(tau) + log p(lam)
+ *             [+ log p(sigma)] + t + SUM_j l_j [+ log sigma] ),     tau = e^t, lam_j = e^(l_j)
+ *   grad[c,:] = dU / dz[c,:]
+ * kind: B2_GLM_BERNOULLI, B2_GLM_CATEGORICAL, B2_GLM_POISSON (as b2_glm_potential), B2_GLM_NORMAL (as
+ * b2_glm_normal_potential: s_off, s_prior, sp0, sp1 and sigma; s_off must be < 0 for every other kind) or
+ * B2_GLM_BINOMIAL (as b2_glm_binomial_potential: trials, trials_per_row), with their scopes of D and K.
+ * z: [C, Dz] fp32 row-major; w (K*D values) at w_off, b (K values, has_bias) at b_off, log sigma at s_off (>= 0),
+ * t = log tau at scale->tau_off (>= 0: one column) and l = log lam at scale->lam_off (>= 0: K*D columns, lam_j scales
+ * w_j); a -1 offset means absent, and at least one of tau and lam is latent.  Dz is exactly the sum of the present
+ * blocks' widths, none overlapping another or leaving the row.  The priors of tau and of every lam_j are
+ * B2_SIGMA_* codes with parameters (p0, p1), as for sigma: positive, and for LogNormal a finite loc.
+ * X, y (and per-row trials) 16-byte aligned.  Anything else returns B2_ERR_NULL / B2_ERR_BAD_SHAPE /
+ * B2_ERR_TOO_LARGE before any CUDA call.  Four launches with no host sync (CUDA graph capturable): the pack kernel,
+ * the kind's likelihood call with weight -1 (kernel + finish, every logit fp32-exact), and a potential finish that
+ * adds every prior term and Jacobian in fp64 in a fixed order.  workspace: b2_glm_scaled_potential_workspace()
+ * bytes, zero-initialised once.
+ */
+#define B2_GLM_NORMAL 3
+#define B2_GLM_BINOMIAL 4
+typedef struct b2_glm_weight_scale {
+  int64_t tau_off, lam_off;     /* z columns of log tau / log lam, -1 when absent */
+  int tau_prior, lam_prior;     /* B2_SIGMA_HALFNORMAL .. B2_SIGMA_LOGNORMAL */
+  double tau_p0, tau_p1, lam_p0, lam_p1;
+} b2_glm_weight_scale;
+int b2_glm_scaled_potential(int kind, const float* X, const void* y, const float* trials, int trials_per_row,
+                            int64_t N, int D, int K, int has_bias, const float* z, int64_t C, int64_t Dz,
+                            int64_t w_off, int64_t b_off, int64_t s_off, double s_b, int s_prior, double sp0,
+                            double sp1, double sigma, const b2_glm_weight_scale* scale, float* U, float* grad,
+                            void* workspace, size_t workspace_bytes, void* stream);
+size_t b2_glm_scaled_potential_workspace(int kind, int64_t N, int D, int K, int64_t C);
+
 /* ---- optimisers --------------------------------------------------------------------------
  * Multi-tensor fused updates replacing PyroOptim's per-parameter Python loop
  * (pyro/optim/optim.py:117-155).  Per-tensor scalar state lives in DEVICE arrays so a captured

@@ -35,7 +35,7 @@ EMULATE_RSAMPLE = False   # tests/cpu_emulation.py flips this to exercise the fu
 SITE_SMALL_N = 8192   # B2_SITE_SMALL_N: one-CTA kernel with fused stored-shape gradient reductions
 DIRICHLET, CATEGORICAL, MVN_TRIL = 32, 33, 34
 MODEL_HIER_NORMAL, MODEL_LOGISTIC = 0, 1
-GLM_BERNOULLI, GLM_CATEGORICAL, GLM_POISSON = 0, 1, 2
+GLM_BERNOULLI, GLM_CATEGORICAL, GLM_POISSON, GLM_NORMAL, GLM_BINOMIAL = 0, 1, 2, 3, 4
 SIGMA_CONST, SIGMA_HALFNORMAL, SIGMA_HALFCAUCHY, SIGMA_EXPONENTIAL, SIGMA_LOGNORMAL = 0, 1, 2, 3, 4
 NUTS_SMALL_MAX_D = 64
 
@@ -72,6 +72,13 @@ class b2_model(ctypes.Structure):
     _fields_ = [("model", ctypes.c_int32), ("dtype", ctypes.c_int32), ("J", ctypes.c_int64),
                 ("D", ctypes.c_int64), ("data0", ctypes.c_void_p), ("data1", ctypes.c_void_p),
                 ("hyper", ctypes.c_double * 4)]
+
+
+class b2_glm_weight_scale(ctypes.Structure):
+    """Mirror of ``b2_glm_weight_scale`` (include/pyro_b200.h): the latent weight scale of a regression potential."""
+    _fields_ = [("tau_off", ctypes.c_int64), ("lam_off", ctypes.c_int64), ("tau_prior", ctypes.c_int32),
+                ("lam_prior", ctypes.c_int32), ("tau_p0", ctypes.c_double), ("tau_p1", ctypes.c_double),
+                ("lam_p0", ctypes.c_double), ("lam_p1", ctypes.c_double)]
 
 
 class b2_nuts_lockstep(ctypes.Structure):
@@ -142,6 +149,10 @@ SIGNATURES = {
     "b2_glm_potential": (_i32, [_i32, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _i64, _i64, _f64, _f64,
                                 _vp, _vp, _vp, _sz, _vp]),
     "b2_glm_potential_workspace": (_sz, [_i32, _i64, _i32, _i32, _i64]),
+    "b2_glm_scaled_potential": (_i32, [_i32, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _i64,
+                                       _i64, _i64, _f64, _i32, _f64, _f64, _f64,
+                                       ctypes.POINTER(b2_glm_weight_scale), _vp, _vp, _vp, _sz, _vp]),
+    "b2_glm_scaled_potential_workspace": (_sz, [_i32, _i64, _i32, _i32, _i64]),
     "b2_clipped_adam": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _vp]),
     "b2_adagrad_rmsprop": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _vp]),
     "b2_leapfrog_half_kick_drift": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _i32, _vp]),

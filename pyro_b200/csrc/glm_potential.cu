@@ -18,7 +18,8 @@
 // so the sampler targets the posterior of the data as given, not of X rounded to TF32.
 // With a noise scale (linear regression) the pack also writes each chain's sigma_c = exp(z[c, s_off]) (or the
 // constant), and the finish adds sigma's prior and the Jacobian of sigma = e^t in fp64.  Binomial regression passes
-// the trial counts to its likelihood call as a fixed operand.
+// the trial counts to its likelihood call as a fixed operand.  b2_glm_scaled_potential runs the same sequence for a
+// latent weight scale (w ~ Normal(0, tau * lam)), with glm_scaled_potential_finish_kernel as step 3.
 #include <math.h>
 
 #include "b2_common.cuh"
@@ -40,6 +41,40 @@ __global__ void __launch_bounds__(256) glm_potential_pack_kernel(const float* __
   const int64_t j = i - c * per;
   if (j < KD) Wp[c * KD + j] = z[c * Dz + w_off + j];
   else bp[c * Kb + (j - KD)] = z[c * Dz + b_off + (j - KD)];
+}
+
+constexpr double kHalfLog2Pi = 0.91893853320467274178;
+
+// log p(v) and d log p / dv of a positive scale v under prior code `prior` (B2_SIGMA_*): HalfNormal(p0),
+// HalfCauchy(p0), Exponential(p0) or LogNormal(p0, p1).  The priors of a noise scale and of a weight scale.
+__device__ __forceinline__ void positive_prior(int prior, double p0, double p1, double v, double& lp, double& dlp) {
+  constexpr double kLog2 = 0.69314718055994531, kLogPi = 1.14472988584940017;
+  if (prior == B2_SIGMA_HALFNORMAL) {             // p0 = scale
+    lp = kLog2 - log(p0) - kHalfLog2Pi - v * v / (2.0 * p0 * p0);
+    dlp = -v / (p0 * p0);
+  } else if (prior == B2_SIGMA_HALFCAUCHY) {      // p0 = scale
+    lp = kLog2 - kLogPi - log(p0) - log1p(v * v / (p0 * p0));
+    dlp = -2.0 * v / (p0 * p0 + v * v);
+  } else if (prior == B2_SIGMA_EXPONENTIAL) {     // p0 = rate
+    lp = log(p0) - p0 * v;
+    dlp = -p0;
+  } else {                                        // B2_SIGMA_LOGNORMAL: p0 = loc, p1 = scale
+    const double lv = log(v), q = (lv - p0) / p1;
+    lp = -lv - log(p1) - kHalfLog2Pi - 0.5 * q * q;
+    dlp = -1.0 / v - q / (p1 * v);
+  }
+}
+
+// a latent noise scale v = e^t, t = z[c, s_off]: U += -log p(v) - t (the Jacobian of v = e^t), and
+// dU/dt = v (dU/dv) - 1 with dU/dv = dsig (the likelihood's, already negated) - d log p(v) / dv
+__device__ __forceinline__ void add_latent_sigma_terms(const float* zc, float* gc, int64_t s_off, const float* sig,
+                                                       const float* dsig, int64_t c, int s_prior, double sp0,
+                                                       double sp1, double& u) {
+  const double t = (double)zc[s_off], v = (double)sig[c];
+  double lp, dlp;
+  positive_prior(s_prior, sp0, sp1, v, lp, dlp);
+  u += -lp - t;
+  gc[s_off] = (float)(v * ((double)dsig[c] - dlp) - 1.0);
 }
 
 __global__ void __launch_bounds__(256) glm_potential_finish_kernel(
@@ -68,31 +103,69 @@ __global__ void __launch_bounds__(256) glm_potential_finish_kernel(
   qw = warp_sum(qw);
   qb = warp_sum(qb);
   if (lane == 0) {
-    constexpr double kHalfLog2Pi = 0.91893853320467274178;
     double u = -(double)sum_p[c] + 0.5 * qw + (double)KD * (log(s_w) + kHalfLog2Pi);
     if (Kb) u += 0.5 * qb + (double)Kb * (log(s_b) + kHalfLog2Pi);
-    if (sig != nullptr && s_off >= 0) {
-      // a latent noise scale v = e^t, t = z[c, s_off]: U += -log p(v) - t (the Jacobian of v = e^t), and
-      // dU/dt = v (dU/dv) - 1 with dU/dv = dsig (the likelihood's, already negated) - d log p(v) / dv
-      constexpr double kLog2 = 0.69314718055994531, kLogPi = 1.14472988584940017;
-      const double t = (double)zc[s_off], v = (double)sig[c];
-      double lp = 0.0, dlp = 0.0;
-      if (s_prior == B2_SIGMA_HALFNORMAL) {             // sp0 = scale
-        lp = kLog2 - log(sp0) - kHalfLog2Pi - v * v / (2.0 * sp0 * sp0);
-        dlp = -v / (sp0 * sp0);
-      } else if (s_prior == B2_SIGMA_HALFCAUCHY) {      // sp0 = scale
-        lp = kLog2 - kLogPi - log(sp0) - log1p(v * v / (sp0 * sp0));
-        dlp = -2.0 * v / (sp0 * sp0 + v * v);
-      } else if (s_prior == B2_SIGMA_EXPONENTIAL) {     // sp0 = rate
-        lp = log(sp0) - sp0 * v;
-        dlp = -sp0;
-      } else {                                          // B2_SIGMA_LOGNORMAL: sp0 = loc, sp1 = scale
-        const double lv = log(v), q = (lv - sp0) / sp1;
-        lp = -lv - log(sp1) - kHalfLog2Pi - 0.5 * q * q;
-        dlp = -1.0 / v - q / (sp1 * v);
-      }
+    if (sig != nullptr && s_off >= 0) add_latent_sigma_terms(zc, gc, s_off, sig, dsig, c, s_prior, sp0, sp1, u);
+    U[c] = (float)u;
+  }
+}
+
+// glm_potential_finish_kernel with a latent weight scale: one warp per chain, fp64, lane-strided over the KD
+// coefficients and then the shuffle tree, so every result is in a fixed order.  Per coefficient j, with
+// s_j = tau lam_j and a_j = 1 - w_j^2 / s_j^2:
+//   U += w_j^2 / (2 s_j^2) + log s_j + log(2 pi) / 2           dU/dw_j = dW_j + w_j / s_j^2
+//   U += -log p(lam_j) - l_j                                   dU/dl_j = a_j - lam_j (d log p / d lam)(lam_j) - 1
+// and once per chain U += -log p(tau) - t, dU/dt = SUM_j a_j - tau (d log p / d tau)(tau) - 1.  The bias prior and
+// the noise scale's terms are those of glm_potential_finish_kernel.
+__global__ void __launch_bounds__(256) glm_scaled_potential_finish_kernel(
+    const float* __restrict__ z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int KD, int Kb, double s_b,
+    const float* __restrict__ sum_p, const float* __restrict__ dW, const float* __restrict__ db,
+    float* __restrict__ U, float* __restrict__ grad, const float* __restrict__ sig, const float* __restrict__ dsig,
+    int64_t s_off, int s_prior, double sp0, double sp1, b2_glm_weight_scale ws) {
+  const int64_t c = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (c >= C) return;
+  const double ib = Kb ? 1.0 / (s_b * s_b) : 0.0;
+  const float* zc = z + c * Dz;
+  float* gc = grad + c * Dz;
+  const double t = ws.tau_off >= 0 ? (double)zc[ws.tau_off] : 0.0;
+  double uw = 0.0, asum = 0.0, qb = 0.0;  // the weight and lam terms of U, SUM a_j, SUM b^2 / s_b^2
+  for (int j = lane; j < KD; j += 32) {
+    const double v = (double)zc[w_off + j];
+    const double l = ws.lam_off >= 0 ? (double)zc[ws.lam_off + j] : 0.0;
+    const double ls = t + l;               // log s_j
+    const double is2 = exp(-2.0 * ls);     // 1 / s_j^2
+    const double q = v * v * is2;
+    uw += 0.5 * q + ls + kHalfLog2Pi;
+    gc[w_off + j] = (float)((double)dW[c * KD + j] + v * is2);
+    const double a = 1.0 - q;
+    asum += a;
+    if (ws.lam_off >= 0) {
+      const double lam = exp(l);
+      double lp, dlp;
+      positive_prior(ws.lam_prior, ws.lam_p0, ws.lam_p1, lam, lp, dlp);
+      uw += -lp - l;
+      gc[ws.lam_off + j] = (float)(a - lam * dlp - 1.0);
+    }
+  }
+  for (int j = lane; j < Kb; j += 32) {
+    const double v = (double)zc[b_off + j];
+    qb += v * v * ib;
+    gc[b_off + j] = (float)((double)db[c * Kb + j] + v * ib);
+  }
+  uw = warp_sum(uw);
+  asum = warp_sum(asum);
+  qb = warp_sum(qb);
+  if (lane == 0) {
+    double u = -(double)sum_p[c] + uw;
+    if (Kb) u += 0.5 * qb + (double)Kb * (log(s_b) + kHalfLog2Pi);
+    if (sig != nullptr && s_off >= 0) add_latent_sigma_terms(zc, gc, s_off, sig, dsig, c, s_prior, sp0, sp1, u);
+    if (ws.tau_off >= 0) {
+      const double tau = exp(t);
+      double lp, dlp;
+      positive_prior(ws.tau_prior, ws.tau_p0, ws.tau_p1, tau, lp, dlp);
       u += -lp - t;
-      gc[s_off] = (float)(v * ((double)dsig[c] - dlp) - 1.0);
+      gc[ws.tau_off] = (float)(asum - tau * dlp - 1.0);
     }
     U[c] = (float)u;
   }
@@ -136,11 +209,13 @@ struct PotentialSigma {
 // One potential evaluation after the entry point's own checks: pack -> likelihood -> potential finish.
 // lik(Wp, bp, sig, dsig, sum_p, dW, db, ws, ws_bytes) makes the likelihood call on the chains' packed operands
 // with weight -1, writing sum_p, dW, db (and dsig) into the layout's areas, and returns its B2 code.  sg is
-// null without a noise scale.
+// null without a noise scale; wsc is null for a constant weight scale s_w, else the latent weight scale, finished
+// by glm_scaled_potential_finish_kernel.
 template <class Likelihood>
 int glm_potential_run(size_t lik_bytes, const float* z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int KD,
-                      int K, int has_bias, double s_w, double s_b, const PotentialSigma* sg, float* U, float* grad,
-                      void* workspace, size_t workspace_bytes, cudaStream_t s, Likelihood lik) {
+                      int K, int has_bias, double s_w, double s_b, const PotentialSigma* sg,
+                      const b2_glm_weight_scale* wsc, float* U, float* grad, void* workspace,
+                      size_t workspace_bytes, cudaStream_t s, Likelihood lik) {
   const GlmPotentialLayout L = glm_potential_layout(lik_bytes, KD, K, C, sg != nullptr);
   if (!workspace || workspace_bytes < L.total) return B2_ERR_WORKSPACE;
   const int Kb = has_bias ? K : 0;
@@ -162,26 +237,75 @@ int glm_potential_run(size_t lik_bytes, const float* z, int64_t C, int64_t Dz, i
   if (rc != 0) return rc;
   rc = lik(Wp, bp, sig, dsig, sum_p, dW, db, ws, L.wp);
   if (rc != 0) return rc;
-  glm_potential_finish_kernel<<<(unsigned)((C * 32 + 255) / 256), 256, 0, s>>>(
-      z, C, Dz, w_off, b_off, KD, Kb, s_w, s_b, sum_p, dW, db, U, grad, sig, dsig, s_off, sg ? sg->s_prior : 0,
-      sg ? sg->sp0 : 0.0, sg ? sg->sp1 : 0.0);
+  const unsigned grid = (unsigned)((C * 32 + 255) / 256);
+  if (wsc == nullptr)
+    glm_potential_finish_kernel<<<grid, 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, s_w, s_b, sum_p, dW, db, U, grad,
+                                                     sig, dsig, s_off, sg ? sg->s_prior : 0, sg ? sg->sp0 : 0.0,
+                                                     sg ? sg->sp1 : 0.0);
+  else
+    glm_scaled_potential_finish_kernel<<<grid, 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, s_b, sum_p, dW, db, U,
+                                                            grad, sig, dsig, s_off, sg ? sg->s_prior : 0,
+                                                            sg ? sg->sp0 : 0.0, sg ? sg->sp1 : 0.0, *wsc);
   count_launch(1);
   return check_launch();
 }
 
+// Scope of the likelihood kernels (K == 1 except for softmax); the kind codes of b2_glm_scaled_potential
 inline bool glm_potential_in_scope(int kind, int64_t N, int D, int K, int64_t C) {
   if (N < 1 || C < 1 || C >= ((int64_t)1 << 31)) return false;
   if (kind == B2_GLM_BERNOULLI) return K == 1 && (D == 4 || D == 8 || D == 16 || D == 32);
   if (kind == B2_GLM_CATEGORICAL) return D == 32 && K >= 2 && K <= 16;
-  if (kind == B2_GLM_POISSON) return K == 1 && D >= 1 && D <= 128;
+  if (kind == B2_GLM_POISSON || kind == B2_GLM_NORMAL || kind == B2_GLM_BINOMIAL)
+    return K == 1 && D >= 1 && D <= 128;
   return false;
 }
 
-// the likelihood workspace of an in-scope b2_glm_potential kind
+// the kinds b2_glm_potential takes (Normal and Binomial regression have their own entry points)
+inline bool glm_plain_kind(int kind) {
+  return kind == B2_GLM_BERNOULLI || kind == B2_GLM_CATEGORICAL || kind == B2_GLM_POISSON;
+}
+
+// the likelihood workspace of an in-scope kind
 inline size_t glm_potential_lik_bytes(int kind, int64_t N, int D, int K, int64_t C) {
-  return kind == B2_GLM_BERNOULLI ? b2_glm_workspace(N, D, (int)C)
-         : kind == B2_GLM_POISSON ? b2_glm_poisson_workspace(N, D, (int)C)
-                                  : b2_glm_categorical_workspace(N, D, K, (int)C);
+  switch (kind) {
+    case B2_GLM_BERNOULLI: return b2_glm_workspace(N, D, (int)C);
+    case B2_GLM_POISSON: return b2_glm_poisson_workspace(N, D, (int)C);
+    case B2_GLM_NORMAL: return b2_glm_normal_workspace(N, D, (int)C);
+    case B2_GLM_BINOMIAL: return b2_glm_binomial_workspace(N, D, (int)C);
+    default: return b2_glm_categorical_workspace(N, D, K, (int)C);
+  }
+}
+
+// The likelihood call of glm_potential_run for every kind: weight = -1, so dW, db (and dsig) are derivatives of
+// -loglik; every logit fp32-exact (B2_FLAG_GLM_3XTF32; the Normal kernels always split X).  The noise scale `sig`
+// and its gradient `dsig` (null for a constant noise scale) are Normal regression's, trials Binomial's.
+inline int glm_potential_likelihood(int kind, const float* X, const void* y, const float* trials, int trials_per_row,
+                                    int64_t N, int D, int K, int64_t C, const float* Wp, const float* bp,
+                                    const float* sig, float* dsig, float* sum_p, float* dW, float* db, void* ws,
+                                    size_t ws_bytes, void* stream) {
+  const float* yf = static_cast<const float*>(y);
+  switch (kind) {
+    case B2_GLM_BERNOULLI:
+      return b2_glm_bernoulli_logits(X, yf, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0, B2_FLAG_GLM_3XTF32, sum_p, nullptr,
+                                     dW, db, ws, ws_bytes, stream);
+    case B2_GLM_POISSON:
+      return b2_glm_poisson_log_rate(X, yf, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0, B2_FLAG_GLM_3XTF32, sum_p, nullptr,
+                                     dW, db, ws, ws_bytes, stream);
+    case B2_GLM_NORMAL:
+      return b2_glm_normal_loc(X, yf, Wp, bp, sig, 1, N, D, (int)C, 1.0, -1.0, 1.0, 0, sum_p, nullptr, dW, db, dsig,
+                               ws, ws_bytes, stream);
+    case B2_GLM_BINOMIAL:
+      return b2_glm_binomial_logits(X, yf, trials, trials_per_row, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
+                                    B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, stream);
+    default:
+      return b2_glm_categorical_logits(X, static_cast<const int64_t*>(y), Wp, bp, N, D, K, (int)C, 1.0, -1.0, 1.0,
+                                       B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, stream);
+  }
+}
+
+inline bool positive_prior_ok(int prior, double p0, double p1) {
+  return prior == B2_SIGMA_LOGNORMAL ? p1 > 0.0 && fabs(p0) < INFINITY
+                                     : prior >= B2_SIGMA_HALFNORMAL && prior <= B2_SIGMA_EXPONENTIAL && p0 > 0.0;
 }
 
 }  // namespace b2
@@ -189,7 +313,7 @@ inline size_t glm_potential_lik_bytes(int kind, int64_t N, int D, int K, int64_t
 using namespace b2;
 
 extern "C" size_t b2_glm_potential_workspace(int kind, int64_t N, int D, int K, int64_t C) {
-  if (!glm_potential_in_scope(kind, N, D, K, C)) return 256;
+  if (!glm_plain_kind(kind) || !glm_potential_in_scope(kind, N, D, K, C)) return 256;
   return glm_potential_layout(glm_potential_lik_bytes(kind, N, D, K, C), (int64_t)K * D, K, C, false).total;
 }
 
@@ -198,7 +322,7 @@ extern "C" int b2_glm_potential(int kind, const float* X, const void* y, int64_t
                                 double s_b, float* U, float* grad, void* workspace, size_t workspace_bytes,
                                 void* stream) {
   if (!X || !y || !z || !U || !grad) return B2_ERR_NULL;
-  if (!glm_potential_in_scope(kind, N, D, K, C)) return B2_ERR_BAD_SHAPE;
+  if (!glm_plain_kind(kind) || !glm_potential_in_scope(kind, N, D, K, C)) return B2_ERR_BAD_SHAPE;
   const int KD = K * D, Kb = has_bias ? K : 0;
   // z's row is exactly the weight block and the bias block, neither overlapping nor out of the row
   if (Dz != (int64_t)KD + Kb || w_off < 0 || w_off + KD > Dz) return B2_ERR_BAD_SHAPE;
@@ -206,18 +330,12 @@ extern "C" int b2_glm_potential(int kind, const float* X, const void* y, int64_t
     return B2_ERR_BAD_SHAPE;
   if (!(s_w > 0.0) || (has_bias && !(s_b > 0.0))) return B2_ERR_BAD_SHAPE;
   return glm_potential_run(
-      glm_potential_lik_bytes(kind, N, D, K, C), z, C, Dz, w_off, b_off, KD, K, has_bias, s_w, s_b, nullptr, U, grad,
-      workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
+      glm_potential_lik_bytes(kind, N, D, K, C), z, C, Dz, w_off, b_off, KD, K, has_bias, s_w, s_b, nullptr, nullptr,
+      U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
       [&](const float* Wp, const float* bp, const float*, float*, float* sum_p, float* dW, float* db, void* ws,
           size_t ws_bytes) {
-        if (kind == B2_GLM_BERNOULLI)
-          return b2_glm_bernoulli_logits(X, static_cast<const float*>(y), Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
-                                         B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, stream);
-        if (kind == B2_GLM_POISSON)
-          return b2_glm_poisson_log_rate(X, static_cast<const float*>(y), Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
-                                         B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, stream);
-        return b2_glm_categorical_logits(X, static_cast<const int64_t*>(y), Wp, bp, N, D, K, (int)C, 1.0, -1.0, 1.0,
-                                         B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, stream);
+        return glm_potential_likelihood(kind, X, y, nullptr, 0, N, D, K, C, Wp, bp, nullptr, nullptr, sum_p, dW, db,
+                                        ws, ws_bytes, stream);
       });
 }
 
@@ -242,22 +360,19 @@ extern "C" int b2_glm_normal_potential(const float* X, const float* y, int64_t N
     return B2_ERR_BAD_SHAPE;
   if (!(s_w > 0.0) || (has_bias && !(s_b > 0.0))) return B2_ERR_BAD_SHAPE;
   if (Ks) {
-    if (s_prior == B2_SIGMA_LOGNORMAL ? !(sp1 > 0.0) || !(fabs(sp0) < INFINITY)
-        : (s_prior < B2_SIGMA_HALFNORMAL || s_prior > B2_SIGMA_EXPONENTIAL || !(sp0 > 0.0)))
-      return B2_ERR_BAD_SHAPE;
+    if (!positive_prior_ok(s_prior, sp0, sp1)) return B2_ERR_BAD_SHAPE;
   } else if (!(sigma > 0.0) || !((float)sigma > 0.f)) {
     return B2_ERR_BAD_SHAPE;
   }
   if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
   const PotentialSigma sg = {Ks ? s_off : (int64_t)-1, (float)sigma, s_prior, sp0, sp1};
-  // weight = -1: dW, db and dsig are derivatives of -loglik; X is always split (every mean fp32-exact)
   return glm_potential_run(
-      b2_glm_normal_workspace(N, D, (int)C), z, C, Dz, w_off, b_off, D, 1, has_bias, s_w, s_b, &sg, U, grad,
+      b2_glm_normal_workspace(N, D, (int)C), z, C, Dz, w_off, b_off, D, 1, has_bias, s_w, s_b, &sg, nullptr, U, grad,
       workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
       [&](const float* Wp, const float* bp, const float* sig, float* dsig, float* sum_p, float* dW, float* db,
           void* ws, size_t ws_bytes) {
-        return b2_glm_normal_loc(X, y, Wp, bp, sig, 1, N, D, (int)C, 1.0, -1.0, 1.0, 0, sum_p, nullptr, dW, db,
-                                 Ks ? dsig : nullptr, ws, ws_bytes, stream);
+        return glm_potential_likelihood(B2_GLM_NORMAL, X, y, nullptr, 0, N, D, 1, C, Wp, bp, sig, Ks ? dsig : nullptr,
+                                        sum_p, dW, db, ws, ws_bytes, stream);
       });
 }
 
@@ -281,13 +396,68 @@ extern "C" int b2_glm_binomial_potential(const float* X, const float* y, const f
   if (!(s_w > 0.0) || (has_bias && !(s_b > 0.0))) return B2_ERR_BAD_SHAPE;
   if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
   if (trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0) return B2_ERR_BAD_SHAPE;
-  // weight = -1: dW and db are derivatives of -loglik; every logit fp32-exact (X split)
   return glm_potential_run(
-      b2_glm_binomial_workspace(N, D, (int)C), z, C, Dz, w_off, b_off, D, 1, has_bias, s_w, s_b, nullptr, U, grad,
-      workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
+      b2_glm_binomial_workspace(N, D, (int)C), z, C, Dz, w_off, b_off, D, 1, has_bias, s_w, s_b, nullptr, nullptr, U,
+      grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
       [&](const float* Wp, const float* bp, const float*, float*, float* sum_p, float* dW, float* db, void* ws,
           size_t ws_bytes) {
-        return b2_glm_binomial_logits(X, y, trials, trials_per_row, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
-                                      B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, stream);
+        return glm_potential_likelihood(B2_GLM_BINOMIAL, X, y, trials, trials_per_row, N, D, 1, C, Wp, bp, nullptr,
+                                        nullptr, sum_p, dW, db, ws, ws_bytes, stream);
+      });
+}
+
+// ---- any kind with a latent weight scale: w ~ Normal(0, tau * lam) -------------------------------------------
+extern "C" size_t b2_glm_scaled_potential_workspace(int kind, int64_t N, int D, int K, int64_t C) {
+  if (!glm_potential_in_scope(kind, N, D, K, C)) return 256;
+  return glm_potential_layout(glm_potential_lik_bytes(kind, N, D, K, C), (int64_t)K * D, K, C,
+                              kind == B2_GLM_NORMAL).total;
+}
+
+extern "C" int b2_glm_scaled_potential(int kind, const float* X, const void* y, const float* trials,
+                                       int trials_per_row, int64_t N, int D, int K, int has_bias, const float* z,
+                                       int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int64_t s_off, double s_b,
+                                       int s_prior, double sp0, double sp1, double sigma,
+                                       const b2_glm_weight_scale* scale, float* U, float* grad, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+  if (!X || !y || !z || !U || !grad || !scale) return B2_ERR_NULL;
+  if (kind == B2_GLM_BINOMIAL && !trials) return B2_ERR_NULL;
+  if (!glm_potential_in_scope(kind, N, D, K, C)) return B2_ERR_BAD_SHAPE;
+  if (N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
+  const b2_glm_weight_scale sc = *scale;
+  const bool normal = kind == B2_GLM_NORMAL, has_tau = sc.tau_off >= 0, has_lam = sc.lam_off >= 0;
+  if (!has_tau && !has_lam) return B2_ERR_BAD_SHAPE;    // a constant weight scale is b2_glm_potential's
+  if (!normal && s_off >= 0) return B2_ERR_BAD_SHAPE;   // only linear regression has a noise scale
+  const int64_t KD = (int64_t)K * D;
+  // z's row is exactly w, b, log sigma, log tau and log lam: each block inside the row, no two overlapping, and
+  // their widths summing to Dz
+  const int64_t off[5] = {w_off, has_bias ? b_off : -1, s_off, sc.tau_off, sc.lam_off};
+  const int64_t len[5] = {KD, has_bias ? K : 0, s_off >= 0 ? 1 : 0, has_tau ? 1 : 0, has_lam ? KD : 0};
+  int64_t width = 0;
+  for (int i = 0; i < 5; ++i) {
+    if (len[i] == 0) continue;
+    if (off[i] < 0 || off[i] > Dz - len[i]) return B2_ERR_BAD_SHAPE;
+    for (int j = 0; j < i; ++j)
+      if (len[j] && off[i] < off[j] + len[j] && off[j] < off[i] + len[i]) return B2_ERR_BAD_SHAPE;
+    width += len[i];
+  }
+  if (width != Dz) return B2_ERR_BAD_SHAPE;
+  if (has_bias && !(s_b > 0.0)) return B2_ERR_BAD_SHAPE;
+  if (has_tau && !positive_prior_ok(sc.tau_prior, sc.tau_p0, sc.tau_p1)) return B2_ERR_BAD_SHAPE;
+  if (has_lam && !positive_prior_ok(sc.lam_prior, sc.lam_p0, sc.lam_p1)) return B2_ERR_BAD_SHAPE;
+  if (normal && s_off >= 0 && !positive_prior_ok(s_prior, sp0, sp1)) return B2_ERR_BAD_SHAPE;
+  if (normal && s_off < 0 && (!(sigma > 0.0) || !((float)sigma > 0.f))) return B2_ERR_BAD_SHAPE;
+  if (kind == B2_GLM_BINOMIAL && trials_per_row != 0 && trials_per_row != 1) return B2_ERR_BAD_SHAPE;
+  if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
+  if (kind == B2_GLM_BINOMIAL && trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0)
+    return B2_ERR_BAD_SHAPE;
+  const PotentialSigma sg = {s_off >= 0 ? s_off : (int64_t)-1, (float)sigma, s_prior, sp0, sp1};
+  const bool latent_sigma = normal && s_off >= 0;
+  return glm_potential_run(
+      glm_potential_lik_bytes(kind, N, D, K, C), z, C, Dz, w_off, b_off, (int)KD, K, has_bias, 1.0, s_b,
+      normal ? &sg : nullptr, &sc, U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
+      [&](const float* Wp, const float* bp, const float* sig, float* dsig, float* sum_p, float* dW, float* db,
+          void* ws, size_t ws_bytes) {
+        return glm_potential_likelihood(kind, X, y, trials, trials_per_row, N, D, K, C, Wp, bp, sig,
+                                        latent_sigma ? dsig : nullptr, sum_p, dW, db, ws, ws_bytes, stream);
       });
 }

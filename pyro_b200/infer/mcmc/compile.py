@@ -16,6 +16,8 @@ WITHOUT touching the user's code, whether a model belongs to such a class:
 
 The returned potential uses the model's own site names, so ``MCMC.get_samples()`` is unchanged.
 """
+import math
+
 import torch
 
 
@@ -181,14 +183,37 @@ def _try_logistic(poutine, model, args, kwargs, latent, observed):
     return LogisticPotential(X, y.to(X.dtype), prior_scale=s, site_name=bname)
 
 
+_POSITIVE = ("HalfNormal", "HalfCauchy", "Exponential", "LogNormal")
+
+
+def _positive_prior(fn, cls):
+    """``(cls, p0, p1)`` of a HalfNormal(p0), HalfCauchy(p0), Exponential(p0) or LogNormal(p0, p1) prior whose
+    parameters are each one repeated gradient-free value, else None."""
+    if cls == "LogNormal":
+        p0, p1 = _const(fn.loc), _const(fn.scale)
+    else:
+        p0, p1 = _const(fn.rate if cls == "Exponential" else fn.scale), 1.0
+    if p0 is None or p1 is None or not p1 > 0.0 or not math.isfinite(p0) or (cls != "LogNormal" and not p0 > 0.0):
+        return None
+    return cls, p0, p1
+
+
 def _try_glm(poutine, model, args, kwargs, latent, observed):
     """Logistic regression with an intercept, or softmax, Poisson (log link), Binomial (logit link) or linear
     regression with or without one, in fp32, within the GLM kernels' scope: Bernoulli D in {4, 8, 16, 32};
     Categorical D == 32, 2 <= K <= 16; Poisson, Binomial and Normal 1 <= D <= 128.  Binomial's total_count is a
-    constant or gradient-free fp32 [N] counts, the same at every probe.  Linear regression's noise scale is a constant or one latent scalar site with
-    a constant-parameter HalfNormal, HalfCauchy, Exponential or LogNormal prior."""
+    constant or gradient-free fp32 [N] counts, the same at every probe.
+
+    The weight prior is ``Normal(0, S)`` and the bias prior ``Normal(0, s_b)`` with a constant ``s_b``.  ``S`` is a
+    constant, or latent: ``tau`` (one positive scalar site), ``lam`` (a positive site of the weight's shape) or
+    ``tau * lam``.  Linear regression's noise scale is a constant or one latent positive scalar site.  Every
+    latent positive site has a HalfNormal, HalfCauchy, Exponential or LogNormal prior with constant parameters
+    (for ``lam`` one value for every coefficient), and exactly one role -- noise scale, ``tau`` or ``lam`` -- which
+    the probes establish: the observation's scale equals the drawn noise scale and the weight site's scale equals
+    the drawn ``tau``, ``lam`` or ``tau * lam`` at every probe.  Intercept-free logistic regression with a constant
+    weight scale keeps LogisticPotential's route."""
     from .potential import GlmPotential
-    if len(observed) != 1 or len(latent) not in (1, 2, 3):
+    if len(observed) != 1 or not 1 <= len(latent) <= 5:
         return None
     (obs_name, obs), = observed.items()
     _, kind = _base(obs["fn"])
@@ -198,29 +223,22 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
             "PoissonLinear": "Poisson", "NormalLinear": "Normal", "BinomialLinear": "Binomial"}.get(kind, kind)
     if kind not in ("Bernoulli", "Categorical", "Poisson", "Normal", "Binomial") or not _plain_site(obs):
         return None
-    # linear regression: at most one latent noise-scale site, positive support (z holds its log)
     order = list(latent)                   # TracePotential's site order
-    sigma_site, sigma_prior, shapes_sigma = None, None, None
-    if kind == "Normal":
-        for name, site in latent.items():
-            fn, cls = _base(site["fn"])
-            if cls not in ("HalfNormal", "HalfCauchy", "Exponential", "LogNormal"):
-                continue
-            v = site["value"]
-            if sigma_site is not None or not _plain_site(site) or not isinstance(v, torch.Tensor) \
-                    or v.dtype != torch.float32 or v.numel() != 1:
-                return None
-            if cls == "LogNormal":
-                p0, p1 = _const(fn.loc), _const(fn.scale)
-            else:
-                p0, p1 = _const(fn.rate if cls == "Exponential" else fn.scale), 1.0
-            if p0 is None or p1 is None or not p1 > 0.0 or (cls != "LogNormal" and not p0 > 0.0):
-                return None
-            sigma_site, sigma_prior, shapes_sigma = name, (cls, p0, p1), tuple(v.shape)
-        latent = {k: v for k, v in latent.items() if k != sigma_site}
-        if len(latent) not in (1, 2):
+    # positive-support sites (z holds their logs): the noise scale and the weight scales, roles decided by probing
+    positive, priors = {}, {}
+    for name, site in latent.items():
+        fn, cls = _base(site["fn"])
+        if cls not in _POSITIVE:
+            continue
+        v = site["value"]
+        if not _plain_site(site) or not isinstance(v, torch.Tensor) or v.dtype != torch.float32:
             return None
-    elif len(latent) == 3:
+        priors[name] = _positive_prior(fn, cls)
+        if priors[name] is None:
+            return None
+        positive[name] = tuple(v.shape)
+    latent = {k: v for k, v in latent.items() if k not in positive}
+    if len(latent) not in (1, 2):
         return None
     y = obs["value"]
     if not isinstance(y, torch.Tensor) or y.dim() != 1:
@@ -241,10 +259,7 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
         if cls != "Normal" or not _plain_site(site) or not isinstance(v, torch.Tensor) \
                 or v.dtype != torch.float32 or _const(fn.loc) != 0.0:
             return None
-        s = _const(fn.scale)
-        if s is None or not s > 0.0:
-            return None
-        scales[name], shapes[name] = s, tuple(v.shape)
+        scales[name], shapes[name] = _const(fn.scale), tuple(v.shape)
     if kind == "Bernoulli":
         K = 1
         wshapes, bshapes = [(D,)], [(), (1,)]
@@ -266,40 +281,88 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
     if len(weight) != 1 or len(bias) + 1 != len(latent):
         return None
     weight, bias = weight[0], (bias[0] if bias else None)
-    if kind == "Bernoulli" and bias is None:
-        return None   # intercept-free logistic regression keeps LogisticPotential's route
+    if bias is not None and not (scales[bias] is not None and scales[bias] > 0.0):
+        return None
+    # candidates by shape: tau (and the noise scale) one value, lam the weight's shape
+    scalars = [name for name, s in positive.items() if s in ((), (1,))]
+    lams = [name for name, s in positive.items() if s == shapes[weight]]
     # ---- functional probe: logits == X @ w + b  /  log_softmax(logits) == log_softmax(X @ W.mT + b)  /
-    # log(rate) == X @ w + b ----------------------------------------------------------------------------------
+    # log(rate) == X @ w + b, and the scales' roles ------------------------------------------------------------------
     gen = torch.Generator(device="cpu").manual_seed(20240302)
-    sigma_const = None
+    sigma_site, sigma_const = None, None
+    wform = None                           # (tau site or None, lam site or None); (None, None): the constant s_w
     trials = None                          # Binomial: the constant count, or the [N] counts of the prototype
     if kind == "Binomial":
         trials = _binomial_trials(_base(obs["fn"])[0], n)
         if trials is None:
             return None
-    for _ in range(3):
+
+    def as_t(v):
+        return torch.as_tensor(v, dtype=X.dtype, device=X.device)
+
+    for i in range(3):
         wv = torch.randn(shapes[weight], generator=gen).to(X)
         if kind == "Poisson":
             wv = wv / D ** 0.5            # log-rates of a few units: exp neither overflows nor underflows
         bv = torch.randn(shapes[bias], generator=gen).to(X) if bias is not None else None
         data = {weight: wv} if bias is None else {weight: wv, bias: bv}
-        if sigma_site is not None:
-            sv = torch.exp(0.5 * torch.randn((), generator=gen)).to(X)
-            data[sigma_site] = sv.reshape(shapes_sigma)
-        pfn = _probe(poutine, model, args, kwargs, data, obs_name)
+        for name, shape in positive.items():
+            data[name] = torch.exp(0.5 * torch.randn(shape, generator=gen)).to(X)
+        tr = poutine.trace(poutine.condition(model, data=data)).get_trace(*args, **kwargs)
+        pfn = _base(tr.nodes[obs_name]["fn"])[0]
+        # the priors: constant parameters that do not move with any latent
+        for name in positive:
+            fn, cls = _base(tr.nodes[name]["fn"])
+            if cls != priors[name][0] or _positive_prior(fn, cls) != priors[name]:
+                return None
+        if bias is not None:
+            bfn = _base(tr.nodes[bias]["fn"])[0]
+            if _const(bfn.loc) != 0.0 or _const(bfn.scale) != scales[bias]:
+                return None
+        wfn = _base(tr.nodes[weight]["fn"])[0]
+        if _const(wfn.loc) != 0.0:
+            return None
         if kind == "Normal":
-            # scale: the latent sigma as drawn, or one constant that does not move with the weights
-            sc = pfn.scale
+            # scale: a latent noise scale as drawn, or one constant that does not move with the latents
+            sc = as_t(pfn.scale)
+            if i == 0:
+                hits = [name for name in scalars if _close(sc, data[name].reshape(()), X.dtype)]
+                if len(hits) > 1:
+                    return None
+                sigma_site = hits[0] if hits else None
             if sigma_site is not None:
-                if not isinstance(sc, torch.Tensor) or not _close(sc, sv, X.dtype):
+                if not _close(sc, data[sigma_site].reshape(()), X.dtype):
                     return None
             else:
                 c = _const(sc)
                 if c is None or not c > 0.0 or (sigma_const is not None and c != sigma_const):
                     return None
                 sigma_const = c
-            logits = pfn.loc
-        elif kind == "Binomial":
+        # the weight scale: the constant of the prototype, or the drawn tau, lam or tau * lam
+        def want_scale(form):
+            t, lam = form
+            if t is None and lam is None:
+                return as_t(scales[weight]) if scales[weight] is not None and scales[weight] > 0.0 else None
+            v = data[t].reshape(()) if t is not None else 1.0
+            return v * data[lam] if lam is not None else v
+        ws = as_t(wfn.scale)
+        if i == 0:
+            free_s = [name for name in scalars if name != sigma_site]
+            forms = [(None, None)] + [(t, None) for t in free_s] + [(None, lam) for lam in lams] + \
+                [(t, lam) for t in free_s for lam in lams if t != lam]
+            hits = [f for f in forms if want_scale(f) is not None and _close(ws, want_scale(f), X.dtype)]
+            if len(hits) != 1:
+                return None
+            wform = hits[0]
+            # every positive site has exactly one role
+            roles = [r for r in (sigma_site,) + wform if r is not None]
+            if sorted(roles) != sorted(positive):
+                return None
+        want = want_scale(wform)
+        if tuple(torch.broadcast_shapes(ws.shape, want.shape, shapes[weight])) != shapes[weight] \
+                or not _close(ws, want, X.dtype):
+            return None
+        if kind == "Binomial":
             # logits as the model gave them (not probs), and the same trial counts at every probe
             t = _binomial_trials(pfn, n)
             if t is None or type(t) is not type(trials) or (
@@ -307,34 +370,37 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
                     isinstance(t, torch.Tensor) and not torch.equal(t, trials)):
                 return None
             logits = pfn.logits
+        elif kind == "Normal":
+            logits = pfn.loc
         else:
             logits = torch.log(pfn.rate) if kind == "Poisson" else pfn.logits
         if hasattr(logits, "dense"):
             logits = logits.dense()
-        if kind in ("Poisson", "Normal", "Binomial"):
+        if kind != "Categorical":
             want = X @ wv + (bv.reshape(()) if bv is not None else 0.0)
-        elif kind == "Bernoulli":
-            want = X @ wv + bv.reshape(())
         else:
             want = X @ wv.mT + (bv if bv is not None else 0.0)
             logits, want = torch.log_softmax(logits, -1), torch.log_softmax(want, -1)
         if tuple(logits.shape) != tuple(want.shape) or not _close(logits, want, X.dtype):
             return None
+    tau_site, lam_site = wform
+    if kind == "Bernoulli" and bias is None and tau_site is None and lam_site is None:
+        return None   # intercept-free logistic regression with a constant weight scale keeps LogisticPotential
     off, sites = 0, {}
     for name in order:
-        if name == sigma_site:
-            sites[name] = (slice(off, off + 1), "exp", shapes_sigma)
-            off += 1
-            continue
+        shape = positive.get(name, shapes.get(name))
         width = 1
-        for d in shapes[name]:
+        for d in shape:
             width *= d
-        sites[name] = (slice(off, off + width), "identity", shapes[name])
+        sites[name] = (slice(off, off + width), "exp" if name in positive else "identity", shape)
         off += width
-    return GlmPotential(X, y.detach(), kind, sites, weight, bias, s_w=scales[weight],
+    return GlmPotential(X, y.detach(), kind, sites, weight, bias,
+                        s_w=scales[weight] if wform == (None, None) else 1.0,
                         s_b=scales[bias] if bias is not None else 1.0,
                         sigma=sigma_const if sigma_const is not None else 1.0, sigma_site=sigma_site,
-                        sigma_prior=sigma_prior, trials=trials)
+                        sigma_prior=priors.get(sigma_site), trials=trials,
+                        tau_site=tau_site, tau_prior=priors.get(tau_site),
+                        lam_site=lam_site, lam_prior=priors.get(lam_site))
 
 
 def _binomial_trials(fn, n):

@@ -123,9 +123,15 @@ class GlmPotential:
     HalfCauchy(p0), Exponential(p0) or LogNormal(p0, p1); z then holds ``log sigma`` (transform ``"exp"``) and U
     carries the Jacobian ``-log sigma``, as ``TracePotential`` gives it (``b2_glm_normal_potential``).
 
+    The weight scale may instead be latent (``b2_glm_scaled_potential``): ``w ~ Normal(0, S)`` with ``S`` the
+    positive scalar site ``tau_site``, the positive site ``lam_site`` of the weight's shape, or their product (the
+    hierarchical, ARD and horseshoe priors).  ``tau_prior`` / ``lam_prior`` are ``(kind, p0, p1)`` as
+    ``sigma_prior``, one value for every coefficient; z holds their logs (transform ``"exp"``), and U carries
+    their Jacobians.
+
     ``value_and_grad`` is ``b2_glm_potential``: the likelihood of all chains comes from one pass of the
     fused GLM kernel over X, the chains being its particles.  ``sites`` maps each site name to
-    ``(slice into z, "identity", value shape)`` in the order and layout ``TracePotential`` gives the same
+    ``(slice into z, transform, value shape)`` in the order and layout ``TracePotential`` gives the same
     model, so samples, ``initial_params`` and ``full_mass`` behave the same on either.  Every chain is
     evaluated; the sampler masks inactive chains, as it does for ``TracePotential``."""
 
@@ -133,7 +139,7 @@ class GlmPotential:
                      "Exponential": N.SIGMA_EXPONENTIAL, "LogNormal": N.SIGMA_LOGNORMAL}
 
     def __init__(self, X, y, kind, sites, weight, bias=None, s_w=1.0, s_b=1.0, sigma=1.0, sigma_site=None,
-                 sigma_prior=None, trials=None):
+                 sigma_prior=None, trials=None, tau_site=None, tau_prior=None, lam_site=None, lam_prior=None):
         N.require_cuda(X, "GlmPotential")
         if X.dtype != torch.float32 or X.dim() != 2:
             raise ValueError("GlmPotential needs fp32 X of shape [N, D]")
@@ -145,6 +151,23 @@ class GlmPotential:
             self.sigma_prior = (self._SIGMA_PRIORS[pk], float(p0), float(p1))
         else:
             self.sigma_prior = (N.SIGMA_CONST, 0.0, 0.0)
+        # a latent weight scale: b2_glm_weight_scale with the z columns of log tau / log lam (-1 when absent)
+        self.tau_site, self.lam_site = tau_site, lam_site
+        self.weight_scale = None
+        if tau_site is not None or lam_site is not None:
+            sc = N.b2_glm_weight_scale()
+            sc.tau_off = sites[tau_site][0].start if tau_site is not None else -1
+            sc.lam_off = sites[lam_site][0].start if lam_site is not None else -1
+            for part, site, prior in (("tau", tau_site, tau_prior), ("lam", lam_site, lam_prior)):
+                if site is None:
+                    continue
+                pk, p0, p1 = prior
+                setattr(sc, part + "_prior", self._SIGMA_PRIORS[pk])
+                setattr(sc, part + "_p0", float(p0))
+                setattr(sc, part + "_p1", float(p1))
+            self.weight_scale = sc
+        self.scaled_kind = {"Bernoulli": N.GLM_BERNOULLI, "Categorical": N.GLM_CATEGORICAL,
+                            "Poisson": N.GLM_POISSON, "Normal": N.GLM_NORMAL, "Binomial": N.GLM_BINOMIAL}[kind]
         self.kind = {"Bernoulli": N.GLM_BERNOULLI, "Categorical": N.GLM_CATEGORICAL, "Poisson": N.GLM_POISSON,
                      "Normal": None, "Binomial": None}[kind]
         self.binomial = kind == "Binomial"
@@ -181,6 +204,8 @@ class GlmPotential:
         U = torch.empty(C, dtype=torch.float32, device=z.device)
         g = torch.empty_like(z)
         lib = N.lib()
+        if self.weight_scale is not None:
+            return self._scaled_value_and_grad(lib, z, C, U, g)
         if self.normal:
             need = int(lib.b2_glm_normal_potential_workspace(self.n, self.Dx, C))
             ws = N.workspace(z.device, need, tag="glm_potential")
@@ -206,6 +231,19 @@ class GlmPotential:
             self.kind, self.X.data_ptr(), self.y.data_ptr(), self.n, self.Dx, self.K, int(self.has_bias),
             z.data_ptr(), C, self.D, self.w_off, self.b_off, self.s_w, self.s_b, U.data_ptr(), g.data_ptr(),
             ws.data_ptr(), ws.numel(), N.stream_ptr(z.device)), "b2_glm_potential")
+        return U, g
+
+    def _scaled_value_and_grad(self, lib, z, C, U, g):
+        need = int(lib.b2_glm_scaled_potential_workspace(self.scaled_kind, self.n, self.Dx, self.K, C))
+        ws = N.workspace(z.device, need, tag="glm_potential")
+        s_off = self.sites[self.sigma_site][0].start if self.sigma_site is not None else -1
+        pk, p0, p1 = self.sigma_prior
+        trials, per_row = (self.trials.data_ptr(), self.trials_per_row) if self.binomial else (None, 0)
+        N.check(lib.b2_glm_scaled_potential(
+            self.scaled_kind, self.X.data_ptr(), self.y.data_ptr(), trials, per_row, self.n, self.Dx, self.K,
+            int(self.has_bias), z.data_ptr(), C, self.D, self.w_off, self.b_off, s_off, self.s_b, pk, p0, p1,
+            self.sigma, ctypes.byref(self.weight_scale), U.data_ptr(), g.data_ptr(), ws.data_ptr(), ws.numel(),
+            N.stream_ptr(z.device)), "b2_glm_scaled_potential")
         return U, g
 
     def unpack(self, z):
