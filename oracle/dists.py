@@ -32,8 +32,9 @@ def normal(x, loc, scale):
 
 def bernoulli_logits(x, logits):
     """torch/distributions/bernoulli.py:121-125: -binary_cross_entropy_with_logits(logits, x)
-    = x*l - softplus(l)"""
-    return x * logits - torch.nn.functional.softplus(logits)
+    = x*l - softplus(l), with softplus(l) = log(1 + e^l) evaluated stably as that loss does (torch's
+    nn.functional.softplus returns l itself above its threshold of 20)"""
+    return x * logits - torch.logaddexp(logits, torch.zeros_like(logits))
 
 
 def bernoulli_probs(x, probs):
@@ -67,6 +68,27 @@ def beta(x, concentration1, concentration0):
 def poisson(x, rate):
     """torch/distributions/poisson.py:75-79"""
     return torch.xlogy(x, rate) - rate - torch.lgamma(x + 1)
+
+
+def binomial_logits(x, total_count, logits):
+    """pyro/distributions/torch.py:83-101 with log_binomial at tol = 0 (pyro/ops/special.py:93-108):
+    k*l - n*(max(l, 0) + log1p(exp(-|l|))) + lgamma(n + 1) - lgamma(k + 1) - lgamma(n - k + 1).
+    log_binomial runs under torch.no_grad, so the lgamma terms carry no gradient.
+    max(l, 0) + log1p(exp(-|l|)) is log(1 + e^l), evaluated here by logaddexp in the same way.  Its gradient is
+    sigmoid(l), 0.5 at l = 0 as with the reference's _clamp_by_zero (pyro/distributions/torch.py:18-20), whose
+    backward instead adds and cancels +-n/2 and so rounds n*sigmoid(l) at the scale of ulp(n/2)."""
+    with torch.no_grad():
+        n1 = total_count + 1
+        log_binom = n1.lgamma() - (x + 1).lgamma() - (n1 - x).lgamma()
+    norm = total_count * torch.logaddexp(logits, torch.zeros_like(logits))
+    return x * logits - norm + log_binom
+
+
+def binomial_probs(x, total_count, probs):
+    """Binomial(total_count, probs): logits from torch's probs_to_logits with the clamp, as bernoulli_probs"""
+    eps = torch.finfo(probs.dtype).eps
+    p = probs.clamp(min=eps, max=1 - eps)
+    return binomial_logits(x, total_count, torch.log(p) - torch.log1p(-p))
 
 
 def cauchy(x, loc, scale):
@@ -154,5 +176,6 @@ ELEMENTWISE = {
     9: (half_normal, 1), 10: (bernoulli_probs, 1), 11: (uniform, 2),
     12: (lambda x, a, b, c, d: kl_normal_normal(a, b, c, d), 4),
     13: (lambda x, a, b, c, d: kl_gamma_gamma(a, b, c, d), 4),
+    16: (binomial_logits, 2), 17: (binomial_probs, 2),
 }
 EVENT = {32: dirichlet, 33: categorical, 34: mvn_tril}

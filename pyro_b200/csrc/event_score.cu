@@ -285,7 +285,8 @@ __global__ void __launch_bounds__(256) categorical_rowthread_kernel(const EventA
 #pragma unroll
         for (int j = 1; j < V; ++j) cm = b2_max(cm, lv.v[j]);
         const T nm = b2_max(mx, cm);
-        T sacc = (k == 0) ? (T)0 : se * fast_exp(mx - nm);
+        // no finite logit yet: the running sum (0, or NaN from exp(-inf - -inf)) is dropped, as in the vec kernel
+        T sacc = (mx == -b2_inf<T>()) ? (T)0 : se * fast_exp(mx - nm);
 #pragma unroll
         for (int j = 0; j < V; ++j) sacc += fast_exp(lv.v[j] - nm);
         se = sacc;
