@@ -565,6 +565,43 @@ int b2_glm_scaled_potential(int kind, const float* X, const void* y, const float
                             void* workspace, size_t workspace_bytes, void* stream);
 size_t b2_glm_scaled_potential_workspace(int kind, int64_t N, int D, int K, int64_t C);
 
+/*
+ * b2_glm_group_potential -- HMC / NUTS potential energy and gradient of multilevel regression: the regressions of
+ * b2_glm_scaled_potential with a constant weight scale and a varying intercept by group,
+ *   eta[c,n] = <X[n,:], w[c,:]> + b[c] + alpha[c, g[n]],   alpha ~ Normal(0, s_a)[G]         (centred)
+ *                                                          alpha = s_a * e, e ~ Normal(0, 1)[G] (non-centred)
+ * with s_a the constant s_const or latent (z holds t = log s_a at s_off, prior s_prior with (sp0, sp1) as for a
+ * latent sigma).  U is the potential of pyro/infer/mcmc/util.py:275-286, with the Jacobian -t of a latent s_a.
+ * The likelihood of all chains is one pass of the kind's fused kernel over [X | onehot(g)]: the group effect is G
+ * more columns of the contraction, synthesised in shared memory from g, so X is read once and no [C, N] tensor is
+ * made.  A group index outside [0, G) makes U and the group effect's gradient NaN.
+ * kind: B2_GLM_BERNOULLI (any D), B2_GLM_POISSON, B2_GLM_NORMAL (s_off, s_prior, sp0, sp1 and sigma as for
+ * b2_glm_normal_potential; s_off < 0 for every other kind) or B2_GLM_BINOMIAL (trials, trials_per_row), with
+ * 1 <= D, 1 <= G and D + G <= 128.  z: [C, Dz] fp32 row-major; w (D values) at w_off, b at b_off (has_bias), log
+ * sigma at s_off, alpha or e (G values) at ge->a_off and log s_a at ge->s_off (-1: the constant ge->s_const).  Dz is
+ * exactly the sum of the present blocks' widths, none overlapping another or leaving the row.  X, y, ge->groups (and
+ * per-row trials) 16-byte aligned.  Anything else returns B2_ERR_NULL / B2_ERR_BAD_SHAPE / B2_ERR_TOO_LARGE before
+ * any CUDA call.  Four launches with no host sync (CUDA graph capturable): the pack kernel (each chain's [w | alpha]
+ * row), the kind's likelihood call with weight -1 (kernel + finish, every logit fp32-exact), and a potential finish
+ * that adds every prior term and Jacobian in fp64 in a fixed order.  workspace: b2_glm_group_potential_workspace()
+ * bytes, zero-initialised once.
+ */
+typedef struct b2_glm_group_effect {
+  const int32_t* groups;        /* [N] group of each row, 16-byte aligned */
+  int64_t a_off;                /* z columns of alpha (centred) or e (non-centred), G of them */
+  int64_t s_off;                /* z column of log s_a, -1 for the constant s_const */
+  int G;                        /* number of groups: 1 <= G, D + G <= 128 */
+  int noncentred;               /* 0: alpha ~ Normal(0, s_a); 1: alpha = s_a * e, e ~ Normal(0, 1) */
+  int s_prior;                  /* B2_SIGMA_HALFNORMAL .. B2_SIGMA_LOGNORMAL (latent s_a) */
+  double s_const, sp0, sp1;
+} b2_glm_group_effect;
+int b2_glm_group_potential(int kind, const float* X, const void* y, const float* trials, int trials_per_row,
+                           int64_t N, int D, int has_bias, const float* z, int64_t C, int64_t Dz, int64_t w_off,
+                           int64_t b_off, int64_t s_off, double s_w, double s_b, int s_prior, double sp0, double sp1,
+                           double sigma, const b2_glm_group_effect* ge, float* U, float* grad, void* workspace,
+                           size_t workspace_bytes, void* stream);
+size_t b2_glm_group_potential_workspace(int kind, int64_t N, int D, int G, int64_t C);
+
 /* ---- optimisers --------------------------------------------------------------------------
  * Multi-tensor fused updates replacing PyroOptim's per-parameter Python loop
  * (pyro/optim/optim.py:117-155).  Per-tensor scalar state lives in DEVICE arrays so a captured

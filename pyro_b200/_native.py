@@ -81,6 +81,14 @@ class b2_glm_weight_scale(ctypes.Structure):
                 ("lam_p0", ctypes.c_double), ("lam_p1", ctypes.c_double)]
 
 
+class b2_glm_group_effect(ctypes.Structure):
+    """Mirror of ``b2_glm_group_effect`` (include/pyro_b200.h): the varying intercept by group of a regression
+    potential."""
+    _fields_ = [("groups", ctypes.c_void_p), ("a_off", ctypes.c_int64), ("s_off", ctypes.c_int64),
+                ("G", ctypes.c_int32), ("noncentred", ctypes.c_int32), ("s_prior", ctypes.c_int32),
+                ("s_const", ctypes.c_double), ("sp0", ctypes.c_double), ("sp1", ctypes.c_double)]
+
+
 class b2_nuts_lockstep(ctypes.Structure):
     """Mirror of ``b2_nuts_lockstep`` (include/pyro_b200.h): device pointers of the lockstep tree state."""
     _fields_ = [("zL", ctypes.c_void_p), ("rL", ctypes.c_void_p), ("zR", ctypes.c_void_p),
@@ -153,6 +161,10 @@ SIGNATURES = {
                                        _i64, _i64, _f64, _i32, _f64, _f64, _f64,
                                        ctypes.POINTER(b2_glm_weight_scale), _vp, _vp, _vp, _sz, _vp]),
     "b2_glm_scaled_potential_workspace": (_sz, [_i32, _i64, _i32, _i32, _i64]),
+    "b2_glm_group_potential": (_i32, [_i32, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _vp, _i64, _i64, _i64, _i64,
+                                      _i64, _f64, _f64, _i32, _f64, _f64, _f64,
+                                      ctypes.POINTER(b2_glm_group_effect), _vp, _vp, _vp, _sz, _vp]),
+    "b2_glm_group_potential_workspace": (_sz, [_i32, _i64, _i32, _i32, _i64]),
     "b2_clipped_adam": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _vp]),
     "b2_adagrad_rmsprop": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _vp]),
     "b2_leapfrog_half_kick_drift": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _i32, _vp]),

@@ -364,18 +364,22 @@ extern "C" size_t b2_glm_workspace(int64_t N, int D, int P) {
 static int glm_bernoulli(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
                          double scale, double weight, double sum_coeff, int flags, float* out_sum_p,
                          float* out_total, float* out_dW, float* out_db, void* workspace, size_t workspace_bytes,
-                         cudaStream_t s, const GlmElbo* E) {
+                         cudaStream_t s, const GlmElbo* E, GlmGroups grp = {}) {
   if (!X || !y || !W) return B2_ERR_NULL;
   if (N <= 0 || P <= 0) return B2_ERR_BAD_SHAPE;
   if (reinterpret_cast<uintptr_t>(X) % 16 != 0) return B2_ERR_BAD_SHAPE;
-  if (D < 1 || D > 128) return B2_ERR_BAD_SHAPE;
-  // D in {4, 8, 16, 32} keep their kernels; every other D takes the wgmma kernel of glm_flat_tc.cu, which
-  // has no fp32 SIMT counterpart and loads y by 16-byte bulk copies with 32-bit row counts
-  const bool flat = !(D == 4 || D == 8 || D == 16 || D == 32);
+  // with a group effect the contraction is D + G columns wide (W, dW, partials)
+  const int Da = D + (grp.idx ? grp.G : 0);
+  if (D < 1 || Da > 128) return B2_ERR_BAD_SHAPE;
+  if (grp.idx && (grp.G < 1 || reinterpret_cast<uintptr_t>(grp.idx) % 16 != 0)) return B2_ERR_BAD_SHAPE;
+  // D in {4, 8, 16, 32} keep their kernels; every other D, and every D with a group effect, takes the wgmma
+  // kernel of glm_flat_tc.cu, which has no fp32 SIMT counterpart and loads y by 16-byte bulk copies with 32-bit
+  // row counts
+  const bool flat = grp.idx || !(D == 4 || D == 8 || D == 16 || D == 32);
   if (flat && (flags & B2_FLAG_GLM_FP32)) return B2_ERR_BAD_SHAPE;
   if (flat && reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
   if (flat && N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
-  if (!workspace || workspace_bytes < b2_glm_workspace(N, D, P)) return B2_ERR_WORKSPACE;
+  if (!workspace || workspace_bytes < b2_glm_workspace(N, Da, P)) return B2_ERR_WORKSPACE;
   // below 8 Ki rows the single-pass TF32 gradient contraction has not averaged its operand rounding
   // (2^-12 relative per term) below the fp32 tolerance yet: those sizes take the exact fp32 SIMT kernel
   // unless the tensor-core kernel is asked for explicitly (B2_FLAG_GLM_3XTF32).  The TMA loads need a
@@ -388,7 +392,7 @@ static int glm_bernoulli(const float* X, const float* y, const float* W, const f
   float* partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
   if (flat || use_tc) {
     const bool split_x = glm_split_x(flags, N);
-    const int rc = flat ? launch_glm_flat_tc(X, y, W, b, N, D, P, partials, gx, split_x, s)
+    const int rc = flat ? launch_glm_flat_tc(X, y, W, b, N, D, P, partials, gx, split_x, s, grp)
                         : launch_glm_tc(X, y, W, b, N, P, partials, gx, split_x, s);
     if (rc != 0) return rc;
   } else
@@ -406,11 +410,19 @@ static int glm_bernoulli(const float* X, const float* y, const float* W, const f
                P, 1, D, scale, weight, glm_sum_p(partials, out_sum_p, gx, total), out_dW, out_db, sum_coeff, flags,
                out_total, ticket, *E);
   } else {
-    launch_glm_finish(partials, ticket, gx, P, 1, D, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW,
+    launch_glm_finish(partials, ticket, gx, P, 1, Da, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW,
                       out_db, nullptr, s);
   }
   count_launch(2);
   return check_launch();
+}
+
+int b2::glm_bernoulli_logits(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
+                             double scale, double weight, double sum_coeff, int flags, float* out_sum_p,
+                             float* out_total, float* out_dW, float* out_db, void* workspace, size_t workspace_bytes,
+                             cudaStream_t s, GlmGroups grp) {
+  return glm_bernoulli(X, y, W, b, N, D, P, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW, out_db,
+                       workspace, workspace_bytes, s, nullptr, grp);
 }
 
 extern "C" int b2_glm_bernoulli_logits(const float* X, const float* y, const float* W,

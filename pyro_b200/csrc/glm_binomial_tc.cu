@@ -91,10 +91,28 @@ glm_binomial_flat_tc_kernel(const float* __restrict__ X, const float* __restrict
   if (blockIdx.y == 0) lbinom_partial<tcf::Cfg<DC>::kThreads, ROW>(y, trials, N, lg);
 }
 
+// with a group effect: D + G columns, X split
+template <bool ROW, int DC>
+__global__ void __launch_bounds__(tcf::Cfg<DC, true>::kThreads, 1)
+glm_binomial_group_tc_kernel(const float* __restrict__ X, const float* __restrict__ y,
+                             const float* __restrict__ trials, const float* __restrict__ W,
+                             const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
+                             float* __restrict__ lg, const int32_t* __restrict__ groups, int G) {
+  tcf::glm_flat_pipeline<Binomial<ROW>, DC, true, true>(X, y, W, bvec, N, D, P, partials, trials, groups, G);
+  if (blockIdx.y == 0) lbinom_partial<tcf::Cfg<DC, true>::kThreads, ROW>(y, trials, N, lg);
+}
+
 template <bool ROW>
 int launch(const float* X, const float* y, const float* m, const float* W, const float* b, int64_t N, int D, int P,
-           float* partials, float* lg, int gx, bool split_x, cudaStream_t s) {
+           float* partials, float* lg, int gx, bool split_x, cudaStream_t s, GlmGroups grp) {
   const dim3 grid = slab_grid(gx, P);
+  // D + G < 32 runs the two-atom loop too (see below)
+  if (grp.idx)
+    return glm_dispatch_dc<2>(D + grp.G, true, [&](auto dc, auto) {
+      using C = tcf::Cfg<decltype(dc)::value, true>;
+      return launch_tc(glm_binomial_group_tc_kernel<ROW, decltype(dc)::value>, grid, dim3(C::kThreads),
+                       C::kSmemBytes, s, X, y, m, W, b, N, D, P, partials, lg, grp.idx, grp.G);
+    });
   if (D == 32) {
     using namespace tile32;
     using Fam = Binomial<ROW>;
@@ -124,23 +142,32 @@ using namespace b2;
 
 extern "C" size_t b2_glm_binomial_workspace(int64_t N, int D, int P) { return glm_row_workspace(N, D, P, true); }
 
+int b2::glm_binomial_logits(const float* X, const float* y, const float* trials, int trials_per_row, const float* W,
+                            const float* b, int64_t N, int D, int P, double scale, double weight, double sum_coeff,
+                            int flags, float* out_sum_p, float* out_total, float* out_dW, float* out_db,
+                            void* workspace, size_t workspace_bytes, cudaStream_t s, GlmGroups grp) {
+  const bool bad_trials = (trials_per_row != 0 && trials_per_row != 1) ||
+                          (trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0);
+  int rc = glm_row_check(X, y, W, !trials, N, D, P, bad_trials, flags, workspace, workspace_bytes, true, grp);
+  if (rc != B2_OK) return rc;
+  const int Da = D + (grp.idx ? grp.G : 0);
+  const GlmRowWorkspace w = glm_row_areas(workspace, N, Da, P, true);
+  const bool split_x = glm_split_x(flags, N);
+  rc = trials_per_row ? tcbi::launch<true>(X, y, trials, W, b, N, D, P, w.partials, w.lg, w.gx, split_x, s, grp)
+                      : tcbi::launch<false>(X, y, trials, W, b, N, D, P, w.partials, w.lg, w.gx, split_x, s, grp);
+  if (rc != 0) return rc;
+  launch_glm_finish(w.partials, w.ticket, w.gx, P, 1, Da, scale, weight, sum_coeff, flags, out_sum_p, out_total,
+                    out_dW, out_db, w.lg, s);
+  count_launch(2);
+  return check_launch();
+}
+
 extern "C" int b2_glm_binomial_logits(const float* X, const float* y, const float* trials, int trials_per_row,
                                       const float* W, const float* b, int64_t N, int D, int P, double scale,
                                       double weight, double sum_coeff, int flags, float* out_sum_p,
                                       float* out_total, float* out_dW, float* out_db, void* workspace,
                                       size_t workspace_bytes, void* stream) {
-  const bool bad_trials = (trials_per_row != 0 && trials_per_row != 1) ||
-                          (trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0);
-  int rc = glm_row_check(X, y, W, !trials, N, D, P, bad_trials, flags, workspace, workspace_bytes, true);
-  if (rc != B2_OK) return rc;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const GlmRowWorkspace w = glm_row_areas(workspace, N, D, P, true);
-  const bool split_x = glm_split_x(flags, N);
-  rc = trials_per_row ? tcbi::launch<true>(X, y, trials, W, b, N, D, P, w.partials, w.lg, w.gx, split_x, s)
-                      : tcbi::launch<false>(X, y, trials, W, b, N, D, P, w.partials, w.lg, w.gx, split_x, s);
-  if (rc != 0) return rc;
-  launch_glm_finish(w.partials, w.ticket, w.gx, P, 1, D, scale, weight, sum_coeff, flags, out_sum_p, out_total,
-                    out_dW, out_db, w.lg, s);
-  count_launch(2);
-  return check_launch();
+  return glm_binomial_logits(X, y, trials, trials_per_row, W, b, N, D, P, scale, weight, sum_coeff, flags, out_sum_p,
+                             out_total, out_dW, out_db, workspace, workspace_bytes,
+                             reinterpret_cast<cudaStream_t>(stream), {});
 }

@@ -23,12 +23,28 @@ glm_bernoulli_flat_tc_kernel(const float* __restrict__ X, const float* __restric
   glm_flat_pipeline<Bernoulli, DC, SPLIT_X>(X, y, W, bvec, N, D, P, partials);
 }
 
+// with a group effect: D + G columns, X split
+template <int DC>
+__global__ void __launch_bounds__(Cfg<DC, true>::kThreads, 1)
+glm_bernoulli_group_tc_kernel(const float* __restrict__ X, const float* __restrict__ y, const float* __restrict__ W,
+                              const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
+                              const int32_t* __restrict__ groups, int G) {
+  glm_flat_pipeline<Bernoulli, DC, true, true>(X, y, W, bvec, N, D, P, partials, nullptr, groups, G);
+}
+
 }  // namespace tcf
 
 // ---- host side -------------------------------------------------------------------------------------------
-// The caller (b2_glm_bernoulli_logits) has checked 1 <= D <= 128, N < 2^31 and 16-byte aligned X and y.
+// The caller (b2_glm_bernoulli_logits) has checked 1 <= D <= 128 (D + G with groups), N < 2^31 and 16-byte
+// aligned X and y.
 int launch_glm_flat_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
-                       float* partials, int gx, bool split_x, cudaStream_t s) {
+                       float* partials, int gx, bool split_x, cudaStream_t s, GlmGroups grp) {
+  if (grp.idx)
+    return glm_dispatch_dc<1>(D + grp.G, true, [&](auto dc, auto) {
+      using C = tcf::Cfg<decltype(dc)::value, true>;
+      return launch_tc(tcf::glm_bernoulli_group_tc_kernel<decltype(dc)::value>, tc::slab_grid(gx, P),
+                       dim3(C::kThreads), C::kSmemBytes, s, X, y, W, b, N, D, P, partials, grp.idx, grp.G);
+    });
   return glm_dispatch_dc<1>(D, split_x, [&](auto dc, auto sx) {
     using C = tcf::Cfg<decltype(dc)::value>;
     return launch_tc(tcf::glm_bernoulli_flat_tc_kernel<decltype(dc)::value, decltype(sx)::value>,

@@ -30,9 +30,18 @@
 //
 // Precision policy of glm_tc.cu: W always split, X split under SPLIT_X, g rounded to nearest TF32.
 //
-// Budget: at DC = 4 one warpgroup holds W hi + lo (64 KB), X hi + lo (64 KB), X^T (34 KB) and a landing tile
-// (32 KB), and its GEMM 2 accumulator alone takes 68 registers.  So DC = 1 runs four warpgroups per CTA (the
+// Budget: at DC = 4 one warpgroup holds W hi + lo (64 KB), X hi + lo (64 KB), X^T (34 KB), a landing tile
+// (32 KB), 1 KB of labels and with GROUPS 1 KB of group indices (197 KB in all), and its GEMM 2 accumulator alone takes 68 registers.  So DC = 1 runs four warpgroups per CTA (the
 // 128-register cap of glm_tc.cu), DC = 2 two and DC >= 3 one, each with a single landing stage.
+//
+// Group columns (GROUPS, a varying intercept alpha[g_n] by group): X @ w + b + alpha[g] is [X | onehot(g)] @
+// [w ; alpha] + b, so the kernel runs at D_aug = D + G (<= 128) with G synthesised columns.  The group index g[N]
+// (int32) is bulk-copied next to y into its own 1 KB region; the landing buffer keeps X's stride D, and the split
+// pass writes column D + j of a row as 1 when g_n == j and 0 otherwise, in X (exact in TF32: X_lo is zero) and in
+// X^T, so GEMM 1 gathers alpha and GEMM 2's dW columns D .. D+G-1 are the segment sums d loglik / d alpha_g.
+// W, the partials and the finish are D_aug wide.  A row whose index is outside [0, G) gets NaN in every group
+// column, so the likelihood and the group columns of dW come out NaN rather than silently dropping the row.  (The
+// other gradients need not: the epilogues clamp a logit before they take its gradient.)
 //
 // Determinism: every CTA writes its partials once (warpgroups summed in a fixed order); no float atomics.
 #pragma once
@@ -46,7 +55,7 @@ namespace tcf {
 
 using namespace tc;
 
-template <int DC>
+template <int DC, bool GROUPS = false>
 struct Cfg {
   static constexpr int kKD = 32 * DC;                          // padded feature count
   static constexpr int kN2 = kKD + 8;                          // GEMM 2 width: dW columns, db, 7 unused
@@ -59,8 +68,9 @@ struct Cfg {
   static constexpr uint32_t WG_XLO = WG_XOP + kOp;             // X_lo (SPLIT_X)
   static constexpr uint32_t WG_XT = WG_XLO + kOp;              // X^T [kb 2][c KD + 8][32 n], n permuted (kt_pos)
   static constexpr uint32_t WG_LAND = WG_XT + 2 * kXtBlock;    // landing buffer [64][D], unswizzled
-  static constexpr uint32_t WG_Y = WG_LAND + kOp;              // y [64]
-  static constexpr uint32_t kWGBytes = WG_Y + 1024;
+  static constexpr uint32_t WG_Y = WG_LAND + kOp;              // y [64] (Binomial: two slots of y, trials)
+  static constexpr uint32_t WG_G = WG_Y + 1024;                // group index [64] int32 (GROUPS)
+  static constexpr uint32_t kWGBytes = WG_G + (GROUPS ? 1024 : 0);
   // CTA layout (operand regions 1024-byte aligned: the 128-byte swizzle pattern is taken from address bits)
   static constexpr uint32_t OFF_WHI = 0;                       // [DC][p 64][32] SW128
   static constexpr uint32_t OFF_WLO = OFF_WHI + kOp;
@@ -85,13 +95,16 @@ __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_
 // d[4j + 2h + e] = D[16 w4 + gid + 8h][8j + 2 t4 + e].
 // Binomial only (glm_tc_common.cuh): trials are the per-row counts [N] (kRowTrials, bulk-copied behind y) or
 // the one count of every row (kConstTrials).
-template <class Fam, int DC, bool SPLIT_X>
+// GROUPS: groups[N] the group index of each row, G groups; W is [P][D + G], the partials [gx][P][D + G + 2].
+template <class Fam, int DC, bool SPLIT_X, bool GROUPS = false>
 __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, const float* __restrict__ y,
                                                   const float* __restrict__ W, const float* __restrict__ bvec,
                                                   int64_t N, int D, int P, float* __restrict__ partials,
-                                                  const float* __restrict__ trials = nullptr) {
-  using C = Cfg<DC>;
+                                                  const float* __restrict__ trials = nullptr,
+                                                  const int32_t* __restrict__ groups = nullptr, int G = 0) {
+  using C = Cfg<DC, GROUPS>;
   constexpr int kKD = C::kKD, kWG = C::kWG;
+  const int Da = GROUPS ? D + G : D;           // columns of the contraction
   pdl_enter();   // lets glm_finish_kernel be resident (blocked in its griddepcontrol.wait) before this kernel ends
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
@@ -112,7 +125,7 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
   // weight tiles, zero in the padding columns d >= D, and the ones rows of X^T
   stage_w_and_ones<1, kKD, C::kThreads>(reinterpret_cast<float*>(sm + C::OFF_WHI),
                                         reinterpret_cast<float*>(sm + C::OFF_WLO), sm + C::OFF_WG + C::WG_XT,
-                                        C::kWGBytes, W, slab, P, 1, D);
+                                        C::kWGBytes, W, slab, P, 1, Da);
   fence_proxy_async();
   __syncthreads();
 
@@ -130,6 +143,7 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
     const uint32_t bar = base + C::OFF_BAR + 8u * (uint32_t)wg;
     float* land = reinterpret_cast<float*>(my + C::WG_LAND);
     float* ys = reinterpret_cast<float*>(my + C::WG_Y);
+    int32_t* gs = reinterpret_cast<int32_t*>(my + C::WG_G);   // GROUPS only
     float bias[2];                             // of particles 16 w4 + gid + 8h
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -154,13 +168,17 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
         for (int i = (int)(ybulk / 4); i < kRows; ++i) ys[yo + i] = (i < rows) ? y[row0 + i] : 0.f;
         if constexpr (kRowM)
           for (int i = (int)(ybulk / 4); i < kRows; ++i) ys[yo + kRows + i] = (i < rows) ? trials[row0 + i] : 0.f;
+        if constexpr (GROUPS)
+          for (int i = (int)(ybulk / 4); i < kRows; ++i) gs[i] = (i < rows) ? groups[row0 + i] : 0;
       }
       // the arrive releases the ordinary stores above to the warpgroup's mbar_wait
-      mbar_expect_tx(bar, xbulk + (kRowM ? 2 : 1) * ybulk);
+      mbar_expect_tx(bar, xbulk + ((kRowM ? 2 : 1) + (GROUPS ? 1 : 0)) * ybulk);
       if (xbulk) bulk_load(my_s + C::WG_LAND, X + row0 * D, xbulk, bar);
       if (ybulk) bulk_load(my_s + C::WG_Y + 4 * yo, y + row0, ybulk, bar);
       if constexpr (kRowM)
         if (ybulk) bulk_load(my_s + C::WG_Y + 4 * (yo + kRows), trials + row0, ybulk, bar);
+      if constexpr (GROUPS)
+        if (ybulk) bulk_load(my_s + C::WG_G, groups + row0, ybulk, bar);
     };
     if (t == 0 && wg < nt) load(wg);
     for (int k = 0, it = wg; it < nt; ++k, it += kWG) {
@@ -171,7 +189,7 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
       wgmma_wait0();
       fence_regs(acc2);
       // ---- split pass, once per 32-column atom, with the thread mapping of the D = 32 pipeline
-      // (glm_tc_common.cuh): columns d >= D and rows past N are exact zeros --------------------------------
+      // (glm_tc_common.cuh): columns d >= D (GROUPS: d >= D + G) and rows past N are exact zeros ------------
       {
         const int lam = t & 7, mu = t >> 3;
         const int e = lam & 1, q8 = ((mu >> 3) << 2) | (lam >> 1);
@@ -180,6 +198,19 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
         float4* xs = reinterpret_cast<float4*>(my + C::WG_XOP);
         float4* xl = reinterpret_cast<float4*>(my + C::WG_XLO);
         float4* xt = reinterpret_cast<float4*>(my + C::WG_XT + (q8 >> 2) * C::kXtBlock);
+        // GROUPS: the one group column of each of the thread's rows, and the value of its other group columns
+        // (0, or NaN in every group column for an index outside [0, G))
+        int gcol[4];
+        float goff[4];
+        if constexpr (GROUPS) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int gi = gs[8 * q8 + 2 * i + e];
+            const bool ok = (unsigned)gi < (unsigned)G;
+            gcol[i] = ok ? D + gi : -1;
+            goff[i] = ok ? 0.f : __int_as_float(0x7fc00000);
+          }
+        }
 #pragma unroll
         for (int a = 0; a < DC; ++a) {
           float xr[4][4];                      // [i][q] = X[8 q8 + 2i + e][32 a + 4c + q] rounded to TF32
@@ -192,7 +223,10 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
             for (int q = 0; q < 4; ++q) {
               const int d = 32 * a + 4 * c + q;
               const float v = land[r * D + min(d, D - 1)];
-              x[q] = (d < D && r < rows) ? v : 0.f;
+              if constexpr (GROUPS)
+                x[q] = (d < Da && r < rows) ? (d < D ? v : (d == gcol[i] ? 1.f : goff[i])) : 0.f;
+              else
+                x[q] = (d < D && r < rows) ? v : 0.f;
               xr[i][q] = tf32_rn(x[q]);
             }
             if (SPLIT_X) {
@@ -251,7 +285,7 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
     }
   }
   // CTA results through the warpgroup regions, idle now
-  cta_partials<1, C::kN2, C::kThreads>(reinterpret_cast<float*>(sm + C::OFF_WG), acc2, lpa, wg, nt, slab, P, 1, D,
+  cta_partials<1, C::kN2, C::kThreads>(reinterpret_cast<float*>(sm + C::OFF_WG), acc2, lpa, wg, nt, slab, P, 1, Da,
                                        partials);
 }
 

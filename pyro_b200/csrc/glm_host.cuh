@@ -9,6 +9,15 @@
 
 namespace b2 {
 
+// A varying intercept by group (glm_flat_pipeline's GROUPS): idx[N] is the int32 group of each row, 16-byte
+// aligned, and G the number of groups; no group effect when idx is null.  With one, a likelihood call runs the flat
+// pipeline at D + G columns whatever D is: W, dW, the CTA partials and the workspace are D + G wide, and dW's
+// columns D .. D+G-1 are the derivatives with respect to the group effects.
+struct GlmGroups {
+  const int32_t* idx = nullptr;
+  int G = 0;
+};
+
 // ---- glm.cu ----
 // The second launch of every GLM likelihood call: glm_finish_kernel over the CTA partials [gx][P][K (D + 1) + 1].
 // lg (one more partial per CTA that every particle's sum subtracts) and the Normal noise scale sigma[p *
@@ -29,10 +38,31 @@ int launch_glm_tc(const float* X, const float* y, const float* W, const float* b
 // device, under a lock; false when CUDA refuses it
 bool set_max_dynamic_smem(const void* kernel, int bytes);
 
+// b2_glm_bernoulli_logits with an optional group effect
+int glm_bernoulli_logits(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
+                         double scale, double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
+                         float* out_dW, float* out_db, void* workspace, size_t workspace_bytes, cudaStream_t s,
+                         GlmGroups grp);
+
 // ---- glm_flat_tc.cu ----
-// Bernoulli at every other D in 1..128 on glm_flat_pipeline
+// Bernoulli at every other D in 1..128 on glm_flat_pipeline, and at every D with a group effect (X split)
 int launch_glm_flat_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
-                       float* partials, int gx, bool split_x, cudaStream_t s);
+                       float* partials, int gx, bool split_x, cudaStream_t s, GlmGroups grp = {});
+
+// ---- glm_poisson_tc.cu, glm_normal_tc.cu, glm_binomial_tc.cu ----
+// b2_glm_poisson_log_rate, b2_glm_normal_loc and b2_glm_binomial_logits with an optional group effect
+int glm_poisson_log_rate(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
+                         double scale, double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
+                         float* out_dW, float* out_db, void* workspace, size_t workspace_bytes, cudaStream_t s,
+                         GlmGroups grp);
+int glm_normal_loc(const float* X, const float* y, const float* W, const float* b, const float* sigma,
+                   int sigma_stride, int64_t N, int D, int P, double scale, double weight, double sum_coeff, int flags,
+                   float* out_sum_p, float* out_total, float* out_dW, float* out_db, float* out_dsigma,
+                   void* workspace, size_t workspace_bytes, cudaStream_t s, GlmGroups grp);
+int glm_binomial_logits(const float* X, const float* y, const float* trials, int trials_per_row, const float* W,
+                        const float* b, int64_t N, int D, int P, double scale, double weight, double sum_coeff,
+                        int flags, float* out_sum_p, float* out_total, float* out_dW, float* out_db, void* workspace,
+                        size_t workspace_bytes, cudaStream_t s, GlmGroups grp);
 
 // Launch of a kernel that needs more than 48 KB of dynamic shared memory: 0, or B2_ERR_LAUNCH when its
 // shared-memory limit could not be raised.
@@ -87,15 +117,18 @@ inline GlmRowWorkspace glm_row_areas(void* workspace, int64_t N, int D, int P, b
 // The argument checks of the per-row entry points, in order; null_operand and bad_operand are the family's own
 // (a null sigma or trial-count pointer; a bad sigma_stride, trials_per_row or trial-count alignment).  The tiles
 // arrive by TMA / bulk copies (16-byte aligned sources, 32-bit row coordinates), and these families have no fp32
-// SIMT kernel.
+// SIMT kernel.  With a group effect D + G columns must fit and the workspace is theirs.
 inline int glm_row_check(const float* X, const float* y, const float* W, bool null_operand, int64_t N, int D, int P,
-                         bool bad_operand, int flags, const void* workspace, size_t workspace_bytes, bool with_lg) {
+                         bool bad_operand, int flags, const void* workspace, size_t workspace_bytes, bool with_lg,
+                         GlmGroups grp = {}) {
   if (!X || !y || !W || null_operand) return B2_ERR_NULL;
-  if (N <= 0 || P <= 0 || D < 1 || D > 128 || bad_operand) return B2_ERR_BAD_SHAPE;
+  const int Da = D + (grp.idx ? grp.G : 0);
+  if (N <= 0 || P <= 0 || D < 1 || Da > 128 || bad_operand) return B2_ERR_BAD_SHAPE;
+  if (grp.idx && (grp.G < 1 || reinterpret_cast<uintptr_t>(grp.idx) % 16 != 0)) return B2_ERR_BAD_SHAPE;
   if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
   if (flags & B2_FLAG_GLM_FP32) return B2_ERR_BAD_SHAPE;
   if (N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
-  if (!workspace || workspace_bytes < glm_row_workspace(N, D, P, with_lg)) return B2_ERR_WORKSPACE;
+  if (!workspace || workspace_bytes < glm_row_workspace(N, Da, P, with_lg)) return B2_ERR_WORKSPACE;
   return B2_OK;
 }
 

@@ -60,9 +60,24 @@ glm_normal_flat_tc_kernel(const float* __restrict__ X, const float* __restrict__
   tcf::glm_flat_pipeline<Normal, DC, true>(X, y, W, bvec, N, D, P, partials);
 }
 
+// with a group effect: D + G columns
+template <int DC>
+__global__ void __launch_bounds__(tcf::Cfg<DC, true>::kThreads, 1)
+glm_normal_group_tc_kernel(const float* __restrict__ X, const float* __restrict__ y, const float* __restrict__ W,
+                           const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
+                           const int32_t* __restrict__ groups, int G) {
+  tcf::glm_flat_pipeline<Normal, DC, true, true>(X, y, W, bvec, N, D, P, partials, nullptr, groups, G);
+}
+
 int launch(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
-           float* partials, int gx, cudaStream_t s) {
+           float* partials, int gx, cudaStream_t s, GlmGroups grp) {
   const dim3 grid = slab_grid(gx, P);
+  if (grp.idx)
+    return glm_dispatch_dc<1>(D + grp.G, true, [&](auto dc, auto) {
+      using C = tcf::Cfg<decltype(dc)::value, true>;
+      return launch_tc(glm_normal_group_tc_kernel<decltype(dc)::value>, grid, dim3(C::kThreads), C::kSmemBytes, s, X,
+                       y, W, b, N, D, P, partials, grp.idx, grp.G);
+    });
   if (D == 32) {
     using namespace tile32;
     CUtensorMap mx, my;
@@ -85,20 +100,29 @@ using namespace b2;
 
 extern "C" size_t b2_glm_normal_workspace(int64_t N, int D, int P) { return glm_row_workspace(N, D, P, false); }
 
+int b2::glm_normal_loc(const float* X, const float* y, const float* W, const float* b, const float* sigma,
+                       int sigma_stride, int64_t N, int D, int P, double scale, double weight, double sum_coeff,
+                       int flags, float* out_sum_p, float* out_total, float* out_dW, float* out_db, float* out_dsigma,
+                       void* workspace, size_t workspace_bytes, cudaStream_t s, GlmGroups grp) {
+  int rc = glm_row_check(X, y, W, !sigma, N, D, P, sigma_stride != 0 && sigma_stride != 1, flags, workspace,
+                         workspace_bytes, false, grp);
+  if (rc != B2_OK) return rc;
+  const int Da = D + (grp.idx ? grp.G : 0);
+  const GlmRowWorkspace w = glm_row_areas(workspace, N, Da, P, false);
+  rc = tcn::launch(X, y, W, b, N, D, P, w.partials, w.gx, s, grp);
+  if (rc != 0) return rc;
+  launch_glm_finish(w.partials, w.ticket, w.gx, P, 1, Da, scale, weight, sum_coeff, flags, out_sum_p, out_total,
+                    out_dW, out_db, nullptr, s, sigma, sigma_stride, N, out_dsigma);
+  count_launch(2);
+  return check_launch();
+}
+
 extern "C" int b2_glm_normal_loc(const float* X, const float* y, const float* W, const float* b,
                                  const float* sigma, int sigma_stride, int64_t N, int D, int P, double scale,
                                  double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
                                  float* out_dW, float* out_db, float* out_dsigma, void* workspace,
                                  size_t workspace_bytes, void* stream) {
-  int rc = glm_row_check(X, y, W, !sigma, N, D, P, sigma_stride != 0 && sigma_stride != 1, flags, workspace,
-                         workspace_bytes, false);
-  if (rc != B2_OK) return rc;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const GlmRowWorkspace w = glm_row_areas(workspace, N, D, P, false);
-  rc = tcn::launch(X, y, W, b, N, D, P, w.partials, w.gx, s);
-  if (rc != 0) return rc;
-  launch_glm_finish(w.partials, w.ticket, w.gx, P, 1, D, scale, weight, sum_coeff, flags, out_sum_p, out_total,
-                    out_dW, out_db, nullptr, s, sigma, sigma_stride, N, out_dsigma);
-  count_launch(2);
-  return check_launch();
+  return glm_normal_loc(X, y, W, b, sigma, sigma_stride, N, D, P, scale, weight, sum_coeff, flags, out_sum_p,
+                        out_total, out_dW, out_db, out_dsigma, workspace, workspace_bytes,
+                        reinterpret_cast<cudaStream_t>(stream), {});
 }

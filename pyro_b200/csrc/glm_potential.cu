@@ -19,28 +19,39 @@
 // With a noise scale (linear regression) the pack also writes each chain's sigma_c = exp(z[c, s_off]) (or the
 // constant), and the finish adds sigma's prior and the Jacobian of sigma = e^t in fp64.  Binomial regression passes
 // the trial counts to its likelihood call as a fixed operand.  b2_glm_scaled_potential runs the same sequence for a
-// latent weight scale (w ~ Normal(0, tau * lam)), with glm_scaled_potential_finish_kernel as step 3.
+// latent weight scale (w ~ Normal(0, tau * lam)), with glm_scaled_potential_finish_kernel as step 3, and
+// b2_glm_group_potential for a varying intercept alpha[g] by group: the pack writes [w | alpha] as each chain's
+// weight row, the likelihood runs on [X | onehot(g)] (glm_flat_tc.cuh GROUPS), and
+// glm_group_potential_finish_kernel is step 3.
 #include <math.h>
 
 #include "b2_common.cuh"
+#include "glm_host.cuh"
 
 namespace b2 {
 
 // sig (linear regression only, else null): sig[c] = exp(z[c, s_off]) for a latent noise scale (z holds its log),
-// the constant s_const when s_off < 0
+// the constant s_const when s_off < 0.  With a group effect (ge.G > 0) the last ge.G of the KD weight columns are
+// alpha: z's alpha columns, or s_a * eta (non-centred).
 __global__ void __launch_bounds__(256) glm_potential_pack_kernel(const float* __restrict__ z, int64_t C,
                                                                  int64_t Dz, int64_t w_off, int64_t b_off,
                                                                  int KD, int Kb, float* __restrict__ Wp,
                                                                  float* __restrict__ bp, int64_t s_off,
-                                                                 float s_const, float* __restrict__ sig) {
+                                                                 float s_const, float* __restrict__ sig,
+                                                                 b2_glm_group_effect ge) {
   const int64_t per = KD + Kb;
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (sig != nullptr && i < C) sig[i] = s_off >= 0 ? expf(z[i * Dz + s_off]) : s_const;
   if (i >= C * per) return;
   const int64_t c = i / per;
   const int64_t j = i - c * per;
-  if (j < KD) Wp[c * KD + j] = z[c * Dz + w_off + j];
-  else bp[c * Kb + (j - KD)] = z[c * Dz + b_off + (j - KD)];
+  const int64_t a = j - (KD - ge.G);           // the group of a weight column, negative for w
+  if (j < KD && a < 0) Wp[c * KD + j] = z[c * Dz + w_off + j];
+  else if (j < KD) {
+    float v = z[c * Dz + ge.a_off + a];
+    if (ge.noncentred) v *= ge.s_off >= 0 ? expf(z[c * Dz + ge.s_off]) : (float)ge.s_const;
+    Wp[c * KD + j] = v;
+  } else bp[c * Kb + (j - KD)] = z[c * Dz + b_off + (j - KD)];
 }
 
 constexpr double kHalfLog2Pi = 0.91893853320467274178;
@@ -63,6 +74,16 @@ __device__ __forceinline__ void positive_prior(int prior, double p0, double p1, 
     lp = -lv - log(p1) - kHalfLog2Pi - 0.5 * q * q;
     dlp = -1.0 / v - q / (p1 * v);
   }
+}
+
+// a latent positive scale v = e^t under prior (prior, p0, p1): U += -log p(v) - t (the Jacobian of v = e^t), and
+// dU/dt = h - v (d log p / dv)(v) - 1, h being the derivative of the rest of U with respect to t
+__device__ __forceinline__ double latent_scale_terms(int prior, double p0, double p1, double t, double h, double& u) {
+  const double v = exp(t);
+  double lp, dlp;
+  positive_prior(prior, p0, p1, v, lp, dlp);
+  u += -lp - t;
+  return h - v * dlp - 1.0;
 }
 
 // a latent noise scale v = e^t, t = z[c, s_off]: U += -log p(v) - t (the Jacobian of v = e^t), and
@@ -140,13 +161,7 @@ __global__ void __launch_bounds__(256) glm_scaled_potential_finish_kernel(
     gc[w_off + j] = (float)((double)dW[c * KD + j] + v * is2);
     const double a = 1.0 - q;
     asum += a;
-    if (ws.lam_off >= 0) {
-      const double lam = exp(l);
-      double lp, dlp;
-      positive_prior(ws.lam_prior, ws.lam_p0, ws.lam_p1, lam, lp, dlp);
-      uw += -lp - l;
-      gc[ws.lam_off + j] = (float)(a - lam * dlp - 1.0);
-    }
+    if (ws.lam_off >= 0) gc[ws.lam_off + j] = (float)latent_scale_terms(ws.lam_prior, ws.lam_p0, ws.lam_p1, l, a, uw);
   }
   for (int j = lane; j < Kb; j += 32) {
     const double v = (double)zc[b_off + j];
@@ -160,13 +175,70 @@ __global__ void __launch_bounds__(256) glm_scaled_potential_finish_kernel(
     double u = -(double)sum_p[c] + uw;
     if (Kb) u += 0.5 * qb + (double)Kb * (log(s_b) + kHalfLog2Pi);
     if (sig != nullptr && s_off >= 0) add_latent_sigma_terms(zc, gc, s_off, sig, dsig, c, s_prior, sp0, sp1, u);
-    if (ws.tau_off >= 0) {
-      const double tau = exp(t);
-      double lp, dlp;
-      positive_prior(ws.tau_prior, ws.tau_p0, ws.tau_p1, tau, lp, dlp);
-      u += -lp - t;
-      gc[ws.tau_off] = (float)(asum - tau * dlp - 1.0);
+    if (ws.tau_off >= 0) gc[ws.tau_off] = (float)latent_scale_terms(ws.tau_prior, ws.tau_p0, ws.tau_p1, t, asum, u);
+    U[c] = (float)u;
+  }
+}
+
+// glm_potential_finish_kernel with a group effect alpha (ge.G values at the end of each chain's [w | alpha] row of
+// dW, KD = D + G wide): one warp per chain, fp64, lane-strided over the coefficients and then the shuffle tree, so
+// every result is in a fixed order.  With s = s_a (= e^t when latent) and dW_g = d(-loglik)/d alpha_g:
+//   centred      U += alpha_g^2 / (2 s^2) + log s + log(2 pi) / 2    dU/dalpha_g = dW_g + alpha_g / s^2
+//                dU/dt = SUM_g (1 - alpha_g^2 / s^2) - s (d log p / ds)(s) - 1
+//   non-centred  U += eta_g^2 / 2 + log(2 pi) / 2                    dU/deta_g = s dW_g + eta_g
+//                dU/dt = s SUM_g eta_g dW_g - s (d log p / ds)(s) - 1
+// and for a latent s once per chain U += -log p(s) - t.  The weight and bias priors and the noise scale's terms
+// are those of glm_potential_finish_kernel.
+__global__ void __launch_bounds__(256) glm_group_potential_finish_kernel(
+    const float* __restrict__ z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int KD, int Kb, double s_w,
+    double s_b, const float* __restrict__ sum_p, const float* __restrict__ dW, const float* __restrict__ db,
+    float* __restrict__ U, float* __restrict__ grad, const float* __restrict__ sig, const float* __restrict__ dsig,
+    int64_t s_off, int s_prior, double sp0, double sp1, b2_glm_group_effect ge) {
+  const int64_t c = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (c >= C) return;
+  const int D = KD - ge.G;
+  const double iw = 1.0 / (s_w * s_w);
+  const double ib = Kb ? 1.0 / (s_b * s_b) : 0.0;
+  const float* zc = z + c * Dz;
+  float* gc = grad + c * Dz;
+  const float* dWc = dW + c * KD;
+  const double t = ge.s_off >= 0 ? (double)zc[ge.s_off] : 0.0;
+  const double sa = ge.s_off >= 0 ? exp(t) : ge.s_const, isa2 = 1.0 / (sa * sa);
+  double qw = 0.0, qb = 0.0, ua = 0.0, h = 0.0;  // SUM w^2 / s_w^2, SUM b^2 / s_b^2, the alpha terms of U, dU/dt
+  for (int j = lane; j < D; j += 32) {
+    const double v = (double)zc[w_off + j];
+    qw += v * v * iw;
+    gc[w_off + j] = (float)((double)dWc[j] + v * iw);
+  }
+  for (int j = lane; j < ge.G; j += 32) {
+    const double v = (double)zc[ge.a_off + j], g = (double)dWc[D + j];
+    if (ge.noncentred) {
+      ua += 0.5 * v * v + kHalfLog2Pi;
+      h += sa * v * g;
+      gc[ge.a_off + j] = (float)(sa * g + v);
+    } else {
+      const double q = v * v * isa2;
+      ua += 0.5 * q + kHalfLog2Pi;
+      h += 1.0 - q;
+      gc[ge.a_off + j] = (float)(g + v * isa2);
     }
+  }
+  for (int j = lane; j < Kb; j += 32) {
+    const double v = (double)zc[b_off + j];
+    qb += v * v * ib;
+    gc[b_off + j] = (float)((double)db[c * Kb + j] + v * ib);
+  }
+  qw = warp_sum(qw);
+  qb = warp_sum(qb);
+  ua = warp_sum(ua);
+  h = warp_sum(h);
+  if (lane == 0) {
+    double u = -(double)sum_p[c] + 0.5 * qw + (double)D * (log(s_w) + kHalfLog2Pi) + ua;
+    if (!ge.noncentred) u += (double)ge.G * log(sa);
+    if (Kb) u += 0.5 * qb + (double)Kb * (log(s_b) + kHalfLog2Pi);
+    if (sig != nullptr && s_off >= 0) add_latent_sigma_terms(zc, gc, s_off, sig, dsig, c, s_prior, sp0, sp1, u);
+    if (ge.s_off >= 0) gc[ge.s_off] = (float)latent_scale_terms(ge.s_prior, ge.sp0, ge.sp1, t, h, u);
     U[c] = (float)u;
   }
 }
@@ -210,12 +282,13 @@ struct PotentialSigma {
 // lik(Wp, bp, sig, dsig, sum_p, dW, db, ws, ws_bytes) makes the likelihood call on the chains' packed operands
 // with weight -1, writing sum_p, dW, db (and dsig) into the layout's areas, and returns its B2 code.  sg is
 // null without a noise scale; wsc is null for a constant weight scale s_w, else the latent weight scale, finished
-// by glm_scaled_potential_finish_kernel.
+// by glm_scaled_potential_finish_kernel.  ge is null without a group effect, else KD counts its G columns and
+// glm_group_potential_finish_kernel finishes.
 template <class Likelihood>
 int glm_potential_run(size_t lik_bytes, const float* z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int KD,
                       int K, int has_bias, double s_w, double s_b, const PotentialSigma* sg,
-                      const b2_glm_weight_scale* wsc, float* U, float* grad, void* workspace,
-                      size_t workspace_bytes, cudaStream_t s, Likelihood lik) {
+                      const b2_glm_weight_scale* wsc, const b2_glm_group_effect* ge, float* U, float* grad,
+                      void* workspace, size_t workspace_bytes, cudaStream_t s, Likelihood lik) {
   const GlmPotentialLayout L = glm_potential_layout(lik_bytes, KD, K, C, sg != nullptr);
   if (!workspace || workspace_bytes < L.total) return B2_ERR_WORKSPACE;
   const int Kb = has_bias ? K : 0;
@@ -230,15 +303,21 @@ int glm_potential_run(size_t lik_bytes, const float* z, int64_t C, int64_t Dz, i
   const int64_t s_off = sg ? sg->s_off : -1;
 
   const int64_t npack = C * (KD + Kb);
+  b2_glm_group_effect none = {};
+  const b2_glm_group_effect& gef = ge ? *ge : none;
   glm_potential_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, Wp, bp,
-                                                                             s_off, sg ? sg->s_const : 0.f, sig);
+                                                                             s_off, sg ? sg->s_const : 0.f, sig, gef);
   count_launch(1);
   int rc = check_launch();
   if (rc != 0) return rc;
   rc = lik(Wp, bp, sig, dsig, sum_p, dW, db, ws, L.wp);
   if (rc != 0) return rc;
   const unsigned grid = (unsigned)((C * 32 + 255) / 256);
-  if (wsc == nullptr)
+  if (ge != nullptr)
+    glm_group_potential_finish_kernel<<<grid, 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, s_w, s_b, sum_p, dW, db, U,
+                                                           grad, sig, dsig, s_off, sg ? sg->s_prior : 0,
+                                                           sg ? sg->sp0 : 0.0, sg ? sg->sp1 : 0.0, *ge);
+  else if (wsc == nullptr)
     glm_potential_finish_kernel<<<grid, 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, s_w, s_b, sum_p, dW, db, U, grad,
                                                      sig, dsig, s_off, sg ? sg->s_prior : 0, sg ? sg->sp0 : 0.0,
                                                      sg ? sg->sp1 : 0.0);
@@ -278,25 +357,27 @@ inline size_t glm_potential_lik_bytes(int kind, int64_t N, int D, int K, int64_t
 
 // The likelihood call of glm_potential_run for every kind: weight = -1, so dW, db (and dsig) are derivatives of
 // -loglik; every logit fp32-exact (B2_FLAG_GLM_3XTF32; the Normal kernels always split X).  The noise scale `sig`
-// and its gradient `dsig` (null for a constant noise scale) are Normal regression's, trials Binomial's.
+// and its gradient `dsig` (null for a constant noise scale) are Normal regression's, trials Binomial's; grp the
+// group effect of every kind but Categorical (Wp and dW then D + G wide).
 inline int glm_potential_likelihood(int kind, const float* X, const void* y, const float* trials, int trials_per_row,
                                     int64_t N, int D, int K, int64_t C, const float* Wp, const float* bp,
                                     const float* sig, float* dsig, float* sum_p, float* dW, float* db, void* ws,
-                                    size_t ws_bytes, void* stream) {
+                                    size_t ws_bytes, void* stream, GlmGroups grp = {}) {
   const float* yf = static_cast<const float*>(y);
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   switch (kind) {
     case B2_GLM_BERNOULLI:
-      return b2_glm_bernoulli_logits(X, yf, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0, B2_FLAG_GLM_3XTF32, sum_p, nullptr,
-                                     dW, db, ws, ws_bytes, stream);
+      return glm_bernoulli_logits(X, yf, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0, B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW,
+                                  db, ws, ws_bytes, s, grp);
     case B2_GLM_POISSON:
-      return b2_glm_poisson_log_rate(X, yf, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0, B2_FLAG_GLM_3XTF32, sum_p, nullptr,
-                                     dW, db, ws, ws_bytes, stream);
+      return glm_poisson_log_rate(X, yf, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0, B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW,
+                                  db, ws, ws_bytes, s, grp);
     case B2_GLM_NORMAL:
-      return b2_glm_normal_loc(X, yf, Wp, bp, sig, 1, N, D, (int)C, 1.0, -1.0, 1.0, 0, sum_p, nullptr, dW, db, dsig,
-                               ws, ws_bytes, stream);
+      return glm_normal_loc(X, yf, Wp, bp, sig, 1, N, D, (int)C, 1.0, -1.0, 1.0, 0, sum_p, nullptr, dW, db, dsig, ws,
+                            ws_bytes, s, grp);
     case B2_GLM_BINOMIAL:
-      return b2_glm_binomial_logits(X, yf, trials, trials_per_row, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
-                                    B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, stream);
+      return glm_binomial_logits(X, yf, trials, trials_per_row, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
+                                 B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, s, grp);
     default:
       return b2_glm_categorical_logits(X, static_cast<const int64_t*>(y), Wp, bp, N, D, K, (int)C, 1.0, -1.0, 1.0,
                                        B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, stream);
@@ -331,7 +412,7 @@ extern "C" int b2_glm_potential(int kind, const float* X, const void* y, int64_t
   if (!(s_w > 0.0) || (has_bias && !(s_b > 0.0))) return B2_ERR_BAD_SHAPE;
   return glm_potential_run(
       glm_potential_lik_bytes(kind, N, D, K, C), z, C, Dz, w_off, b_off, KD, K, has_bias, s_w, s_b, nullptr, nullptr,
-      U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
+      nullptr, U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
       [&](const float* Wp, const float* bp, const float*, float*, float* sum_p, float* dW, float* db, void* ws,
           size_t ws_bytes) {
         return glm_potential_likelihood(kind, X, y, nullptr, 0, N, D, K, C, Wp, bp, nullptr, nullptr, sum_p, dW, db,
@@ -367,8 +448,8 @@ extern "C" int b2_glm_normal_potential(const float* X, const float* y, int64_t N
   if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
   const PotentialSigma sg = {Ks ? s_off : (int64_t)-1, (float)sigma, s_prior, sp0, sp1};
   return glm_potential_run(
-      b2_glm_normal_workspace(N, D, (int)C), z, C, Dz, w_off, b_off, D, 1, has_bias, s_w, s_b, &sg, nullptr, U, grad,
-      workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
+      b2_glm_normal_workspace(N, D, (int)C), z, C, Dz, w_off, b_off, D, 1, has_bias, s_w, s_b, &sg, nullptr, nullptr,
+      U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
       [&](const float* Wp, const float* bp, const float* sig, float* dsig, float* sum_p, float* dW, float* db,
           void* ws, size_t ws_bytes) {
         return glm_potential_likelihood(B2_GLM_NORMAL, X, y, nullptr, 0, N, D, 1, C, Wp, bp, sig, Ks ? dsig : nullptr,
@@ -397,8 +478,8 @@ extern "C" int b2_glm_binomial_potential(const float* X, const float* y, const f
   if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
   if (trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0) return B2_ERR_BAD_SHAPE;
   return glm_potential_run(
-      b2_glm_binomial_workspace(N, D, (int)C), z, C, Dz, w_off, b_off, D, 1, has_bias, s_w, s_b, nullptr, nullptr, U,
-      grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
+      b2_glm_binomial_workspace(N, D, (int)C), z, C, Dz, w_off, b_off, D, 1, has_bias, s_w, s_b, nullptr, nullptr,
+      nullptr, U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
       [&](const float* Wp, const float* bp, const float*, float*, float* sum_p, float* dW, float* db, void* ws,
           size_t ws_bytes) {
         return glm_potential_likelihood(B2_GLM_BINOMIAL, X, y, trials, trials_per_row, N, D, 1, C, Wp, bp, nullptr,
@@ -454,10 +535,76 @@ extern "C" int b2_glm_scaled_potential(int kind, const float* X, const void* y, 
   const bool latent_sigma = normal && s_off >= 0;
   return glm_potential_run(
       glm_potential_lik_bytes(kind, N, D, K, C), z, C, Dz, w_off, b_off, (int)KD, K, has_bias, 1.0, s_b,
-      normal ? &sg : nullptr, &sc, U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
+      normal ? &sg : nullptr, &sc, nullptr, U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
       [&](const float* Wp, const float* bp, const float* sig, float* dsig, float* sum_p, float* dW, float* db,
           void* ws, size_t ws_bytes) {
         return glm_potential_likelihood(kind, X, y, trials, trials_per_row, N, D, K, C, Wp, bp, sig,
                                         latent_sigma ? dsig : nullptr, sum_p, dW, db, ws, ws_bytes, stream);
+      });
+}
+
+// ---- a varying intercept by group: alpha[g], centred or non-centred, with a constant or latent scale s_a -------
+// Scope: kinds Bernoulli, Poisson, Normal and Binomial, 1 <= G and D + G <= 128.
+inline bool glm_group_in_scope(int kind, int64_t N, int D, int G, int64_t C) {
+  if (kind != B2_GLM_BERNOULLI && kind != B2_GLM_POISSON && kind != B2_GLM_NORMAL && kind != B2_GLM_BINOMIAL)
+    return false;
+  return N >= 1 && C >= 1 && C < ((int64_t)1 << 31) && D >= 1 && G >= 1 && D + G <= 128;
+}
+
+extern "C" size_t b2_glm_group_potential_workspace(int kind, int64_t N, int D, int G, int64_t C) {
+  if (!glm_group_in_scope(kind, N, D, G, C)) return 256;
+  return glm_potential_layout(glm_potential_lik_bytes(kind, N, D + G, 1, C), D + G, 1, C, kind == B2_GLM_NORMAL).total;
+}
+
+extern "C" int b2_glm_group_potential(int kind, const float* X, const void* y, const float* trials,
+                                      int trials_per_row, int64_t N, int D, int has_bias, const float* z, int64_t C,
+                                      int64_t Dz, int64_t w_off, int64_t b_off, int64_t s_off, double s_w,
+                                      double s_b, int s_prior, double sp0, double sp1, double sigma,
+                                      const b2_glm_group_effect* ge, float* U, float* grad, void* workspace,
+                                      size_t workspace_bytes, void* stream) {
+  if (!X || !y || !z || !U || !grad || !ge || !ge->groups) return B2_ERR_NULL;
+  if (kind == B2_GLM_BINOMIAL && !trials) return B2_ERR_NULL;
+  const b2_glm_group_effect g = *ge;
+  if (!glm_group_in_scope(kind, N, D, g.G, C)) return B2_ERR_BAD_SHAPE;
+  if (N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
+  const bool normal = kind == B2_GLM_NORMAL;
+  if (!normal && s_off >= 0) return B2_ERR_BAD_SHAPE;   // only linear regression has a noise scale
+  if (g.noncentred != 0 && g.noncentred != 1) return B2_ERR_BAD_SHAPE;
+  // z's row is exactly w, b, log sigma, alpha (or eta) and log s_a: each block inside the row, no two overlapping,
+  // and their widths summing to Dz
+  const int64_t off[5] = {w_off, has_bias ? b_off : -1, s_off, g.a_off, g.s_off};
+  const int64_t len[5] = {D, has_bias ? 1 : 0, s_off >= 0 ? 1 : 0, g.G, g.s_off >= 0 ? 1 : 0};
+  int64_t width = 0;
+  for (int i = 0; i < 5; ++i) {
+    if (len[i] == 0) continue;
+    if (off[i] < 0 || off[i] > Dz - len[i]) return B2_ERR_BAD_SHAPE;
+    for (int j = 0; j < i; ++j)
+      if (len[j] && off[i] < off[j] + len[j] && off[j] < off[i] + len[i]) return B2_ERR_BAD_SHAPE;
+    width += len[i];
+  }
+  if (width != Dz) return B2_ERR_BAD_SHAPE;
+  if (!(s_w > 0.0) || (has_bias && !(s_b > 0.0))) return B2_ERR_BAD_SHAPE;
+  if (g.s_off >= 0 && !positive_prior_ok(g.s_prior, g.sp0, g.sp1)) return B2_ERR_BAD_SHAPE;
+  if (g.s_off < 0 && (!(g.s_const > 0.0) || !((float)g.s_const > 0.f))) return B2_ERR_BAD_SHAPE;
+  if (normal && s_off >= 0 && !positive_prior_ok(s_prior, sp0, sp1)) return B2_ERR_BAD_SHAPE;
+  if (normal && s_off < 0 && (!(sigma > 0.0) || !((float)sigma > 0.f))) return B2_ERR_BAD_SHAPE;
+  if (kind == B2_GLM_BINOMIAL && trials_per_row != 0 && trials_per_row != 1) return B2_ERR_BAD_SHAPE;
+  if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0 ||
+      reinterpret_cast<uintptr_t>(g.groups) % 16 != 0)
+    return B2_ERR_BAD_SHAPE;
+  if (kind == B2_GLM_BINOMIAL && trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0)
+    return B2_ERR_BAD_SHAPE;
+  const PotentialSigma sg = {s_off >= 0 ? s_off : (int64_t)-1, (float)sigma, s_prior, sp0, sp1};
+  const bool latent_sigma = normal && s_off >= 0;
+  GlmGroups grp;
+  grp.idx = g.groups;
+  grp.G = g.G;
+  return glm_potential_run(
+      glm_potential_lik_bytes(kind, N, D + g.G, 1, C), z, C, Dz, w_off, b_off, D + g.G, 1, has_bias, s_w, s_b,
+      normal ? &sg : nullptr, nullptr, &g, U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
+      [&](const float* Wp, const float* bp, const float* sig, float* dsig, float* sum_p, float* dW, float* db,
+          void* ws, size_t ws_bytes) {
+        return glm_potential_likelihood(kind, X, y, trials, trials_per_row, N, D, 1, C, Wp, bp, sig,
+                                        latent_sigma ? dsig : nullptr, sum_p, dW, db, ws, ws_bytes, stream, grp);
       });
 }

@@ -208,11 +208,17 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
     constant, or latent: ``tau`` (one positive scalar site), ``lam`` (a positive site of the weight's shape) or
     ``tau * lam``.  Linear regression's noise scale is a constant or one latent positive scalar site.  Every
     latent positive site has a HalfNormal, HalfCauchy, Exponential or LogNormal prior with constant parameters
-    (for ``lam`` one value for every coefficient), and exactly one role -- noise scale, ``tau`` or ``lam`` -- which
-    the probes establish: the observation's scale equals the drawn noise scale and the weight site's scale equals
-    the drawn ``tau``, ``lam`` or ``tau * lam`` at every probe.  Intercept-free logistic regression with a constant
-    weight scale keeps LogisticPotential's route."""
-    from .potential import GlmPotential
+    (for ``lam`` one value for every coefficient), and exactly one role -- noise scale, ``tau``, ``lam`` or the group
+    scale ``s_a`` -- which the probes establish: the observation's scale equals the drawn noise scale and the weight
+    site's scale equals the drawn ``tau``, ``lam`` or ``tau * lam`` at every probe.  Intercept-free logistic
+    regression with a constant weight scale keeps LogisticPotential's route.
+
+    A varying intercept by group (every kind but softmax, with a constant weight scale, any D with D + G <= 128):
+    the group index is the one gradient-free int64 ``[N]`` tensor among the arguments, and the group effect a
+    latent ``Normal`` site of shape ``(G,)``, tried after the model without one fails.  The probes decide the form:
+    the observation's logits (log-rate, loc) equal ``X @ w + b + alpha[g]`` with ``alpha ~ Normal(0, s_a)``
+    (centred), or ``X @ w + b + s_a * eta[g]`` with ``eta ~ Normal(0, 1)`` (non-centred), ``s_a`` a constant or a
+    drawn positive scalar site, at every probe.  So how the model writes the gather does not matter."""
     if len(observed) != 1 or not 1 <= len(latent) <= 5:
         return None
     (obs_name, obs), = observed.items()
@@ -238,7 +244,7 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
             return None
         positive[name] = tuple(v.shape)
     latent = {k: v for k, v in latent.items() if k not in positive}
-    if len(latent) not in (1, 2):
+    if len(latent) not in (1, 2, 3):
         return None
     y = obs["value"]
     if not isinstance(y, torch.Tensor) or y.dim() != 1:
@@ -260,10 +266,34 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
                 or v.dtype != torch.float32 or _const(fn.loc) != 0.0:
             return None
         scales[name], shapes[name] = _const(fn.scale), tuple(v.shape)
+    attempts = [None]                      # the group-effect site: none, then each candidate
+    ints = [a for a in list(args) + list(kwargs.values())
+            if isinstance(a, torch.Tensor) and a is not y and a.dtype == torch.int64 and a.dim() == 1
+            and a.numel() == n and not a.requires_grad]
+    if kind != "Categorical" and len(ints) == 1 and len(latent) >= 2 and ints[0].numel() > 0:
+        # only sites with a group for every index: the probes gather with it
+        lo, hi = int(ints[0].min()), int(ints[0].max())
+        attempts += [name for name, s in shapes.items() if len(s) == 1 and D + s[0] <= 128 and lo >= 0 and hi < s[0]]
+    for group_site in attempts:
+        pot = _glm_roles(poutine, model, args, kwargs, kind, obs_name, obs, order, positive, priors, latent, X, y,
+                         scales, shapes, group_site, ints[0] if group_site is not None else None)
+        if pot is not None:
+            return pot
+    return None
+
+
+def _glm_roles(poutine, model, args, kwargs, kind, obs_name, obs, order, positive, priors, latent, X, y, scales,
+               shapes, group_site, gidx):
+    """``_try_glm`` with the Normal site ``group_site`` (None: no group effect) as the group effect."""
+    from .potential import GlmPotential
+    n, D = y.numel(), X.shape[1]
+    latent = {k: v for k, v in latent.items() if k != group_site}
+    if len(latent) not in (1, 2):
+        return None
     if kind == "Bernoulli":
         K = 1
         wshapes, bshapes = [(D,)], [(), (1,)]
-        if D not in (4, 8, 16, 32) or y.dtype != torch.float32:
+        if (group_site is None and D not in (4, 8, 16, 32)) or y.dtype != torch.float32:
             return None
     elif kind in ("Poisson", "Normal", "Binomial"):
         K = 1
@@ -271,13 +301,13 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
         if not 1 <= D <= 128 or y.dtype != torch.float32:
             return None
     else:
-        wmat = [s for s in shapes.values() if len(s) == 2]
+        wmat = [shapes[name] for name in latent if len(shapes[name]) == 2]
         K = wmat[0][0] if len(wmat) == 1 else 0
         wshapes, bshapes = [(K, D)], [(K,)]
         if D != 32 or not 2 <= K <= 16 or y.dtype != torch.int64:
             return None
-    weight = [name for name, s in shapes.items() if s in wshapes]
-    bias = [name for name, s in shapes.items() if s in bshapes]
+    weight = [name for name in latent if shapes[name] in wshapes]
+    bias = [name for name in latent if shapes[name] in bshapes]
     if len(weight) != 1 or len(bias) + 1 != len(latent):
         return None
     weight, bias = weight[0], (bias[0] if bias else None)
@@ -292,6 +322,7 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
     sigma_site, sigma_const = None, None
     wform = None                           # (tau site or None, lam site or None); (None, None): the constant s_w
     trials = None                          # Binomial: the constant count, or the [N] counts of the prototype
+    group = None                           # the group effect's form, once the first probe has found it
     if kind == "Binomial":
         trials = _binomial_trials(_base(obs["fn"])[0], n)
         if trials is None:
@@ -308,6 +339,8 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
         data = {weight: wv} if bias is None else {weight: wv, bias: bv}
         for name, shape in positive.items():
             data[name] = torch.exp(0.5 * torch.randn(shape, generator=gen)).to(X)
+        if group_site is not None:
+            data[group_site] = torch.randn(shapes[group_site], generator=gen).to(X)
         tr = poutine.trace(poutine.condition(model, data=data)).get_trace(*args, **kwargs)
         pfn = _base(tr.nodes[obs_name]["fn"])[0]
         # the priors: constant parameters that do not move with any latent
@@ -338,6 +371,7 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
                 if c is None or not c > 0.0 or (sigma_const is not None and c != sigma_const):
                     return None
                 sigma_const = c
+        free_s = [name for name in scalars if name != sigma_site]
         # the weight scale: the constant of the prototype, or the drawn tau, lam or tau * lam
         def want_scale(form):
             t, lam = form
@@ -347,17 +381,14 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
             return v * data[lam] if lam is not None else v
         ws = as_t(wfn.scale)
         if i == 0:
-            free_s = [name for name in scalars if name != sigma_site]
-            forms = [(None, None)] + [(t, None) for t in free_s] + [(None, lam) for lam in lams] + \
-                [(t, lam) for t in free_s for lam in lams if t != lam]
+            forms = [(None, None)]
+            if group_site is None:
+                forms += [(t, None) for t in free_s] + [(None, lam) for lam in lams] + \
+                    [(t, lam) for t in free_s for lam in lams if t != lam]
             hits = [f for f in forms if want_scale(f) is not None and _close(ws, want_scale(f), X.dtype)]
             if len(hits) != 1:
                 return None
             wform = hits[0]
-            # every positive site has exactly one role
-            roles = [r for r in (sigma_site,) + wform if r is not None]
-            if sorted(roles) != sorted(positive):
-                return None
         want = want_scale(wform)
         if tuple(torch.broadcast_shapes(ws.shape, want.shape, shapes[weight])) != shapes[weight] \
                 or not _close(ws, want, X.dtype):
@@ -381,10 +412,21 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
         else:
             want = X @ wv.mT + (bv if bv is not None else 0.0)
             logits, want = torch.log_softmax(logits, -1), torch.log_softmax(want, -1)
+        if group_site is not None:
+            group = _group_form(tr, group_site, data, gidx, logits, want, free_s, group, X.dtype)
+            if group is None:
+                return None
+            sa = data[group["s_site"]].reshape(()) if group["s_site"] is not None else as_t(group["s_const"])
+            e = data[group_site][gidx]
+            want = want + (sa * e if group["noncentred"] else e)
         if tuple(logits.shape) != tuple(want.shape) or not _close(logits, want, X.dtype):
             return None
     tau_site, lam_site = wform
-    if kind == "Bernoulli" and bias is None and tau_site is None and lam_site is None:
+    # every positive site has exactly one role
+    roles = [r for r in (sigma_site,) + wform + ((group["s_site"],) if group else ()) if r is not None]
+    if sorted(roles) != sorted(positive):
+        return None
+    if kind == "Bernoulli" and bias is None and tau_site is None and lam_site is None and group is None:
         return None   # intercept-free logistic regression with a constant weight scale keeps LogisticPotential
     off, sites = 0, {}
     for name in order:
@@ -394,13 +436,50 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
             width *= d
         sites[name] = (slice(off, off + width), "exp" if name in positive else "identity", shape)
         off += width
+    if group is not None:
+        group = dict(group, site=group_site, index=gidx, s_prior=priors.get(group["s_site"]))
     return GlmPotential(X, y.detach(), kind, sites, weight, bias,
                         s_w=scales[weight] if wform == (None, None) else 1.0,
                         s_b=scales[bias] if bias is not None else 1.0,
                         sigma=sigma_const if sigma_const is not None else 1.0, sigma_site=sigma_site,
                         sigma_prior=priors.get(sigma_site), trials=trials,
                         tau_site=tau_site, tau_prior=priors.get(tau_site),
-                        lam_site=lam_site, lam_prior=priors.get(lam_site))
+                        lam_site=lam_site, lam_prior=priors.get(lam_site), group=group)
+
+
+def _group_form(tr, group_site, data, gidx, logits, want, free_s, group, dtype):
+    """The group effect's form at one probe: ``{"noncentred", "s_site", "s_const"}`` when the residual
+    ``logits - want`` is ``alpha[g]`` with ``alpha ~ Normal(0, s_a)`` or ``s_a * eta[g]`` with ``eta ~ Normal(0, 1)``,
+    ``s_a`` the drawn site of ``free_s`` or one constant; ``group`` is the first probe's answer, which later probes
+    must repeat.  None otherwise."""
+    afn = _base(tr.nodes[group_site]["fn"])[0]
+    if _const(afn.loc) != 0.0:
+        return None
+    G = data[group_site].numel()
+    scale = torch.as_tensor(afn.scale, dtype=dtype, device=logits.device).detach()
+    if tuple(torch.broadcast_shapes(scale.shape, (G,))) != (G,):
+        return None
+    e = data[group_site][gidx]
+    r = logits - want
+    if group is None:
+        if _close(r, e, dtype):
+            s, noncentred = scale, False
+        elif _const(scale) == 1.0:
+            # the least-squares s_a of r = s_a e; the comparison below confirms it
+            s, noncentred = (r * e).sum() / (e * e).sum().clamp(min=1e-30), True
+        else:
+            return None
+        hits = [name for name in free_s if _close(s, data[name].reshape(()), dtype)]
+        if len(hits) > 1:
+            return None
+        c = _const(s) if not hits else None
+        if not hits and not (c is not None and c > 0.0 and math.isfinite(c)):
+            return None
+        group = {"noncentred": noncentred, "s_site": hits[0] if hits else None, "s_const": c}
+    sa = data[group["s_site"]].reshape(()) if group["s_site"] is not None else group["s_const"]
+    if group["noncentred"]:
+        return group if _const(scale) == 1.0 else None
+    return group if _close(scale, torch.as_tensor(sa, dtype=dtype, device=scale.device), dtype) else None
 
 
 def _binomial_trials(fn, n):

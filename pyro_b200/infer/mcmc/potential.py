@@ -129,6 +129,14 @@ class GlmPotential:
     ``sigma_prior``, one value for every coefficient; z holds their logs (transform ``"exp"``), and U carries
     their Jacobians.
 
+    A varying intercept by group (``b2_glm_group_potential``, every kind but softmax, constant weight scale): the
+    linear predictor gains ``alpha[g]``, ``g`` the int64 ``[N]`` group index and ``alpha`` the ``G`` values of the
+    site ``group["site"]``, drawn as ``Normal(0, s_a)`` (centred) or as ``eta ~ Normal(0, 1)`` with
+    ``alpha = s_a * eta`` (``group["noncentred"]``).  ``s_a`` is the constant ``group["s_const"]`` or the positive
+    scalar site ``group["s_site"]`` with prior ``group["s_prior"]`` (as ``sigma_prior``).  ``group["index"]`` must
+    lie in ``[0, G)``; a private int32 copy is made once.  The likelihood runs on ``[X | onehot(g)]``, so
+    ``D + G <= 128``.
+
     ``value_and_grad`` is ``b2_glm_potential``: the likelihood of all chains comes from one pass of the
     fused GLM kernel over X, the chains being its particles.  ``sites`` maps each site name to
     ``(slice into z, transform, value shape)`` in the order and layout ``TracePotential`` gives the same
@@ -139,7 +147,8 @@ class GlmPotential:
                      "Exponential": N.SIGMA_EXPONENTIAL, "LogNormal": N.SIGMA_LOGNORMAL}
 
     def __init__(self, X, y, kind, sites, weight, bias=None, s_w=1.0, s_b=1.0, sigma=1.0, sigma_site=None,
-                 sigma_prior=None, trials=None, tau_site=None, tau_prior=None, lam_site=None, lam_prior=None):
+                 sigma_prior=None, trials=None, tau_site=None, tau_prior=None, lam_site=None, lam_prior=None,
+                 group=None):
         N.require_cuda(X, "GlmPotential")
         if X.dtype != torch.float32 or X.dim() != 2:
             raise ValueError("GlmPotential needs fp32 X of shape [N, D]")
@@ -192,6 +201,30 @@ class GlmPotential:
         self.D = sum(sl.stop - sl.start for sl, _, _ in self.sites.values())
         self.dtype = torch.float32
         self.device = self.X.device
+        self.group, self.group_effect = group, None
+        if group is not None:
+            self.group_effect = self._group_effect(group)
+
+    def _group_effect(self, group):
+        """b2_glm_group_effect of ``group``, with the private int32 copy of the index it points to."""
+        sl, _, shape = self.sites[group["site"]]
+        G = int(shape[0])
+        g = group["index"].detach().to(self.device).reshape(-1)
+        if g.numel() != self.n or g.is_floating_point():
+            raise ValueError("the group index must be an integer tensor of shape [N]")
+        if bool((g < 0).any()) or bool((g >= G).any()):
+            raise ValueError("group index outside [0, %d)" % G)
+        self.groups = g.to(torch.int32).clone()
+        ge = N.b2_glm_group_effect()
+        ge.groups = self.groups.data_ptr()
+        ge.a_off, ge.G, ge.noncentred = sl.start, G, int(bool(group["noncentred"]))
+        s_site = group.get("s_site")
+        if s_site is not None:
+            pk, p0, p1 = group["s_prior"]
+            ge.s_off, ge.s_prior, ge.sp0, ge.sp1 = self.sites[s_site][0].start, self._SIGMA_PRIORS[pk], p0, p1
+        else:
+            ge.s_off, ge.s_const = -1, float(group["s_const"])
+        return ge
 
     @property
     def dim(self):
@@ -204,6 +237,8 @@ class GlmPotential:
         U = torch.empty(C, dtype=torch.float32, device=z.device)
         g = torch.empty_like(z)
         lib = N.lib()
+        if self.group_effect is not None:
+            return self._group_value_and_grad(lib, z, C, U, g)
         if self.weight_scale is not None:
             return self._scaled_value_and_grad(lib, z, C, U, g)
         if self.normal:
@@ -244,6 +279,19 @@ class GlmPotential:
             int(self.has_bias), z.data_ptr(), C, self.D, self.w_off, self.b_off, s_off, self.s_b, pk, p0, p1,
             self.sigma, ctypes.byref(self.weight_scale), U.data_ptr(), g.data_ptr(), ws.data_ptr(), ws.numel(),
             N.stream_ptr(z.device)), "b2_glm_scaled_potential")
+        return U, g
+
+    def _group_value_and_grad(self, lib, z, C, U, g):
+        need = int(lib.b2_glm_group_potential_workspace(self.scaled_kind, self.n, self.Dx, self.group_effect.G, C))
+        ws = N.workspace(z.device, need, tag="glm_potential")
+        s_off = self.sites[self.sigma_site][0].start if self.sigma_site is not None else -1
+        pk, p0, p1 = self.sigma_prior
+        trials, per_row = (self.trials.data_ptr(), self.trials_per_row) if self.binomial else (None, 0)
+        N.check(lib.b2_glm_group_potential(
+            self.scaled_kind, self.X.data_ptr(), self.y.data_ptr(), trials, per_row, self.n, self.Dx,
+            int(self.has_bias), z.data_ptr(), C, self.D, self.w_off, self.b_off, s_off, self.s_w, self.s_b, pk, p0, p1,
+            self.sigma, ctypes.byref(self.group_effect), U.data_ptr(), g.data_ptr(), ws.data_ptr(), ws.numel(),
+            N.stream_ptr(z.device)), "b2_glm_group_potential")
         return U, g
 
     def unpack(self, z):
