@@ -573,6 +573,23 @@ struct ValueAux {
 #if defined(__CUDACC__)
 static __device__ const float kLogFactorialF32[64] = {0.0f, 0.0f, 0.693147181f, 1.79175947f, 3.17805383f, 4.78749174f, 6.57925121f, 8.52516136f, 10.6046029f, 12.8018275f, 15.1044126f, 17.5023078f, 19.9872145f, 22.5521639f, 25.1912212f, 27.8992714f, 30.6718601f, 33.5050735f, 36.3954452f, 39.3398842f, 42.3356165f, 45.3801389f, 48.4711814f, 51.6066756f, 54.7847294f, 58.0036052f, 61.2617018f, 64.5575386f, 67.8897431f, 71.257039f, 74.6582363f, 78.0922236f, 81.5579595f, 85.054467f, 88.5808275f, 92.1361756f, 95.7196945f, 99.3306125f, 102.968199f, 106.63176f, 110.32064f, 114.034212f, 117.771881f, 121.533082f, 125.317271f, 129.123934f, 132.952575f, 136.802723f, 140.673924f, 144.565744f, 148.477767f, 152.409593f, 156.360836f, 160.331128f, 164.320112f, 168.327445f, 172.352797f, 176.395848f, 180.456291f, 184.533829f, 188.628173f, 192.739047f, 196.866182f, 201.009316f};
 static __device__ const float kDigammaIntF32[64] = {-0.577215665f, 0.422784335f, 0.922784335f, 1.25611767f, 1.50611767f, 1.70611767f, 1.87278434f, 2.01564148f, 2.14064148f, 2.25175259f, 2.35175259f, 2.44266168f, 2.52599501f, 2.60291809f, 2.67434666f, 2.74101333f, 2.80351333f, 2.86233686f, 2.91789241f, 2.97052399f, 3.02052399f, 3.06814304f, 3.11359759f, 3.15707585f, 3.19874251f, 3.23874251f, 3.27720405f, 3.31424109f, 3.34995537f, 3.38443813f, 3.41777147f, 3.45002953f, 3.48127953f, 3.51158256f, 3.54099433f, 3.56956575f, 3.59734353f, 3.62437056f, 3.65068635f, 3.67632737f, 3.70132737f, 3.72571762f, 3.74952714f, 3.77278296f, 3.79551023f, 3.81773245f, 3.83947158f, 3.86074818f, 3.88158151f, 3.90198967f, 3.92198967f, 3.94159752f, 3.96082829f, 3.97969621f, 3.99821473f, 4.01639655f, 4.03425369f, 4.05179755f, 4.06903893f, 4.08598808f, 4.10265475f, 4.11904819f, 4.13517722f, 4.15105024f};
+// log(k!) for k = 0..63 in fp64, for the data terms of the GLM kernels (glm_tc_common.cuh): summed over millions of
+// rows, the rounding of an fp32 entry repeats on every row with that count and no longer averages out.
+static __device__ const double kLogFactorialF64[64] = {0.0, 0.0, 0.693147180559945, 1.7917594692280554, 3.178053830347945, 4.787491742782047, 6.579251212010102, 8.525161361065415, 10.604602902745249, 12.801827480081467, 15.104412573075514, 17.502307845873887, 19.987214495661885, 22.55216385312342, 25.191221182738683, 27.89927138384089, 30.671860106080672, 33.50507345013689, 36.39544520803305, 39.339884187199495, 42.335616460753485, 45.38013889847691, 48.47118135183522, 51.60667556776438, 54.78472939811232, 58.00360522298052, 61.26170176100201, 64.55753862700634, 67.88974313718153, 71.257038967168, 74.65823634883017, 78.0922235533153, 81.55795945611503, 85.05446701758152, 88.58082754219768, 92.1361756036871, 95.7196945421432, 99.33061245478743, 102.96819861451381, 106.63176026064346, 110.32063971475738, 114.03421178146169, 117.77188139974507, 121.53308151543864, 125.3172711493569, 129.12393363912722, 132.95257503561632, 136.80272263732635, 140.67392364823425, 144.5657439463449, 148.47776695177305, 152.40959258449732, 156.3608363030788, 160.3311282166309, 164.32011226319514, 168.32744544842765, 172.35279713916282, 176.39584840699737, 180.45629141754375, 184.53382886144948, 188.62817342367163, 192.7390472878449, 196.86618167288998, 201.00931639928152};
+// log(v!) = lgamma(v + 1) in fp64: the table for integer v < 64, Stirling's series from 64 on (the first omitted
+// term, 1/(1680 x^7), is below 2e-16 there), CUDA's lgamma for every other v (fractional, negative, huge, NaN).
+__device__ __forceinline__ double log_factorial_f64(float v) {
+  const int k = __float2int_rz(v);
+  if ((unsigned)k < 64u && (float)k == v) return __ldg(&kLogFactorialF64[k]);
+  const double x = (double)v + 1.0;
+  if (v >= 64.f && v < 1e15f) {
+    // 1/x only scales the correction terms (below 1.3e-3 here): a rounded fp32 reciprocal is exact enough
+    const double inv = (double)__frcp_rn((float)x), inv2 = inv * inv;
+    return (x - 0.5) * log(x) - x + 0.91893853320467274178 +
+           inv * (1.0 / 12.0 - inv2 * (1.0 / 360.0 - inv2 * (1.0 / 1260.0)));
+  }
+  return lgamma(x);
+}
 #endif
 
 // Poisson(rate): torch/distributions/poisson.py:75-79   xlogy(x, rate) - rate - lgamma(x + 1)

@@ -157,9 +157,8 @@ struct GlmElbo {
 };
 
 // second stage: fixed-order sum over the CTAs' partials [nblocks][P][K (D + 1) + 1] (per class dW[0..D-1]
-// and db, then the particle's lp sum; K = 1 but for softmax); applies weight / scale.  lg (Poisson and
-// Binomial, else null) holds one more partial per CTA, of a data term every particle's sum subtracts: SUM
-// lgamma(y + 1), SUM log C(m, y).  sigma (Normal only, else null; sigma[p * sigma_stride] for particle p) turns the sufficient
+// and db, then the particle's lp sum; K = 1 but for softmax); applies weight / scale.  (The Poisson and Binomial
+// kernels have already folded their data terms into the lp partials.)  sigma (Normal only, else null; sigma[p * sigma_stride] for particle p) turns the sufficient
 // statistics of the Normal tile kernel into the lp sum and gradients: the lp slot holds S = SUM (y - l)^2 and
 // dW / db hold SUM (y - l) [x | 1]; the warp of sum_p[p] also writes out_dsigma[p] (nullable), n is N.
 // One WARP per entry of the [P, K (D + 1) + 1] table: lanes stride over the CTAs (L2-resident partials),
@@ -178,7 +177,7 @@ __device__ __forceinline__ void glm_finish_body(const float* __restrict__ partia
                                                 double scale, double weight, float* __restrict__ sum_p,
                                                 float* __restrict__ out_dW, float* __restrict__ out_db,
                                                 double sum_coeff, int flags, float* __restrict__ out_total,
-                                                unsigned int* __restrict__ ticket, const float* __restrict__ lg,
+                                                unsigned int* __restrict__ ticket,
                                                 const float* __restrict__ sigma, int sigma_stride, int64_t n,
                                                 float* __restrict__ out_dsigma, const GlmElbo* E) {
   pdl_enter();
@@ -244,11 +243,6 @@ __device__ __forceinline__ void glm_finish_body(const float* __restrict__ partia
       }
       return;
     }
-    if (lg != nullptr) {
-      double l = 0.0;
-      for (int bl = lane; bl < nblocks; bl += 32) l += (double)lg[bl];
-      s -= warp_sum(l);
-    }
     if (sigma) {
       // Normal: s is S = SUM (y - l)^2; lp sum = -S / (2 sigma^2) - n (log sigma + log(2 pi) / 2) and
       // d/dsigma = S / sigma^3 - n / sigma, all in fp64
@@ -310,11 +304,10 @@ __global__ void __launch_bounds__(kFinishThreads) glm_finish_kernel(const float*
                                                          float* __restrict__ out_db, double sum_coeff, int flags,
                                                          float* __restrict__ out_total,
                                                          unsigned int* __restrict__ ticket,
-                                                         const float* __restrict__ lg,
                                                          const float* __restrict__ sigma, int sigma_stride,
                                                          int64_t n, float* __restrict__ out_dsigma) {
   glm_finish_body(partials, nblocks, P, K, D, scale, weight, sum_p, out_dW, out_db, sum_coeff, flags, out_total,
-                  ticket, lg, sigma, sigma_stride, n, out_dsigma, nullptr);
+                  ticket, sigma, sigma_stride, n, out_dsigma, nullptr);
 }
 
 __global__ void __launch_bounds__(kFinishThreads) glm_finish_elbo_kernel(const float* __restrict__ partials, int nblocks, int P,
@@ -324,7 +317,7 @@ __global__ void __launch_bounds__(kFinishThreads) glm_finish_elbo_kernel(const f
                                                               int flags, float* __restrict__ out_total,
                                                               unsigned int* __restrict__ ticket, const GlmElbo E) {
   glm_finish_body(partials, nblocks, P, K, D, scale, weight, sum_p, out_dW, out_db, sum_coeff, flags, out_total,
-                  ticket, nullptr, nullptr, 0, 0, nullptr, &E);
+                  ticket, nullptr, 0, 0, nullptr, &E);
 }
 
 // The per-particle sums go to out_sum_p, or without one to the [P] row of the workspace after the partials.
@@ -334,12 +327,12 @@ static float* glm_sum_p(const float* partials, float* out_sum_p, int gx, int tot
 
 void launch_glm_finish(const float* partials, unsigned int* ticket, int gx, int P, int K, int D, double scale,
                        double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
-                       float* out_dW, float* out_db, const float* lg, cudaStream_t s, const float* sigma,
+                       float* out_dW, float* out_db, cudaStream_t s, const float* sigma,
                        int sigma_stride, int64_t n, float* out_dsigma) {
   const int total = P * (K * (D + 1) + 1);
   launch_pdl(glm_finish_kernel, dim3((total + kFinishEntries - 1) / kFinishEntries), dim3(kFinishThreads), 0, s,
              partials, gx, P, K, D, scale, weight, glm_sum_p(partials, out_sum_p, gx, total), out_dW, out_db,
-             sum_coeff, flags, out_total, ticket, lg, sigma, sigma_stride, n, out_dsigma);
+             sum_coeff, flags, out_total, ticket, sigma, sigma_stride, n, out_dsigma);
 }
 
 inline int glm_grid_x(int64_t N) {
@@ -411,7 +404,7 @@ static int glm_bernoulli(const float* X, const float* y, const float* W, const f
                out_total, ticket, *E);
   } else {
     launch_glm_finish(partials, ticket, gx, P, 1, Da, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW,
-                      out_db, nullptr, s);
+                      out_db, s);
   }
   count_launch(2);
   return check_launch();

@@ -17,10 +17,11 @@
 // Precision policy of the Poisson kernels: W always split hi + lo, X split too under SPLIT_X; GEMM 1 starts from
 // zero and the epilogue adds the bias, rounded to nearest (see poisson_epilogue); g rounded to nearest TF32.
 //
-// SUM log C(m, y) = SUM [lgamma(y + 1) + lgamma(m - y + 1) - lgamma(m + 1)] depends on the data alone: after its
-// tile loop each CTA of particle slab 0 sums it over the rows of its own tiles (read again from L2, outside the
-// wgmma pipeline) into one more partial, and glm_finish_kernel subtracts the sum of those partials from every
-// particle's sum.  Every sum has a fixed order; no float atomics, and a call is two launches (kernel + finish).
+// SUM log C(m, y) = -SUM [lgamma(y + 1) + lgamma(m - y + 1) - lgamma(m + 1)] depends on the data alone: after its
+// tile loop each CTA sums it in fp64 over the rows of its own tiles (read again from L2, outside the wgmma
+// pipeline) and adds it to each particle's fp64 lp sum before rounding that to its fp32 partial (Binomial in
+// glm_tc_common.cuh): at m = 1000 a row's y l - m softplus(l) is about -690 nats and its lp a few.  Every sum has
+// a fixed order; no float atomics, and a call is two launches (kernel + finish).
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -35,38 +36,6 @@ namespace tcbi {
 
 using namespace tc;
 
-// lgamma(v + 1): the table of integer counts below 64, the shifted Stirling series above
-__device__ __forceinline__ float lgamma1(float v) { return ValueAux<kPoisson, float, false>::make(v).lgx; }
-
-// lg[blockIdx.x] = SUM [lgamma(y_n + 1) + lgamma(m_n - y_n + 1) - lgamma(m_n + 1)] over the rows of the CTA's
-// tiles (blockIdx.x, blockIdx.x + gridDim.x, ...), in a fixed order; called by every thread of a CTA of slab 0
-// after its tile loop
-template <int NT, bool ROW>
-__device__ __forceinline__ void lbinom_partial(const float* __restrict__ y, const float* __restrict__ trials,
-                                               int64_t N, float* __restrict__ lg) {
-  __shared__ float red[NT / 32];
-  const int64_t ntiles = (N + kRows - 1) / kRows;
-  const int nt = (int)((ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x);
-  const float mc = ROW ? 0.f : __ldg(trials);
-  const float lgm = ROW ? 0.f : lgamma1(mc);
-  float s = 0.f;
-  for (int64_t i = threadIdx.x; i < (int64_t)nt * kRows; i += NT) {
-    const int64_t n = (blockIdx.x + (i / kRows) * (int64_t)gridDim.x) * kRows + i % kRows;
-    if (n < N) {
-      const float yv = __ldg(y + n), m = ROW ? __ldg(trials + n) : mc;
-      s += (lgamma1(yv) + lgamma1(m - yv)) - (ROW ? lgamma1(m) : lgm);
-    }
-  }
-  s = warp_sum(s);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float v = 0.f;
-    for (int w = 0; w < NT / 32; ++w) v += red[w];
-    lg[blockIdx.x] = v;
-  }
-}
-
 // D = 32.  SPLIT_X = false (default): W split hi/lo, X rounded to nearest.  SPLIT_X = true: X split as well.
 // ROW: per-row trial counts (map_m); else the one count trials[0].
 template <bool ROW, bool SPLIT_X>
@@ -74,10 +43,8 @@ __global__ void __launch_bounds__(tile32::kThreads, 1)
 glm_binomial_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_y,
                        const __grid_constant__ CUtensorMap map_m, const float* __restrict__ y,
                        const float* __restrict__ trials, const float* __restrict__ W,
-                       const float* __restrict__ bvec, int64_t N, int P, float* __restrict__ partials,
-                       float* __restrict__ lg) {
-  tile32::glm_tile_pipeline<Binomial<ROW>, SPLIT_X>(map_x, map_y, W, bvec, N, P, 1, partials, &map_m, trials);
-  if (blockIdx.y == 0) lbinom_partial<tile32::kThreads, ROW>(y, trials, N, lg);
+                       const float* __restrict__ bvec, int64_t N, int P, float* __restrict__ partials) {
+  tile32::glm_tile_pipeline<Binomial<ROW>, SPLIT_X>(map_x, map_y, W, bvec, N, P, 1, partials, &map_m, trials, y);
 }
 
 // every other D in 1..128, padded to DC atoms of 32 columns
@@ -85,10 +52,8 @@ template <bool ROW, int DC, bool SPLIT_X>
 __global__ void __launch_bounds__(tcf::Cfg<DC>::kThreads, 1)
 glm_binomial_flat_tc_kernel(const float* __restrict__ X, const float* __restrict__ y,
                             const float* __restrict__ trials, const float* __restrict__ W,
-                            const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
-                            float* __restrict__ lg) {
+                            const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials) {
   tcf::glm_flat_pipeline<Binomial<ROW>, DC, SPLIT_X>(X, y, W, bvec, N, D, P, partials, trials);
-  if (blockIdx.y == 0) lbinom_partial<tcf::Cfg<DC>::kThreads, ROW>(y, trials, N, lg);
 }
 
 // with a group effect: D + G columns, X split
@@ -97,21 +62,20 @@ __global__ void __launch_bounds__(tcf::Cfg<DC, true>::kThreads, 1)
 glm_binomial_group_tc_kernel(const float* __restrict__ X, const float* __restrict__ y,
                              const float* __restrict__ trials, const float* __restrict__ W,
                              const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
-                             float* __restrict__ lg, const int32_t* __restrict__ groups, int G) {
+                             const int32_t* __restrict__ groups, int G) {
   tcf::glm_flat_pipeline<Binomial<ROW>, DC, true, true>(X, y, W, bvec, N, D, P, partials, trials, groups, G);
-  if (blockIdx.y == 0) lbinom_partial<tcf::Cfg<DC, true>::kThreads, ROW>(y, trials, N, lg);
 }
 
 template <bool ROW>
 int launch(const float* X, const float* y, const float* m, const float* W, const float* b, int64_t N, int D, int P,
-           float* partials, float* lg, int gx, bool split_x, cudaStream_t s, GlmGroups grp) {
+           float* partials, int gx, bool split_x, cudaStream_t s, GlmGroups grp) {
   const dim3 grid = slab_grid(gx, P);
   // D + G < 32 runs the two-atom loop too (see below)
   if (grp.idx)
     return glm_dispatch_dc<2>(D + grp.G, true, [&](auto dc, auto) {
       using C = tcf::Cfg<decltype(dc)::value, true>;
       return launch_tc(glm_binomial_group_tc_kernel<ROW, decltype(dc)::value>, grid, dim3(C::kThreads),
-                       C::kSmemBytes, s, X, y, m, W, b, N, D, P, partials, lg, grp.idx, grp.G);
+                       C::kSmemBytes, s, X, y, m, W, b, N, D, P, partials, grp.idx, grp.G);
     });
   if (D == 32) {
     using namespace tile32;
@@ -122,16 +86,16 @@ int launch(const float* X, const float* y, const float* m, const float* W, const
     if (!ROW) mm = my;                           // not read
     constexpr uint32_t kSmemBytes = Smem32<Fam::kYBytes>::kBytes;
     return split_x ? launch_tc(glm_binomial_tc_kernel<ROW, true>, grid, dim3(kThreads), kSmemBytes, s, mx, my, mm, y,
-                               m, W, b, N, P, partials, lg)
+                               m, W, b, N, P, partials)
                    : launch_tc(glm_binomial_tc_kernel<ROW, false>, grid, dim3(kThreads), kSmemBytes, s, mx, my, mm, y,
-                               m, W, b, N, P, partials, lg);
+                               m, W, b, N, P, partials);
   }
   // D < 32 runs the two-atom loop (two warpgroups, 255 registers): with one atom and four warpgroups the
   // 128-register cap made this epilogue spill
   return glm_dispatch_dc<2>(D, split_x, [&](auto dc, auto sx) {
     using C = tcf::Cfg<decltype(dc)::value>;
     return launch_tc(glm_binomial_flat_tc_kernel<ROW, decltype(dc)::value, decltype(sx)::value>, grid,
-                     dim3(C::kThreads), C::kSmemBytes, s, X, y, m, W, b, N, D, P, partials, lg);
+                     dim3(C::kThreads), C::kSmemBytes, s, X, y, m, W, b, N, D, P, partials);
   });
 }
 
@@ -140,7 +104,7 @@ int launch(const float* X, const float* y, const float* m, const float* W, const
 
 using namespace b2;
 
-extern "C" size_t b2_glm_binomial_workspace(int64_t N, int D, int P) { return glm_row_workspace(N, D, P, true); }
+extern "C" size_t b2_glm_binomial_workspace(int64_t N, int D, int P) { return glm_row_workspace(N, D, P); }
 
 int b2::glm_binomial_logits(const float* X, const float* y, const float* trials, int trials_per_row, const float* W,
                             const float* b, int64_t N, int D, int P, double scale, double weight, double sum_coeff,
@@ -148,16 +112,16 @@ int b2::glm_binomial_logits(const float* X, const float* y, const float* trials,
                             void* workspace, size_t workspace_bytes, cudaStream_t s, GlmGroups grp) {
   const bool bad_trials = (trials_per_row != 0 && trials_per_row != 1) ||
                           (trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0);
-  int rc = glm_row_check(X, y, W, !trials, N, D, P, bad_trials, flags, workspace, workspace_bytes, true, grp);
+  int rc = glm_row_check(X, y, W, !trials, N, D, P, bad_trials, flags, workspace, workspace_bytes, grp);
   if (rc != B2_OK) return rc;
   const int Da = D + (grp.idx ? grp.G : 0);
-  const GlmRowWorkspace w = glm_row_areas(workspace, N, Da, P, true);
+  const GlmRowWorkspace w = glm_row_areas(workspace, N, Da, P);
   const bool split_x = glm_split_x(flags, N);
-  rc = trials_per_row ? tcbi::launch<true>(X, y, trials, W, b, N, D, P, w.partials, w.lg, w.gx, split_x, s, grp)
-                      : tcbi::launch<false>(X, y, trials, W, b, N, D, P, w.partials, w.lg, w.gx, split_x, s, grp);
+  rc = trials_per_row ? tcbi::launch<true>(X, y, trials, W, b, N, D, P, w.partials, w.gx, split_x, s, grp)
+                      : tcbi::launch<false>(X, y, trials, W, b, N, D, P, w.partials, w.gx, split_x, s, grp);
   if (rc != 0) return rc;
   launch_glm_finish(w.partials, w.ticket, w.gx, P, 1, Da, scale, weight, sum_coeff, flags, out_sum_p, out_total,
-                    out_dW, out_db, w.lg, s);
+                    out_dW, out_db, s);
   count_launch(2);
   return check_launch();
 }

@@ -64,6 +64,8 @@ template <int KP>
 struct Softmax {
   static_assert(KP == 2 || KP == 4 || KP == 8 || KP == 16, "class padding");
   static constexpr int kTrials = kNoTrials;
+  using LpAcc = float;
+  static constexpr bool kDataTerm = false;
   static constexpr bool kBiasInEpilogue = false;
   static constexpr int kKP = KP;
   static constexpr uint32_t kYBytes = kRows * 8;  // 512 B of int64 labels
@@ -203,7 +205,7 @@ extern "C" int b2_glm_categorical_logits(const float* X, const int64_t* y, const
   }
   if (rc != 0) return rc;
   launch_glm_finish(partials, ticket, gx, P, K, kD, scale, weight, sum_coeff, flags, out_sum_p, out_total, out_dW,
-                    out_db, nullptr, s);
+                    out_db, s);
   count_launch(2);
   return check_launch();
 }

@@ -77,11 +77,12 @@ struct Cfg {
   static constexpr uint32_t OFF_WG = OFF_WLO + kOp;
   static constexpr uint32_t OFF_BAR = OFF_WG + kWG * kWGBytes;
   static constexpr uint32_t kSmemBytes = OFF_BAR + 64 + 1024;  // + slack for the 1024-byte alignment
-  // the final reduction reuses the warpgroup regions: [kWG][64 p][KD + 1] + [kWG][64 p] floats
+  // the final reduction reuses the warpgroup regions: [kWG][64 p][KD + 1] floats + [kWG][64 p] lp sums (at most
+  // fp64)
   static constexpr int kRS = kKD + 1;
   static_assert(kSmemBytes <= 232448, "shared memory budget");
   static_assert(kXtBlock % 1024 == 0 && kWGBytes % 1024 == 0, "operand alignment");
-  static_assert((kWG * kM * kRS + kWG * kM) * 4 <= kWG * kWGBytes, "reduction scratch");
+  static_assert(kWG * kM * kRS * 4 + kWG * kM * 8 <= kWG * kWGBytes, "reduction scratch");
 };
 
 // one 1-D bulk copy global -> shared, completing `bytes` (a non-zero multiple of 16) on the mbarrier
@@ -129,7 +130,7 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
   fence_proxy_async();
   __syncthreads();
 
-  float lpa[2] = {0.f, 0.f};                   // lp sums of the thread's two particles
+  typename Fam::LpAcc lpa[2] = {0, 0};         // lp sums of the thread's two particles
   // GEMM 2 accumulator [p][c]: dW in c < D, db in c = KD.  Started by the warpgroup's first GEMM 2 k-step
   // with scale-d = 0, never written by ordinary instructions before the tile loop (C7515, see glm_tc.cu).
   float acc2[C::kN2 / 2];
@@ -278,15 +279,17 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
     fence_regs(acc2);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      float v = lpa[h];
+      auto v = lpa[h];
       v += __shfl_xor_sync(0xffffffffu, v, 1);
       v += __shfl_xor_sync(0xffffffffu, v, 2);
       lpa[h] = v;
     }
   }
+  double dterm = 0.0;
+  if constexpr (Fam::kDataTerm) dterm = Fam::template data_term<C::kThreads>(y, trials, N);
   // CTA results through the warpgroup regions, idle now
   cta_partials<1, C::kN2, C::kThreads>(reinterpret_cast<float*>(sm + C::OFF_WG), acc2, lpa, wg, nt, slab, P, 1, Da,
-                                       partials);
+                                       partials, dterm);
 }
 
 }  // namespace tcf

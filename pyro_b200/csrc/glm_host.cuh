@@ -20,12 +20,11 @@ struct GlmGroups {
 
 // ---- glm.cu ----
 // The second launch of every GLM likelihood call: glm_finish_kernel over the CTA partials [gx][P][K (D + 1) + 1].
-// lg (one more partial per CTA that every particle's sum subtracts) and the Normal noise scale sigma[p *
-// sigma_stride] with n = N rows and out_dsigma are optional.  The per-particle sums go to out_sum_p, or without
-// one to the [P] row of the workspace after the partials.
+// The Normal noise scale sigma[p * sigma_stride] with n = N rows and out_dsigma are optional.  The per-particle sums
+// go to out_sum_p, or without one to the [P] row of the workspace after the partials.
 void launch_glm_finish(const float* partials, unsigned int* ticket, int gx, int P, int K, int D, double scale,
                        double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
-                       float* out_dW, float* out_db, const float* lg, cudaStream_t s, const float* sigma = nullptr,
+                       float* out_dW, float* out_db, cudaStream_t s, const float* sigma = nullptr,
                        int sigma_stride = 0, int64_t n = 0, float* out_dsigma = nullptr);
 
 // ---- glm_tc.cu ----
@@ -90,27 +89,24 @@ int glm_dispatch_dc(int D, bool split_x, F&& f) {
 }
 
 // ---- the per-row entry points: b2_glm_poisson_log_rate, b2_glm_normal_loc, b2_glm_binomial_logits ----
-// workspace: [ticket, 256 B][CTA partials gx * P * (D + 2)][one [P] row for the per-particle sums], then with lg
-// the [gx] partials of the data term of the finish (Poisson, Binomial)
-inline size_t glm_row_workspace(int64_t N, int D, int P, bool with_lg) {
+// workspace: [ticket, 256 B][CTA partials gx * P * (D + 2)][one [P] row for the per-particle sums]
+inline size_t glm_row_workspace(int64_t N, int D, int P) {
   if (N < 1 || D < 1 || D > 128 || P < 1) return 256;
   const size_t gx = (size_t)glm_tc_grid_x(N);
-  return 256 + (gx * (size_t)P * (size_t)(D + 2) + (size_t)P + (with_lg ? gx : 0)) * sizeof(float);
+  return 256 + (gx * (size_t)P * (size_t)(D + 2) + (size_t)P) * sizeof(float);
 }
 
 struct GlmRowWorkspace {
   int gx;
   unsigned int* ticket;
   float* partials;
-  float* lg;          // null without lg
 };
 
-inline GlmRowWorkspace glm_row_areas(void* workspace, int64_t N, int D, int P, bool with_lg) {
+inline GlmRowWorkspace glm_row_areas(void* workspace, int64_t N, int D, int P) {
   GlmRowWorkspace w;
   w.gx = glm_tc_grid_x(N);
   w.ticket = reinterpret_cast<unsigned int*>(workspace);
   w.partials = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  w.lg = with_lg ? w.partials + (size_t)w.gx * P * (D + 2) + P : nullptr;
   return w;
 }
 
@@ -119,7 +115,7 @@ inline GlmRowWorkspace glm_row_areas(void* workspace, int64_t N, int D, int P, b
 // arrive by TMA / bulk copies (16-byte aligned sources, 32-bit row coordinates), and these families have no fp32
 // SIMT kernel.  With a group effect D + G columns must fit and the workspace is theirs.
 inline int glm_row_check(const float* X, const float* y, const float* W, bool null_operand, int64_t N, int D, int P,
-                         bool bad_operand, int flags, const void* workspace, size_t workspace_bytes, bool with_lg,
+                         bool bad_operand, int flags, const void* workspace, size_t workspace_bytes,
                          GlmGroups grp = {}) {
   if (!X || !y || !W || null_operand) return B2_ERR_NULL;
   const int Da = D + (grp.idx ? grp.G : 0);
@@ -128,7 +124,7 @@ inline int glm_row_check(const float* X, const float* y, const float* W, bool nu
   if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
   if (flags & B2_FLAG_GLM_FP32) return B2_ERR_BAD_SHAPE;
   if (N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
-  if (!workspace || workspace_bytes < glm_row_workspace(N, Da, P, with_lg)) return B2_ERR_WORKSPACE;
+  if (!workspace || workspace_bytes < glm_row_workspace(N, Da, P)) return B2_ERR_WORKSPACE;
   return B2_OK;
 }
 

@@ -98,21 +98,21 @@ int launch(const float* X, const float* y, const float* W, const float* b, int64
 
 using namespace b2;
 
-extern "C" size_t b2_glm_normal_workspace(int64_t N, int D, int P) { return glm_row_workspace(N, D, P, false); }
+extern "C" size_t b2_glm_normal_workspace(int64_t N, int D, int P) { return glm_row_workspace(N, D, P); }
 
 int b2::glm_normal_loc(const float* X, const float* y, const float* W, const float* b, const float* sigma,
                        int sigma_stride, int64_t N, int D, int P, double scale, double weight, double sum_coeff,
                        int flags, float* out_sum_p, float* out_total, float* out_dW, float* out_db, float* out_dsigma,
                        void* workspace, size_t workspace_bytes, cudaStream_t s, GlmGroups grp) {
   int rc = glm_row_check(X, y, W, !sigma, N, D, P, sigma_stride != 0 && sigma_stride != 1, flags, workspace,
-                         workspace_bytes, false, grp);
+                         workspace_bytes, grp);
   if (rc != B2_OK) return rc;
   const int Da = D + (grp.idx ? grp.G : 0);
-  const GlmRowWorkspace w = glm_row_areas(workspace, N, Da, P, false);
+  const GlmRowWorkspace w = glm_row_areas(workspace, N, Da, P);
   rc = tcn::launch(X, y, W, b, N, D, P, w.partials, w.gx, s, grp);
   if (rc != 0) return rc;
   launch_glm_finish(w.partials, w.ticket, w.gx, P, 1, Da, scale, weight, sum_coeff, flags, out_sum_p, out_total,
-                    out_dW, out_db, nullptr, s, sigma, sigma_stride, N, out_dsigma);
+                    out_dW, out_db, s, sigma, sigma_stride, N, out_dsigma);
   count_launch(2);
   return check_launch();
 }

@@ -13,10 +13,11 @@
 // under SPLIT_X; unlike theirs, GEMM 1 starts from zero and the epilogue adds the bias, rounded to nearest
 // (the tensor cores' truncating accumulation biases a log-rate held from the first k-step; see poisson_epilogue).
 //
-// SUM lgamma(y + 1) depends on y alone: after its tile loop each CTA of particle slab 0 sums it over the rows
-// of its own tiles (read again from L2, outside the wgmma pipeline) into one more partial, and glm_finish_kernel
-// subtracts the sum of those partials from every particle's sum.  Every sum has a fixed order; no float
-// atomics, and a call is still two launches (kernel + finish).
+// SUM lgamma(y + 1) depends on y alone: after its tile loop each CTA sums it in fp64 over the rows of its own
+// tiles (read again from L2, outside the wgmma pipeline) and subtracts it from each particle's fp64 lp sum before
+// rounding that to its fp32 partial (Poisson in glm_tc_common.cuh).  At counts of 100 a row's y l - e^l is about
+// +360 nats and its lp about -3, so the cancellation happens before anything is rounded at the scale of the
+// terms.  Every sum has a fixed order; no float atomics, and a call is still two launches (kernel + finish).
 //
 // Overflow: above l = 88.72 e^l is +inf in fp32.  Such a row's lp and g are -inf (y l - inf, y - inf), so sum_p
 // is -inf and db is -inf * weight; dW is non-finite (inf, or NaN where the row's x is zero or infinities of
@@ -35,46 +36,21 @@ namespace tcpr {
 
 using namespace tc;
 
-// lg[blockIdx.x] = SUM lgamma(y_n + 1) over the rows of the CTA's tiles (blockIdx.x, blockIdx.x + gridDim.x,
-// ...), in a fixed order; called by every thread of a CTA of slab 0 after its tile loop
-template <int NT>
-__device__ __forceinline__ void lgamma_partial(const float* __restrict__ y, int64_t N, float* __restrict__ lg) {
-  __shared__ float red[NT / 32];
-  const int64_t ntiles = (N + kRows - 1) / kRows;
-  const int nt = (int)((ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x);
-  float s = 0.f;
-  for (int64_t i = threadIdx.x; i < (int64_t)nt * kRows; i += NT) {
-    const int64_t n = (blockIdx.x + (i / kRows) * (int64_t)gridDim.x) * kRows + i % kRows;
-    if (n < N) s += ValueAux<kPoisson, float, false>::make(__ldg(y + n)).lgx;
-  }
-  s = warp_sum(s);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float v = 0.f;
-    for (int w = 0; w < NT / 32; ++w) v += red[w];
-    lg[blockIdx.x] = v;
-  }
-}
-
 // D = 32.  SPLIT_X = false (default): W split hi/lo, X rounded to nearest.  SPLIT_X = true: X split as well.
 template <bool SPLIT_X>
 __global__ void __launch_bounds__(tile32::kThreads, 1)
 glm_poisson_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_y,
                       const float* __restrict__ y, const float* __restrict__ W, const float* __restrict__ bvec,
-                      int64_t N, int P, float* __restrict__ partials, float* __restrict__ lg) {
-  tile32::glm_tile_pipeline<Poisson, SPLIT_X>(map_x, map_y, W, bvec, N, P, 1, partials);
-  if (blockIdx.y == 0) lgamma_partial<tile32::kThreads>(y, N, lg);
+                      int64_t N, int P, float* __restrict__ partials) {
+  tile32::glm_tile_pipeline<Poisson, SPLIT_X>(map_x, map_y, W, bvec, N, P, 1, partials, nullptr, nullptr, y);
 }
 
 // every other D in 1..128, padded to DC atoms of 32 columns
 template <int DC, bool SPLIT_X>
 __global__ void __launch_bounds__(tcf::Cfg<DC>::kThreads, 1)
 glm_poisson_flat_tc_kernel(const float* __restrict__ X, const float* __restrict__ y, const float* __restrict__ W,
-                           const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
-                           float* __restrict__ lg) {
+                           const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials) {
   tcf::glm_flat_pipeline<Poisson, DC, SPLIT_X>(X, y, W, bvec, N, D, P, partials);
-  if (blockIdx.y == 0) lgamma_partial<tcf::Cfg<DC>::kThreads>(y, N, lg);
 }
 
 // with a group effect: D + G columns, X split
@@ -82,19 +58,18 @@ template <int DC>
 __global__ void __launch_bounds__(tcf::Cfg<DC, true>::kThreads, 1)
 glm_poisson_group_tc_kernel(const float* __restrict__ X, const float* __restrict__ y, const float* __restrict__ W,
                             const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
-                            float* __restrict__ lg, const int32_t* __restrict__ groups, int G) {
+                            const int32_t* __restrict__ groups, int G) {
   tcf::glm_flat_pipeline<Poisson, DC, true, true>(X, y, W, bvec, N, D, P, partials, nullptr, groups, G);
-  if (blockIdx.y == 0) lgamma_partial<tcf::Cfg<DC, true>::kThreads>(y, N, lg);
 }
 
 int launch(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
-           float* partials, float* lg, int gx, bool split_x, cudaStream_t s, GlmGroups grp) {
+           float* partials, int gx, bool split_x, cudaStream_t s, GlmGroups grp) {
   const dim3 grid = slab_grid(gx, P);
   if (grp.idx)
     return glm_dispatch_dc<1>(D + grp.G, true, [&](auto dc, auto) {
       using C = tcf::Cfg<decltype(dc)::value, true>;
       return launch_tc(glm_poisson_group_tc_kernel<decltype(dc)::value>, grid, dim3(C::kThreads), C::kSmemBytes, s,
-                       X, y, W, b, N, D, P, partials, lg, grp.idx, grp.G);
+                       X, y, W, b, N, D, P, partials, grp.idx, grp.G);
     });
   if (D == 32) {
     using namespace tile32;
@@ -102,14 +77,14 @@ int launch(const float* X, const float* y, const float* W, const float* b, int64
     if (!encode_x_map(&mx, X, N) || !encode_label_map(&my, y, N, Poisson::kYType)) return B2_ERR_LAUNCH;
     constexpr uint32_t kSmemBytes = Smem32<Poisson::kYBytes>::kBytes;
     return split_x ? launch_tc(glm_poisson_tc_kernel<true>, grid, dim3(kThreads), kSmemBytes, s, mx, my, y, W, b, N,
-                               P, partials, lg)
+                               P, partials)
                    : launch_tc(glm_poisson_tc_kernel<false>, grid, dim3(kThreads), kSmemBytes, s, mx, my, y, W, b, N,
-                               P, partials, lg);
+                               P, partials);
   }
   return glm_dispatch_dc<1>(D, split_x, [&](auto dc, auto sx) {
     using C = tcf::Cfg<decltype(dc)::value>;
     return launch_tc(glm_poisson_flat_tc_kernel<decltype(dc)::value, decltype(sx)::value>, grid, dim3(C::kThreads),
-                     C::kSmemBytes, s, X, y, W, b, N, D, P, partials, lg);
+                     C::kSmemBytes, s, X, y, W, b, N, D, P, partials);
   });
 }
 
@@ -118,20 +93,20 @@ int launch(const float* X, const float* y, const float* W, const float* b, int64
 
 using namespace b2;
 
-extern "C" size_t b2_glm_poisson_workspace(int64_t N, int D, int P) { return glm_row_workspace(N, D, P, true); }
+extern "C" size_t b2_glm_poisson_workspace(int64_t N, int D, int P) { return glm_row_workspace(N, D, P); }
 
 int b2::glm_poisson_log_rate(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
                              double scale, double weight, double sum_coeff, int flags, float* out_sum_p,
                              float* out_total, float* out_dW, float* out_db, void* workspace, size_t workspace_bytes,
                              cudaStream_t s, GlmGroups grp) {
-  int rc = glm_row_check(X, y, W, false, N, D, P, false, flags, workspace, workspace_bytes, true, grp);
+  int rc = glm_row_check(X, y, W, false, N, D, P, false, flags, workspace, workspace_bytes, grp);
   if (rc != B2_OK) return rc;
   const int Da = D + (grp.idx ? grp.G : 0);
-  const GlmRowWorkspace w = glm_row_areas(workspace, N, Da, P, true);
-  rc = tcpr::launch(X, y, W, b, N, D, P, w.partials, w.lg, w.gx, glm_split_x(flags, N), s, grp);
+  const GlmRowWorkspace w = glm_row_areas(workspace, N, Da, P);
+  rc = tcpr::launch(X, y, W, b, N, D, P, w.partials, w.gx, glm_split_x(flags, N), s, grp);
   if (rc != 0) return rc;
   launch_glm_finish(w.partials, w.ticket, w.gx, P, 1, Da, scale, weight, sum_coeff, flags, out_sum_p, out_total,
-                    out_dW, out_db, w.lg, s);
+                    out_dW, out_db, s);
   count_launch(2);
   return check_launch();
 }

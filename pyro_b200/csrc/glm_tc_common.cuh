@@ -7,6 +7,7 @@
 #include <cuda.h>
 
 #include "b2_common.cuh"
+#include "b2_math.cuh"
 
 namespace b2 {
 namespace tc {
@@ -322,6 +323,9 @@ __device__ __forceinline__ void bernoulli_epilogue(const float (&acc1)[32], cons
 // lp = y*l - e^l (the parameter-free -lgamma(y + 1) is summed once per call, not here) and g = y - e^l rounded
 // to nearest TF32: ONE MUFU op (ex2) per logit.  MASK (the last, partial tile only) zeroes rows past N.
 // Above l = 88.72 e^l is +inf: lp and g are then -inf, never NaN.
+// lpa is fp64 (see Poisson): a row's y*l - e^l is hundreds of nats at counts of 100 and cancels against lgamma(y + 1)
+// to a few, so the sum over a thread's tiles must not round at the scale of the terms; the 16 rows of one tile are
+// still summed in fp32.
 // The bias is added here, rounded to nearest, not carried by GEMM 1's accumulator: the tensor cores truncate
 // each fp32 accumulation, and from an accumulator of |b| (a log-rate of a few units) every k-step shifts l
 // toward zero by about half an ulp of b.  That shift enters the sum as SUM (y - e^l) dl, which does not cancel
@@ -330,7 +334,7 @@ __device__ __forceinline__ void bernoulli_epilogue(const float (&acc1)[32], cons
 template <bool MASK>
 __device__ __forceinline__ void poisson_epilogue(const float (&acc1)[32], const float (&bias)[2],
                                                  const float2 (&yr)[8], int64_t row0, int64_t N, int t4,
-                                                 float (&lpa)[2], uint32_t (&g)[32]) {
+                                                 double (&lpa)[2], uint32_t (&g)[32]) {
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     float s[2] = {0.f, 0.f};                    // two chains of adds (k-blocks j even / odd)
@@ -350,7 +354,7 @@ __device__ __forceinline__ void poisson_epilogue(const float (&acc1)[32], const 
         s[j & 1] += lp;
         g[i] = __float_as_uint(tf32_rn(gg));
       }
-    lpa[h] += s[0] + s[1];
+    lpa[h] += (double)(s[0] + s[1]);
   }
 }
 
@@ -385,14 +389,14 @@ __device__ __forceinline__ void normal_epilogue(const float (&acc1)[32], const f
 // lp = y*l - m*softplus(l) (the parameter-free log binomial coefficient is summed once per call, not here) and
 // g = y - m*sigmoid(l) rounded to nearest TF32, for y successes out of m trials: ex2, rcp and lg2 per logit.  The
 // linear part is y*l for l < 0 and (y - m)*l otherwise, exact for integer counts.  y and m are read from shared
-// memory here (ROW: one m per row, else the count mc of every row).  The bias is added here, as in
+// memory here (ROW: one m per row, else the count mc of every row).  The bias is added here and lpa is fp64, as in
 // poisson_epilogue.  MASK (the last, partial tile only) zeroes rows past N.
 // (The running product of epi_batch, one lg2 per particle and tile for one count of every row, made the 128-register
 // kernels spill.)
 template <bool MASK, bool ROW>
 __device__ __forceinline__ void binomial_epilogue(const float (&acc1)[32], const float (&bias)[2],
                                                   const float2* yr, const float2* mr, float mc, int64_t row0,
-                                                  int64_t N, int t4, float (&lpa)[2], uint32_t (&g)[32]) {
+                                                  int64_t N, int t4, double (&lpa)[2], uint32_t (&g)[32]) {
   // k-block outermost: the labels of a k-block serve both particles of the thread and are dead after it
   float s[2] = {0.f, 0.f};
 #pragma unroll
@@ -418,8 +422,29 @@ __device__ __forceinline__ void binomial_epilogue(const float (&acc1)[32], const
         g[i] = __float_as_uint(tf32_rn(gg));
       }
   }
-  lpa[0] += s[0];
-  lpa[1] += s[1];
+  lpa[0] += (double)s[0];
+  lpa[1] += (double)s[1];
+}
+
+// SUM f(n) over the rows n < N of the CTA's tiles (blockIdx.x, blockIdx.x + gridDim.x, ...), in fp64 and a fixed
+// order; called by every thread of the CTA, each of which gets the sum
+template <int NT, class F>
+__device__ __forceinline__ double cta_row_sum(int64_t N, F f) {
+  __shared__ double red[NT / 32];
+  const int64_t ntiles = (N + kRows - 1) / kRows;
+  const int nt = (int)((ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x);
+  double s = 0.0;
+  for (int64_t i = threadIdx.x; i < (int64_t)nt * kRows; i += NT) {
+    const int64_t n = (blockIdx.x + (i / kRows) * (int64_t)gridDim.x) * kRows + i % kRows;
+    if (n < N) s += f(n);
+  }
+  s = warp_sum(s);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  double v = 0.0;
+#pragma unroll
+  for (int w = 0; w < NT / 32; ++w) v += red[w];
+  return v;
 }
 
 // ---- likelihood families of the GLM tile pipelines ----------------------------------------------------------
@@ -430,12 +455,18 @@ __device__ __forceinline__ void binomial_epilogue(const float (&acc1)[32], const
 // of the thread's two rows to lpa; the any-D tile loop (glm_flat_tc.cuh) calls tile_epilogue(acc1, labels,
 // row0, N, t4, last, lpa, g) instead.  kTrials (Binomial only) adds a second label operand, the trial counts:
 // one device value for every row (kConstTrials) or one per row (kRowTrials, loaded next to y on the same
-// mbarrier); read_trials(stage + 256, t4, m, labels) then completes the labels.
+// mbarrier); read_trials(stage + 256, t4, m, labels) then completes the labels.  LpAcc is the type of the lp sums
+// lpa.  kDataTerm families (Poisson, Binomial) leave a parameter-free term of each row's lp out of the tile loop:
+// data_term<NT>(y, trials, N) is its fp64 sum over the CTA's rows, which cta_partials subtracts from every
+// particle's fp64 lp sum before rounding it to the fp32 partial.  So the partial is of the size of the lp sum, not
+// of its terms, and glm_finish_kernel adds no data term.
 enum : int { kNoTrials = 0, kConstTrials = 1, kRowTrials = 2 };
 
 // logistic regression: one GEMM 1 row per particle, fp32 labels y
 struct Bernoulli {
   static constexpr int kTrials = kNoTrials;
+  using LpAcc = float;
+  static constexpr bool kDataTerm = false;
   static constexpr bool kBiasInEpilogue = false;  // GEMM 1's accumulator starts at the bias
   static constexpr int kKP = 1;
   static constexpr uint32_t kYBytes = kRows * 4;  // 256 B of y
@@ -460,12 +491,18 @@ struct Bernoulli {
 };
 
 // Poisson regression (log link): the labels of Bernoulli, fp32 counts y
-// (GEMM 1 starts from zero and the epilogue adds the bias, see poisson_epilogue)
+// (GEMM 1 starts from zero and the epilogue adds the bias, see poisson_epilogue); the data term is SUM lgamma(y + 1)
 struct Poisson : Bernoulli {
   static constexpr bool kBiasInEpilogue = true;
+  using LpAcc = double;
+  static constexpr bool kDataTerm = true;
+  template <int NT>
+  static __device__ __forceinline__ double data_term(const float* __restrict__ y, const float*, int64_t N) {
+    return cta_row_sum<NT>(N, [&](int64_t n) { return log_factorial_f64(__ldg(y + n)); });
+  }
   static __device__ __forceinline__ void tile_epilogue(const float (&acc1)[32], const float (&bias)[2],
                                                        const Labels& y, int64_t row0, int64_t N, int t4, bool last,
-                                                       float (&lpa)[2], uint32_t (&g)[32]) {
+                                                       double (&lpa)[2], uint32_t (&g)[32]) {
     if (last)
       poisson_epilogue<true>(acc1, bias, y, row0, N, t4, lpa, g);
     else
@@ -473,7 +510,7 @@ struct Poisson : Bernoulli {
   }
   static __device__ __forceinline__ void epilogue(const float (&acc1)[32], const float (&bias)[2], const Labels& y,
                                                   const int (&)[2], int, int64_t row0, int64_t N, int t4,
-                                                  float (&lpa)[2], uint32_t (&g)[32]) {
+                                                  double (&lpa)[2], uint32_t (&g)[32]) {
     tile_epilogue(acc1, bias, y, row0, N, t4, row0 + kRows > N, lpa, g);
   }
 };
@@ -499,11 +536,23 @@ struct Normal : Bernoulli {
 
 // Binomial regression (logit link): fp32 successes y and trial counts m, one for every row (ROW = false, a
 // device value read once per call) or one per row (ROW: [N] fp32, loaded next to y).  GEMM 1 starts from zero
-// and the epilogue adds the bias, see binomial_epilogue.
+// and the epilogue adds the bias, see binomial_epilogue.  The data term is -SUM log C(m, y).
 template <bool ROW>
 struct Binomial : Bernoulli {
   static constexpr int kTrials = ROW ? kRowTrials : kConstTrials;
   static constexpr bool kBiasInEpilogue = true;
+  using LpAcc = double;
+  static constexpr bool kDataTerm = true;
+  template <int NT>
+  static __device__ __forceinline__ double data_term(const float* __restrict__ y, const float* __restrict__ trials,
+                                                     int64_t N) {
+    const float mc = ROW ? 0.f : __ldg(trials);
+    const double lgm = ROW ? 0.0 : log_factorial_f64(mc);
+    return cta_row_sum<NT>(N, [&](int64_t n) {
+      const float yv = __ldg(y + n), m = ROW ? __ldg(trials + n) : mc;
+      return (log_factorial_f64(yv) + log_factorial_f64(m - yv)) - (ROW ? log_factorial_f64(m) : lgm);
+    });
+  }
   static constexpr uint32_t kYBytes = (ROW ? 2 : 1) * kRows * 4;   // y, then the trials of the tile
   // The labels stay in shared memory until the epilogue reads them (y and m of the thread's rows n = 8j + 2 t4 + e
   // at y[4j], m[4j]): held in registers across GEMM 1 they made the 128-register kernels spill.  So the tile
@@ -523,7 +572,7 @@ struct Binomial : Bernoulli {
   }
   static __device__ __forceinline__ void tile_epilogue(const float (&acc1)[32], const float (&bias)[2],
                                                        const Labels& lab, int64_t row0, int64_t N, int t4,
-                                                       bool last, float (&lpa)[2], uint32_t (&g)[32]) {
+                                                       bool last, double (&lpa)[2], uint32_t (&g)[32]) {
     if (last)
       binomial_epilogue<true, ROW>(acc1, bias, lab.y, lab.m, lab.mc, row0, N, t4, lpa, g);
     else
@@ -531,7 +580,7 @@ struct Binomial : Bernoulli {
   }
   static __device__ __forceinline__ void epilogue(const float (&acc1)[32], const float (&bias)[2],
                                                   const Labels& lab, const int (&)[2], int, int64_t row0,
-                                                  int64_t N, int t4, float (&lpa)[2], uint32_t (&g)[32]) {
+                                                  int64_t N, int t4, double (&lpa)[2], uint32_t (&g)[32]) {
     tile_epilogue(acc1, bias, lab, row0, N, t4, row0 + kRows > N, lpa, g);
   }
 };
@@ -606,16 +655,17 @@ __device__ __forceinline__ void gemm2(float (&acc2)[N2 / 2], uint32_t (&g)[32], 
 }
 
 // CTA results through the idle shared memory red, in a fixed summation order: [NT / 128][64 m][KD + 1] GEMM 2
-// accumulators (dW in columns < D, db in column KD) and [NT / 128][64 m] lp sums (lpa already summed over the
-// four lanes of a row), then each row summed over the warpgroups that had a tile.  The CTA's partials are
-// [P][K (D + 1) + 1]: per class dW[0..D-1] and db, then the particle's lp sum.
-template <int KP, int N2, int NT>
-__device__ __forceinline__ void cta_partials(float* red, const float (&acc2)[N2 / 2], const float (&lpa)[2], int wg,
-                                             int nt, int slab, int P, int K, int D, float* partials) {
+// accumulators (dW in columns < D, db in column KD) and [NT / 128][64 m] lp sums of type A (lpa already summed
+// over the four lanes of a row), then each row summed over the warpgroups that had a tile.  The CTA's partials are
+// [P][K (D + 1) + 1]: per class dW[0..D-1] and db, then the particle's lp sum, less dterm (fp64 lp sums only).
+template <int KP, int N2, int NT, typename A>
+__device__ __forceinline__ void cta_partials(float* red, const float (&acc2)[N2 / 2], const A (&lpa)[2], int wg,
+                                             int nt, int slab, int P, int K, int D, float* partials,
+                                             double dterm = 0.0) {
   constexpr int KD = N2 - 8, kWG = NT / 128;
   const int tid = threadIdx.x, w4 = (tid >> 5) & 3, gid = (tid & 31) >> 2, t4 = tid & 3;
   float* red2 = red;
-  float* redlp = red2 + kWG * kM * (KD + 1);
+  A* redlp = reinterpret_cast<A*>(red2 + kWG * kM * (KD + 1));   // 8-byte aligned: kM * (KD + 1) is even
   __syncthreads();
 #pragma unroll
   for (int j = 0; j < N2 / 8; ++j)
@@ -643,10 +693,11 @@ __device__ __forceinline__ void cta_partials(float* red, const float (&acc2)[N2 
     }
   }
   if (tid < kM / KP && slab * (kM / KP) + tid < P) {
-    float v = 0.f;
+    A v = 0;
     for (int q = 0; q < nwg; ++q)
       for (int k = 0; k < KP; ++k) v += redlp[q * kM + tid * KP + k];
-    partials[((int64_t)blockIdx.x * P + slab * (kM / KP) + tid) * S + K * (D + 1)] = v;
+    if constexpr (sizeof(A) == 8) v -= dterm;
+    partials[((int64_t)blockIdx.x * P + slab * (kM / KP) + tid) * S + K * (D + 1)] = (float)v;
   }
 }
 
@@ -680,17 +731,18 @@ struct Smem32 {
   static constexpr uint32_t kBytes = OFF_BAR + 256 + 1024;   // + slack for the 1024-byte alignment
   static_assert(kBytes <= 232448, "shared memory budget");
   static_assert(OFF_WHI % 1024 == 0 && kWGBytes % 1024 == 0 && kXtBlock % 1024 == 0, "operand alignment");
-  // the final reduction reuses the X ring: [kWG][64 m][33] + [kWG][64 m] floats
-  static_assert((kWG * kM * 33 + kWG * kM) * 4 <= kStages * kTile, "reduction scratch");
+  // the final reduction reuses the X ring: [kWG][64 m][33] floats + [kWG][64 m] lp sums (at most fp64)
+  static_assert(kWG * kM * 33 * 4 + kWG * kM * 8 <= kStages * kTile, "reduction scratch");
 };
 
 // Fam is the likelihood family (Bernoulli, Poisson, Normal, Binomial above, Softmax of glm_categorical_tc.cu).
-// Binomial only: map_m is the trials' label map (kRowTrials), trials the one device count (kConstTrials).
+// Binomial only: map_m is the trials' label map (kRowTrials), trials the trial counts (one device count for
+// kConstTrials).  y, the labels in global memory, is read by the data term of kDataTerm families only.
 template <class Fam, bool SPLIT_X>
 __device__ __forceinline__ void glm_tile_pipeline(const CUtensorMap& map_x, const CUtensorMap& map_y,
                                                   const float* W, const float* bvec, int64_t N, int P, int K,
                                                   float* partials, const CUtensorMap* map_m = nullptr,
-                                                  const float* trials = nullptr) {
+                                                  const float* trials = nullptr, const float* y = nullptr) {
   using L = Smem32<Fam::kYBytes>;
   constexpr int KP = Fam::kKP;
   constexpr uint32_t kYBytes = Fam::kYBytes;
@@ -739,7 +791,7 @@ __device__ __forceinline__ void glm_tile_pipeline(const CUtensorMap& map_x, cons
   fence_proxy_async();
   __syncthreads();
 
-  float lpa[2] = {0.f, 0.f};                   // lp sums of the thread's two rows
+  typename Fam::LpAcc lpa[2] = {0, 0};         // lp sums of the thread's two rows
   // GEMM 2 accumulator [m][c]: dW in c < 32, db in c = 32.  Never written by ordinary instructions before
   // the tile loop (C7515): the warpgroup's first GEMM 2 k-step starts it with scale-d = 0, and a warpgroup
   // without a tile is left out of the CTA reduction.
@@ -842,14 +894,16 @@ __device__ __forceinline__ void glm_tile_pipeline(const CUtensorMap& map_x, cons
     fence_regs(acc2);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      float v = lpa[h];
+      auto v = lpa[h];
       v += __shfl_xor_sync(0xffffffffu, v, 1);
       v += __shfl_xor_sync(0xffffffffu, v, 2);
       lpa[h] = v;
     }
   }
+  double dterm = 0.0;
+  if constexpr (Fam::kDataTerm) dterm = Fam::template data_term<kThreads>(y, trials, N);
   cta_partials<KP, kD + 8, kThreads>(reinterpret_cast<float*>(sm + L::OFF_X), acc2, lpa, wg, nt, slab, P, K, kD,
-                                     partials);
+                                     partials, dterm);
 }
 
 }  // namespace tile32
