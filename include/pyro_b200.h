@@ -602,6 +602,34 @@ int b2_glm_group_potential(int kind, const float* X, const void* y, const float*
                            size_t workspace_bytes, void* stream);
 size_t b2_glm_group_potential_workspace(int kind, int64_t N, int D, int G, int64_t C);
 
+/*
+ * b2_glm_group_sum -- the fused likelihood term of a regression with a varying intercept by group, for P particles:
+ *   eta[p,n] = <X[n,:], W[p,:]> + b[p] + alpha[p, groups[n]]
+ * scored as b2_glm_bernoulli_logits / b2_glm_poisson_log_rate / b2_glm_normal_loc / b2_glm_binomial_logits score
+ * their eta (kind B2_GLM_BERNOULLI, B2_GLM_POISSON, B2_GLM_NORMAL or B2_GLM_BINOMIAL; Categorical is refused), with
+ * their outputs, and out_dW [P][D + G] whose columns D .. D+G-1 are the derivatives with respect to alpha[p, :].
+ * The group effect is G more columns of the one tensor-core pass over [X | onehot(groups)], so X is read once and no
+ * [P, N] tensor is written.  X: [N, D] fp32 row-major, y: [N] fp32, both 16-byte aligned; trials / trials_per_row as
+ * for b2_glm_binomial_logits (Binomial only); sigma / sigma_stride / out_dsigma as for b2_glm_normal_loc (Normal
+ * only); groups: [N] int32, 16-byte aligned, each in [0, G) (a row outside makes sum_p and d/dalpha NaN);
+ * W: row p at W + p * w_stride (D values), alpha: row p at alpha + p * alpha_stride (G values), a stride of 0 sharing
+ * one row with every particle; b: [P] (nullable).  1 <= D, 1 <= G, D + G <= 128, N < 2^31.  Precision policy of the
+ * kind's plain entry point (Normal: X always split; the others: X rounded to TF32 from 65536 rows, split below that
+ * and with B2_FLAG_GLM_3XTF32); the one-hot columns are exact either way.  B2_FLAG_GLM_FP32 returns
+ * B2_ERR_BAD_SHAPE.  Every argument is checked before any CUDA call: B2_ERR_NULL, B2_ERR_BAD_SHAPE (kind, shapes,
+ * strides, alignment, trials_per_row, sigma_stride), B2_ERR_TOO_LARGE, B2_ERR_WORKSPACE.
+ * workspace: b2_glm_group_sum_workspace() bytes, zero-initialised ONCE by the caller.  Three launches with no host
+ * sync (CUDA graph capturable): the pack of each particle's [w | alpha] row, the kind's group kernel and
+ * glm_finish_kernel, which sums the CTA partials in a fixed order (deterministic, no float atomics).
+ */
+int b2_glm_group_sum(int kind, const float* X, const float* y, const float* trials, int trials_per_row,
+                     const float* sigma, int sigma_stride, const int32_t* groups, int G, const float* W,
+                     int64_t w_stride, const float* alpha, int64_t alpha_stride, const float* b, int64_t N, int D,
+                     int P, double scale, double weight, double sum_coeff, int flags, float* out_sum_p,
+                     float* out_total, float* out_dW, float* out_db, float* out_dsigma, void* workspace,
+                     size_t workspace_bytes, void* stream);
+size_t b2_glm_group_sum_workspace(int kind, int64_t N, int D, int G, int P);
+
 /* ---- optimisers --------------------------------------------------------------------------
  * Multi-tensor fused updates replacing PyroOptim's per-parameter Python loop
  * (pyro/optim/optim.py:117-155).  Per-tensor scalar state lives in DEVICE arrays so a captured

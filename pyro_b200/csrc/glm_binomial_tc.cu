@@ -56,7 +56,7 @@ glm_binomial_flat_tc_kernel(const float* __restrict__ X, const float* __restrict
   tcf::glm_flat_pipeline<Binomial<ROW>, DC, SPLIT_X>(X, y, W, bvec, N, D, P, partials, trials);
 }
 
-// with a group effect: D + G columns, X split
+// with a group effect: D + G columns, X split (X rounded to TF32: glm_group.cu)
 template <bool ROW, int DC>
 __global__ void __launch_bounds__(tcf::Cfg<DC, true>::kThreads, 1)
 glm_binomial_group_tc_kernel(const float* __restrict__ X, const float* __restrict__ y,
@@ -71,6 +71,8 @@ int launch(const float* X, const float* y, const float* m, const float* W, const
            float* partials, int gx, bool split_x, cudaStream_t s, GlmGroups grp) {
   const dim3 grid = slab_grid(gx, P);
   // D + G < 32 runs the two-atom loop too (see below)
+  if (grp.idx && !split_x)
+    return launch_glm_group_rn(B2_GLM_BINOMIAL, X, y, m, ROW, W, b, N, D, P, partials, gx, s, grp);
   if (grp.idx)
     return glm_dispatch_dc<2>(D + grp.G, true, [&](auto dc, auto) {
       using C = tcf::Cfg<decltype(dc)::value, true>;

@@ -23,7 +23,7 @@ glm_bernoulli_flat_tc_kernel(const float* __restrict__ X, const float* __restric
   glm_flat_pipeline<Bernoulli, DC, SPLIT_X>(X, y, W, bvec, N, D, P, partials);
 }
 
-// with a group effect: D + G columns, X split
+// with a group effect: D + G columns, X split (X rounded to TF32: glm_group.cu)
 template <int DC>
 __global__ void __launch_bounds__(Cfg<DC, true>::kThreads, 1)
 glm_bernoulli_group_tc_kernel(const float* __restrict__ X, const float* __restrict__ y, const float* __restrict__ W,
@@ -39,6 +39,8 @@ glm_bernoulli_group_tc_kernel(const float* __restrict__ X, const float* __restri
 // aligned X and y.
 int launch_glm_flat_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
                        float* partials, int gx, bool split_x, cudaStream_t s, GlmGroups grp) {
+  if (grp.idx && !split_x)
+    return launch_glm_group_rn(B2_GLM_BERNOULLI, X, y, nullptr, false, W, b, N, D, P, partials, gx, s, grp);
   if (grp.idx)
     return glm_dispatch_dc<1>(D + grp.G, true, [&](auto dc, auto) {
       using C = tcf::Cfg<decltype(dc)::value, true>;

@@ -44,7 +44,7 @@ int glm_bernoulli_logits(const float* X, const float* y, const float* W, const f
                          GlmGroups grp);
 
 // ---- glm_flat_tc.cu ----
-// Bernoulli at every other D in 1..128 on glm_flat_pipeline, and at every D with a group effect (X split)
+// Bernoulli at every other D in 1..128 on glm_flat_pipeline, and at every D with a group effect
 int launch_glm_flat_tc(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
                        float* partials, int gx, bool split_x, cudaStream_t s, GlmGroups grp = {});
 
@@ -62,6 +62,14 @@ int glm_binomial_logits(const float* X, const float* y, const float* trials, int
                         const float* b, int64_t N, int D, int P, double scale, double weight, double sum_coeff,
                         int flags, float* out_sum_p, float* out_total, float* out_dW, float* out_db, void* workspace,
                         size_t workspace_bytes, cudaStream_t s, GlmGroups grp);
+
+// ---- glm_group.cu ----
+// The group kernel of kind B2_GLM_BERNOULLI, B2_GLM_POISSON or B2_GLM_BINOMIAL (row_trials: per-row counts m) with X
+// rounded to nearest TF32, for the family launchers when glm_split_x is false; the X-split group kernels stay with
+// their families.
+int launch_glm_group_rn(int kind, const float* X, const float* y, const float* m, bool row_trials, const float* W,
+                        const float* b, int64_t N, int D, int P, float* partials, int gx, cudaStream_t s,
+                        GlmGroups grp);
 
 // Launch of a kernel that needs more than 48 KB of dynamic shared memory: 0, or B2_ERR_LAUNCH when its
 // shared-memory limit could not be raised.

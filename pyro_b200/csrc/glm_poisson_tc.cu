@@ -53,7 +53,7 @@ glm_poisson_flat_tc_kernel(const float* __restrict__ X, const float* __restrict_
   tcf::glm_flat_pipeline<Poisson, DC, SPLIT_X>(X, y, W, bvec, N, D, P, partials);
 }
 
-// with a group effect: D + G columns, X split
+// with a group effect: D + G columns, X split (X rounded to TF32: glm_group.cu)
 template <int DC>
 __global__ void __launch_bounds__(tcf::Cfg<DC, true>::kThreads, 1)
 glm_poisson_group_tc_kernel(const float* __restrict__ X, const float* __restrict__ y, const float* __restrict__ W,
@@ -65,6 +65,8 @@ glm_poisson_group_tc_kernel(const float* __restrict__ X, const float* __restrict
 int launch(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
            float* partials, int gx, bool split_x, cudaStream_t s, GlmGroups grp) {
   const dim3 grid = slab_grid(gx, P);
+  if (grp.idx && !split_x)
+    return launch_glm_group_rn(B2_GLM_POISSON, X, y, nullptr, false, W, b, N, D, P, partials, gx, s, grp);
   if (grp.idx)
     return glm_dispatch_dc<1>(D + grp.G, true, [&](auto dc, auto) {
       using C = tcf::Cfg<decltype(dc)::value, true>;

@@ -15,6 +15,7 @@ Sampling (``rsample``/``sample``) uses torch's generators; fusing it with scorin
 row of the scope table (SURVEY.md 8f rank 1).
 """
 import math
+import weakref
 from collections import namedtuple
 from numbers import Number
 
@@ -1050,15 +1051,22 @@ class LinearPredictor:
     that reads X and y once and emits sum, dW and db (``b2_glm_bernoulli_logits``) instead of
     materialising the [P, N] logits, log_prob and gradient tensors.
 
-    ``w``: [D], [P, D] or [P, 1, D] (vectorised particles);  ``b``: None, [], [P] or [P, 1]."""
+    ``w``: [D], [P, D] or [P, 1, D] (vectorised particles);  ``b``: None, [], [P] or [P, 1].
 
-    def __init__(self, X, w, b=None, tensor_cores=True):
+    ``group`` (a :class:`GroupGather`, or None): a varying intercept by group, ``+ table[..., index]``, which the
+    unchanged model added (pyro_b200/lazy.py); its table has one row, or one per particle.  ``eager`` then computes the
+    predictor the way the model wrote it, so that :meth:`dense` is that value bit for bit.  A consumer that does not
+    score the group (``_weights``) must not see such a predictor: it is scored by ``b2_glm_group_sum`` or
+    materialised."""
+
+    def __init__(self, X, w, b=None, tensor_cores=True, group=None, eager=None):
         # latent values may arrive as lazy-aware SiteValue tensors (pyro_b200/lazy.py): score plain ones
         if type(w).__name__ == "SiteValue":
             w = _ops.plain_value(w)
         if type(b).__name__ == "SiteValue":
             b = _ops.plain_value(b)
         self.X, self.w, self.b = X, w, b
+        self.group, self.eager = group, eager
         self.tensor_cores = tensor_cores  # False: fp32 SIMT contractions (B2_FLAG_GLM_FP32)
         D = X.shape[-1]
         self.vectorised = w.dim() > 1
@@ -1067,11 +1075,56 @@ class LinearPredictor:
         self.dtype, self.device = X.dtype, X.device
 
     def dense(self):
+        if self.eager is not None:
+            return self.eager()
         W = self.w.reshape(self.P, -1)
         out = W @ self.X.t()
         if self.b is not None:
             out = out + self.b.reshape(self.P, 1)
-        return out if self.vectorised else out.squeeze(0)
+        out = out if self.vectorised else out.squeeze(0)
+        return out if self.group is None else out + self.group.dense()
+
+
+class GroupGather:
+    """Lazy ``table[..., index]``: a latent table of G values per row (``[G]``, ``[P, G]``, ``[P, 1, G]``) gathered
+    along its last dim by a gradient-free int64 ``[N]`` group index.  It stands for the ``[..., N]`` tensor only until
+    it is added to a lazy ``X @ w + b`` (:class:`LinearPredictor` ``group``); every other use materialises it."""
+
+    def __init__(self, table, index):
+        if type(table).__name__ == "SiteValue":
+            table = _ops.plain_value(table)
+        self.table, self.index = table, index
+        self.G = table.shape[-1]
+        self.shape = table.shape[:-1] + index.shape
+        self.dtype, self.device = table.dtype, table.device
+
+    def dense(self):
+        return self.table[..., self.index]
+
+
+# int32 copies of group indices for b2_glm_group_sum and GlmPotential: id(index) -> (weakref, _version, device, G,
+# copy).  A copy is built (one conversion, one host sync for its range check) the first time an index is scored, e.g.
+# in SVI's eager warm-up step, so a graph-captured step reuses it without a sync; a fresh index tensor every step
+# (subsampling) pays the conversion and the check every step.
+_INDEX32 = {}
+
+
+def group_index_int32(index, G):
+    """The int32 copy of the int64 group index ``index`` ([N], any device), checked once against ``[0, G)``: an index
+    outside raises IndexError before anything reads it.  None while a CUDA graph is captured and no copy exists yet
+    (the check needs a host sync), so the caller can materialise instead."""
+    key = id(index)
+    hit = _INDEX32.get(key)
+    if hit is not None and hit[0]() is index and hit[1:4] == (index._version, index.device, G):
+        return hit[4]
+    if N.capturing():
+        return None
+    g = index.detach().reshape(-1)
+    if bool(((g < 0) | (g >= G)).any()):
+        raise IndexError("group index outside [0, %d)" % G)
+    copy = g.to(torch.int32, copy=True)
+    _INDEX32[key] = (weakref.ref(index, lambda _, k=key: _INDEX32.pop(k, None)), index._version, index.device, G, copy)
+    return copy
 
 
 def linear_predictor(X, w, b=None, tensor_cores=True):
@@ -1173,25 +1226,80 @@ def _lazy_as(x, cls):
 
 
 def _weights(lp):
-    """``(W [P, D], b [P] or None)`` of a LinearPredictor."""
+    """``(W [P, D], b [P] or None)`` of a LinearPredictor without a group effect."""
+    if lp.group is not None:
+        raise RuntimeError("pyro_b200: a linear predictor with a group effect reached a kernel that does not score it")
     return lp.w.reshape(lp.P, lp.X.shape[-1]), lp.b.reshape(lp.P) if lp.b is not None else None
 
 
-def _per_row_scope(lp, value, mask, batch_shape):
-    """``(X, y, W, b)`` for the tensor-core kernels of the per-row GLM families (Bernoulli, Poisson, Normal,
-    Binomial) at any D in 1..128, or None outside their scope.  They take tensor cores asked for, fp32, contiguous
+def _row_scope(lp, value, mask, batch_shape, D):
+    """``(X, y)`` for the tensor-core kernels of the per-row GLM families (Bernoulli, Poisson, Normal, Binomial) at
+    D contraction columns (1..128), or None outside their scope.  They take tensor cores asked for, fp32, contiguous
     16-byte aligned X and y, no mask, one value per row and the predictor's batch shape, from 8192 rows: below that
     the single-pass TF32 gradient has not averaged its rounding down to fp32 accuracy yet, and these kernels have no
     fp32 counterpart."""
     X = lp.X
     ok = (mask is None and X.dtype == torch.float32 and X.is_contiguous() and X.data_ptr() % 16 == 0
-          and 1 <= X.shape[-1] <= 128 and getattr(lp, "tensor_cores", True) and X.shape[0] >= 8192
+          and 1 <= D <= 128 and getattr(lp, "tensor_cores", True) and X.shape[0] >= 8192
           and isinstance(value, torch.Tensor) and value.numel() == X.shape[0]
           and tuple(batch_shape) == tuple(lp.shape))
     y = value.reshape(-1).to(torch.float32).contiguous() if ok else None
     if not ok or y.data_ptr() % 16 != 0:
         return None
-    return (X, y) + _weights(lp)
+    return X, y
+
+
+def _per_row_scope(lp, value, mask, batch_shape):
+    """``(X, y, W, b)`` of :func:`_row_scope` for a predictor without a group effect, or None."""
+    rs = _row_scope(lp, value, mask, batch_shape, lp.X.shape[-1]) if lp.group is None else None
+    return None if rs is None else rs + _weights(lp)
+
+
+def _glm_group(meta, X, y, W, b, A, sigma):
+    scale, weight, coeff, _, kind, idx, trials, per_row, s_stride = meta
+    N.require_cuda(X, "fused multilevel-regression likelihood")
+    P, D = W.shape
+    G = A.shape[-1]
+    n = X.shape[0]
+    dev = X.device
+    total = torch.empty((), dtype=torch.float32, device=dev)
+    dWA = torch.empty((P, D + G), dtype=torch.float32, device=dev)       # [d/dw | d/dalpha] per particle
+    db = torch.empty(P, dtype=torch.float32, device=dev)
+    dsig = torch.empty(P, dtype=torch.float32, device=dev) if sigma is not None and sigma.requires_grad else None
+    ws = N.workspace(dev, int(N.lib().b2_glm_group_sum_workspace(kind, n, D, G, P)), tag="glm")
+    Wc, Ac = W.contiguous(), A.contiguous()
+    bc = b.contiguous() if b is not None else None
+    sc = sigma.contiguous() if sigma is not None else None
+    a_stride = 0 if Ac.numel() == G else G        # one table row shared by every particle, or one per particle
+    N.check(N.lib().b2_glm_group_sum(
+        kind, X.data_ptr(), y.data_ptr(), _ptr(trials), per_row, _ptr(sc), s_stride, idx.data_ptr(), G,
+        Wc.data_ptr(), D, Ac.data_ptr(), a_stride, _ptr(bc), n, D, P, float(scale), float(weight), float(coeff), 0,
+        None, total.data_ptr(), dWA.data_ptr(), db.data_ptr(), _ptr(dsig), ws.data_ptr(), ws.numel(),
+        N.stream_ptr(dev)), "b2_glm_group_sum")
+    dA = dWA[:, D:]
+    dA = (dA.sum(0) if a_stride == 0 else dA).reshape(A.shape)
+    if dsig is not None and s_stride == 0:
+        dsig = dsig.sum().reshape(sigma.shape)      # one sigma shared by every particle
+    return total, None, None, dWA[:, :D], db if b is not None else None, dA, dsig
+
+
+_GlmGroupFn = _FusedSum(_glm_group)
+
+
+def _group_sum(kind, lp, value, mask, batch_shape, coeffs, trials=(None, 0), sigma=(None, 0)):
+    """The site sum of a predictor with a group effect through ``b2_glm_group_sum``, or None outside its scope:
+    :func:`_row_scope` at D + G columns, and a table of X's dtype and device.  An index outside ``[0, G)`` raises
+    IndexError before any launch."""
+    grp = lp.group
+    D = lp.X.shape[-1]
+    rs = _row_scope(lp, value, mask, batch_shape, D + grp.G)
+    if rs is None or grp.table.dtype != torch.float32 or grp.table.device != lp.X.device:
+        return None
+    idx = group_index_int32(grp.index, grp.G)
+    if idx is None:
+        return None
+    W, b = lp.w.reshape(lp.P, D), lp.b.reshape(lp.P) if lp.b is not None else None
+    return _GlmGroupFn.apply(coeffs + (kind, idx) + tuple(trials) + (sigma[1],), *rs, W, b, grp.table, sigma[0])
 
 
 class _BernoulliLinear(Bernoulli):
@@ -1218,6 +1326,9 @@ class _BernoulliLinear(Bernoulli):
 
     def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
         lz = self._lazy
+        if lz.group is not None:
+            out = _group_sum(N.GLM_BERNOULLI, lz, value, mask, self.batch_shape, (scale, weight, sum_coeff, unit))
+            return out if out is not None else super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
         X = lz.X
         tc = getattr(lz, "tensor_cores", True)
         if X.shape[-1] in (4, 8, 16, 32):
@@ -1511,7 +1622,11 @@ class _PoissonLinear(Poisson):
         return self._params[0]
 
     def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
-        args = _per_row_scope(self._lazy.lp, value, mask, self.batch_shape)
+        lp = self._lazy.lp
+        if lp.group is not None:
+            out = _group_sum(N.GLM_POISSON, lp, value, mask, self.batch_shape, (scale, weight, sum_coeff, unit))
+            return out if out is not None else super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
+        args = _per_row_scope(lp, value, mask, self.batch_shape)
         if args is None:
             return super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
         return _GlmPoissonFn.apply((scale, weight, sum_coeff, unit), *args)
@@ -1610,6 +1725,11 @@ class _NormalLinear(Normal):
 
     def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
         lp = self._loc_lazy.lazy
+        if lp.group is not None:
+            sig = _per_particle_sigma(self._scale, lp)
+            out = None if sig is None else _group_sum(N.GLM_NORMAL, lp, value, mask, self.batch_shape,
+                                                      (scale, weight, sum_coeff, unit), sigma=sig)
+            return out if out is not None else super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
         args = _per_row_scope(lp, value, mask, self.batch_shape)
         sig = _per_particle_sigma(self._scale, lp) if args is not None else None     # one noise scale per particle
         if sig is None:
@@ -1721,6 +1841,11 @@ class _BinomialLinear(Binomial):
         return self._params[1]
 
     def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
+        if self._lazy.group is not None:
+            trials = _binomial_trials(self._total_count, self._lazy)
+            out = None if trials is None else _group_sum(N.GLM_BINOMIAL, self._lazy, value, mask, self.batch_shape,
+                                                         (scale, weight, sum_coeff, unit), trials=trials)
+            return out if out is not None else super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
         args = _per_row_scope(self._lazy, value, mask, self.batch_shape)
         # the counts as the kernel reads them, passed in meta: they are data, never differentiated
         trials = _binomial_trials(self._total_count, self._lazy) if args is not None else None
@@ -1737,7 +1862,7 @@ def _binomial_new(cls, total_count=1, probs=None, logits=None, validate_args=Non
 
 
 Binomial.__new__ = staticmethod(_binomial_new)
-__all__ += ["LinearPredictor", "linear_predictor", "ExpLinearPredictor", "ClassLinearPredictor",
+__all__ += ["LinearPredictor", "linear_predictor", "ExpLinearPredictor", "GroupGather", "ClassLinearPredictor",
             "class_linear_predictor", "FactorProduct", "constant"]
 
 from .hmm import GaussianHMM  # noqa: E402,F401

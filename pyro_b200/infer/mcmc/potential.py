@@ -19,7 +19,7 @@ from torch.distributions import biject_to
 
 from ... import _native as N
 from ... import poutine
-from ...distributions import scale_and_mask
+from ...distributions import group_index_int32, scale_and_mask
 from ...primitives import plate
 
 
@@ -212,9 +212,10 @@ class GlmPotential:
         g = group["index"].detach().to(self.device).reshape(-1)
         if g.numel() != self.n or g.is_floating_point():
             raise ValueError("the group index must be an integer tensor of shape [N]")
-        if bool((g < 0).any()) or bool((g >= G).any()):
-            raise ValueError("group index outside [0, %d)" % G)
-        self.groups = g.to(torch.int32).clone()
+        try:
+            self.groups = group_index_int32(g, G)
+        except IndexError as e:
+            raise ValueError(str(e)) from None
         ge = N.b2_glm_group_effect()
         ge.groups = self.groups.data_ptr()
         ge.a_off, ge.G, ge.noncentred = sl.start, G, int(bool(group["noncentred"]))

@@ -37,13 +37,23 @@ Poisson matrix factorisation (the bottom layer of the sparse gamma DEF) has one 
 (fp32, one CUDA device, 1 <= K <= 16) gives a :class:`FactorProduct`, and ``Poisson(lazy)`` scores the site with
 ``b2_poisson_product`` without writing the ``[P, N, J]`` rate.  Any other use, ``+`` included, materialises it.
 
+Multilevel regression has one more: a gather of a latent table along its last dim by a gradient-free int64 ``[N]``
+group index on the table's device -- ``alpha[g]`` of a ``[G]`` value, ``alpha[..., g]``, ``alpha.index_select(-1, g)``,
+``torch.index_select(alpha, -1, g)``, with the table ``[G]``, ``[P, G]`` or ``[P, 1, G]`` or a view kept as a site
+value -- gives a :class:`GroupGather`, and so does ``s * eta[..., g]`` with ``s`` a number or one scalar per particle
+(``[]``, ``[1]``, ``[P, 1]``: the ``[P, G]`` table ``s * eta`` is formed eagerly, so autograd covers ``s``).  Added to a
+lazy ``X @ w (+ b)``, before or after the bias and in either order, it becomes the predictor's group effect, and the
+four families above score ``X @ w + b + alpha[g]`` with ``b2_glm_group_sum``: G more columns of the one pass over X.
+Any other use of the gather, a second group effect included, materialises it exactly as torch computes it.
+
 This is trace-time pattern matching at the seam where Pyro already passes values around (the replayed
 guide value of pyro/poutine/replay_messenger.py:50-61); nothing in the model is rewritten.
 """
 import torch
 
 from ._lazyparam import LazyExpParam
-from .distributions import ClassLinearPredictor, ExpLinearPredictor, FactorProduct, LinearPredictor, _ops
+from .distributions import (ClassLinearPredictor, ExpLinearPredictor, FactorProduct, GroupGather, LinearPredictor,
+                            _ops)
 
 _VIEW_FUNCS = {"squeeze", "unsqueeze", "reshape", "view", "transpose", "t", "permute", "expand",
                "expand_as", "flatten", "contiguous", "__getitem__", "movedim", "swapaxes", "detach_",
@@ -55,6 +65,7 @@ _FACTOR_MATMUL_FUNCS = {"matmul", "__matmul__", "__rmatmul__", "bmm"}
 # tests widen this to check the lazy semantics without a GPU)
 _FACTOR_DEVICE_TYPES = ("cuda",)
 _ADD_FUNCS = {"add", "__add__", "__radd__", "__iadd__", "add_"}
+_MUL_FUNCS = {"mul", "__mul__", "__rmul__"}
 _CHEAP_TRUE = {"eq", "__eq__", "isfinite"}
 _CHEAP_FALSE = {"ne", "__ne__", "isnan", "isinf"}
 _META_FUNCS = {"size", "dim", "ndimension", "numel", "nelement", "__len__", "is_floating_point",
@@ -126,6 +137,10 @@ class SiteValue(torch.Tensor):
             if lazy is not None:
                 if isinstance(lazy, LinearPredictorTensor) and isinstance(lazy.lazy, LinearPredictor):
                     lazy._eager = _eager_call(func, args, kwargs)   # read by exp (ExpLinearPredictor)
+                return lazy
+        if name in ("__getitem__", "index_select") and not kwargs:
+            lazy = _try_group_gather(name, args)
+            if lazy is not None:
                 return lazy
         if any(isinstance(a, LinearPredictorTensor) for a in args):
             return LinearPredictorTensor.__torch_function__(func, types, args, kwargs)
@@ -207,6 +222,33 @@ def _try_lazy_matmul(name, args):
     return None
 
 
+def _try_group_gather(name, args):
+    """``alpha[g]`` (``alpha`` 1-d), ``alpha[..., g]`` or ``index_select(alpha, -1, g)`` of a site value ``[G]``,
+    ``[P, G]`` or ``[P, 1, G]`` and a gradient-free int64 ``[N]`` index on its device: a lazy gather, or None."""
+    if name == "__getitem__":
+        if len(args) != 2:
+            return None
+        t, key = args
+        if isinstance(key, tuple) and len(key) == 2 and key[0] is Ellipsis:
+            idx = key[1]
+        elif isinstance(key, torch.Tensor) and isinstance(t, torch.Tensor) and t.dim() == 1:
+            idx = key
+        else:
+            return None
+    else:
+        if len(args) != 3:
+            return None
+        t, dim, idx = args
+        if not isinstance(t, torch.Tensor) or isinstance(dim, bool) or dim not in (-1, t.dim() - 1):
+            return None
+    if not isinstance(t, SiteValue) or not (t.dim() in (1, 2) or (t.dim() == 3 and t.shape[1] == 1)):
+        return None
+    if (not isinstance(idx, torch.Tensor) or isinstance(idx, (SiteValue, LinearPredictorTensor, LazyExpParam))
+            or idx.dtype != torch.int64 or idx.dim() != 1 or idx.requires_grad or idx.device != t.device):
+        return None
+    return LinearPredictorTensor(GroupGather(t, idx))
+
+
 def _try_factor_product(name, a, b):
     """``z [N, K] @ w [K, J]`` or ``z [P, N, K] @ w [P, K, J]`` of two site values: a lazy rate, or None."""
     if name not in _FACTOR_MATMUL_FUNCS or a.dtype != torch.float32 or b.dtype != torch.float32:
@@ -275,8 +317,52 @@ class LinearPredictorTensor(torch.Tensor):
         another order)."""
         return self._eager() if self._eager is not None else self.dense()
 
+    def _with_group(self, gg):
+        """This ``X @ w (+ b)`` plus the lazy gather ``gg`` as its group effect, or None: one group effect per
+        predictor, an index of one value per row, and a gather that broadcasts to the predictor's shape with one
+        table row, or one per particle."""
+        lz = self._lazy
+        if lz.group is not None or gg.index.numel() != lz.X.shape[0] or gg.dtype != lz.dtype or gg.device != lz.device:
+            return None
+        try:
+            if torch.broadcast_shapes(gg.shape, lz.shape) != lz.shape:
+                return None
+        except RuntimeError:
+            return None
+        if gg.table.numel() // gg.G not in (1, lz.P):
+            return None
+        return LinearPredictorTensor(LinearPredictor(lz.X, lz.w, lz.b, lz.tensor_cores, group=gg))
+
+    def _scaled(self, s):
+        """``s * table[..., index]`` as the gather of the table ``s * table``, or None: ``s`` a number or one scalar
+        per particle (``[]``, ``[1]``, ``[P, 1]``), and a table of at most two dims."""
+        gg = self._lazy
+        if isinstance(s, (int, float)) and not isinstance(s, bool):
+            shape = torch.Size(())
+        elif (isinstance(s, torch.Tensor) and not isinstance(s, (LinearPredictorTensor, LazyExpParam))
+              and s.dtype == gg.dtype and s.device == gg.device
+              and ((s.numel() == 1 and s.dim() <= 2) or (s.dim() == 2 and s.shape[1] == 1))):
+            shape = s.shape
+            s = _ops.plain_value(s) if isinstance(s, SiteValue) else s
+        else:
+            return None
+        try:
+            tshape = torch.broadcast_shapes(shape, gg.table.shape)
+            if len(tshape) > 2 or tshape[:-1] + gg.index.shape != torch.broadcast_shapes(shape, gg.shape):
+                return None
+        except RuntimeError:
+            return None
+        return LinearPredictorTensor(GroupGather(s * gg.table, gg.index))
+
     def _with_bias(self, b):
         lz = self._lazy
+        if isinstance(lz, GroupGather):
+            if isinstance(b, LinearPredictorTensor) and isinstance(b._lazy, LinearPredictor):
+                return b._with_group(lz)
+            return None
+        if isinstance(lz, LinearPredictor) and isinstance(b, LinearPredictorTensor) and isinstance(b._lazy,
+                                                                                                  GroupGather):
+            return self._with_group(b._lazy)
         if isinstance(lz, (FactorProduct, ExpLinearPredictor)):
             return None
         if isinstance(lz, ClassLinearPredictor):
@@ -301,7 +387,7 @@ class LinearPredictorTensor(torch.Tensor):
             return None
         if bp.numel() == 1 and lz.P > 1:
             bp = bp.reshape(()).expand(lz.P)
-        return LinearPredictorTensor(LinearPredictor(lz.X, lz.w, bp, lz.tensor_cores))
+        return LinearPredictorTensor(LinearPredictor(lz.X, lz.w, bp, lz.tensor_cores, group=lz.group))
 
     @classmethod
     def __torch_dispatch__(cls, func, types, args=(), kwargs=None):
@@ -327,7 +413,17 @@ class LinearPredictorTensor(torch.Tensor):
                 if out is not None:
                     if isinstance(out.lazy, LinearPredictor):
                         out._eager = _eager_call(func, args, kwargs)
+                        if out.lazy.group is not None:
+                            out.lazy.eager = out._eager      # dense() is the sum in the order the model wrote it
                     return out
+            if name in _MUL_FUNCS and len(args) == 2 and not kwargs and isinstance(self._lazy, GroupGather):
+                out = self._scaled(args[1] if args[0] is self else args[0])
+                if out is not None:
+                    return out
+            # a lazy gather answers nothing else: every other use materialises it
+            if any(isinstance(a, LinearPredictorTensor) and isinstance(a._lazy, GroupGather) for a in args):
+                with torch._C.DisableTorchFunctionSubclass():
+                    return func(*_plain(args), **{k: _plain(v) for k, v in kwargs.items()})
             if name == "exp" and len(args) == 1 and not kwargs and isinstance(self._lazy, LinearPredictor):
                 return LinearPredictorTensor(ExpLinearPredictor(self._lazy, self.eager))
             # Poisson's rate check (constraints.nonnegative: rate >= 0) answered from the operation: exp >= 0
