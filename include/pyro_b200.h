@@ -575,17 +575,32 @@ size_t b2_glm_scaled_potential_workspace(int kind, int64_t N, int D, int K, int6
  * The likelihood of all chains is one pass of the kind's fused kernel over [X | onehot(g)]: the group effect is G
  * more columns of the contraction, synthesised in shared memory from g, so X is read once and no [C, N] tensor is
  * made.  A group index outside [0, G) makes U and the group effect's gradient NaN.
+ * Varying slopes (ge->S = 1..3; 0, as all-zero trailing fields give, for none): slope k adds beta_k[c, g[n]] *
+ * X[n, col_k] to eta, with beta_k ~ Normal(0, s_k)[G] (centred) or beta_k = s_k * e_k, e_k ~ Normal(0, 1)[G]
+ * (non-centred), and s_k constant or latent as s_a is.  Its covariate is column col_k of X (0 <= col_k < D, the
+ * S columns distinct), so it costs G more columns of the same pass: the likelihood runs at D + G (1 + S) <= 128
+ * columns, and a bad group index makes every slope's gradient NaN too.  Each slope's table and latent scale are
+ * blocks of z's row like alpha and log s_a.
  * kind: B2_GLM_BERNOULLI (any D), B2_GLM_POISSON, B2_GLM_NORMAL (s_off, s_prior, sp0, sp1 and sigma as for
  * b2_glm_normal_potential; s_off < 0 for every other kind) or B2_GLM_BINOMIAL (trials, trials_per_row), with
- * 1 <= D, 1 <= G and D + G <= 128.  z: [C, Dz] fp32 row-major; w (D values) at w_off, b at b_off (has_bias), log
+ * 1 <= D, 1 <= G and D + G (1 + S) <= 128.  z: [C, Dz] fp32 row-major; w (D values) at w_off, b at b_off (has_bias), log
  * sigma at s_off, alpha or e (G values) at ge->a_off and log s_a at ge->s_off (-1: the constant ge->s_const).  Dz is
  * exactly the sum of the present blocks' widths, none overlapping another or leaving the row.  X, y, ge->groups (and
  * per-row trials) 16-byte aligned.  Anything else returns B2_ERR_NULL / B2_ERR_BAD_SHAPE / B2_ERR_TOO_LARGE before
- * any CUDA call.  Four launches with no host sync (CUDA graph capturable): the pack kernel (each chain's [w | alpha]
- * row), the kind's likelihood call with weight -1 (kernel + finish, every logit fp32-exact), and a potential finish
- * that adds every prior term and Jacobian in fp64 in a fixed order.  workspace: b2_glm_group_potential_workspace()
- * bytes, zero-initialised once.
+ * any CUDA call.  Four launches with no host sync (CUDA graph capturable): the pack kernel (each chain's
+ * [w | alpha | beta_1 .. beta_S] row), the kind's likelihood call with weight -1 (kernel + finish, every logit fp32-exact), and a potential finish
+ * that adds every prior term and Jacobian in fp64 in a fixed order (the slopes' after the intercept's).
+ * workspace: b2_glm_group_potential_workspace() bytes, zero-initialised once; its G argument is the number of group
+ * columns, G (1 + S).
  */
+typedef struct b2_glm_group_slope {
+  int64_t b_off;                /* z columns of beta_k (centred) or e_k (non-centred), G of them */
+  int64_t s_off;                /* z column of log s_k, -1 for the constant s_const */
+  int col;                      /* the covariate: column col of X */
+  int noncentred;               /* 0: beta_k ~ Normal(0, s_k); 1: beta_k = s_k * e_k, e_k ~ Normal(0, 1) */
+  int s_prior;                  /* B2_SIGMA_HALFNORMAL .. B2_SIGMA_LOGNORMAL (latent s_k) */
+  double s_const, sp0, sp1;
+} b2_glm_group_slope;
 typedef struct b2_glm_group_effect {
   const int32_t* groups;        /* [N] group of each row, 16-byte aligned */
   int64_t a_off;                /* z columns of alpha (centred) or e (non-centred), G of them */
@@ -594,6 +609,8 @@ typedef struct b2_glm_group_effect {
   int noncentred;               /* 0: alpha ~ Normal(0, s_a); 1: alpha = s_a * e, e ~ Normal(0, 1) */
   int s_prior;                  /* B2_SIGMA_HALFNORMAL .. B2_SIGMA_LOGNORMAL (latent s_a) */
   double s_const, sp0, sp1;
+  int S;                        /* varying slopes, 0 <= S <= 3 */
+  b2_glm_group_slope slope[3];  /* the first S are read */
 } b2_glm_group_effect;
 int b2_glm_group_potential(int kind, const float* X, const void* y, const float* trials, int trials_per_row,
                            int64_t N, int D, int has_bias, const float* z, int64_t C, int64_t Dz, int64_t w_off,

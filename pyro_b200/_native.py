@@ -81,12 +81,20 @@ class b2_glm_weight_scale(ctypes.Structure):
                 ("lam_p0", ctypes.c_double), ("lam_p1", ctypes.c_double)]
 
 
+class b2_glm_group_slope(ctypes.Structure):
+    """Mirror of ``b2_glm_group_slope`` (include/pyro_b200.h): one varying slope by group on a column of X."""
+    _fields_ = [("b_off", ctypes.c_int64), ("s_off", ctypes.c_int64), ("col", ctypes.c_int32),
+                ("noncentred", ctypes.c_int32), ("s_prior", ctypes.c_int32),
+                ("s_const", ctypes.c_double), ("sp0", ctypes.c_double), ("sp1", ctypes.c_double)]
+
+
 class b2_glm_group_effect(ctypes.Structure):
     """Mirror of ``b2_glm_group_effect`` (include/pyro_b200.h): the varying intercept by group of a regression
-    potential."""
+    potential, and its varying slopes."""
     _fields_ = [("groups", ctypes.c_void_p), ("a_off", ctypes.c_int64), ("s_off", ctypes.c_int64),
                 ("G", ctypes.c_int32), ("noncentred", ctypes.c_int32), ("s_prior", ctypes.c_int32),
-                ("s_const", ctypes.c_double), ("sp0", ctypes.c_double), ("sp1", ctypes.c_double)]
+                ("s_const", ctypes.c_double), ("sp0", ctypes.c_double), ("sp1", ctypes.c_double),
+                ("S", ctypes.c_int32), ("slope", b2_glm_group_slope * 3)]
 
 
 class b2_nuts_lockstep(ctypes.Structure):

@@ -362,7 +362,7 @@ static int glm_bernoulli(const float* X, const float* y, const float* W, const f
   if (N <= 0 || P <= 0) return B2_ERR_BAD_SHAPE;
   if (reinterpret_cast<uintptr_t>(X) % 16 != 0) return B2_ERR_BAD_SHAPE;
   // with a group effect the contraction is D + G columns wide (W, dW, partials)
-  const int Da = D + (grp.idx ? grp.G : 0);
+  const int Da = D + grp.cols();
   if (D < 1 || Da > 128) return B2_ERR_BAD_SHAPE;
   if (grp.idx && (grp.G < 1 || reinterpret_cast<uintptr_t>(grp.idx) % 16 != 0)) return B2_ERR_BAD_SHAPE;
   // D in {4, 8, 16, 32} keep their kernels; every other D, and every D with a group effect, takes the wgmma

@@ -63,7 +63,17 @@ glm_binomial_group_tc_kernel(const float* __restrict__ X, const float* __restric
                              const float* __restrict__ trials, const float* __restrict__ W,
                              const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
                              const int32_t* __restrict__ groups, int G) {
-  tcf::glm_flat_pipeline<Binomial<ROW>, DC, true, true>(X, y, W, bvec, N, D, P, partials, trials, groups, G);
+  tcf::glm_flat_pipeline<Binomial<ROW>, DC, true, true>(X, y, W, bvec, N, D, P, partials, trials, GlmGroups{groups, G});
+}
+
+// with varying slopes as well (S > 0): D + G (1 + S) columns, X split
+template <bool ROW, int DC>
+__global__ void __launch_bounds__(tcf::Cfg<DC, true>::kThreads, 1)
+glm_binomial_slope_tc_kernel(const float* __restrict__ X, const float* __restrict__ y,
+                             const float* __restrict__ trials, const float* __restrict__ W,
+                             const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
+                             GlmGroups grp) {
+  tcf::glm_flat_pipeline<Binomial<ROW>, DC, true, true, true>(X, y, W, bvec, N, D, P, partials, trials, grp);
 }
 
 template <bool ROW>
@@ -74,10 +84,14 @@ int launch(const float* X, const float* y, const float* m, const float* W, const
   if (grp.idx && !split_x)
     return launch_glm_group_rn(B2_GLM_BINOMIAL, X, y, m, ROW, W, b, N, D, P, partials, gx, s, grp);
   if (grp.idx)
-    return glm_dispatch_dc<2>(D + grp.G, true, [&](auto dc, auto) {
+    return glm_dispatch_dc<2>(D + grp.cols(), true, [&](auto dc, auto) {
       using C = tcf::Cfg<decltype(dc)::value, true>;
-      return launch_tc(glm_binomial_group_tc_kernel<ROW, decltype(dc)::value>, grid, dim3(C::kThreads),
-                       C::kSmemBytes, s, X, y, m, W, b, N, D, P, partials, grp.idx, grp.G);
+      constexpr int kDC = decltype(dc)::value;
+      if (grp.S)
+        return launch_tc(glm_binomial_slope_tc_kernel<ROW, kDC>, grid, dim3(C::kThreads), C::kSmemBytes, s, X, y, m,
+                         W, b, N, D, P, partials, grp);
+      return launch_tc(glm_binomial_group_tc_kernel<ROW, kDC>, grid, dim3(C::kThreads), C::kSmemBytes, s, X, y, m, W,
+                       b, N, D, P, partials, grp.idx, grp.G);
     });
   if (D == 32) {
     using namespace tile32;
@@ -116,7 +130,7 @@ int b2::glm_binomial_logits(const float* X, const float* y, const float* trials,
                           (trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0);
   int rc = glm_row_check(X, y, W, !trials, N, D, P, bad_trials, flags, workspace, workspace_bytes, grp);
   if (rc != B2_OK) return rc;
-  const int Da = D + (grp.idx ? grp.G : 0);
+  const int Da = D + grp.cols();
   const GlmRowWorkspace w = glm_row_areas(workspace, N, Da, P);
   const bool split_x = glm_split_x(flags, N);
   rc = trials_per_row ? tcbi::launch<true>(X, y, trials, W, b, N, D, P, w.partials, w.gx, split_x, s, grp)

@@ -29,7 +29,16 @@ __global__ void __launch_bounds__(Cfg<DC, true>::kThreads, 1)
 glm_bernoulli_group_tc_kernel(const float* __restrict__ X, const float* __restrict__ y, const float* __restrict__ W,
                               const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
                               const int32_t* __restrict__ groups, int G) {
-  glm_flat_pipeline<Bernoulli, DC, true, true>(X, y, W, bvec, N, D, P, partials, nullptr, groups, G);
+  glm_flat_pipeline<Bernoulli, DC, true, true>(X, y, W, bvec, N, D, P, partials, nullptr, GlmGroups{groups, G});
+}
+
+// with varying slopes as well (S > 0): D + G (1 + S) columns, X split
+template <int DC>
+__global__ void __launch_bounds__(Cfg<DC, true>::kThreads, 1)
+glm_bernoulli_slope_tc_kernel(const float* __restrict__ X, const float* __restrict__ y, const float* __restrict__ W,
+                              const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
+                              GlmGroups grp) {
+  glm_flat_pipeline<Bernoulli, DC, true, true, true>(X, y, W, bvec, N, D, P, partials, nullptr, grp);
 }
 
 }  // namespace tcf
@@ -42,10 +51,14 @@ int launch_glm_flat_tc(const float* X, const float* y, const float* W, const flo
   if (grp.idx && !split_x)
     return launch_glm_group_rn(B2_GLM_BERNOULLI, X, y, nullptr, false, W, b, N, D, P, partials, gx, s, grp);
   if (grp.idx)
-    return glm_dispatch_dc<1>(D + grp.G, true, [&](auto dc, auto) {
+    return glm_dispatch_dc<1>(D + grp.cols(), true, [&](auto dc, auto) {
       using C = tcf::Cfg<decltype(dc)::value, true>;
-      return launch_tc(tcf::glm_bernoulli_group_tc_kernel<decltype(dc)::value>, tc::slab_grid(gx, P),
-                       dim3(C::kThreads), C::kSmemBytes, s, X, y, W, b, N, D, P, partials, grp.idx, grp.G);
+      constexpr int kDC = decltype(dc)::value;
+      if (grp.S)
+        return launch_tc(tcf::glm_bernoulli_slope_tc_kernel<kDC>, tc::slab_grid(gx, P), dim3(C::kThreads),
+                         C::kSmemBytes, s, X, y, W, b, N, D, P, partials, grp);
+      return launch_tc(tcf::glm_bernoulli_group_tc_kernel<kDC>, tc::slab_grid(gx, P), dim3(C::kThreads),
+                       C::kSmemBytes, s, X, y, W, b, N, D, P, partials, grp.idx, grp.G);
     });
   return glm_dispatch_dc<1>(D, split_x, [&](auto dc, auto sx) {
     using C = tcf::Cfg<decltype(dc)::value>;

@@ -43,11 +43,19 @@
 // column, so the likelihood and the group columns of dW come out NaN rather than silently dropping the row.  (The
 // other gradients need not: the epilogues clamp a logit before they take its gradient.)
 //
+// Varying slopes (GROUPS and SLOPES, GlmGroups::S > 0 read at run time; the S = 0 kernels are built without them): X @ w + b + alpha[g] + SUM_k beta_k[g] x_{c_k} is
+// [X | onehot(g) | x_{c_1} onehot(g) | ..] @ [w ; alpha ; beta_1 ; ..] + b, D_aug = D + G (1 + S).  Slope k's
+// column D + kG + j of a row is its covariate X[n, c_k], read from the landing buffer row the split pass is on,
+// when g_n == j and 0 otherwise.  It is split hi + lo and transposed into X^T as X's own columns are, so GEMM 1's
+// logits stay fp32-exact under SPLIT_X and GEMM 2's columns D + kG .. D + (k+1)G - 1 are d loglik / d beta_k.  A
+// row with an index outside [0, G) gets NaN in the slope columns too.
+//
 // Determinism: every CTA writes its partials once (warpgroups summed in a fixed order); no float atomics.
 #pragma once
 #include <cuda.h>
 
 #include "b2_common.cuh"
+#include "glm_host.cuh"
 #include "glm_tc_common.cuh"
 
 namespace b2 {
@@ -96,16 +104,19 @@ __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_
 // d[4j + 2h + e] = D[16 w4 + gid + 8h][8j + 2 t4 + e].
 // Binomial only (glm_tc_common.cuh): trials are the per-row counts [N] (kRowTrials, bulk-copied behind y) or
 // the one count of every row (kConstTrials).
-// GROUPS: groups[N] the group index of each row, G groups; W is [P][D + G], the partials [gx][P][D + G + 2].
-template <class Fam, int DC, bool SPLIT_X, bool GROUPS = false>
+// GROUPS: grp.idx[N] the group index of each row, grp.G groups and (SLOPES) grp.S slopes on X's columns grp.col;
+// W is [P][D + G (1 + S)], the partials [gx][P][D + G (1 + S) + 2].  Without SLOPES, S is 0.
+template <class Fam, int DC, bool SPLIT_X, bool GROUPS = false, bool SLOPES = false>
 __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, const float* __restrict__ y,
                                                   const float* __restrict__ W, const float* __restrict__ bvec,
                                                   int64_t N, int D, int P, float* __restrict__ partials,
                                                   const float* __restrict__ trials = nullptr,
-                                                  const int32_t* __restrict__ groups = nullptr, int G = 0) {
+                                                  GlmGroups grp = {}) {
   using C = Cfg<DC, GROUPS>;
   constexpr int kKD = C::kKD, kWG = C::kWG;
-  const int Da = GROUPS ? D + G : D;           // columns of the contraction
+  const int32_t* __restrict__ groups = grp.idx;
+  const int G = grp.G;
+  const int Da = GROUPS ? D + (SLOPES ? grp.cols() : G) : D;   // columns of the contraction
   pdl_enter();   // lets glm_finish_kernel be resident (blocked in its griddepcontrol.wait) before this kernel ends
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
@@ -190,7 +201,7 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
       wgmma_wait0();
       fence_regs(acc2);
       // ---- split pass, once per 32-column atom, with the thread mapping of the D = 32 pipeline
-      // (glm_tc_common.cuh): columns d >= D (GROUPS: d >= D + G) and rows past N are exact zeros ------------
+      // (glm_tc_common.cuh): columns d >= D (GROUPS: d >= D_aug) and rows past N are exact zeros -------------
       {
         const int lam = t & 7, mu = t >> 3;
         const int e = lam & 1, q8 = ((mu >> 3) << 2) | (lam >> 1);
@@ -199,17 +210,23 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
         float4* xs = reinterpret_cast<float4*>(my + C::WG_XOP);
         float4* xl = reinterpret_cast<float4*>(my + C::WG_XLO);
         float4* xt = reinterpret_cast<float4*>(my + C::WG_XT + (q8 >> 2) * C::kXtBlock);
-        // GROUPS: the one group column of each of the thread's rows, and the value of its other group columns
-        // (0, or NaN in every group column for an index outside [0, G))
+        // GROUPS: the intercept column of each of the thread's rows, the covariates of its slope columns (k G
+        // further on), and the value of its other group columns (0, or NaN in every group column for an index
+        // outside [0, G): its intercept column is then far enough below 0 that no column matches)
         int gcol[4];
-        float goff[4];
+        float goff[4], gx[4][3];
         if constexpr (GROUPS) {
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
-            const int gi = gs[8 * q8 + 2 * i + e];
+            const int r = 8 * q8 + 2 * i + e;
+            const int gi = gs[r];
             const bool ok = (unsigned)gi < (unsigned)G;
-            gcol[i] = ok ? D + gi : -1;
+            gcol[i] = ok ? D + gi : (SLOPES ? -512 : -1);
             goff[i] = ok ? 0.f : __int_as_float(0x7fc00000);
+            if constexpr (SLOPES) {
+#pragma unroll
+              for (int k = 0; k < 3; ++k) gx[i][k] = k < grp.S ? land[r * D + grp.col[k]] : 0.f;
+            }
           }
         }
 #pragma unroll
@@ -224,8 +241,14 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
             for (int q = 0; q < 4; ++q) {
               const int d = 32 * a + 4 * c + q;
               const float v = land[r * D + min(d, D - 1)];
-              if constexpr (GROUPS)
+              if constexpr (SLOPES) {
+                const int o = d - gcol[i];     // k G in slope k's column of the row's group, 0 in its intercept's
+                const float gv = o == 0 ? 1.f : o == G ? gx[i][0] : o == 2 * G ? gx[i][1] : o == 3 * G ? gx[i][2]
+                                                                                                      : goff[i];
+                x[q] = (d < Da && r < rows) ? (d < D ? v : gv) : 0.f;
+              } else if constexpr (GROUPS) {
                 x[q] = (d < Da && r < rows) ? (d < D ? v : (d == gcol[i] ? 1.f : goff[i])) : 0.f;
+              }
               else
                 x[q] = (d < D && r < rows) ? v : 0.f;
               xr[i][q] = tf32_rn(x[q]);

@@ -25,14 +25,14 @@ __global__ void __launch_bounds__(tcf::Cfg<DC, true>::kThreads, 1)
 glm_group_rn_tc_kernel(const float* __restrict__ X, const float* __restrict__ y, const float* __restrict__ trials,
                        const float* __restrict__ W, const float* __restrict__ bvec, int64_t N, int D, int P,
                        float* __restrict__ partials, const int32_t* __restrict__ groups, int G) {
-  tcf::glm_flat_pipeline<Fam, DC, false, true>(X, y, W, bvec, N, D, P, partials, trials, groups, G);
+  tcf::glm_flat_pipeline<Fam, DC, false, true>(X, y, W, bvec, N, D, P, partials, trials, GlmGroups{groups, G});
 }
 
 // MinDC: Binomial runs D + G < 32 on the two-atom loop, as its plain kernels do (glm_binomial_tc.cu)
 template <class Fam, int MinDC>
 int launch_group_rn(const float* X, const float* y, const float* m, const float* W, const float* b, int64_t N, int D,
                     int P, float* partials, int gx, cudaStream_t s, GlmGroups grp) {
-  return glm_dispatch_dc<MinDC>(D + grp.G, false, [&](auto dc, auto) {
+  return glm_dispatch_dc<MinDC>(D + grp.cols(), false, [&](auto dc, auto) {
     using C = tcf::Cfg<decltype(dc)::value, true>;
     return launch_tc(glm_group_rn_tc_kernel<Fam, decltype(dc)::value>, tc::slab_grid(gx, P), dim3(C::kThreads),
                      C::kSmemBytes, s, X, y, m, W, b, N, D, P, partials, grp.idx, grp.G);
@@ -42,6 +42,7 @@ int launch_group_rn(const float* X, const float* y, const float* m, const float*
 int launch_glm_group_rn(int kind, const float* X, const float* y, const float* m, bool row_trials, const float* W,
                         const float* b, int64_t N, int D, int P, float* partials, int gx, cudaStream_t s,
                         GlmGroups grp) {
+  if (grp.S != 0) return B2_ERR_BAD_SHAPE;   // varying slopes run on the X-split group kernels only
   switch (kind) {
     case B2_GLM_BERNOULLI: return launch_group_rn<tc::Bernoulli, 1>(X, y, m, W, b, N, D, P, partials, gx, s, grp);
     case B2_GLM_POISSON: return launch_group_rn<tc::Poisson, 1>(X, y, m, W, b, N, D, P, partials, gx, s, grp);

@@ -12,10 +12,16 @@ namespace b2 {
 // A varying intercept by group (glm_flat_pipeline's GROUPS): idx[N] is the int32 group of each row, 16-byte
 // aligned, and G the number of groups; no group effect when idx is null.  With one, a likelihood call runs the flat
 // pipeline at D + G columns whatever D is: W, dW, the CTA partials and the workspace are D + G wide, and dW's
-// columns D .. D+G-1 are the derivatives with respect to the group effects.
+// columns D .. D+G-1 are the derivatives with respect to the group effects.  S (0..3) varying slopes by group add G
+// columns each: slope k's columns D + kG + j (k = 1..S) hold X[n, col[k - 1]] where g_n == j, so the call is
+// D + G (1 + S) wide and dW's slope columns are the derivatives with respect to the slopes.
 struct GlmGroups {
   const int32_t* idx = nullptr;
   int G = 0;
+  int S = 0;
+  int col[3] = {0, 0, 0};
+  // the synthesised columns of the contraction, G (1 + S); none without a group effect
+  __host__ __device__ int cols() const { return idx ? G * (1 + S) : 0; }
 };
 
 // ---- glm.cu ----
@@ -126,7 +132,7 @@ inline int glm_row_check(const float* X, const float* y, const float* W, bool nu
                          bool bad_operand, int flags, const void* workspace, size_t workspace_bytes,
                          GlmGroups grp = {}) {
   if (!X || !y || !W || null_operand) return B2_ERR_NULL;
-  const int Da = D + (grp.idx ? grp.G : 0);
+  const int Da = D + grp.cols();
   if (N <= 0 || P <= 0 || D < 1 || Da > 128 || bad_operand) return B2_ERR_BAD_SHAPE;
   if (grp.idx && (grp.G < 1 || reinterpret_cast<uintptr_t>(grp.idx) % 16 != 0)) return B2_ERR_BAD_SHAPE;
   if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;

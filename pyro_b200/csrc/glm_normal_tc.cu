@@ -66,17 +66,30 @@ __global__ void __launch_bounds__(tcf::Cfg<DC, true>::kThreads, 1)
 glm_normal_group_tc_kernel(const float* __restrict__ X, const float* __restrict__ y, const float* __restrict__ W,
                            const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
                            const int32_t* __restrict__ groups, int G) {
-  tcf::glm_flat_pipeline<Normal, DC, true, true>(X, y, W, bvec, N, D, P, partials, nullptr, groups, G);
+  tcf::glm_flat_pipeline<Normal, DC, true, true>(X, y, W, bvec, N, D, P, partials, nullptr, GlmGroups{groups, G});
+}
+
+// with varying slopes as well (S > 0): D + G (1 + S) columns
+template <int DC>
+__global__ void __launch_bounds__(tcf::Cfg<DC, true>::kThreads, 1)
+glm_normal_slope_tc_kernel(const float* __restrict__ X, const float* __restrict__ y, const float* __restrict__ W,
+                           const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
+                           GlmGroups grp) {
+  tcf::glm_flat_pipeline<Normal, DC, true, true, true>(X, y, W, bvec, N, D, P, partials, nullptr, grp);
 }
 
 int launch(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
            float* partials, int gx, cudaStream_t s, GlmGroups grp) {
   const dim3 grid = slab_grid(gx, P);
   if (grp.idx)
-    return glm_dispatch_dc<1>(D + grp.G, true, [&](auto dc, auto) {
+    return glm_dispatch_dc<1>(D + grp.cols(), true, [&](auto dc, auto) {
       using C = tcf::Cfg<decltype(dc)::value, true>;
-      return launch_tc(glm_normal_group_tc_kernel<decltype(dc)::value>, grid, dim3(C::kThreads), C::kSmemBytes, s, X,
-                       y, W, b, N, D, P, partials, grp.idx, grp.G);
+      constexpr int kDC = decltype(dc)::value;
+      if (grp.S)
+        return launch_tc(glm_normal_slope_tc_kernel<kDC>, grid, dim3(C::kThreads), C::kSmemBytes, s, X, y, W, b, N, D,
+                         P, partials, grp);
+      return launch_tc(glm_normal_group_tc_kernel<kDC>, grid, dim3(C::kThreads), C::kSmemBytes, s, X, y, W, b, N, D, P,
+                       partials, grp.idx, grp.G);
     });
   if (D == 32) {
     using namespace tile32;
@@ -107,7 +120,7 @@ int b2::glm_normal_loc(const float* X, const float* y, const float* W, const flo
   int rc = glm_row_check(X, y, W, !sigma, N, D, P, sigma_stride != 0 && sigma_stride != 1, flags, workspace,
                          workspace_bytes, grp);
   if (rc != B2_OK) return rc;
-  const int Da = D + (grp.idx ? grp.G : 0);
+  const int Da = D + grp.cols();
   const GlmRowWorkspace w = glm_row_areas(workspace, N, Da, P);
   rc = tcn::launch(X, y, W, b, N, D, P, w.partials, w.gx, s, grp);
   if (rc != 0) return rc;

@@ -59,7 +59,16 @@ __global__ void __launch_bounds__(tcf::Cfg<DC, true>::kThreads, 1)
 glm_poisson_group_tc_kernel(const float* __restrict__ X, const float* __restrict__ y, const float* __restrict__ W,
                             const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
                             const int32_t* __restrict__ groups, int G) {
-  tcf::glm_flat_pipeline<Poisson, DC, true, true>(X, y, W, bvec, N, D, P, partials, nullptr, groups, G);
+  tcf::glm_flat_pipeline<Poisson, DC, true, true>(X, y, W, bvec, N, D, P, partials, nullptr, GlmGroups{groups, G});
+}
+
+// with varying slopes as well (S > 0): D + G (1 + S) columns, X split
+template <int DC>
+__global__ void __launch_bounds__(tcf::Cfg<DC, true>::kThreads, 1)
+glm_poisson_slope_tc_kernel(const float* __restrict__ X, const float* __restrict__ y, const float* __restrict__ W,
+                            const float* __restrict__ bvec, int64_t N, int D, int P, float* __restrict__ partials,
+                            GlmGroups grp) {
+  tcf::glm_flat_pipeline<Poisson, DC, true, true, true>(X, y, W, bvec, N, D, P, partials, nullptr, grp);
 }
 
 int launch(const float* X, const float* y, const float* W, const float* b, int64_t N, int D, int P,
@@ -68,10 +77,14 @@ int launch(const float* X, const float* y, const float* W, const float* b, int64
   if (grp.idx && !split_x)
     return launch_glm_group_rn(B2_GLM_POISSON, X, y, nullptr, false, W, b, N, D, P, partials, gx, s, grp);
   if (grp.idx)
-    return glm_dispatch_dc<1>(D + grp.G, true, [&](auto dc, auto) {
+    return glm_dispatch_dc<1>(D + grp.cols(), true, [&](auto dc, auto) {
       using C = tcf::Cfg<decltype(dc)::value, true>;
-      return launch_tc(glm_poisson_group_tc_kernel<decltype(dc)::value>, grid, dim3(C::kThreads), C::kSmemBytes, s,
-                       X, y, W, b, N, D, P, partials, grp.idx, grp.G);
+      constexpr int kDC = decltype(dc)::value;
+      if (grp.S)
+        return launch_tc(glm_poisson_slope_tc_kernel<kDC>, grid, dim3(C::kThreads), C::kSmemBytes, s, X, y, W, b, N, D,
+                         P, partials, grp);
+      return launch_tc(glm_poisson_group_tc_kernel<kDC>, grid, dim3(C::kThreads), C::kSmemBytes, s, X, y, W, b, N, D, P,
+                       partials, grp.idx, grp.G);
     });
   if (D == 32) {
     using namespace tile32;
@@ -103,7 +116,7 @@ int b2::glm_poisson_log_rate(const float* X, const float* y, const float* W, con
                              cudaStream_t s, GlmGroups grp) {
   int rc = glm_row_check(X, y, W, false, N, D, P, false, flags, workspace, workspace_bytes, grp);
   if (rc != B2_OK) return rc;
-  const int Da = D + (grp.idx ? grp.G : 0);
+  const int Da = D + grp.cols();
   const GlmRowWorkspace w = glm_row_areas(workspace, N, Da, P);
   rc = tcpr::launch(X, y, W, b, N, D, P, w.partials, w.gx, glm_split_x(flags, N), s, grp);
   if (rc != 0) return rc;

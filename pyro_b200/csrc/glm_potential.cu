@@ -20,8 +20,9 @@
 // constant), and the finish adds sigma's prior and the Jacobian of sigma = e^t in fp64.  Binomial regression passes
 // the trial counts to its likelihood call as a fixed operand.  b2_glm_scaled_potential runs the same sequence for a
 // latent weight scale (w ~ Normal(0, tau * lam)), with glm_scaled_potential_finish_kernel as step 3, and
-// b2_glm_group_potential for a varying intercept alpha[g] by group: the pack writes [w | alpha] as each chain's
-// weight row, the likelihood runs on [X | onehot(g)] (glm_flat_tc.cuh GROUPS), and
+// b2_glm_group_potential for a varying intercept alpha[g] by group and up to three varying slopes beta_k[g] on
+// columns of X: glm_group_potential_pack_kernel writes [w | alpha | beta_1 ..] as each chain's weight row, the
+// likelihood runs on [X | onehot(g) | x_{c_1} onehot(g) ..] (glm_flat_tc.cuh GROUPS), and
 // glm_group_potential_finish_kernel is step 3.
 #include <math.h>
 
@@ -31,27 +32,59 @@
 namespace b2 {
 
 // sig (linear regression only, else null): sig[c] = exp(z[c, s_off]) for a latent noise scale (z holds its log),
-// the constant s_const when s_off < 0.  With a group effect (ge.G > 0) the last ge.G of the KD weight columns are
-// alpha: z's alpha columns, or s_a * eta (non-centred).
+// the constant s_const when s_off < 0.  A group effect's weight rows are glm_group_potential_pack_kernel's.
 __global__ void __launch_bounds__(256) glm_potential_pack_kernel(const float* __restrict__ z, int64_t C,
                                                                  int64_t Dz, int64_t w_off, int64_t b_off,
                                                                  int KD, int Kb, float* __restrict__ Wp,
                                                                  float* __restrict__ bp, int64_t s_off,
-                                                                 float s_const, float* __restrict__ sig,
-                                                                 b2_glm_group_effect ge) {
+                                                                 float s_const, float* __restrict__ sig) {
   const int64_t per = KD + Kb;
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (sig != nullptr && i < C) sig[i] = s_off >= 0 ? expf(z[i * Dz + s_off]) : s_const;
   if (i >= C * per) return;
   const int64_t c = i / per;
   const int64_t j = i - c * per;
-  const int64_t a = j - (KD - ge.G);           // the group of a weight column, negative for w
-  if (j < KD && a < 0) Wp[c * KD + j] = z[c * Dz + w_off + j];
-  else if (j < KD) {
-    float v = z[c * Dz + ge.a_off + a];
-    if (ge.noncentred) v *= ge.s_off >= 0 ? expf(z[c * Dz + ge.s_off]) : (float)ge.s_const;
+  if (j < KD) Wp[c * KD + j] = z[c * Dz + w_off + j];
+  else bp[c * Kb + (j - KD)] = z[c * Dz + b_off + (j - KD)];
+}
+
+// glm_potential_pack_kernel for a group effect: each chain's weight row is [w | alpha | beta_1 .. beta_S], KD =
+// D + G (1 + S) wide.  Block 0 is alpha, block k slope k; each is z's columns, or s * eta for a non-centred block
+// (s its scale: exp of its z column, or its constant).
+__global__ void __launch_bounds__(256) glm_group_potential_pack_kernel(const float* __restrict__ z, int64_t C,
+                                                                       int64_t Dz, int64_t w_off, int64_t b_off,
+                                                                       int KD, int Kb, float* __restrict__ Wp,
+                                                                       float* __restrict__ bp, int64_t s_off,
+                                                                       float s_const, float* __restrict__ sig,
+                                                                       b2_glm_group_effect ge) {
+  const int64_t per = KD + Kb;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (sig != nullptr && i < C) sig[i] = s_off >= 0 ? expf(z[i * Dz + s_off]) : s_const;
+  if (i >= C * per) return;
+  const int64_t c = i / per;
+  const int64_t j = i - c * per;
+  const int D = KD - ge.G * (1 + ge.S);
+  if (j < D) {
+    Wp[c * KD + j] = z[c * Dz + w_off + j];
+  } else if (j < KD) {
+    const int k = (int)(j - D) / ge.G, a = (int)(j - D) - k * ge.G;   // block k, group a
+    int64_t off = ge.a_off, so = ge.s_off;
+    int nc = ge.noncentred;
+    double sc = ge.s_const;
+#pragma unroll
+    for (int m = 0; m < 3; ++m)                // selected, not indexed: the parameter struct stays in param space
+      if (k == m + 1) {
+        off = ge.slope[m].b_off;
+        so = ge.slope[m].s_off;
+        nc = ge.slope[m].noncentred;
+        sc = ge.slope[m].s_const;
+      }
+    float v = z[c * Dz + off + a];
+    if (nc) v *= so >= 0 ? expf(z[c * Dz + so]) : (float)sc;
     Wp[c * KD + j] = v;
-  } else bp[c * Kb + (j - KD)] = z[c * Dz + b_off + (j - KD)];
+  } else {
+    bp[c * Kb + (j - KD)] = z[c * Dz + b_off + (j - KD)];
+  }
 }
 
 constexpr double kHalfLog2Pi = 0.91893853320467274178;
@@ -180,15 +213,16 @@ __global__ void __launch_bounds__(256) glm_scaled_potential_finish_kernel(
   }
 }
 
-// glm_potential_finish_kernel with a group effect alpha (ge.G values at the end of each chain's [w | alpha] row of
-// dW, KD = D + G wide): one warp per chain, fp64, lane-strided over the coefficients and then the shuffle tree, so
-// every result is in a fixed order.  With s = s_a (= e^t when latent) and dW_g = d(-loglik)/d alpha_g:
+// glm_potential_finish_kernel with a group effect alpha (ge.G values after w in each chain's [w | alpha | beta_1 ..]
+// row of dW, KD = D + G (1 + S) wide): one warp per chain, fp64, lane-strided over the coefficients and then the
+// shuffle tree, so every result is in a fixed order.  With s = s_a (= e^t when latent) and dW_g = d(-loglik)/d alpha_g:
 //   centred      U += alpha_g^2 / (2 s^2) + log s + log(2 pi) / 2    dU/dalpha_g = dW_g + alpha_g / s^2
 //                dU/dt = SUM_g (1 - alpha_g^2 / s^2) - s (d log p / ds)(s) - 1
 //   non-centred  U += eta_g^2 / 2 + log(2 pi) / 2                    dU/deta_g = s dW_g + eta_g
 //                dU/dt = s SUM_g eta_g dW_g - s (d log p / ds)(s) - 1
 // and for a latent s once per chain U += -log p(s) - t.  The weight and bias priors and the noise scale's terms
-// are those of glm_potential_finish_kernel.
+// are those of glm_potential_finish_kernel.  Each slope block k (beta_k or e_k, scale s_k) then adds the same terms
+// with its own dW columns and scale, after every term of the intercept-only potential, in the order of k.
 __global__ void __launch_bounds__(256) glm_group_potential_finish_kernel(
     const float* __restrict__ z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int KD, int Kb, double s_w,
     double s_b, const float* __restrict__ sum_p, const float* __restrict__ dW, const float* __restrict__ db,
@@ -197,7 +231,7 @@ __global__ void __launch_bounds__(256) glm_group_potential_finish_kernel(
   const int64_t c = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (c >= C) return;
-  const int D = KD - ge.G;
+  const int D = KD - ge.G * (1 + ge.S);
   const double iw = 1.0 / (s_w * s_w);
   const double ib = Kb ? 1.0 / (s_b * s_b) : 0.0;
   const float* zc = z + c * Dz;
@@ -233,14 +267,42 @@ __global__ void __launch_bounds__(256) glm_group_potential_finish_kernel(
   qb = warp_sum(qb);
   ua = warp_sum(ua);
   h = warp_sum(h);
+  double u = 0.0;
   if (lane == 0) {
-    double u = -(double)sum_p[c] + 0.5 * qw + (double)D * (log(s_w) + kHalfLog2Pi) + ua;
+    u = -(double)sum_p[c] + 0.5 * qw + (double)D * (log(s_w) + kHalfLog2Pi) + ua;
     if (!ge.noncentred) u += (double)ge.G * log(sa);
     if (Kb) u += 0.5 * qb + (double)Kb * (log(s_b) + kHalfLog2Pi);
     if (sig != nullptr && s_off >= 0) add_latent_sigma_terms(zc, gc, s_off, sig, dsig, c, s_prior, sp0, sp1, u);
     if (ge.s_off >= 0) gc[ge.s_off] = (float)latent_scale_terms(ge.s_prior, ge.sp0, ge.sp1, t, h, u);
-    U[c] = (float)u;
   }
+  for (int k = 0; k < ge.S; ++k) {
+    const b2_glm_group_slope& sl = ge.slope[k];
+    const float* dWk = dWc + D + (k + 1) * ge.G;
+    const double tk = sl.s_off >= 0 ? (double)zc[sl.s_off] : 0.0;
+    const double sk = sl.s_off >= 0 ? exp(tk) : sl.s_const, isk2 = 1.0 / (sk * sk);
+    double ub = 0.0, hb = 0.0;                 // the block's terms of U, dU/dt_k
+    for (int j = lane; j < ge.G; j += 32) {
+      const double v = (double)zc[sl.b_off + j], g = (double)dWk[j];
+      if (sl.noncentred) {
+        ub += 0.5 * v * v + kHalfLog2Pi;
+        hb += sk * v * g;
+        gc[sl.b_off + j] = (float)(sk * g + v);
+      } else {
+        const double q = v * v * isk2;
+        ub += 0.5 * q + kHalfLog2Pi;
+        hb += 1.0 - q;
+        gc[sl.b_off + j] = (float)(g + v * isk2);
+      }
+    }
+    ub = warp_sum(ub);
+    hb = warp_sum(hb);
+    if (lane == 0) {
+      u += ub;
+      if (!sl.noncentred) u += (double)ge.G * log(sk);
+      if (sl.s_off >= 0) gc[sl.s_off] = (float)latent_scale_terms(sl.s_prior, sl.sp0, sl.sp1, tk, hb, u);
+    }
+  }
+  if (lane == 0) U[c] = (float)u;
 }
 
 // workspace areas, each 256-byte aligned: [likelihood workspace of lik_bytes][Wp][bp][dW][db][sum_p], then with a
@@ -303,10 +365,12 @@ int glm_potential_run(size_t lik_bytes, const float* z, int64_t C, int64_t Dz, i
   const int64_t s_off = sg ? sg->s_off : -1;
 
   const int64_t npack = C * (KD + Kb);
-  b2_glm_group_effect none = {};
-  const b2_glm_group_effect& gef = ge ? *ge : none;
-  glm_potential_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, Wp, bp,
-                                                                             s_off, sg ? sg->s_const : 0.f, sig, gef);
+  if (ge != nullptr)
+    glm_group_potential_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(
+        z, C, Dz, w_off, b_off, KD, Kb, Wp, bp, s_off, sg ? sg->s_const : 0.f, sig, *ge);
+  else
+    glm_potential_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, Wp, bp,
+                                                                               s_off, sg ? sg->s_const : 0.f, sig);
   count_launch(1);
   int rc = check_launch();
   if (rc != 0) return rc;
@@ -543,8 +607,9 @@ extern "C" int b2_glm_scaled_potential(int kind, const float* X, const void* y, 
       });
 }
 
-// ---- a varying intercept by group: alpha[g], centred or non-centred, with a constant or latent scale s_a -------
-// Scope: kinds Bernoulli, Poisson, Normal and Binomial, 1 <= G and D + G <= 128.
+// ---- a varying intercept by group: alpha[g], centred or non-centred, with a constant or latent scale s_a, and up to
+// three varying slopes beta_k[g] X[n, c_k] with scales of the same forms ------------------------------------------
+// Scope: kinds Bernoulli, Poisson, Normal and Binomial, 1 <= G and D + G (1 + S) <= 128 (G here: the group columns).
 inline bool glm_group_in_scope(int kind, int64_t N, int D, int G, int64_t C) {
   if (kind != B2_GLM_BERNOULLI && kind != B2_GLM_POISSON && kind != B2_GLM_NORMAL && kind != B2_GLM_BINOMIAL)
     return false;
@@ -565,17 +630,34 @@ extern "C" int b2_glm_group_potential(int kind, const float* X, const void* y, c
   if (!X || !y || !z || !U || !grad || !ge || !ge->groups) return B2_ERR_NULL;
   if (kind == B2_GLM_BINOMIAL && !trials) return B2_ERR_NULL;
   const b2_glm_group_effect g = *ge;
-  if (!glm_group_in_scope(kind, N, D, g.G, C)) return B2_ERR_BAD_SHAPE;
+  if (g.S < 0 || g.S > 3 || g.G < 1 || g.G > 128) return B2_ERR_BAD_SHAPE;
+  const int Da = D + g.G * (1 + g.S);
+  if (!glm_group_in_scope(kind, N, D, g.G * (1 + g.S), C)) return B2_ERR_BAD_SHAPE;
   if (N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
   const bool normal = kind == B2_GLM_NORMAL;
   if (!normal && s_off >= 0) return B2_ERR_BAD_SHAPE;   // only linear regression has a noise scale
   if (g.noncentred != 0 && g.noncentred != 1) return B2_ERR_BAD_SHAPE;
-  // z's row is exactly w, b, log sigma, alpha (or eta) and log s_a: each block inside the row, no two overlapping,
-  // and their widths summing to Dz
-  const int64_t off[5] = {w_off, has_bias ? b_off : -1, s_off, g.a_off, g.s_off};
-  const int64_t len[5] = {D, has_bias ? 1 : 0, s_off >= 0 ? 1 : 0, g.G, g.s_off >= 0 ? 1 : 0};
+  for (int k = 0; k < g.S; ++k) {
+    const b2_glm_group_slope& sl = g.slope[k];
+    if (sl.col < 0 || sl.col >= D || (sl.noncentred != 0 && sl.noncentred != 1)) return B2_ERR_BAD_SHAPE;
+    for (int j = 0; j < k; ++j)
+      if (g.slope[j].col == sl.col) return B2_ERR_BAD_SHAPE;
+    if (sl.s_off >= 0 && !positive_prior_ok(sl.s_prior, sl.sp0, sl.sp1)) return B2_ERR_BAD_SHAPE;
+    if (sl.s_off < 0 && (!(sl.s_const > 0.0) || !((float)sl.s_const > 0.f))) return B2_ERR_BAD_SHAPE;
+  }
+  // z's row is exactly w, b, log sigma, alpha (or eta), log s_a and each slope's beta_k (or e_k) and log s_k: each
+  // block inside the row, no two overlapping, and their widths summing to Dz
+  int64_t off[11] = {w_off, has_bias ? b_off : -1, s_off, g.a_off, g.s_off};
+  int64_t len[11] = {D, has_bias ? 1 : 0, s_off >= 0 ? 1 : 0, g.G, g.s_off >= 0 ? 1 : 0};
+  const int nblk = 5 + 2 * g.S;
+  for (int k = 0; k < g.S; ++k) {
+    off[5 + 2 * k] = g.slope[k].b_off;
+    len[5 + 2 * k] = g.G;
+    off[6 + 2 * k] = g.slope[k].s_off;
+    len[6 + 2 * k] = g.slope[k].s_off >= 0 ? 1 : 0;
+  }
   int64_t width = 0;
-  for (int i = 0; i < 5; ++i) {
+  for (int i = 0; i < nblk; ++i) {
     if (len[i] == 0) continue;
     if (off[i] < 0 || off[i] > Dz - len[i]) return B2_ERR_BAD_SHAPE;
     for (int j = 0; j < i; ++j)
@@ -599,8 +681,10 @@ extern "C" int b2_glm_group_potential(int kind, const float* X, const void* y, c
   GlmGroups grp;
   grp.idx = g.groups;
   grp.G = g.G;
+  grp.S = g.S;
+  for (int k = 0; k < g.S; ++k) grp.col[k] = g.slope[k].col;
   return glm_potential_run(
-      glm_potential_lik_bytes(kind, N, D + g.G, 1, C), z, C, Dz, w_off, b_off, D + g.G, 1, has_bias, s_w, s_b,
+      glm_potential_lik_bytes(kind, N, Da, 1, C), z, C, Dz, w_off, b_off, Da, 1, has_bias, s_w, s_b,
       normal ? &sg : nullptr, nullptr, &g, U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
       [&](const float* Wp, const float* bp, const float* sig, float* dsig, float* sum_p, float* dW, float* db,
           void* ws, size_t ws_bytes) {

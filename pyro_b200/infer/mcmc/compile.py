@@ -218,8 +218,15 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
     latent ``Normal`` site of shape ``(G,)``, tried after the model without one fails.  The probes decide the form:
     the observation's logits (log-rate, loc) equal ``X @ w + b + alpha[g]`` with ``alpha ~ Normal(0, s_a)``
     (centred), or ``X @ w + b + s_a * eta[g]`` with ``eta ~ Normal(0, 1)`` (non-centred), ``s_a`` a constant or a
-    drawn positive scalar site, at every probe.  So how the model writes the gather does not matter."""
-    if len(observed) != 1 or not 1 <= len(latent) <= 5:
+    drawn positive scalar site, at every probe.  So how the model writes the gather does not matter.
+
+    Varying slopes (up to three, with a varying intercept, D + G (1 + S) <= 128): further latent ``Normal`` sites of
+    shape ``(G,)``, tried after the intercept-only model fails.  Slope k adds ``beta_k[g] * X[:, c_k]`` to the linear
+    predictor, ``beta_k`` centred or non-centred with its own constant or latent scale, as the intercept.  A probe
+    with only table k non-zero finds ``c_k``: the residual after ``X @ w + b + alpha[g]`` must be ``beta_k[g]`` times
+    a column of X (the lowest such column when columns repeat); then the three probes with every table drawn confirm
+    the whole sum.  So the covariate must be a column of X, whatever the model writes to take it."""
+    if len(observed) != 1 or not 1 <= len(latent) <= 11:
         return None
     (obs_name, obs), = observed.items()
     _, kind = _base(obs["fn"])
@@ -244,7 +251,7 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
             return None
         positive[name] = tuple(v.shape)
     latent = {k: v for k, v in latent.items() if k not in positive}
-    if len(latent) not in (1, 2, 3):
+    if not 1 <= len(latent) <= 6:
         return None
     y = obs["value"]
     if not isinstance(y, torch.Tensor) or y.dim() != 1:
@@ -266,28 +273,36 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
                 or v.dtype != torch.float32 or _const(fn.loc) != 0.0:
             return None
         scales[name], shapes[name] = _const(fn.scale), tuple(v.shape)
-    attempts = [None]                      # the group-effect site: none, then each candidate
+    attempts = [(None, ())]                # (the group-effect site, its slope sites): none, then each candidate
     ints = [a for a in list(args) + list(kwargs.values())
             if isinstance(a, torch.Tensor) and a is not y and a.dtype == torch.int64 and a.dim() == 1
             and a.numel() == n and not a.requires_grad]
     if kind != "Categorical" and len(ints) == 1 and len(latent) >= 2 and ints[0].numel() > 0:
         # only sites with a group for every index: the probes gather with it
         lo, hi = int(ints[0].min()), int(ints[0].max())
-        attempts += [name for name, s in shapes.items() if len(s) == 1 and D + s[0] <= 128 and lo >= 0 and hi < s[0]]
-    for group_site in attempts:
+        groups = [name for name, s in shapes.items() if len(s) == 1 and lo >= 0 and hi < s[0]]
+        attempts += [(a, ()) for a in groups if D + shapes[a][0] <= 128]
+        # then with slopes: the other sites of the intercept's shape (when D == G, bar one that may be the weight)
+        for a in groups:
+            G = shapes[a][0]
+            rest = [name for name in groups if name != a and shapes[name] == (G,)]
+            sets = [rest] + ([[b for b in rest if b != w] for w in rest] if D == G else [])
+            attempts += [(a, tuple(b)) for b in sets if 1 <= len(b) <= 3 and D + G * (1 + len(b)) <= 128]
+    for group_site, slope_sites in attempts:
         pot = _glm_roles(poutine, model, args, kwargs, kind, obs_name, obs, order, positive, priors, latent, X, y,
-                         scales, shapes, group_site, ints[0] if group_site is not None else None)
+                         scales, shapes, group_site, ints[0] if group_site is not None else None, slope_sites)
         if pot is not None:
             return pot
     return None
 
 
 def _glm_roles(poutine, model, args, kwargs, kind, obs_name, obs, order, positive, priors, latent, X, y, scales,
-               shapes, group_site, gidx):
-    """``_try_glm`` with the Normal site ``group_site`` (None: no group effect) as the group effect."""
+               shapes, group_site, gidx, slope_sites=()):
+    """``_try_glm`` with the Normal site ``group_site`` (None: no group effect) as the group effect, and the Normal
+    sites ``slope_sites`` as its varying slopes."""
     from .potential import GlmPotential
     n, D = y.numel(), X.shape[1]
-    latent = {k: v for k, v in latent.items() if k != group_site}
+    latent = {k: v for k, v in latent.items() if k != group_site and k not in slope_sites}
     if len(latent) not in (1, 2):
         return None
     if kind == "Bernoulli":
@@ -323,6 +338,10 @@ def _glm_roles(poutine, model, args, kwargs, kind, obs_name, obs, order, positiv
     wform = None                           # (tau site or None, lam site or None); (None, None): the constant s_w
     trials = None                          # Binomial: the constant count, or the [N] counts of the prototype
     group = None                           # the group effect's form, once the first probe has found it
+    slopes = {k: None for k in slope_sites}   # each slope's column and form, once its own probe has found them
+    # with slopes, a probe of the intercept alone and one of each slope alone (the other tables zero) come first
+    probes = [()] + [(k,) for k in slope_sites] if slope_sites else []
+    probes += [tuple(slope_sites)] * 3
     if kind == "Binomial":
         trials = _binomial_trials(_base(obs["fn"])[0], n)
         if trials is None:
@@ -331,7 +350,7 @@ def _glm_roles(poutine, model, args, kwargs, kind, obs_name, obs, order, positiv
     def as_t(v):
         return torch.as_tensor(v, dtype=X.dtype, device=X.device)
 
-    for i in range(3):
+    for i, drawn in enumerate(probes):
         wv = torch.randn(shapes[weight], generator=gen).to(X)
         if kind == "Poisson":
             wv = wv / D ** 0.5            # log-rates of a few units: exp neither overflows nor underflows
@@ -341,6 +360,8 @@ def _glm_roles(poutine, model, args, kwargs, kind, obs_name, obs, order, positiv
             data[name] = torch.exp(0.5 * torch.randn(shape, generator=gen)).to(X)
         if group_site is not None:
             data[group_site] = torch.randn(shapes[group_site], generator=gen).to(X)
+        for k in slope_sites:
+            data[k] = torch.randn(shapes[k], generator=gen).to(X) if k in drawn else X.new_zeros(shapes[k])
         tr = poutine.trace(poutine.condition(model, data=data)).get_trace(*args, **kwargs)
         pfn = _base(tr.nodes[obs_name]["fn"])[0]
         # the priors: constant parameters that do not move with any latent
@@ -419,11 +440,34 @@ def _glm_roles(poutine, model, args, kwargs, kind, obs_name, obs, order, positiv
             sa = data[group["s_site"]].reshape(()) if group["s_site"] is not None else as_t(group["s_const"])
             e = data[group_site][gidx]
             want = want + (sa * e if group["noncentred"] else e)
+        for k in drawn:
+            claimed = [sigma_site, group["s_site"]] + [v["form"]["s_site"] for j, v in slopes.items()
+                                                        if j != k and v is not None]
+            free_k = [s for s in free_s if s not in claimed]
+            if slopes[k] is None:
+                # its own probe: the only table drawn, so the residual is its term alone.  The first column whose
+                # form is found wins, one with a drawn scale before a constant one: over very few rows several
+                # columns can fit, and only the drawn scale tells them apart.
+                found = [(c, _group_form(tr, k, data, gidx, logits, want, free_k, None, X.dtype, cov=X[:, c]))
+                         for c in _slope_columns(logits - want, data[k][gidx], X)]
+                found = [f for f in found if f[1] is not None]
+                found = [f for f in found if f[1]["s_site"] is not None] or found
+                if not found:
+                    return None
+                slopes[k] = {"col": found[0][0], "form": found[0][1]}
+            cov = X[:, slopes[k]["col"]]
+            form = _group_form(tr, k, data, gidx, logits, want, free_k, slopes[k]["form"], X.dtype, cov=cov)
+            if form is None:
+                return None
+            sk = data[form["s_site"]].reshape(()) if form["s_site"] is not None else as_t(form["s_const"])
+            e = data[k][gidx] * cov
+            want = want + (sk * e if form["noncentred"] else e)
         if tuple(logits.shape) != tuple(want.shape) or not _close(logits, want, X.dtype):
             return None
     tau_site, lam_site = wform
     # every positive site has exactly one role
-    roles = [r for r in (sigma_site,) + wform + ((group["s_site"],) if group else ()) if r is not None]
+    roles = [r for r in (sigma_site,) + wform + ((group["s_site"],) if group else ())
+             + tuple(v["form"]["s_site"] for v in slopes.values()) if r is not None]
     if sorted(roles) != sorted(positive):
         return None
     if kind == "Bernoulli" and bias is None and tau_site is None and lam_site is None and group is None:
@@ -437,7 +481,9 @@ def _glm_roles(poutine, model, args, kwargs, kind, obs_name, obs, order, positiv
         sites[name] = (slice(off, off + width), "exp" if name in positive else "identity", shape)
         off += width
     if group is not None:
-        group = dict(group, site=group_site, index=gidx, s_prior=priors.get(group["s_site"]))
+        group = dict(group, site=group_site, index=gidx, s_prior=priors.get(group["s_site"]),
+                     slopes=[dict(v["form"], site=k, col=v["col"], s_prior=priors.get(v["form"]["s_site"]))
+                             for k, v in slopes.items()])
     return GlmPotential(X, y.detach(), kind, sites, weight, bias,
                         s_w=scales[weight] if wform == (None, None) else 1.0,
                         s_b=scales[bias] if bias is not None else 1.0,
@@ -447,11 +493,22 @@ def _glm_roles(poutine, model, args, kwargs, kind, obs_name, obs, order, positiv
                         lam_site=lam_site, lam_prior=priors.get(lam_site), group=group)
 
 
-def _group_form(tr, group_site, data, gidx, logits, want, free_s, group, dtype):
+def _slope_columns(r, e, X):
+    """The columns c of X, lowest first, with ``r == s * e * X[:, c]`` for one number s."""
+    cols = []
+    for c in range(X.shape[1]):
+        q = e * X[:, c]
+        s = (r * q).sum() / (q * q).sum().clamp(min=1e-30)
+        if _close(r, s * q, X.dtype):
+            cols.append(c)
+    return cols
+
+
+def _group_form(tr, group_site, data, gidx, logits, want, free_s, group, dtype, cov=None):
     """The group effect's form at one probe: ``{"noncentred", "s_site", "s_const"}`` when the residual
     ``logits - want`` is ``alpha[g]`` with ``alpha ~ Normal(0, s_a)`` or ``s_a * eta[g]`` with ``eta ~ Normal(0, 1)``,
     ``s_a`` the drawn site of ``free_s`` or one constant; ``group`` is the first probe's answer, which later probes
-    must repeat.  None otherwise."""
+    must repeat.  A varying slope's residual is that times its covariate ``cov``.  None otherwise."""
     afn = _base(tr.nodes[group_site]["fn"])[0]
     if _const(afn.loc) != 0.0:
         return None
@@ -460,6 +517,8 @@ def _group_form(tr, group_site, data, gidx, logits, want, free_s, group, dtype):
     if tuple(torch.broadcast_shapes(scale.shape, (G,))) != (G,):
         return None
     e = data[group_site][gidx]
+    if cov is not None:
+        e = e * cov
     r = logits - want
     if group is None:
         if _close(r, e, dtype):

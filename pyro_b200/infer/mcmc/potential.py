@@ -135,7 +135,9 @@ class GlmPotential:
     ``alpha = s_a * eta`` (``group["noncentred"]``).  ``s_a`` is the constant ``group["s_const"]`` or the positive
     scalar site ``group["s_site"]`` with prior ``group["s_prior"]`` (as ``sigma_prior``).  ``group["index"]`` must
     lie in ``[0, G)``; a private int32 copy is made once.  The likelihood runs on ``[X | onehot(g)]``, so
-    ``D + G <= 128``.
+    ``D + G <= 128``.  ``group["slopes"]`` lists up to three varying slopes, each a dict with the keys of the intercept
+    (``site``, ``noncentred``, ``s_site``, ``s_const``, ``s_prior``) and ``col``: slope k adds
+    ``beta_k[g] * X[:, col]``, and each takes G more columns of the contraction, so ``D + G (1 + S) <= 128``.
 
     ``value_and_grad`` is ``b2_glm_potential``: the likelihood of all chains comes from one pass of the
     fused GLM kernel over X, the chains being its particles.  ``sites`` maps each site name to
@@ -225,6 +227,21 @@ class GlmPotential:
             ge.s_off, ge.s_prior, ge.sp0, ge.sp1 = self.sites[s_site][0].start, self._SIGMA_PRIORS[pk], p0, p1
         else:
             ge.s_off, ge.s_const = -1, float(group["s_const"])
+        slopes = group.get("slopes", [])
+        if len(slopes) > 3:
+            raise ValueError("at most three varying slopes")
+        ge.S = len(slopes)
+        for k, sl in enumerate(slopes):
+            e = ge.slope[k]
+            bsl, _, bshape = self.sites[sl["site"]]
+            if tuple(bshape) != (G,) or not 0 <= int(sl["col"]) < self.Dx:
+                raise ValueError("a varying slope needs G values and a column of X")
+            e.b_off, e.col, e.noncentred = bsl.start, int(sl["col"]), int(bool(sl["noncentred"]))
+            if sl.get("s_site") is not None:
+                pk, p0, p1 = sl["s_prior"]
+                e.s_off, e.s_prior, e.sp0, e.sp1 = self.sites[sl["s_site"]][0].start, self._SIGMA_PRIORS[pk], p0, p1
+            else:
+                e.s_off, e.s_const = -1, float(sl["s_const"])
         return ge
 
     @property
@@ -283,7 +300,8 @@ class GlmPotential:
         return U, g
 
     def _group_value_and_grad(self, lib, z, C, U, g):
-        need = int(lib.b2_glm_group_potential_workspace(self.scaled_kind, self.n, self.Dx, self.group_effect.G, C))
+        ge = self.group_effect
+        need = int(lib.b2_glm_group_potential_workspace(self.scaled_kind, self.n, self.Dx, ge.G * (1 + ge.S), C))
         ws = N.workspace(z.device, need, tag="glm_potential")
         s_off = self.sites[self.sigma_site][0].start if self.sigma_site is not None else -1
         pk, p0, p1 = self.sigma_prior
