@@ -458,141 +458,71 @@ int b2_poisson_product(const float* A, const float* B, const float* x, int64_t N
 size_t b2_poisson_product_workspace(int64_t N, int K, int64_t J, int P);
 
 /*
- * b2_glm_potential -- HMC / NUTS potential energy and gradient of Bayesian logistic (kind
- * B2_GLM_BERNOULLI), softmax (B2_GLM_CATEGORICAL) or Poisson (B2_GLM_POISSON, log link) regression for C
- * chains, with the likelihood of every chain computed in one pass over X by the kernels of
- * b2_glm_bernoulli_logits / b2_glm_categorical_logits / b2_glm_poisson_log_rate (the chains are their
- * particles):
- *   U[c]       = -( SUM_n log p(y[n] | logits[c,n]) + SUM_i log Normal(w[c,i]; 0, s_w)
- *                   + SUM_k log Normal(b[c,k]; 0, s_b) )
+ * b2_glm_potential -- HMC / NUTS potential energy and gradient of Bayesian regression for C chains, with the
+ * likelihood of every chain computed in one pass over X by the fused GLM kernels (the chains are their particles):
+ *   U[c]       = -( SUM_n log p(y[n] | eta[c,n]) + SUM_i log Normal(w[c,i]; 0, s_i) + SUM_k log Normal(b[c,k]; 0, s_b)
+ *                   [+ log p(sigma_c)] [+ log p(tau_c) + SUM_j log p(lam_c,j)] [+ the group effect's terms] )
+ *                   + the Jacobians of the latent scales
  *   grad[c,:]  = dU / dz[c,:]
- * logits[c,n] = <X[n,:], w[c,:]> + b[c] (Bernoulli, and Poisson's log-rate, K == 1) or logits[c,n,k] =
- * <X[n,:], W[c,k,:]> + b[c,k] (Categorical).  z: [C, Dz] fp32 row-major chain state; the weights (K*D values, W row-major [K, D])
- * start at column w_off, the bias (K values, only if has_bias) at column b_off, and Dz == K*D + (has_bias ? K
- * : 0).  grad has z's layout.  X: [N, D] fp32 row-major, 16-byte aligned; y: [N] fp32 0/1 (Bernoulli) or
- * int64 labels, 16-byte aligned (Categorical), or fp32 counts, 16-byte aligned (Poisson).
- * Scope: Bernoulli with K == 1 and D in {4, 8, 16, 32}; Categorical with D == 32 and 2 <= K <= 16; Poisson
- * with K == 1 and 1 <= D <= 128;
- * s_w > 0 and (with a bias) s_b > 0; anything else returns B2_ERR_BAD_SHAPE.
- * The GLM kernels always run with B2_FLAG_GLM_3XTF32 (every logit fp32-exact).  The prior and the totals
- * are accumulated in fp64 in a fixed order: results are deterministic.
- * workspace: b2_glm_potential_workspace() bytes, zero-initialised ONCE by the caller; it must not be
- * shared with a concurrent call of any GLM entry point.  Four launches (pack, GLM kernel, GLM finish,
- * potential finish), no host synchronisation: one evaluation can be captured in a CUDA graph.
+ * U is the potential of pyro/infer/mcmc/util.py:275-286: every latent positive scale v is held in z as t = log v,
+ * with the Jacobian -t.  One b2_glm_regression describes the model, its data and z's layout; the call and its
+ * workspace query take the same one.  Its parts:
+ *
+ * kind and likelihood, eta[c,n] = <X[n,:], w[c,:]> + b[c] (K == 1) or eta[c,n,k] = <X[n,:], W[c,k,:]> + b[c,k]:
+ *   B2_GLM_BERNOULLI    y ~ Bernoulli(logits = eta), y [N] fp32 0/1; K == 1, D in {4, 8, 16, 32}
+ *   B2_GLM_CATEGORICAL  y ~ Categorical(logits = eta), y [N] int64 labels; D == 32, 2 <= K <= 16
+ *   B2_GLM_POISSON      y ~ Poisson(rate = exp(eta)), y [N] fp32 counts; K == 1, 1 <= D <= 128
+ *   B2_GLM_NORMAL       y ~ Normal(eta, sigma_c), y [N] fp32; K == 1, 1 <= D <= 128
+ *   B2_GLM_BINOMIAL     y ~ Binomial(m, logits = eta), y [N] fp32; K == 1, 1 <= D <= 128; trials as for
+ *                       b2_glm_binomial_logits (trials_per_row 0: one count, 1: [N] counts, on the device)
+ *   X: [N, D] fp32 row-major.  z: [C, Dz] fp32 row-major chain state; the weights (K*D values, W row-major [K, D])
+ *   start at column w_off, the bias (K values, only if has_bias) at b_off.  grad has z's layout.
+ * noise scale (B2_GLM_NORMAL only): latent when s_off >= 0 (z column s_off holds log sigma; prior s_prior, a
+ *   B2_SIGMA_* code: B2_SIGMA_HALFNORMAL (sp0 = scale), B2_SIGMA_HALFCAUCHY (sp0 = scale), B2_SIGMA_EXPONENTIAL
+ *   (sp0 = rate) or B2_SIGMA_LOGNORMAL (sp0 = loc, sp1 = scale)), else the constant sigma.  s_off must be < 0 for
+ *   every other kind.
+ * weight scale: scale == NULL for the constant s_i = s_w; else latent, s_i = tau lam_i, the hierarchical
+ *   (w ~ Normal(0, tau)), ARD (w ~ Normal(0, lam)) and horseshoe (w ~ Normal(0, tau * lam)) priors: t = log tau at
+ *   scale->tau_off (one column) and l = log lam at scale->lam_off (K*D columns, lam_i scales w_i), a -1 offset
+ *   meaning absent and at least one of them latent; their priors are B2_SIGMA_* codes with (p0, p1) as for sigma.
+ *   s_w is then not read.
+ * group effect: group == NULL for none; else a varying intercept by group and up to three varying slopes,
+ *     eta[c,n] += alpha[c, g[n]] + SUM_k beta_k[c, g[n]] * X[n, col_k]
+ *   with alpha ~ Normal(0, s_a)[G] (centred) or alpha = s_a * e, e ~ Normal(0, 1)[G] (non-centred), s_a the
+ *   constant group->s_const or latent (log s_a at group->s_off, prior as for sigma); each slope k (group->S = 1..3)
+ *   has its table, form and scale the same way, on column col_k of X (0 <= col_k < D, the S columns distinct).
+ *   The likelihood runs on [X | onehot(g) | x_{col_1} onehot(g) ..], G (1 + S) more columns synthesised in shared
+ *   memory from g, so X is read once and no [C, N] tensor is made: every kind but B2_GLM_CATEGORICAL, any D >= 1
+ *   with D + G (1 + S) <= 128, and a constant weight scale.  A group index outside [0, G) makes U and the group
+ *   effect's gradients NaN.
+ * Dz is exactly the sum of the present blocks' widths (w, b, log sigma, log tau, log lam, alpha or e, log s_a, each
+ * slope's table and log s_k), none overlapping another or leaving the row.  s_w > 0 (constant weight scale) and,
+ * with a bias, s_b > 0; a constant sigma or group scale is positive in fp32; a prior's parameters are positive,
+ * and a LogNormal loc finite.  X, y, group->groups and per-row trials are 16-byte aligned (Bernoulli, softmax and
+ * Poisson with neither a latent weight scale nor a group effect check X and y in their likelihood call, where
+ * Bernoulli's SIMT kernel needs only X aligned).  Anything else returns B2_ERR_NULL (a NULL m, X, y, z, U, grad,
+ * Binomial trials or group->groups) or B2_ERR_BAD_SHAPE before any CUDA call; with a latent weight scale or a
+ * group effect N >= 2^31 returns B2_ERR_TOO_LARGE there too, and otherwise the likelihood call decides.
+ * The GLM kernels always run with B2_FLAG_GLM_3XTF32 (every logit fp32-exact).  The prior terms and the totals are
+ * accumulated in fp64 in a fixed order: results are deterministic.
+ * workspace: b2_glm_potential_workspace(m, C) bytes (256 for a model out of scope), zero-initialised ONCE by the
+ * caller; it must not be shared with a concurrent call of any GLM entry point.  Four launches (pack, GLM kernel,
+ * GLM finish, potential finish), no host synchronisation: one evaluation can be captured in a CUDA graph.
  */
 #define B2_GLM_BERNOULLI 0
 #define B2_GLM_CATEGORICAL 1
 #define B2_GLM_POISSON 2
-int b2_glm_potential(int kind, const float* X, const void* y, int64_t N, int D, int K, int has_bias,
-                     const float* z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, double s_w,
-                     double s_b, float* U, float* grad, void* workspace, size_t workspace_bytes,
-                     void* stream);
-
-/*
- * b2_glm_normal_potential -- HMC / NUTS potential energy and gradient of Bayesian linear regression for C chains,
- * with the likelihood of every chain from one pass of b2_glm_normal_loc over X (the chains are its particles):
- *   U[c] = -( SUM_n log Normal(y[n] | <X[n,:], w[c,:]> + b[c], sigma_c) + SUM_i log Normal(w[c,i]; 0, s_w)
- *             + log Normal(b[c]; 0, s_b) + log p(sigma_c) + t_c ),       sigma_c = exp(t_c),  t_c = z[c, s_off]
- *   grad[c,:] = dU / dz[c,:]
- * z: [C, Dz] fp32 row-major chain state; w at columns w_off .. w_off + D - 1, b at b_off (only if has_bias), and
- * for a latent noise scale its log at s_off (s_off < 0: the constant noise scale `sigma`, no column), Dz == D +
- * has_bias + (s_off >= 0).  The prior of a latent sigma is s_prior: B2_SIGMA_HALFNORMAL (sp0 = scale),
- * B2_SIGMA_HALFCAUCHY (sp0 = scale), B2_SIGMA_EXPONENTIAL (sp0 = rate) or B2_SIGMA_LOGNORMAL (sp0 = loc, sp1 =
- * scale).  X: [N, D] fp32 row-major, 1 <= D <= 128; y: [N] fp32; both 16-byte aligned.  Any other shape, a
- * non-positive scale or an unknown prior returns B2_ERR_BAD_SHAPE before any CUDA call.  Three launches (pack,
- * kernel + finish of b2_glm_normal_loc, potential finish), no host sync; the prior terms and totals are fp64 in a
- * fixed order.  workspace: b2_glm_normal_potential_workspace() bytes, zero-initialised once.
- */
+#define B2_GLM_NORMAL 3
+#define B2_GLM_BINOMIAL 4
 #define B2_SIGMA_HALFNORMAL 1
 #define B2_SIGMA_HALFCAUCHY 2
 #define B2_SIGMA_EXPONENTIAL 3
 #define B2_SIGMA_LOGNORMAL 4
-int b2_glm_normal_potential(const float* X, const float* y, int64_t N, int D, int has_bias, const float* z,
-                            int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int64_t s_off, double s_w,
-                            double s_b, int s_prior, double sp0, double sp1, double sigma, float* U, float* grad,
-                            void* workspace, size_t workspace_bytes, void* stream);
-size_t b2_glm_normal_potential_workspace(int64_t N, int D, int64_t C);
-
-/*
- * b2_glm_binomial_potential -- HMC / NUTS potential energy and gradient of Bayesian Binomial regression for C
- * chains: w ~ Normal(0, s_w)[D], b ~ Normal(0, s_b) (has_bias), y ~ Binomial(m, logits = X @ w + b), with trials
- * as for b2_glm_binomial_logits (one count or [N] counts, on the device).  z: [C, Dz] fp32 with Dz = D + has_bias,
- * the weights at w_off and the bias at b_off; U: [C], grad: [C, Dz].  Four launches with no host sync (CUDA graph
- * capturable): the pack kernel of b2_glm_potential, b2_glm_binomial_logits with weight -1 and B2_FLAG_GLM_3XTF32
- * (kernel + finish), and the potential finish, which adds the priors in fp64.  Argument checks as for
- * b2_glm_potential and b2_glm_binomial_logits, all before any CUDA call.
- * workspace: b2_glm_binomial_potential_workspace() bytes, zero-initialised once.
- */
-int b2_glm_binomial_potential(const float* X, const float* y, const float* trials, int trials_per_row, int64_t N,
-                              int D, int has_bias, const float* z, int64_t C, int64_t Dz, int64_t w_off,
-                              int64_t b_off, double s_w, double s_b, float* U, float* grad, void* workspace,
-                              size_t workspace_bytes, void* stream);
-size_t b2_glm_binomial_potential_workspace(int64_t N, int D, int64_t C);
-size_t b2_glm_potential_workspace(int kind, int64_t N, int D, int K, int64_t C);
-
-/*
- * b2_glm_scaled_potential -- HMC / NUTS potential energy and gradient of the regressions above with a LATENT
- * weight scale: the hierarchical (w ~ Normal(0, tau)), ARD (w ~ Normal(0, lam)) and horseshoe
- * (w ~ Normal(0, tau * lam)) weight priors, for C chains.  U is the potential of pyro/infer/mcmc/util.py:275-286:
- *   U[c] = -( loglik + SUM_j log Normal(w_j; 0, tau lam_j) + log Normal(b; 0, s_b) + log p(tau) + log p(lam)
- *             [+ log p(sigma)] + t + SUM_j l_j [+ log sigma] ),     tau = e^t, lam_j = e^(l_j)
- *   grad[c,:] = dU / dz[c,:]
- * kind: B2_GLM_BERNOULLI, B2_GLM_CATEGORICAL, B2_GLM_POISSON (as b2_glm_potential), B2_GLM_NORMAL (as
- * b2_glm_normal_potential: s_off, s_prior, sp0, sp1 and sigma; s_off must be < 0 for every other kind) or
- * B2_GLM_BINOMIAL (as b2_glm_binomial_potential: trials, trials_per_row), with their scopes of D and K.
- * z: [C, Dz] fp32 row-major; w (K*D values) at w_off, b (K values, has_bias) at b_off, log sigma at s_off (>= 0),
- * t = log tau at scale->tau_off (>= 0: one column) and l = log lam at scale->lam_off (>= 0: K*D columns, lam_j scales
- * w_j); a -1 offset means absent, and at least one of tau and lam is latent.  Dz is exactly the sum of the present
- * blocks' widths, none overlapping another or leaving the row.  The priors of tau and of every lam_j are
- * B2_SIGMA_* codes with parameters (p0, p1), as for sigma: positive, and for LogNormal a finite loc.
- * X, y (and per-row trials) 16-byte aligned.  Anything else returns B2_ERR_NULL / B2_ERR_BAD_SHAPE /
- * B2_ERR_TOO_LARGE before any CUDA call.  Four launches with no host sync (CUDA graph capturable): the pack kernel,
- * the kind's likelihood call with weight -1 (kernel + finish, every logit fp32-exact), and a potential finish that
- * adds every prior term and Jacobian in fp64 in a fixed order.  workspace: b2_glm_scaled_potential_workspace()
- * bytes, zero-initialised once.
- */
-#define B2_GLM_NORMAL 3
-#define B2_GLM_BINOMIAL 4
 typedef struct b2_glm_weight_scale {
   int64_t tau_off, lam_off;     /* z columns of log tau / log lam, -1 when absent */
   int tau_prior, lam_prior;     /* B2_SIGMA_HALFNORMAL .. B2_SIGMA_LOGNORMAL */
   double tau_p0, tau_p1, lam_p0, lam_p1;
 } b2_glm_weight_scale;
-int b2_glm_scaled_potential(int kind, const float* X, const void* y, const float* trials, int trials_per_row,
-                            int64_t N, int D, int K, int has_bias, const float* z, int64_t C, int64_t Dz,
-                            int64_t w_off, int64_t b_off, int64_t s_off, double s_b, int s_prior, double sp0,
-                            double sp1, double sigma, const b2_glm_weight_scale* scale, float* U, float* grad,
-                            void* workspace, size_t workspace_bytes, void* stream);
-size_t b2_glm_scaled_potential_workspace(int kind, int64_t N, int D, int K, int64_t C);
-
-/*
- * b2_glm_group_potential -- HMC / NUTS potential energy and gradient of multilevel regression: the regressions of
- * b2_glm_scaled_potential with a constant weight scale and a varying intercept by group,
- *   eta[c,n] = <X[n,:], w[c,:]> + b[c] + alpha[c, g[n]],   alpha ~ Normal(0, s_a)[G]         (centred)
- *                                                          alpha = s_a * e, e ~ Normal(0, 1)[G] (non-centred)
- * with s_a the constant s_const or latent (z holds t = log s_a at s_off, prior s_prior with (sp0, sp1) as for a
- * latent sigma).  U is the potential of pyro/infer/mcmc/util.py:275-286, with the Jacobian -t of a latent s_a.
- * The likelihood of all chains is one pass of the kind's fused kernel over [X | onehot(g)]: the group effect is G
- * more columns of the contraction, synthesised in shared memory from g, so X is read once and no [C, N] tensor is
- * made.  A group index outside [0, G) makes U and the group effect's gradient NaN.
- * Varying slopes (ge->S = 1..3; 0, as all-zero trailing fields give, for none): slope k adds beta_k[c, g[n]] *
- * X[n, col_k] to eta, with beta_k ~ Normal(0, s_k)[G] (centred) or beta_k = s_k * e_k, e_k ~ Normal(0, 1)[G]
- * (non-centred), and s_k constant or latent as s_a is.  Its covariate is column col_k of X (0 <= col_k < D, the
- * S columns distinct), so it costs G more columns of the same pass: the likelihood runs at D + G (1 + S) <= 128
- * columns, and a bad group index makes every slope's gradient NaN too.  Each slope's table and latent scale are
- * blocks of z's row like alpha and log s_a.
- * kind: B2_GLM_BERNOULLI (any D), B2_GLM_POISSON, B2_GLM_NORMAL (s_off, s_prior, sp0, sp1 and sigma as for
- * b2_glm_normal_potential; s_off < 0 for every other kind) or B2_GLM_BINOMIAL (trials, trials_per_row), with
- * 1 <= D, 1 <= G and D + G (1 + S) <= 128.  z: [C, Dz] fp32 row-major; w (D values) at w_off, b at b_off (has_bias), log
- * sigma at s_off, alpha or e (G values) at ge->a_off and log s_a at ge->s_off (-1: the constant ge->s_const).  Dz is
- * exactly the sum of the present blocks' widths, none overlapping another or leaving the row.  X, y, ge->groups (and
- * per-row trials) 16-byte aligned.  Anything else returns B2_ERR_NULL / B2_ERR_BAD_SHAPE / B2_ERR_TOO_LARGE before
- * any CUDA call.  Four launches with no host sync (CUDA graph capturable): the pack kernel (each chain's
- * [w | alpha | beta_1 .. beta_S] row), the kind's likelihood call with weight -1 (kernel + finish, every logit fp32-exact), and a potential finish
- * that adds every prior term and Jacobian in fp64 in a fixed order (the slopes' after the intercept's).
- * workspace: b2_glm_group_potential_workspace() bytes, zero-initialised once; its G argument is the number of group
- * columns, G (1 + S).
- */
 typedef struct b2_glm_group_slope {
   int64_t b_off;                /* z columns of beta_k (centred) or e_k (non-centred), G of them */
   int64_t s_off;                /* z column of log s_k, -1 for the constant s_const */
@@ -612,12 +542,26 @@ typedef struct b2_glm_group_effect {
   int S;                        /* varying slopes, 0 <= S <= 3 */
   b2_glm_group_slope slope[3];  /* the first S are read */
 } b2_glm_group_effect;
-int b2_glm_group_potential(int kind, const float* X, const void* y, const float* trials, int trials_per_row,
-                           int64_t N, int D, int has_bias, const float* z, int64_t C, int64_t Dz, int64_t w_off,
-                           int64_t b_off, int64_t s_off, double s_w, double s_b, int s_prior, double sp0, double sp1,
-                           double sigma, const b2_glm_group_effect* ge, float* U, float* grad, void* workspace,
-                           size_t workspace_bytes, void* stream);
-size_t b2_glm_group_potential_workspace(int kind, int64_t N, int D, int G, int64_t C);
+typedef struct b2_glm_regression {
+  int kind;                               /* B2_GLM_BERNOULLI .. B2_GLM_BINOMIAL */
+  const float* X;                         /* [N, D] */
+  const void* y;                          /* [N] */
+  int64_t N;
+  int D, K;
+  const float* trials;                    /* Binomial only: one count or [N] counts */
+  int trials_per_row;
+  int has_bias;
+  int64_t w_off, b_off;                   /* z columns of w (K*D) and b (K, if has_bias) */
+  double s_w, s_b;                        /* constant prior scales of w and b */
+  int64_t s_off;                          /* Normal only: z column of log sigma, -1 for the constant sigma */
+  int s_prior;                            /* B2_SIGMA_* prior of a latent sigma */
+  double sp0, sp1, sigma;
+  const b2_glm_weight_scale* scale;       /* NULL: the constant s_w */
+  const b2_glm_group_effect* group;       /* NULL: no group effect */
+} b2_glm_regression;
+int b2_glm_potential(const b2_glm_regression* m, const float* z, int64_t C, int64_t Dz, float* U, float* grad,
+                     void* workspace, size_t workspace_bytes, void* stream);
+size_t b2_glm_potential_workspace(const b2_glm_regression* m, int64_t C);
 
 /*
  * b2_glm_group_sum -- the fused likelihood term of a regression with a varying intercept by group, for P particles:

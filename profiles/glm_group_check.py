@@ -1,4 +1,4 @@
-"""GPU check of multilevel regression on GlmPotential (b2_glm_group_potential): a varying intercept by group,
+"""GPU check of multilevel regression on GlmPotential (b2_glm_potential): a varying intercept by group,
 ``y ~ Bernoulli(logits = X @ w + b + alpha[g])`` or ``Poisson(rate = exp(X @ w + b + alpha[g]))`` with
 ``alpha ~ Normal(0, s_a)[G]``, ``s_a ~ HalfNormal(1)``:
   * device time of one potential evaluation (U and dU/dz for all chains) at N = 1e5 and 1e6, D = 16, G = 48, C = 64:

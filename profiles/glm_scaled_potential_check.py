@@ -1,4 +1,4 @@
-"""GPU check of the regression potential with a latent weight scale (GlmPotential, b2_glm_scaled_potential) on
+"""GPU check of the regression potential with a latent weight scale (GlmPotential, b2_glm_potential) on
 horseshoe logistic regression, ``tau ~ HalfCauchy(1)``, ``lam ~ HalfCauchy(1)[D]``, ``w ~ Normal(0, tau * lam)``,
 ``b ~ Normal(0, 10)``, ``y ~ Bernoulli(logits = X @ w + b)``:
   * device time of one potential evaluation (U and dU/dz for all chains) at N = 1e6, D = 32 for C = 8, 64, 128

@@ -1,4 +1,4 @@
-"""GPU check of multilevel regression with varying slopes on GlmPotential (b2_glm_group_potential with S slopes):
+"""GPU check of multilevel regression with varying slopes on GlmPotential (b2_glm_potential, S slopes):
 ``y ~ Bernoulli(logits = X @ w + b + alpha[g] + beta[g] * X[:, 0])``, ``alpha ~ Normal(0, s_a)[G]``,
 ``beta ~ Normal(0, s_b)[G]``, latent HalfNormal scales:
   * device time of one potential evaluation (U and dU/dz for all chains) at N = 1e5 and 1e6, D = 16, G = 32, S = 1

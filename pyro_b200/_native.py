@@ -97,6 +97,18 @@ class b2_glm_group_effect(ctypes.Structure):
                 ("S", ctypes.c_int32), ("slope", b2_glm_group_slope * 3)]
 
 
+class b2_glm_regression(ctypes.Structure):
+    """Mirror of ``b2_glm_regression`` (include/pyro_b200.h): the regression model of a potential, its data, z's
+    layout and its optional latent weight scale and group effect."""
+    _fields_ = [("kind", ctypes.c_int32), ("X", ctypes.c_void_p), ("y", ctypes.c_void_p), ("N", ctypes.c_int64),
+                ("D", ctypes.c_int32), ("K", ctypes.c_int32), ("trials", ctypes.c_void_p),
+                ("trials_per_row", ctypes.c_int32), ("has_bias", ctypes.c_int32), ("w_off", ctypes.c_int64),
+                ("b_off", ctypes.c_int64), ("s_w", ctypes.c_double), ("s_b", ctypes.c_double),
+                ("s_off", ctypes.c_int64), ("s_prior", ctypes.c_int32), ("sp0", ctypes.c_double),
+                ("sp1", ctypes.c_double), ("sigma", ctypes.c_double),
+                ("scale", ctypes.POINTER(b2_glm_weight_scale)), ("group", ctypes.POINTER(b2_glm_group_effect))]
+
+
 class b2_nuts_lockstep(ctypes.Structure):
     """Mirror of ``b2_nuts_lockstep`` (include/pyro_b200.h): device pointers of the lockstep tree state."""
     _fields_ = [("zL", ctypes.c_void_p), ("rL", ctypes.c_void_p), ("zR", ctypes.c_void_p),
@@ -153,26 +165,11 @@ SIGNATURES = {
     "b2_glm_binomial_logits": (_i32, [_vp, _vp, _vp, _i32, _vp, _vp, _i64, _i32, _i32, _f64, _f64, _f64, _i32,
                                       _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2_glm_binomial_workspace": (_sz, [_i64, _i32, _i32]),
-    "b2_glm_binomial_potential": (_i32, [_vp, _vp, _vp, _i32, _i64, _i32, _i32, _vp, _i64, _i64, _i64, _i64, _f64,
-                                         _f64, _vp, _vp, _vp, _sz, _vp]),
-    "b2_glm_binomial_potential_workspace": (_sz, [_i64, _i32, _i64]),
-    "b2_glm_normal_potential": (_i32, [_vp, _vp, _i64, _i32, _i32, _vp, _i64, _i64, _i64, _i64, _i64, _f64, _f64,
-                                       _i32, _f64, _f64, _f64, _vp, _vp, _vp, _sz, _vp]),
-    "b2_glm_normal_potential_workspace": (_sz, [_i64, _i32, _i64]),
     "b2_poisson_product": (_i32, [_vp, _vp, _vp, _i64, _i32, _i64, _i32, _f64, _f64, _f64, _i32, _vp, _vp, _vp,
                                   _vp, _vp, _sz, _vp]),
     "b2_poisson_product_workspace": (_sz, [_i64, _i32, _i64, _i32]),
-    "b2_glm_potential": (_i32, [_i32, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _i64, _i64, _f64, _f64,
-                                _vp, _vp, _vp, _sz, _vp]),
-    "b2_glm_potential_workspace": (_sz, [_i32, _i64, _i32, _i32, _i64]),
-    "b2_glm_scaled_potential": (_i32, [_i32, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _i32, _vp, _i64, _i64, _i64,
-                                       _i64, _i64, _f64, _i32, _f64, _f64, _f64,
-                                       ctypes.POINTER(b2_glm_weight_scale), _vp, _vp, _vp, _sz, _vp]),
-    "b2_glm_scaled_potential_workspace": (_sz, [_i32, _i64, _i32, _i32, _i64]),
-    "b2_glm_group_potential": (_i32, [_i32, _vp, _vp, _vp, _i32, _i64, _i32, _i32, _vp, _i64, _i64, _i64, _i64,
-                                      _i64, _f64, _f64, _i32, _f64, _f64, _f64,
-                                      ctypes.POINTER(b2_glm_group_effect), _vp, _vp, _vp, _sz, _vp]),
-    "b2_glm_group_potential_workspace": (_sz, [_i32, _i64, _i32, _i32, _i64]),
+    "b2_glm_potential": (_i32, [ctypes.POINTER(b2_glm_regression), _vp, _i64, _i64, _vp, _vp, _vp, _sz, _vp]),
+    "b2_glm_potential_workspace": (_sz, [ctypes.POINTER(b2_glm_regression), _i64]),
     "b2_glm_group_sum": (_i32, [_i32, _vp, _vp, _vp, _i32, _vp, _i32, _vp, _i32, _vp, _i64, _vp, _i64, _vp, _i64,
                                 _i32, _i32, _f64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2_glm_group_sum_workspace": (_sz, [_i32, _i64, _i32, _i32, _i32]),

@@ -1,29 +1,27 @@
 // glm_potential.cu -- HMC / NUTS potential energy of Bayesian logistic, softmax, Poisson, Binomial and linear
-// regression for C chains.
+// regression for C chains: b2_glm_potential on one b2_glm_regression.
 //
-//   U[c]    = -( SUM_n log p(y_n | logits_cn) + SUM log Normal(w; 0, s_w) + SUM log Normal(b; 0, s_b) )
+//   U[c]    = -( SUM_n log p(y_n | logits_cn) + log p(w) + log p(b) [+ log p(sigma)] [+ group effect] ) + Jacobians
 //   grad[c] = dU / dz[c]                                           (in z's layout)
 //
-// The likelihood and its gradient come from the fused GLM likelihood entry points (b2_glm_bernoulli_logits,
-// b2_glm_categorical_logits, b2_glm_poisson_log_rate, b2_glm_normal_loc, b2_glm_binomial_logits: a tile kernel and
+// The likelihood and its gradient come from the fused GLM likelihood calls (glm_bernoulli_logits,
+// b2_glm_categorical_logits, glm_poisson_log_rate, glm_normal_loc, glm_binomial_logits: a tile kernel and
 // glm_finish_kernel each) with their particle axis set to the chains, so X is read once per evaluation for every
-// chain together.  Each entry point checks its own arguments, then glm_potential_run makes the one fixed launch
-// sequence, with no host sync (CUDA graph capturable):
-//   1. glm_potential_pack_kernel    z's weight / bias columns -> the contiguous [C, K*D] / [C, K] operands
-//                                   (z's rows also hold the other site, so their stride is not the kernels')
+// chain together.  b2_glm_potential checks every argument, then makes the one fixed launch sequence, with no host
+// sync (CUDA graph capturable):
+//   1. glm_potential_pack_kernel    z's weight / bias columns -> the contiguous [C, KD] / [C, K] operands
+//                                   (z's rows also hold the other sites, so their stride is not the kernels')
 //   2. the likelihood call          weight = -1: dW, db are d(-loglik)/dW, d(-loglik)/db; sum_p = loglik
-//   3. glm_potential_finish_kernel  adds the Normal prior value and gradient, one warp per chain, fp64
-//                                   accumulation in a fixed order, and writes U and grad
+//   3. glm_potential_finish_kernel  adds the priors' values and gradients, one warp per chain, fp64 accumulation
+//                                   in a fixed order, and writes U and grad
 // The GLM kernels always run with every logit fp32-exact (B2_FLAG_GLM_3XTF32; the Normal kernels always split X),
 // so the sampler targets the posterior of the data as given, not of X rounded to TF32.
 // With a noise scale (linear regression) the pack also writes each chain's sigma_c = exp(z[c, s_off]) (or the
 // constant), and the finish adds sigma's prior and the Jacobian of sigma = e^t in fp64.  Binomial regression passes
-// the trial counts to its likelihood call as a fixed operand.  b2_glm_scaled_potential runs the same sequence for a
-// latent weight scale (w ~ Normal(0, tau * lam)), with glm_scaled_potential_finish_kernel as step 3, and
-// b2_glm_group_potential for a varying intercept alpha[g] by group and up to three varying slopes beta_k[g] on
-// columns of X: glm_group_potential_pack_kernel writes [w | alpha | beta_1 ..] as each chain's weight row, the
-// likelihood runs on [X | onehot(g) | x_{c_1} onehot(g) ..] (glm_flat_tc.cuh GROUPS), and
-// glm_group_potential_finish_kernel is step 3.
+// the trial counts to its likelihood call as a fixed operand.  A latent weight scale (w ~ Normal(0, tau * lam))
+// changes only the finish's weight terms.  A group effect, a varying intercept alpha[g] and up to three varying
+// slopes beta_k[g] on columns of X, makes each chain's packed weight row [w | alpha | beta_1 ..], and the likelihood
+// runs on [X | onehot(g) | x_{c_1} onehot(g) ..] (glm_flat_tc.cuh GROUPS).
 #include <math.h>
 
 #include "b2_common.cuh"
@@ -31,42 +29,26 @@
 
 namespace b2 {
 
-// sig (linear regression only, else null): sig[c] = exp(z[c, s_off]) for a latent noise scale (z holds its log),
-// the constant s_const when s_off < 0.  A group effect's weight rows are glm_group_potential_pack_kernel's.
-__global__ void __launch_bounds__(256) glm_potential_pack_kernel(const float* __restrict__ z, int64_t C,
-                                                                 int64_t Dz, int64_t w_off, int64_t b_off,
-                                                                 int KD, int Kb, float* __restrict__ Wp,
-                                                                 float* __restrict__ bp, int64_t s_off,
-                                                                 float s_const, float* __restrict__ sig) {
+// Each chain's weight row [w | alpha | beta_1 .. beta_S], KD = D + G (1 + S) wide with a group effect (GROUP; else
+// KD = K*D and ge is not read).  Group block 0 is alpha, block k slope k; each is z's columns, or s * eta for a
+// non-centred block (s its scale: exp of its z column, or its constant).  sig (linear regression only, else null):
+// sig[c] = exp(z[c, s_off]) for a latent noise scale (z holds its log), the constant s_const when s_off < 0.
+template <bool GROUP>
+__global__ void __launch_bounds__(256) glm_potential_pack_kernel(const float* __restrict__ z, int64_t C, int64_t Dz,
+                                                                 int64_t w_off, int64_t b_off, int KD, int Kb,
+                                                                 float* __restrict__ Wp, float* __restrict__ bp,
+                                                                 int64_t s_off, float s_const,
+                                                                 float* __restrict__ sig, b2_glm_group_effect ge) {
   const int64_t per = KD + Kb;
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (sig != nullptr && i < C) sig[i] = s_off >= 0 ? expf(z[i * Dz + s_off]) : s_const;
   if (i >= C * per) return;
   const int64_t c = i / per;
   const int64_t j = i - c * per;
-  if (j < KD) Wp[c * KD + j] = z[c * Dz + w_off + j];
-  else bp[c * Kb + (j - KD)] = z[c * Dz + b_off + (j - KD)];
-}
-
-// glm_potential_pack_kernel for a group effect: each chain's weight row is [w | alpha | beta_1 .. beta_S], KD =
-// D + G (1 + S) wide.  Block 0 is alpha, block k slope k; each is z's columns, or s * eta for a non-centred block
-// (s its scale: exp of its z column, or its constant).
-__global__ void __launch_bounds__(256) glm_group_potential_pack_kernel(const float* __restrict__ z, int64_t C,
-                                                                       int64_t Dz, int64_t w_off, int64_t b_off,
-                                                                       int KD, int Kb, float* __restrict__ Wp,
-                                                                       float* __restrict__ bp, int64_t s_off,
-                                                                       float s_const, float* __restrict__ sig,
-                                                                       b2_glm_group_effect ge) {
-  const int64_t per = KD + Kb;
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (sig != nullptr && i < C) sig[i] = s_off >= 0 ? expf(z[i * Dz + s_off]) : s_const;
-  if (i >= C * per) return;
-  const int64_t c = i / per;
-  const int64_t j = i - c * per;
-  const int D = KD - ge.G * (1 + ge.S);
+  const int D = GROUP ? KD - ge.G * (1 + ge.S) : KD;
   if (j < D) {
     Wp[c * KD + j] = z[c * Dz + w_off + j];
-  } else if (j < KD) {
+  } else if (GROUP && j < KD) {
     const int k = (int)(j - D) / ge.G, a = (int)(j - D) - k * ge.G;   // block k, group a
     int64_t off = ge.a_off, so = ge.s_off;
     int nc = ge.noncentred;
@@ -90,7 +72,8 @@ __global__ void __launch_bounds__(256) glm_group_potential_pack_kernel(const flo
 constexpr double kHalfLog2Pi = 0.91893853320467274178;
 
 // log p(v) and d log p / dv of a positive scale v under prior code `prior` (B2_SIGMA_*): HalfNormal(p0),
-// HalfCauchy(p0), Exponential(p0) or LogNormal(p0, p1).  The priors of a noise scale and of a weight scale.
+// HalfCauchy(p0), Exponential(p0) or LogNormal(p0, p1).  The priors of a noise scale, a weight scale and a group
+// effect's scale.
 __device__ __forceinline__ void positive_prior(int prior, double p0, double p1, double v, double& lp, double& dlp) {
   constexpr double kLog2 = 0.69314718055994531, kLogPi = 1.14472988584940017;
   if (prior == B2_SIGMA_HALFNORMAL) {             // p0 = scale
@@ -131,70 +114,104 @@ __device__ __forceinline__ void add_latent_sigma_terms(const float* zc, float* g
   gc[s_off] = (float)(v * ((double)dsig[c] - dlp) - 1.0);
 }
 
+// One block of a group effect (the intercept, described as a slope, or a slope): its G values v_g at z columns
+// b.b_off (alpha_g or beta_k,g when centred, e_g when non-centred) with the scale s = e^t, t = z[c, b.s_off] (or the
+// constant b.s_const), and dWb[g] = d(-loglik)/d(the block's coefficient of group g):
+//   centred      U += v_g^2 / (2 s^2) + log s + log(2 pi) / 2    dU/dv_g = dWb_g + v_g / s^2
+//                dU/dt = SUM_g (1 - v_g^2 / s^2) - s (d log p / ds)(s) - 1
+//   non-centred  U += v_g^2 / 2 + log(2 pi) / 2                  dU/dv_g = s dWb_g + v_g
+//                dU/dt = s SUM_g v_g dWb_g - s (d log p / ds)(s) - 1
+// and for a latent s once per chain U += -log p(s) - t.  Lane-strided over the G values, then the shuffle tree:
+// writes dU/dv_g and returns, in every lane, t, s and the warp's sums u (the block's terms of U but G log s) and h
+// (dU/dt before the prior's terms).
+struct GroupBlockSums {
+  double t, s, u, h;
+};
+
+__device__ __forceinline__ GroupBlockSums group_block_sums(const b2_glm_group_slope& b, int G, const float* zc,
+                                                           float* gc, const float* dWb, int lane) {
+  GroupBlockSums r;
+  r.t = b.s_off >= 0 ? (double)zc[b.s_off] : 0.0;
+  r.s = b.s_off >= 0 ? exp(r.t) : b.s_const;
+  const double is2 = 1.0 / (r.s * r.s);
+  double u = 0.0, h = 0.0;
+  for (int j = lane; j < G; j += 32) {
+    const double v = (double)zc[b.b_off + j], g = (double)dWb[j];
+    if (b.noncentred) {
+      u += 0.5 * v * v + kHalfLog2Pi;
+      h += r.s * v * g;
+      gc[b.b_off + j] = (float)(r.s * g + v);
+    } else {
+      const double q = v * v * is2;
+      u += 0.5 * q + kHalfLog2Pi;
+      h += 1.0 - q;
+      gc[b.b_off + j] = (float)(g + v * is2);
+    }
+  }
+  r.u = warp_sum(u);
+  r.h = warp_sum(h);
+  return r;
+}
+
+// lane 0: a group block's terms of U, G log s for a centred one last
+__device__ __forceinline__ void add_group_block_u(const b2_glm_group_slope& b, int G, const GroupBlockSums& r,
+                                                  double& u) {
+  u += r.u;
+  if (!b.noncentred) u += (double)G * log(r.s);
+}
+
+// One warp per chain, fp64, lane-strided over each block of coefficients and then the shuffle tree, so every result
+// is in a fixed order.  The weight prior over the D = KD - G (1 + S) coefficients of w is the constant-scale
+//   U += SUM_j w_j^2 / (2 s_w^2) + D (log s_w + log(2 pi) / 2)    dU/dw_j = dW_j + w_j / s_w^2
+// or, with a latent weight scale (LATENT: ws), per coefficient j, with s_j = tau lam_j and a_j = 1 - w_j^2 / s_j^2:
+//   U += w_j^2 / (2 s_j^2) + log s_j + log(2 pi) / 2           dU/dw_j = dW_j + w_j / s_j^2
+//   U += -log p(lam_j) - l_j                                   dU/dl_j = a_j - lam_j (d log p / d lam)(lam_j) - 1
+// and once per chain U += -log p(tau) - t, dU/dt = SUM_j a_j - tau (d log p / d tau)(tau) - 1.  Then come the bias
+// prior, the noise scale's terms and, with a group effect (GROUP: ge), its blocks: the intercept block's U terms
+// before the bias prior and its latent scale's after the noise scale's, then each slope block, in the order of k.
+// LATENT and GROUP are template flags, so each configuration runs only its own code.
+template <bool LATENT, bool GROUP>
 __global__ void __launch_bounds__(256) glm_potential_finish_kernel(
     const float* __restrict__ z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int KD, int Kb, double s_w,
     double s_b, const float* __restrict__ sum_p, const float* __restrict__ dW, const float* __restrict__ db,
     float* __restrict__ U, float* __restrict__ grad, const float* __restrict__ sig, const float* __restrict__ dsig,
-    int64_t s_off, int s_prior, double sp0, double sp1) {
+    int64_t s_off, int s_prior, double sp0, double sp1, b2_glm_weight_scale ws, b2_glm_group_effect ge) {
   const int64_t c = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (c >= C) return;
-  const double iw = 1.0 / (s_w * s_w);
+  const int D = GROUP ? KD - ge.G * (1 + ge.S) : KD;
   const double ib = Kb ? 1.0 / (s_b * s_b) : 0.0;
   const float* zc = z + c * Dz;
   float* gc = grad + c * Dz;
-  double qw = 0.0, qb = 0.0;  // SUM w^2 / s_w^2, SUM b^2 / s_b^2
-  for (int j = lane; j < KD; j += 32) {
-    const double v = (double)zc[w_off + j];
-    qw += v * v * iw;
-    gc[w_off + j] = (float)((double)dW[c * KD + j] + v * iw);
-  }
-  for (int j = lane; j < Kb; j += 32) {
-    const double v = (double)zc[b_off + j];
-    qb += v * v * ib;
-    gc[b_off + j] = (float)((double)db[c * Kb + j] + v * ib);
-  }
-  qw = warp_sum(qw);
-  qb = warp_sum(qb);
-  if (lane == 0) {
-    double u = -(double)sum_p[c] + 0.5 * qw + (double)KD * (log(s_w) + kHalfLog2Pi);
-    if (Kb) u += 0.5 * qb + (double)Kb * (log(s_b) + kHalfLog2Pi);
-    if (sig != nullptr && s_off >= 0) add_latent_sigma_terms(zc, gc, s_off, sig, dsig, c, s_prior, sp0, sp1, u);
-    U[c] = (float)u;
-  }
-}
-
-// glm_potential_finish_kernel with a latent weight scale: one warp per chain, fp64, lane-strided over the KD
-// coefficients and then the shuffle tree, so every result is in a fixed order.  Per coefficient j, with
-// s_j = tau lam_j and a_j = 1 - w_j^2 / s_j^2:
-//   U += w_j^2 / (2 s_j^2) + log s_j + log(2 pi) / 2           dU/dw_j = dW_j + w_j / s_j^2
-//   U += -log p(lam_j) - l_j                                   dU/dl_j = a_j - lam_j (d log p / d lam)(lam_j) - 1
-// and once per chain U += -log p(tau) - t, dU/dt = SUM_j a_j - tau (d log p / d tau)(tau) - 1.  The bias prior and
-// the noise scale's terms are those of glm_potential_finish_kernel.
-__global__ void __launch_bounds__(256) glm_scaled_potential_finish_kernel(
-    const float* __restrict__ z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int KD, int Kb, double s_b,
-    const float* __restrict__ sum_p, const float* __restrict__ dW, const float* __restrict__ db,
-    float* __restrict__ U, float* __restrict__ grad, const float* __restrict__ sig, const float* __restrict__ dsig,
-    int64_t s_off, int s_prior, double sp0, double sp1, b2_glm_weight_scale ws) {
-  const int64_t c = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (c >= C) return;
-  const double ib = Kb ? 1.0 / (s_b * s_b) : 0.0;
-  const float* zc = z + c * Dz;
-  float* gc = grad + c * Dz;
-  const double t = ws.tau_off >= 0 ? (double)zc[ws.tau_off] : 0.0;
-  double uw = 0.0, asum = 0.0, qb = 0.0;  // the weight and lam terms of U, SUM a_j, SUM b^2 / s_b^2
-  for (int j = lane; j < KD; j += 32) {
-    const double v = (double)zc[w_off + j];
-    const double l = ws.lam_off >= 0 ? (double)zc[ws.lam_off + j] : 0.0;
-    const double ls = t + l;               // log s_j
-    const double is2 = exp(-2.0 * ls);     // 1 / s_j^2
-    const double q = v * v * is2;
-    uw += 0.5 * q + ls + kHalfLog2Pi;
-    gc[w_off + j] = (float)((double)dW[c * KD + j] + v * is2);
-    const double a = 1.0 - q;
-    asum += a;
-    if (ws.lam_off >= 0) gc[ws.lam_off + j] = (float)latent_scale_terms(ws.lam_prior, ws.lam_p0, ws.lam_p1, l, a, uw);
+  const float* dWc = dW + c * KD;
+  const double t = LATENT && ws.tau_off >= 0 ? (double)zc[ws.tau_off] : 0.0;
+  const b2_glm_group_slope icpt = {ge.a_off, ge.s_off, 0, ge.noncentred, ge.s_prior, ge.s_const, ge.sp0, ge.sp1};
+  GroupBlockSums a = {};
+  if (GROUP) a = group_block_sums(icpt, ge.G, zc, gc, dWc + D, lane);
+  // uw: SUM w^2 / s_w^2 for a constant weight scale, the weight and lam terms of U for a latent one; asum: SUM a_j;
+  // qb: SUM b^2 / s_b^2
+  double uw = 0.0, asum = 0.0, qb = 0.0;
+  if (LATENT) {
+    for (int j = lane; j < D; j += 32) {
+      const double v = (double)zc[w_off + j];
+      const double l = ws.lam_off >= 0 ? (double)zc[ws.lam_off + j] : 0.0;
+      const double ls = t + l;               // log s_j
+      const double is2 = exp(-2.0 * ls);     // 1 / s_j^2
+      const double q = v * v * is2;
+      uw += 0.5 * q + ls + kHalfLog2Pi;
+      gc[w_off + j] = (float)((double)dWc[j] + v * is2);
+      const double a = 1.0 - q;
+      asum += a;
+      if (ws.lam_off >= 0)
+        gc[ws.lam_off + j] = (float)latent_scale_terms(ws.lam_prior, ws.lam_p0, ws.lam_p1, l, a, uw);
+    }
+  } else {
+    const double iw = 1.0 / (s_w * s_w);
+    for (int j = lane; j < D; j += 32) {
+      const double v = (double)zc[w_off + j];
+      uw += v * v * iw;
+      gc[w_off + j] = (float)((double)dWc[j] + v * iw);
+    }
   }
   for (int j = lane; j < Kb; j += 32) {
     const double v = (double)zc[b_off + j];
@@ -202,128 +219,79 @@ __global__ void __launch_bounds__(256) glm_scaled_potential_finish_kernel(
     gc[b_off + j] = (float)((double)db[c * Kb + j] + v * ib);
   }
   uw = warp_sum(uw);
-  asum = warp_sum(asum);
+  if (LATENT) asum = warp_sum(asum);
   qb = warp_sum(qb);
-  if (lane == 0) {
-    double u = -(double)sum_p[c] + uw;
-    if (Kb) u += 0.5 * qb + (double)Kb * (log(s_b) + kHalfLog2Pi);
-    if (sig != nullptr && s_off >= 0) add_latent_sigma_terms(zc, gc, s_off, sig, dsig, c, s_prior, sp0, sp1, u);
-    if (ws.tau_off >= 0) gc[ws.tau_off] = (float)latent_scale_terms(ws.tau_prior, ws.tau_p0, ws.tau_p1, t, asum, u);
-    U[c] = (float)u;
-  }
-}
-
-// glm_potential_finish_kernel with a group effect alpha (ge.G values after w in each chain's [w | alpha | beta_1 ..]
-// row of dW, KD = D + G (1 + S) wide): one warp per chain, fp64, lane-strided over the coefficients and then the
-// shuffle tree, so every result is in a fixed order.  With s = s_a (= e^t when latent) and dW_g = d(-loglik)/d alpha_g:
-//   centred      U += alpha_g^2 / (2 s^2) + log s + log(2 pi) / 2    dU/dalpha_g = dW_g + alpha_g / s^2
-//                dU/dt = SUM_g (1 - alpha_g^2 / s^2) - s (d log p / ds)(s) - 1
-//   non-centred  U += eta_g^2 / 2 + log(2 pi) / 2                    dU/deta_g = s dW_g + eta_g
-//                dU/dt = s SUM_g eta_g dW_g - s (d log p / ds)(s) - 1
-// and for a latent s once per chain U += -log p(s) - t.  The weight and bias priors and the noise scale's terms
-// are those of glm_potential_finish_kernel.  Each slope block k (beta_k or e_k, scale s_k) then adds the same terms
-// with its own dW columns and scale, after every term of the intercept-only potential, in the order of k.
-__global__ void __launch_bounds__(256) glm_group_potential_finish_kernel(
-    const float* __restrict__ z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int KD, int Kb, double s_w,
-    double s_b, const float* __restrict__ sum_p, const float* __restrict__ dW, const float* __restrict__ db,
-    float* __restrict__ U, float* __restrict__ grad, const float* __restrict__ sig, const float* __restrict__ dsig,
-    int64_t s_off, int s_prior, double sp0, double sp1, b2_glm_group_effect ge) {
-  const int64_t c = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (c >= C) return;
-  const int D = KD - ge.G * (1 + ge.S);
-  const double iw = 1.0 / (s_w * s_w);
-  const double ib = Kb ? 1.0 / (s_b * s_b) : 0.0;
-  const float* zc = z + c * Dz;
-  float* gc = grad + c * Dz;
-  const float* dWc = dW + c * KD;
-  const double t = ge.s_off >= 0 ? (double)zc[ge.s_off] : 0.0;
-  const double sa = ge.s_off >= 0 ? exp(t) : ge.s_const, isa2 = 1.0 / (sa * sa);
-  double qw = 0.0, qb = 0.0, ua = 0.0, h = 0.0;  // SUM w^2 / s_w^2, SUM b^2 / s_b^2, the alpha terms of U, dU/dt
-  for (int j = lane; j < D; j += 32) {
-    const double v = (double)zc[w_off + j];
-    qw += v * v * iw;
-    gc[w_off + j] = (float)((double)dWc[j] + v * iw);
-  }
-  for (int j = lane; j < ge.G; j += 32) {
-    const double v = (double)zc[ge.a_off + j], g = (double)dWc[D + j];
-    if (ge.noncentred) {
-      ua += 0.5 * v * v + kHalfLog2Pi;
-      h += sa * v * g;
-      gc[ge.a_off + j] = (float)(sa * g + v);
-    } else {
-      const double q = v * v * isa2;
-      ua += 0.5 * q + kHalfLog2Pi;
-      h += 1.0 - q;
-      gc[ge.a_off + j] = (float)(g + v * isa2);
-    }
-  }
-  for (int j = lane; j < Kb; j += 32) {
-    const double v = (double)zc[b_off + j];
-    qb += v * v * ib;
-    gc[b_off + j] = (float)((double)db[c * Kb + j] + v * ib);
-  }
-  qw = warp_sum(qw);
-  qb = warp_sum(qb);
-  ua = warp_sum(ua);
-  h = warp_sum(h);
   double u = 0.0;
   if (lane == 0) {
-    u = -(double)sum_p[c] + 0.5 * qw + (double)D * (log(s_w) + kHalfLog2Pi) + ua;
-    if (!ge.noncentred) u += (double)ge.G * log(sa);
+    u = LATENT ? -(double)sum_p[c] + uw : -(double)sum_p[c] + 0.5 * uw + (double)D * (log(s_w) + kHalfLog2Pi);
+    if (GROUP) add_group_block_u(icpt, ge.G, a, u);
     if (Kb) u += 0.5 * qb + (double)Kb * (log(s_b) + kHalfLog2Pi);
     if (sig != nullptr && s_off >= 0) add_latent_sigma_terms(zc, gc, s_off, sig, dsig, c, s_prior, sp0, sp1, u);
-    if (ge.s_off >= 0) gc[ge.s_off] = (float)latent_scale_terms(ge.s_prior, ge.sp0, ge.sp1, t, h, u);
+    if (LATENT && ws.tau_off >= 0)
+      gc[ws.tau_off] = (float)latent_scale_terms(ws.tau_prior, ws.tau_p0, ws.tau_p1, t, asum, u);
+    if (GROUP && ge.s_off >= 0) gc[ge.s_off] = (float)latent_scale_terms(ge.s_prior, ge.sp0, ge.sp1, a.t, a.h, u);
   }
-  for (int k = 0; k < ge.S; ++k) {
+  for (int k = 0; GROUP && k < ge.S; ++k) {
     const b2_glm_group_slope& sl = ge.slope[k];
-    const float* dWk = dWc + D + (k + 1) * ge.G;
-    const double tk = sl.s_off >= 0 ? (double)zc[sl.s_off] : 0.0;
-    const double sk = sl.s_off >= 0 ? exp(tk) : sl.s_const, isk2 = 1.0 / (sk * sk);
-    double ub = 0.0, hb = 0.0;                 // the block's terms of U, dU/dt_k
-    for (int j = lane; j < ge.G; j += 32) {
-      const double v = (double)zc[sl.b_off + j], g = (double)dWk[j];
-      if (sl.noncentred) {
-        ub += 0.5 * v * v + kHalfLog2Pi;
-        hb += sk * v * g;
-        gc[sl.b_off + j] = (float)(sk * g + v);
-      } else {
-        const double q = v * v * isk2;
-        ub += 0.5 * q + kHalfLog2Pi;
-        hb += 1.0 - q;
-        gc[sl.b_off + j] = (float)(g + v * isk2);
-      }
-    }
-    ub = warp_sum(ub);
-    hb = warp_sum(hb);
+    const GroupBlockSums b = group_block_sums(sl, ge.G, zc, gc, dWc + D + (k + 1) * ge.G, lane);
     if (lane == 0) {
-      u += ub;
-      if (!sl.noncentred) u += (double)ge.G * log(sk);
-      if (sl.s_off >= 0) gc[sl.s_off] = (float)latent_scale_terms(sl.s_prior, sl.sp0, sl.sp1, tk, hb, u);
+      add_group_block_u(sl, ge.G, b, u);
+      if (sl.s_off >= 0) gc[sl.s_off] = (float)latent_scale_terms(sl.s_prior, sl.sp0, sl.sp1, b.t, b.h, u);
     }
   }
   if (lane == 0) U[c] = (float)u;
 }
 
-// workspace areas, each 256-byte aligned: [likelihood workspace of lik_bytes][Wp][bp][dW][db][sum_p], then with a
-// noise scale [sig][dsig]
+// the group columns of the likelihood's contraction, G (1 + S); 0 without a group effect
+inline int glm_group_cols(const b2_glm_regression& m) { return m.group ? m.group->G * (1 + m.group->S) : 0; }
+
+// The kinds and widths the likelihood kernels take (K == 1 except for softmax).  With a group effect: every kind
+// but softmax, any D with D + G (1 + S) <= 128 columns, and a constant weight scale.
+inline bool glm_regression_in_scope(const b2_glm_regression& m, int64_t C) {
+  if (m.N < 1 || C < 1 || C >= ((int64_t)1 << 31)) return false;
+  if (m.group) {
+    const b2_glm_group_effect& g = *m.group;
+    if (m.scale || g.S < 0 || g.S > 3 || g.G < 1 || g.G > 128) return false;
+    return (m.kind == B2_GLM_BERNOULLI || m.kind == B2_GLM_POISSON || m.kind == B2_GLM_NORMAL ||
+            m.kind == B2_GLM_BINOMIAL) &&
+           m.K == 1 && m.D >= 1 && m.D + glm_group_cols(m) <= 128;
+  }
+  if (m.kind == B2_GLM_BERNOULLI) return m.K == 1 && (m.D == 4 || m.D == 8 || m.D == 16 || m.D == 32);
+  if (m.kind == B2_GLM_CATEGORICAL) return m.D == 32 && m.K >= 2 && m.K <= 16;
+  if (m.kind == B2_GLM_POISSON || m.kind == B2_GLM_NORMAL || m.kind == B2_GLM_BINOMIAL)
+    return m.K == 1 && m.D >= 1 && m.D <= 128;
+  return false;
+}
+
+// workspace areas, each 256-byte aligned: [likelihood workspace][Wp][bp][dW][db][sum_p], then for linear
+// regression [sig][dsig]
 struct GlmPotentialLayout {
   size_t wp, bp, dw, db, sum_p, sig, dsig, total;
 };
 
 inline size_t round256(size_t b) { return (b + 255) & ~(size_t)255; }
 
-inline GlmPotentialLayout glm_potential_layout(size_t lik_bytes, int64_t KD, int K, int64_t C, bool with_sigma) {
+// the layout of an in-scope regression
+inline GlmPotentialLayout glm_potential_layout(const b2_glm_regression& m, int64_t C) {
+  const int Da = m.D + glm_group_cols(m);
+  size_t lik_bytes;
+  switch (m.kind) {
+    case B2_GLM_BERNOULLI: lik_bytes = b2_glm_workspace(m.N, Da, (int)C); break;
+    case B2_GLM_POISSON: lik_bytes = b2_glm_poisson_workspace(m.N, Da, (int)C); break;
+    case B2_GLM_NORMAL: lik_bytes = b2_glm_normal_workspace(m.N, Da, (int)C); break;
+    case B2_GLM_BINOMIAL: lik_bytes = b2_glm_binomial_workspace(m.N, Da, (int)C); break;
+    default: lik_bytes = b2_glm_categorical_workspace(m.N, Da, m.K, (int)C);
+  }
   GlmPotentialLayout L;
-  const size_t kd = (size_t)KD, c = (size_t)C;
+  const size_t kd = (size_t)m.K * m.D + glm_group_cols(m), k = (size_t)m.K, c = (size_t)C;
   size_t off = round256(lik_bytes);
   L.wp = off; off += round256(c * kd * sizeof(float));
-  L.bp = off; off += round256(c * K * sizeof(float));
+  L.bp = off; off += round256(c * k * sizeof(float));
   L.dw = off; off += round256(c * kd * sizeof(float));
-  L.db = off; off += round256(c * K * sizeof(float));
+  L.db = off; off += round256(c * k * sizeof(float));
   L.sum_p = off; off += round256(c * sizeof(float));
   L.sig = L.dsig = 0;
-  if (with_sigma) {
+  if (m.kind == B2_GLM_NORMAL) {
     L.sig = off; off += round256(c * sizeof(float));
     L.dsig = off; off += round256(c * sizeof(float));
   }
@@ -331,120 +299,31 @@ inline GlmPotentialLayout glm_potential_layout(size_t lik_bytes, int64_t KD, int
   return L;
 }
 
-// The noise scale of linear regression: latent when s_off >= 0 (z[c, s_off] holds its log; prior s_prior with
-// parameters sp0, sp1), else the constant s_const.
-struct PotentialSigma {
-  int64_t s_off;
-  float s_const;
-  int s_prior;
-  double sp0, sp1;
-};
-
-// One potential evaluation after the entry point's own checks: pack -> likelihood -> potential finish.
-// lik(Wp, bp, sig, dsig, sum_p, dW, db, ws, ws_bytes) makes the likelihood call on the chains' packed operands
-// with weight -1, writing sum_p, dW, db (and dsig) into the layout's areas, and returns its B2 code.  sg is
-// null without a noise scale; wsc is null for a constant weight scale s_w, else the latent weight scale, finished
-// by glm_scaled_potential_finish_kernel.  ge is null without a group effect, else KD counts its G columns and
-// glm_group_potential_finish_kernel finishes.
-template <class Likelihood>
-int glm_potential_run(size_t lik_bytes, const float* z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int KD,
-                      int K, int has_bias, double s_w, double s_b, const PotentialSigma* sg,
-                      const b2_glm_weight_scale* wsc, const b2_glm_group_effect* ge, float* U, float* grad,
-                      void* workspace, size_t workspace_bytes, cudaStream_t s, Likelihood lik) {
-  const GlmPotentialLayout L = glm_potential_layout(lik_bytes, KD, K, C, sg != nullptr);
-  if (!workspace || workspace_bytes < L.total) return B2_ERR_WORKSPACE;
-  const int Kb = has_bias ? K : 0;
-  char* ws = reinterpret_cast<char*>(workspace);
-  float* Wp = reinterpret_cast<float*>(ws + L.wp);
-  float* bp = has_bias ? reinterpret_cast<float*>(ws + L.bp) : nullptr;
-  float* dW = reinterpret_cast<float*>(ws + L.dw);
-  float* db = has_bias ? reinterpret_cast<float*>(ws + L.db) : nullptr;
-  float* sum_p = reinterpret_cast<float*>(ws + L.sum_p);
-  float* sig = sg ? reinterpret_cast<float*>(ws + L.sig) : nullptr;
-  float* dsig = sg ? reinterpret_cast<float*>(ws + L.dsig) : nullptr;
-  const int64_t s_off = sg ? sg->s_off : -1;
-
-  const int64_t npack = C * (KD + Kb);
-  if (ge != nullptr)
-    glm_group_potential_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(
-        z, C, Dz, w_off, b_off, KD, Kb, Wp, bp, s_off, sg ? sg->s_const : 0.f, sig, *ge);
-  else
-    glm_potential_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, Wp, bp,
-                                                                               s_off, sg ? sg->s_const : 0.f, sig);
-  count_launch(1);
-  int rc = check_launch();
-  if (rc != 0) return rc;
-  rc = lik(Wp, bp, sig, dsig, sum_p, dW, db, ws, L.wp);
-  if (rc != 0) return rc;
-  const unsigned grid = (unsigned)((C * 32 + 255) / 256);
-  if (ge != nullptr)
-    glm_group_potential_finish_kernel<<<grid, 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, s_w, s_b, sum_p, dW, db, U,
-                                                           grad, sig, dsig, s_off, sg ? sg->s_prior : 0,
-                                                           sg ? sg->sp0 : 0.0, sg ? sg->sp1 : 0.0, *ge);
-  else if (wsc == nullptr)
-    glm_potential_finish_kernel<<<grid, 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, s_w, s_b, sum_p, dW, db, U, grad,
-                                                     sig, dsig, s_off, sg ? sg->s_prior : 0, sg ? sg->sp0 : 0.0,
-                                                     sg ? sg->sp1 : 0.0);
-  else
-    glm_scaled_potential_finish_kernel<<<grid, 256, 0, s>>>(z, C, Dz, w_off, b_off, KD, Kb, s_b, sum_p, dW, db, U,
-                                                            grad, sig, dsig, s_off, sg ? sg->s_prior : 0,
-                                                            sg ? sg->sp0 : 0.0, sg ? sg->sp1 : 0.0, *wsc);
-  count_launch(1);
-  return check_launch();
-}
-
-// Scope of the likelihood kernels (K == 1 except for softmax); the kind codes of b2_glm_scaled_potential
-inline bool glm_potential_in_scope(int kind, int64_t N, int D, int K, int64_t C) {
-  if (N < 1 || C < 1 || C >= ((int64_t)1 << 31)) return false;
-  if (kind == B2_GLM_BERNOULLI) return K == 1 && (D == 4 || D == 8 || D == 16 || D == 32);
-  if (kind == B2_GLM_CATEGORICAL) return D == 32 && K >= 2 && K <= 16;
-  if (kind == B2_GLM_POISSON || kind == B2_GLM_NORMAL || kind == B2_GLM_BINOMIAL)
-    return K == 1 && D >= 1 && D <= 128;
-  return false;
-}
-
-// the kinds b2_glm_potential takes (Normal and Binomial regression have their own entry points)
-inline bool glm_plain_kind(int kind) {
-  return kind == B2_GLM_BERNOULLI || kind == B2_GLM_CATEGORICAL || kind == B2_GLM_POISSON;
-}
-
-// the likelihood workspace of an in-scope kind
-inline size_t glm_potential_lik_bytes(int kind, int64_t N, int D, int K, int64_t C) {
-  switch (kind) {
-    case B2_GLM_BERNOULLI: return b2_glm_workspace(N, D, (int)C);
-    case B2_GLM_POISSON: return b2_glm_poisson_workspace(N, D, (int)C);
-    case B2_GLM_NORMAL: return b2_glm_normal_workspace(N, D, (int)C);
-    case B2_GLM_BINOMIAL: return b2_glm_binomial_workspace(N, D, (int)C);
-    default: return b2_glm_categorical_workspace(N, D, K, (int)C);
-  }
-}
-
-// The likelihood call of glm_potential_run for every kind: weight = -1, so dW, db (and dsig) are derivatives of
-// -loglik; every logit fp32-exact (B2_FLAG_GLM_3XTF32; the Normal kernels always split X).  The noise scale `sig`
-// and its gradient `dsig` (null for a constant noise scale) are Normal regression's, trials Binomial's; grp the
-// group effect of every kind but Categorical (Wp and dW then D + G wide).
-inline int glm_potential_likelihood(int kind, const float* X, const void* y, const float* trials, int trials_per_row,
-                                    int64_t N, int D, int K, int64_t C, const float* Wp, const float* bp,
+// The likelihood call for every kind: weight = -1, so dW, db (and dsig) are derivatives of -loglik; every logit
+// fp32-exact (B2_FLAG_GLM_3XTF32; the Normal kernels always split X).  The noise scale `sig` and its gradient `dsig`
+// (null for a constant noise scale) are Normal regression's, trials Binomial's; grp the group effect of every kind
+// but Categorical (Wp and dW then D + G (1 + S) wide).
+inline int glm_potential_likelihood(const b2_glm_regression& m, int64_t C, const float* Wp, const float* bp,
                                     const float* sig, float* dsig, float* sum_p, float* dW, float* db, void* ws,
-                                    size_t ws_bytes, void* stream, GlmGroups grp = {}) {
-  const float* yf = static_cast<const float*>(y);
+                                    size_t ws_bytes, void* stream, GlmGroups grp) {
+  const float* yf = static_cast<const float*>(m.y);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  switch (kind) {
+  switch (m.kind) {
     case B2_GLM_BERNOULLI:
-      return glm_bernoulli_logits(X, yf, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0, B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW,
-                                  db, ws, ws_bytes, s, grp);
+      return glm_bernoulli_logits(m.X, yf, Wp, bp, m.N, m.D, (int)C, 1.0, -1.0, 1.0, B2_FLAG_GLM_3XTF32, sum_p,
+                                  nullptr, dW, db, ws, ws_bytes, s, grp);
     case B2_GLM_POISSON:
-      return glm_poisson_log_rate(X, yf, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0, B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW,
-                                  db, ws, ws_bytes, s, grp);
+      return glm_poisson_log_rate(m.X, yf, Wp, bp, m.N, m.D, (int)C, 1.0, -1.0, 1.0, B2_FLAG_GLM_3XTF32, sum_p,
+                                  nullptr, dW, db, ws, ws_bytes, s, grp);
     case B2_GLM_NORMAL:
-      return glm_normal_loc(X, yf, Wp, bp, sig, 1, N, D, (int)C, 1.0, -1.0, 1.0, 0, sum_p, nullptr, dW, db, dsig, ws,
-                            ws_bytes, s, grp);
+      return glm_normal_loc(m.X, yf, Wp, bp, sig, 1, m.N, m.D, (int)C, 1.0, -1.0, 1.0, 0, sum_p, nullptr, dW, db,
+                            dsig, ws, ws_bytes, s, grp);
     case B2_GLM_BINOMIAL:
-      return glm_binomial_logits(X, yf, trials, trials_per_row, Wp, bp, N, D, (int)C, 1.0, -1.0, 1.0,
+      return glm_binomial_logits(m.X, yf, m.trials, m.trials_per_row, Wp, bp, m.N, m.D, (int)C, 1.0, -1.0, 1.0,
                                  B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, s, grp);
     default:
-      return b2_glm_categorical_logits(X, static_cast<const int64_t*>(y), Wp, bp, N, D, K, (int)C, 1.0, -1.0, 1.0,
-                                       B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, stream);
+      return b2_glm_categorical_logits(m.X, static_cast<const int64_t*>(m.y), Wp, bp, m.N, m.D, m.K, (int)C, 1.0,
+                                       -1.0, 1.0, B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, ws_bytes, stream);
   }
 }
 
@@ -453,208 +332,52 @@ inline bool positive_prior_ok(int prior, double p0, double p1) {
                                      : prior >= B2_SIGMA_HALFNORMAL && prior <= B2_SIGMA_EXPONENTIAL && p0 > 0.0;
 }
 
-}  // namespace b2
-
-using namespace b2;
-
-extern "C" size_t b2_glm_potential_workspace(int kind, int64_t N, int D, int K, int64_t C) {
-  if (!glm_plain_kind(kind) || !glm_potential_in_scope(kind, N, D, K, C)) return 256;
-  return glm_potential_layout(glm_potential_lik_bytes(kind, N, D, K, C), (int64_t)K * D, K, C, false).total;
+// a scale latent at z column s_off with a valid prior, or else the constant s_const, positive in fp32 too
+inline bool positive_scale_ok(int64_t s_off, int prior, double p0, double p1, double s_const) {
+  return s_off >= 0 ? positive_prior_ok(prior, p0, p1) : s_const > 0.0 && (float)s_const > 0.f;
 }
 
-extern "C" int b2_glm_potential(int kind, const float* X, const void* y, int64_t N, int D, int K, int has_bias,
-                                const float* z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, double s_w,
-                                double s_b, float* U, float* grad, void* workspace, size_t workspace_bytes,
-                                void* stream) {
-  if (!X || !y || !z || !U || !grad) return B2_ERR_NULL;
-  if (!glm_plain_kind(kind) || !glm_potential_in_scope(kind, N, D, K, C)) return B2_ERR_BAD_SHAPE;
-  const int KD = K * D, Kb = has_bias ? K : 0;
-  // z's row is exactly the weight block and the bias block, neither overlapping nor out of the row
-  if (Dz != (int64_t)KD + Kb || w_off < 0 || w_off + KD > Dz) return B2_ERR_BAD_SHAPE;
-  if (has_bias && (b_off < 0 || b_off + Kb > Dz || (b_off < w_off + KD && w_off < b_off + Kb)))
-    return B2_ERR_BAD_SHAPE;
-  if (!(s_w > 0.0) || (has_bias && !(s_b > 0.0))) return B2_ERR_BAD_SHAPE;
-  return glm_potential_run(
-      glm_potential_lik_bytes(kind, N, D, K, C), z, C, Dz, w_off, b_off, KD, K, has_bias, s_w, s_b, nullptr, nullptr,
-      nullptr, U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
-      [&](const float* Wp, const float* bp, const float*, float*, float* sum_p, float* dW, float* db, void* ws,
-          size_t ws_bytes) {
-        return glm_potential_likelihood(kind, X, y, nullptr, 0, N, D, K, C, Wp, bp, nullptr, nullptr, sum_p, dW, db,
-                                        ws, ws_bytes, stream);
-      });
-}
+inline bool misaligned(const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 != 0; }
 
-// ---- linear regression: Normal(X @ w + b, sigma), sigma constant or latent with a positive-support prior ----
-extern "C" size_t b2_glm_normal_potential_workspace(int64_t N, int D, int64_t C) {
-  if (N < 1 || D < 1 || D > 128 || C < 1 || C >= ((int64_t)1 << 31)) return 256;
-  return glm_potential_layout(b2_glm_normal_workspace(N, D, (int)C), D, 1, C, true).total;
-}
-
-extern "C" int b2_glm_normal_potential(const float* X, const float* y, int64_t N, int D, int has_bias,
-                                       const float* z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off,
-                                       int64_t s_off, double s_w, double s_b, int s_prior, double sp0, double sp1,
-                                       double sigma, float* U, float* grad, void* workspace, size_t workspace_bytes,
-                                       void* stream) {
-  if (!X || !y || !z || !U || !grad) return B2_ERR_NULL;
-  if (N < 1 || D < 1 || D > 128 || C < 1 || C >= ((int64_t)1 << 31)) return B2_ERR_BAD_SHAPE;
-  const int Kb = has_bias ? 1 : 0, Ks = s_off >= 0 ? 1 : 0;
-  // z's row is exactly the weight block, the bias and log sigma, none overlapping another or out of the row
-  if (Dz != (int64_t)D + Kb + Ks || w_off < 0 || w_off + D > Dz) return B2_ERR_BAD_SHAPE;
-  if (has_bias && (b_off < 0 || b_off >= Dz || (b_off >= w_off && b_off < w_off + D))) return B2_ERR_BAD_SHAPE;
-  if (Ks && (s_off >= Dz || (s_off >= w_off && s_off < w_off + D) || (has_bias && s_off == b_off)))
-    return B2_ERR_BAD_SHAPE;
-  if (!(s_w > 0.0) || (has_bias && !(s_b > 0.0))) return B2_ERR_BAD_SHAPE;
-  if (Ks) {
-    if (!positive_prior_ok(s_prior, sp0, sp1)) return B2_ERR_BAD_SHAPE;
-  } else if (!(sigma > 0.0) || !((float)sigma > 0.f)) {
-    return B2_ERR_BAD_SHAPE;
+// Every check of b2_glm_potential that needs no workspace: 0, or the B2 code of the first one that fails.
+inline int glm_potential_check(const b2_glm_regression* mp, const float* z, int64_t C, int64_t Dz, const float* U,
+                               const float* grad) {
+  if (!mp || !mp->X || !mp->y || !z || !U || !grad) return B2_ERR_NULL;
+  const b2_glm_regression& m = *mp;
+  if ((m.kind == B2_GLM_BINOMIAL && !m.trials) || (m.group && !m.group->groups)) return B2_ERR_NULL;
+  if (!glm_regression_in_scope(m, C)) return B2_ERR_BAD_SHAPE;
+  // the others leave N to their likelihood call, whose SIMT Bernoulli kernel takes any N
+  if ((m.scale || m.group) && m.N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
+  const bool normal = m.kind == B2_GLM_NORMAL, binomial = m.kind == B2_GLM_BINOMIAL;
+  if (!normal && m.s_off >= 0) return B2_ERR_BAD_SHAPE;   // only linear regression has a noise scale
+  if (normal && !positive_scale_ok(m.s_off, m.s_prior, m.sp0, m.sp1, m.sigma)) return B2_ERR_BAD_SHAPE;
+  if (binomial && m.trials_per_row != 0 && m.trials_per_row != 1) return B2_ERR_BAD_SHAPE;
+  if ((!m.scale && !(m.s_w > 0.0)) || (m.has_bias && !(m.s_b > 0.0))) return B2_ERR_BAD_SHAPE;
+  // z's row is exactly w, b, log sigma, log tau, log lam, alpha (or eta), log s_a and each slope's beta_k (or e_k)
+  // and log s_k: each present block inside the row, no two overlapping, and their widths summing to Dz
+  const int64_t KD = (int64_t)m.K * m.D;
+  int64_t off[13] = {m.w_off, m.b_off, m.s_off}, len[13] = {KD, m.has_bias ? m.K : 0, m.s_off >= 0 ? 1 : 0};
+  int nblk = 3;
+  if (const b2_glm_weight_scale* sc = m.scale) {
+    if (sc->tau_off < 0 && sc->lam_off < 0) return B2_ERR_BAD_SHAPE;   // a constant weight scale is s_w
+    if (sc->tau_off >= 0 && !positive_prior_ok(sc->tau_prior, sc->tau_p0, sc->tau_p1)) return B2_ERR_BAD_SHAPE;
+    if (sc->lam_off >= 0 && !positive_prior_ok(sc->lam_prior, sc->lam_p0, sc->lam_p1)) return B2_ERR_BAD_SHAPE;
+    off[nblk] = sc->tau_off, len[nblk++] = sc->tau_off >= 0 ? 1 : 0;
+    off[nblk] = sc->lam_off, len[nblk++] = sc->lam_off >= 0 ? KD : 0;
   }
-  if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
-  const PotentialSigma sg = {Ks ? s_off : (int64_t)-1, (float)sigma, s_prior, sp0, sp1};
-  return glm_potential_run(
-      b2_glm_normal_workspace(N, D, (int)C), z, C, Dz, w_off, b_off, D, 1, has_bias, s_w, s_b, &sg, nullptr, nullptr,
-      U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
-      [&](const float* Wp, const float* bp, const float* sig, float* dsig, float* sum_p, float* dW, float* db,
-          void* ws, size_t ws_bytes) {
-        return glm_potential_likelihood(B2_GLM_NORMAL, X, y, nullptr, 0, N, D, 1, C, Wp, bp, sig, Ks ? dsig : nullptr,
-                                        sum_p, dW, db, ws, ws_bytes, stream);
-      });
-}
-
-// ---- Binomial regression: Binomial(m, logits = X @ w + b), m one count for every row or one per row ------------
-extern "C" size_t b2_glm_binomial_potential_workspace(int64_t N, int D, int64_t C) {
-  if (N < 1 || D < 1 || D > 128 || C < 1 || C >= ((int64_t)1 << 31)) return 256;
-  return glm_potential_layout(b2_glm_binomial_workspace(N, D, (int)C), D, 1, C, false).total;
-}
-
-extern "C" int b2_glm_binomial_potential(const float* X, const float* y, const float* trials, int trials_per_row,
-                                         int64_t N, int D, int has_bias, const float* z, int64_t C, int64_t Dz,
-                                         int64_t w_off, int64_t b_off, double s_w, double s_b, float* U,
-                                         float* grad, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!X || !y || !trials || !z || !U || !grad) return B2_ERR_NULL;
-  if (N < 1 || D < 1 || D > 128 || C < 1 || C >= ((int64_t)1 << 31)) return B2_ERR_BAD_SHAPE;
-  if (trials_per_row != 0 && trials_per_row != 1) return B2_ERR_BAD_SHAPE;
-  const int Kb = has_bias ? 1 : 0;
-  // z's row is exactly the weight block and the bias, neither overlapping the other or out of the row
-  if (Dz != (int64_t)D + Kb || w_off < 0 || w_off + D > Dz) return B2_ERR_BAD_SHAPE;
-  if (has_bias && (b_off < 0 || b_off >= Dz || (b_off >= w_off && b_off < w_off + D))) return B2_ERR_BAD_SHAPE;
-  if (!(s_w > 0.0) || (has_bias && !(s_b > 0.0))) return B2_ERR_BAD_SHAPE;
-  if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
-  if (trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0) return B2_ERR_BAD_SHAPE;
-  return glm_potential_run(
-      b2_glm_binomial_workspace(N, D, (int)C), z, C, Dz, w_off, b_off, D, 1, has_bias, s_w, s_b, nullptr, nullptr,
-      nullptr, U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
-      [&](const float* Wp, const float* bp, const float*, float*, float* sum_p, float* dW, float* db, void* ws,
-          size_t ws_bytes) {
-        return glm_potential_likelihood(B2_GLM_BINOMIAL, X, y, trials, trials_per_row, N, D, 1, C, Wp, bp, nullptr,
-                                        nullptr, sum_p, dW, db, ws, ws_bytes, stream);
-      });
-}
-
-// ---- any kind with a latent weight scale: w ~ Normal(0, tau * lam) -------------------------------------------
-extern "C" size_t b2_glm_scaled_potential_workspace(int kind, int64_t N, int D, int K, int64_t C) {
-  if (!glm_potential_in_scope(kind, N, D, K, C)) return 256;
-  return glm_potential_layout(glm_potential_lik_bytes(kind, N, D, K, C), (int64_t)K * D, K, C,
-                              kind == B2_GLM_NORMAL).total;
-}
-
-extern "C" int b2_glm_scaled_potential(int kind, const float* X, const void* y, const float* trials,
-                                       int trials_per_row, int64_t N, int D, int K, int has_bias, const float* z,
-                                       int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int64_t s_off, double s_b,
-                                       int s_prior, double sp0, double sp1, double sigma,
-                                       const b2_glm_weight_scale* scale, float* U, float* grad, void* workspace,
-                                       size_t workspace_bytes, void* stream) {
-  if (!X || !y || !z || !U || !grad || !scale) return B2_ERR_NULL;
-  if (kind == B2_GLM_BINOMIAL && !trials) return B2_ERR_NULL;
-  if (!glm_potential_in_scope(kind, N, D, K, C)) return B2_ERR_BAD_SHAPE;
-  if (N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
-  const b2_glm_weight_scale sc = *scale;
-  const bool normal = kind == B2_GLM_NORMAL, has_tau = sc.tau_off >= 0, has_lam = sc.lam_off >= 0;
-  if (!has_tau && !has_lam) return B2_ERR_BAD_SHAPE;    // a constant weight scale is b2_glm_potential's
-  if (!normal && s_off >= 0) return B2_ERR_BAD_SHAPE;   // only linear regression has a noise scale
-  const int64_t KD = (int64_t)K * D;
-  // z's row is exactly w, b, log sigma, log tau and log lam: each block inside the row, no two overlapping, and
-  // their widths summing to Dz
-  const int64_t off[5] = {w_off, has_bias ? b_off : -1, s_off, sc.tau_off, sc.lam_off};
-  const int64_t len[5] = {KD, has_bias ? K : 0, s_off >= 0 ? 1 : 0, has_tau ? 1 : 0, has_lam ? KD : 0};
-  int64_t width = 0;
-  for (int i = 0; i < 5; ++i) {
-    if (len[i] == 0) continue;
-    if (off[i] < 0 || off[i] > Dz - len[i]) return B2_ERR_BAD_SHAPE;
-    for (int j = 0; j < i; ++j)
-      if (len[j] && off[i] < off[j] + len[j] && off[j] < off[i] + len[i]) return B2_ERR_BAD_SHAPE;
-    width += len[i];
-  }
-  if (width != Dz) return B2_ERR_BAD_SHAPE;
-  if (has_bias && !(s_b > 0.0)) return B2_ERR_BAD_SHAPE;
-  if (has_tau && !positive_prior_ok(sc.tau_prior, sc.tau_p0, sc.tau_p1)) return B2_ERR_BAD_SHAPE;
-  if (has_lam && !positive_prior_ok(sc.lam_prior, sc.lam_p0, sc.lam_p1)) return B2_ERR_BAD_SHAPE;
-  if (normal && s_off >= 0 && !positive_prior_ok(s_prior, sp0, sp1)) return B2_ERR_BAD_SHAPE;
-  if (normal && s_off < 0 && (!(sigma > 0.0) || !((float)sigma > 0.f))) return B2_ERR_BAD_SHAPE;
-  if (kind == B2_GLM_BINOMIAL && trials_per_row != 0 && trials_per_row != 1) return B2_ERR_BAD_SHAPE;
-  if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0) return B2_ERR_BAD_SHAPE;
-  if (kind == B2_GLM_BINOMIAL && trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0)
-    return B2_ERR_BAD_SHAPE;
-  const PotentialSigma sg = {s_off >= 0 ? s_off : (int64_t)-1, (float)sigma, s_prior, sp0, sp1};
-  const bool latent_sigma = normal && s_off >= 0;
-  return glm_potential_run(
-      glm_potential_lik_bytes(kind, N, D, K, C), z, C, Dz, w_off, b_off, (int)KD, K, has_bias, 1.0, s_b,
-      normal ? &sg : nullptr, &sc, nullptr, U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
-      [&](const float* Wp, const float* bp, const float* sig, float* dsig, float* sum_p, float* dW, float* db,
-          void* ws, size_t ws_bytes) {
-        return glm_potential_likelihood(kind, X, y, trials, trials_per_row, N, D, K, C, Wp, bp, sig,
-                                        latent_sigma ? dsig : nullptr, sum_p, dW, db, ws, ws_bytes, stream);
-      });
-}
-
-// ---- a varying intercept by group: alpha[g], centred or non-centred, with a constant or latent scale s_a, and up to
-// three varying slopes beta_k[g] X[n, c_k] with scales of the same forms ------------------------------------------
-// Scope: kinds Bernoulli, Poisson, Normal and Binomial, 1 <= G and D + G (1 + S) <= 128 (G here: the group columns).
-inline bool glm_group_in_scope(int kind, int64_t N, int D, int G, int64_t C) {
-  if (kind != B2_GLM_BERNOULLI && kind != B2_GLM_POISSON && kind != B2_GLM_NORMAL && kind != B2_GLM_BINOMIAL)
-    return false;
-  return N >= 1 && C >= 1 && C < ((int64_t)1 << 31) && D >= 1 && G >= 1 && D + G <= 128;
-}
-
-extern "C" size_t b2_glm_group_potential_workspace(int kind, int64_t N, int D, int G, int64_t C) {
-  if (!glm_group_in_scope(kind, N, D, G, C)) return 256;
-  return glm_potential_layout(glm_potential_lik_bytes(kind, N, D + G, 1, C), D + G, 1, C, kind == B2_GLM_NORMAL).total;
-}
-
-extern "C" int b2_glm_group_potential(int kind, const float* X, const void* y, const float* trials,
-                                      int trials_per_row, int64_t N, int D, int has_bias, const float* z, int64_t C,
-                                      int64_t Dz, int64_t w_off, int64_t b_off, int64_t s_off, double s_w,
-                                      double s_b, int s_prior, double sp0, double sp1, double sigma,
-                                      const b2_glm_group_effect* ge, float* U, float* grad, void* workspace,
-                                      size_t workspace_bytes, void* stream) {
-  if (!X || !y || !z || !U || !grad || !ge || !ge->groups) return B2_ERR_NULL;
-  if (kind == B2_GLM_BINOMIAL && !trials) return B2_ERR_NULL;
-  const b2_glm_group_effect g = *ge;
-  if (g.S < 0 || g.S > 3 || g.G < 1 || g.G > 128) return B2_ERR_BAD_SHAPE;
-  const int Da = D + g.G * (1 + g.S);
-  if (!glm_group_in_scope(kind, N, D, g.G * (1 + g.S), C)) return B2_ERR_BAD_SHAPE;
-  if (N >= ((int64_t)1 << 31)) return B2_ERR_TOO_LARGE;
-  const bool normal = kind == B2_GLM_NORMAL;
-  if (!normal && s_off >= 0) return B2_ERR_BAD_SHAPE;   // only linear regression has a noise scale
-  if (g.noncentred != 0 && g.noncentred != 1) return B2_ERR_BAD_SHAPE;
-  for (int k = 0; k < g.S; ++k) {
-    const b2_glm_group_slope& sl = g.slope[k];
-    if (sl.col < 0 || sl.col >= D || (sl.noncentred != 0 && sl.noncentred != 1)) return B2_ERR_BAD_SHAPE;
-    for (int j = 0; j < k; ++j)
-      if (g.slope[j].col == sl.col) return B2_ERR_BAD_SHAPE;
-    if (sl.s_off >= 0 && !positive_prior_ok(sl.s_prior, sl.sp0, sl.sp1)) return B2_ERR_BAD_SHAPE;
-    if (sl.s_off < 0 && (!(sl.s_const > 0.0) || !((float)sl.s_const > 0.f))) return B2_ERR_BAD_SHAPE;
-  }
-  // z's row is exactly w, b, log sigma, alpha (or eta), log s_a and each slope's beta_k (or e_k) and log s_k: each
-  // block inside the row, no two overlapping, and their widths summing to Dz
-  int64_t off[11] = {w_off, has_bias ? b_off : -1, s_off, g.a_off, g.s_off};
-  int64_t len[11] = {D, has_bias ? 1 : 0, s_off >= 0 ? 1 : 0, g.G, g.s_off >= 0 ? 1 : 0};
-  const int nblk = 5 + 2 * g.S;
-  for (int k = 0; k < g.S; ++k) {
-    off[5 + 2 * k] = g.slope[k].b_off;
-    len[5 + 2 * k] = g.G;
-    off[6 + 2 * k] = g.slope[k].s_off;
-    len[6 + 2 * k] = g.slope[k].s_off >= 0 ? 1 : 0;
+  if (const b2_glm_group_effect* g = m.group) {
+    const b2_glm_group_slope icpt = {g->a_off, g->s_off, 0, g->noncentred, g->s_prior, g->s_const, g->sp0, g->sp1};
+    for (int k = -1; k < g->S; ++k) {        // the intercept, then each slope
+      const b2_glm_group_slope& b = k < 0 ? icpt : g->slope[k];
+      if (b.noncentred != 0 && b.noncentred != 1) return B2_ERR_BAD_SHAPE;
+      if (!positive_scale_ok(b.s_off, b.s_prior, b.sp0, b.sp1, b.s_const)) return B2_ERR_BAD_SHAPE;
+      if (k >= 0 && (b.col < 0 || b.col >= m.D)) return B2_ERR_BAD_SHAPE;
+      for (int j = 0; j < k; ++j)
+        if (g->slope[j].col == b.col) return B2_ERR_BAD_SHAPE;
+      off[nblk] = b.b_off, len[nblk++] = g->G;
+      off[nblk] = b.s_off, len[nblk++] = b.s_off >= 0 ? 1 : 0;
+    }
+    if (misaligned(g->groups)) return B2_ERR_BAD_SHAPE;
   }
   int64_t width = 0;
   for (int i = 0; i < nblk; ++i) {
@@ -665,30 +388,66 @@ extern "C" int b2_glm_group_potential(int kind, const float* X, const void* y, c
     width += len[i];
   }
   if (width != Dz) return B2_ERR_BAD_SHAPE;
-  if (!(s_w > 0.0) || (has_bias && !(s_b > 0.0))) return B2_ERR_BAD_SHAPE;
-  if (g.s_off >= 0 && !positive_prior_ok(g.s_prior, g.sp0, g.sp1)) return B2_ERR_BAD_SHAPE;
-  if (g.s_off < 0 && (!(g.s_const > 0.0) || !((float)g.s_const > 0.f))) return B2_ERR_BAD_SHAPE;
-  if (normal && s_off >= 0 && !positive_prior_ok(s_prior, sp0, sp1)) return B2_ERR_BAD_SHAPE;
-  if (normal && s_off < 0 && (!(sigma > 0.0) || !((float)sigma > 0.f))) return B2_ERR_BAD_SHAPE;
-  if (kind == B2_GLM_BINOMIAL && trials_per_row != 0 && trials_per_row != 1) return B2_ERR_BAD_SHAPE;
-  if (reinterpret_cast<uintptr_t>(X) % 16 != 0 || reinterpret_cast<uintptr_t>(y) % 16 != 0 ||
-      reinterpret_cast<uintptr_t>(g.groups) % 16 != 0)
-    return B2_ERR_BAD_SHAPE;
-  if (kind == B2_GLM_BINOMIAL && trials_per_row && reinterpret_cast<uintptr_t>(trials) % 16 != 0)
-    return B2_ERR_BAD_SHAPE;
-  const PotentialSigma sg = {s_off >= 0 ? s_off : (int64_t)-1, (float)sigma, s_prior, sp0, sp1};
-  const bool latent_sigma = normal && s_off >= 0;
+  // Bernoulli, softmax and Poisson with a constant weight scale and no group effect leave X and y to their
+  // likelihood call (the SIMT Bernoulli kernel needs neither aligned)
+  if ((m.scale || m.group || normal || binomial) && (misaligned(m.X) || misaligned(m.y))) return B2_ERR_BAD_SHAPE;
+  if (binomial && m.trials_per_row && misaligned(m.trials)) return B2_ERR_BAD_SHAPE;
+  return 0;
+}
+
+}  // namespace b2
+
+using namespace b2;
+
+extern "C" size_t b2_glm_potential_workspace(const b2_glm_regression* m, int64_t C) {
+  if (!m || !glm_regression_in_scope(*m, C)) return 256;
+  return glm_potential_layout(*m, C).total;
+}
+
+extern "C" int b2_glm_potential(const b2_glm_regression* mp, const float* z, int64_t C, int64_t Dz, float* U,
+                                float* grad, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = glm_potential_check(mp, z, C, Dz, U, grad);
+  if (rc != 0) return rc;
+  const b2_glm_regression& m = *mp;
+  const GlmPotentialLayout L = glm_potential_layout(m, C);
+  if (!workspace || workspace_bytes < L.total) return B2_ERR_WORKSPACE;
+  const bool normal = m.kind == B2_GLM_NORMAL;
+  const int KD = m.K * m.D + glm_group_cols(m), Kb = m.has_bias ? m.K : 0;
+  char* ws = reinterpret_cast<char*>(workspace);
+  float* Wp = reinterpret_cast<float*>(ws + L.wp);
+  float* bp = m.has_bias ? reinterpret_cast<float*>(ws + L.bp) : nullptr;
+  float* dW = reinterpret_cast<float*>(ws + L.dw);
+  float* db = m.has_bias ? reinterpret_cast<float*>(ws + L.db) : nullptr;
+  float* sum_p = reinterpret_cast<float*>(ws + L.sum_p);
+  float* sig = normal ? reinterpret_cast<float*>(ws + L.sig) : nullptr;
+  float* dsig = normal && m.s_off >= 0 ? reinterpret_cast<float*>(ws + L.dsig) : nullptr;
+  const b2_glm_weight_scale no_scale = {-1, -1, 0, 0, 0.0, 0.0, 0.0, 0.0};
+  const b2_glm_group_effect no_group = {};
+  const b2_glm_group_effect& ge = m.group ? *m.group : no_group;
   GlmGroups grp;
-  grp.idx = g.groups;
-  grp.G = g.G;
-  grp.S = g.S;
-  for (int k = 0; k < g.S; ++k) grp.col[k] = g.slope[k].col;
-  return glm_potential_run(
-      glm_potential_lik_bytes(kind, N, Da, 1, C), z, C, Dz, w_off, b_off, Da, 1, has_bias, s_w, s_b,
-      normal ? &sg : nullptr, nullptr, &g, U, grad, workspace, workspace_bytes, reinterpret_cast<cudaStream_t>(stream),
-      [&](const float* Wp, const float* bp, const float* sig, float* dsig, float* sum_p, float* dW, float* db,
-          void* ws, size_t ws_bytes) {
-        return glm_potential_likelihood(kind, X, y, trials, trials_per_row, N, D, 1, C, Wp, bp, sig,
-                                        latent_sigma ? dsig : nullptr, sum_p, dW, db, ws, ws_bytes, stream, grp);
-      });
+  if (m.group) {
+    grp.idx = ge.groups;
+    grp.G = ge.G;
+    grp.S = ge.S;
+    for (int k = 0; k < ge.S; ++k) grp.col[k] = ge.slope[k].col;
+  }
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+
+  const int64_t npack = C * (KD + Kb);
+  const auto pack = m.group ? glm_potential_pack_kernel<true> : glm_potential_pack_kernel<false>;
+  pack<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(z, C, Dz, m.w_off, m.b_off, KD, Kb, Wp, bp, m.s_off,
+                                                       (float)m.sigma, sig, ge);
+  count_launch(1);
+  rc = check_launch();
+  if (rc != 0) return rc;
+  rc = glm_potential_likelihood(m, C, Wp, bp, sig, dsig, sum_p, dW, db, ws, L.wp, stream, grp);
+  if (rc != 0) return rc;
+  const auto finish = m.group   ? glm_potential_finish_kernel<false, true>
+                      : m.scale ? glm_potential_finish_kernel<true, false>
+                                : glm_potential_finish_kernel<false, false>;
+  finish<<<(unsigned)((C * 32 + 255) / 256), 256, 0, s>>>(
+      z, C, Dz, m.w_off, m.b_off, KD, Kb, m.s_w, m.s_b, sum_p, dW, db, U, grad, sig, dsig, m.s_off, m.s_prior, m.sp0,
+      m.sp1, m.scale ? *m.scale : no_scale, ge);
+  count_launch(1);
+  return check_launch();
 }

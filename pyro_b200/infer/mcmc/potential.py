@@ -116,20 +116,19 @@ class GlmPotential:
     ``W ~ Normal(0, s_w)[K, D]``, ``b ~ Normal(0, s_b)[K]`` (optional),
     ``y ~ Categorical(logits = X @ W.mT + b)``, or
     ``w ~ Normal(0, s_w)[D]``, ``b ~ Normal(0, s_b)`` (optional), ``y ~ Poisson(rate = exp(X @ w + b))``, or
-    ``y ~ Binomial(trials, logits = X @ w + b)`` with ``trials`` one count or ``[N]`` counts
-    (``b2_glm_binomial_potential``), or
+    ``y ~ Binomial(trials, logits = X @ w + b)`` with ``trials`` one count or ``[N]`` counts, or
     ``w ~ Normal(0, s_w)[D]``, ``b ~ Normal(0, s_b)`` (optional), ``y ~ Normal(X @ w + b, sigma)`` with a constant
     ``sigma`` or a latent one (``sigma_site``) whose prior ``sigma_prior = (kind, p0, p1)`` is HalfNormal(p0),
     HalfCauchy(p0), Exponential(p0) or LogNormal(p0, p1); z then holds ``log sigma`` (transform ``"exp"``) and U
-    carries the Jacobian ``-log sigma``, as ``TracePotential`` gives it (``b2_glm_normal_potential``).
+    carries the Jacobian ``-log sigma``, as ``TracePotential`` gives it.
 
-    The weight scale may instead be latent (``b2_glm_scaled_potential``): ``w ~ Normal(0, S)`` with ``S`` the
+    The weight scale may instead be latent (``weight_scale``): ``w ~ Normal(0, S)`` with ``S`` the
     positive scalar site ``tau_site``, the positive site ``lam_site`` of the weight's shape, or their product (the
     hierarchical, ARD and horseshoe priors).  ``tau_prior`` / ``lam_prior`` are ``(kind, p0, p1)`` as
     ``sigma_prior``, one value for every coefficient; z holds their logs (transform ``"exp"``), and U carries
     their Jacobians.
 
-    A varying intercept by group (``b2_glm_group_potential``, every kind but softmax, constant weight scale): the
+    A varying intercept by group (``group_effect``, every kind but softmax, constant weight scale): the
     linear predictor gains ``alpha[g]``, ``g`` the int64 ``[N]`` group index and ``alpha`` the ``G`` values of the
     site ``group["site"]``, drawn as ``Normal(0, s_a)`` (centred) or as ``eta ~ Normal(0, 1)`` with
     ``alpha = s_a * eta`` (``group["noncentred"]``).  ``s_a`` is the constant ``group["s_const"]`` or the positive
@@ -139,8 +138,9 @@ class GlmPotential:
     (``site``, ``noncentred``, ``s_site``, ``s_const``, ``s_prior``) and ``col``: slope k adds
     ``beta_k[g] * X[:, col]``, and each takes G more columns of the contraction, so ``D + G (1 + S) <= 128``.
 
-    ``value_and_grad`` is ``b2_glm_potential``: the likelihood of all chains comes from one pass of the
-    fused GLM kernel over X, the chains being its particles.  ``sites`` maps each site name to
+    ``value_and_grad`` is one ``b2_glm_potential`` call on the ``b2_glm_regression`` built once here
+    (``regression``): the likelihood of all chains comes from one pass of the fused GLM kernel over X, the chains
+    being its particles.  ``sites`` maps each site name to
     ``(slice into z, transform, value shape)`` in the order and layout ``TracePotential`` gives the same
     model, so samples, ``initial_params`` and ``full_mass`` behave the same on either.  Every chain is
     evaluated; the sampler masks inactive chains, as it does for ``TracePotential``."""
@@ -177,10 +177,8 @@ class GlmPotential:
                 setattr(sc, part + "_p0", float(p0))
                 setattr(sc, part + "_p1", float(p1))
             self.weight_scale = sc
-        self.scaled_kind = {"Bernoulli": N.GLM_BERNOULLI, "Categorical": N.GLM_CATEGORICAL,
-                            "Poisson": N.GLM_POISSON, "Normal": N.GLM_NORMAL, "Binomial": N.GLM_BINOMIAL}[kind]
         self.kind = {"Bernoulli": N.GLM_BERNOULLI, "Categorical": N.GLM_CATEGORICAL, "Poisson": N.GLM_POISSON,
-                     "Normal": None, "Binomial": None}[kind]
+                     "Normal": N.GLM_NORMAL, "Binomial": N.GLM_BINOMIAL}[kind]
         self.binomial = kind == "Binomial"
         if self.binomial:
             # one count (on the device, read by the kernel) or the [N] counts, private and 16-byte aligned
@@ -206,6 +204,24 @@ class GlmPotential:
         self.group, self.group_effect = group, None
         if group is not None:
             self.group_effect = self._group_effect(group)
+        self.regression = self._regression()
+
+    def _regression(self):
+        """b2_glm_regression of this potential: it points at the private X, y, trials and group-index copies and at
+        the ``weight_scale`` / ``group_effect`` structs (a NULL pointer for a constant scale / no group effect)."""
+        m = N.b2_glm_regression()
+        m.kind, m.X, m.y = self.kind, self.X.data_ptr(), self.y.data_ptr()
+        m.N, m.D, m.K = self.n, self.Dx, self.K
+        if self.binomial:
+            m.trials, m.trials_per_row = self.trials.data_ptr(), self.trials_per_row
+        m.has_bias, m.w_off, m.b_off, m.s_w, m.s_b = int(self.has_bias), self.w_off, self.b_off, self.s_w, self.s_b
+        m.s_off = self.sites[self.sigma_site][0].start if self.sigma_site is not None else -1
+        (m.s_prior, m.sp0, m.sp1), m.sigma = self.sigma_prior, self.sigma
+        if self.weight_scale is not None:
+            m.scale = ctypes.pointer(self.weight_scale)
+        if self.group_effect is not None:
+            m.group = ctypes.pointer(self.group_effect)
+        return m
 
     def _group_effect(self, group):
         """b2_glm_group_effect of ``group``, with the private int32 copy of the index it points to."""
@@ -255,62 +271,11 @@ class GlmPotential:
         U = torch.empty(C, dtype=torch.float32, device=z.device)
         g = torch.empty_like(z)
         lib = N.lib()
-        if self.group_effect is not None:
-            return self._group_value_and_grad(lib, z, C, U, g)
-        if self.weight_scale is not None:
-            return self._scaled_value_and_grad(lib, z, C, U, g)
-        if self.normal:
-            need = int(lib.b2_glm_normal_potential_workspace(self.n, self.Dx, C))
-            ws = N.workspace(z.device, need, tag="glm_potential")
-            s_off = self.sites[self.sigma_site][0].start if self.sigma_site is not None else -1
-            pk, p0, p1 = self.sigma_prior
-            N.check(lib.b2_glm_normal_potential(
-                self.X.data_ptr(), self.y.data_ptr(), self.n, self.Dx, int(self.has_bias), z.data_ptr(), C, self.D,
-                self.w_off, self.b_off, s_off, self.s_w, self.s_b, pk, p0, p1, self.sigma, U.data_ptr(),
-                g.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(z.device)), "b2_glm_normal_potential")
-            return U, g
-        if self.binomial:
-            need = int(lib.b2_glm_binomial_potential_workspace(self.n, self.Dx, C))
-            ws = N.workspace(z.device, need, tag="glm_potential")
-            N.check(lib.b2_glm_binomial_potential(
-                self.X.data_ptr(), self.y.data_ptr(), self.trials.data_ptr(), self.trials_per_row, self.n, self.Dx,
-                int(self.has_bias), z.data_ptr(), C, self.D, self.w_off, self.b_off, self.s_w, self.s_b,
-                U.data_ptr(), g.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(z.device)),
-                "b2_glm_binomial_potential")
-            return U, g
-        need = int(lib.b2_glm_potential_workspace(self.kind, self.n, self.Dx, self.K, C))
+        need = int(lib.b2_glm_potential_workspace(ctypes.byref(self.regression), C))
         ws = N.workspace(z.device, need, tag="glm_potential")
-        N.check(lib.b2_glm_potential(
-            self.kind, self.X.data_ptr(), self.y.data_ptr(), self.n, self.Dx, self.K, int(self.has_bias),
-            z.data_ptr(), C, self.D, self.w_off, self.b_off, self.s_w, self.s_b, U.data_ptr(), g.data_ptr(),
-            ws.data_ptr(), ws.numel(), N.stream_ptr(z.device)), "b2_glm_potential")
-        return U, g
-
-    def _scaled_value_and_grad(self, lib, z, C, U, g):
-        need = int(lib.b2_glm_scaled_potential_workspace(self.scaled_kind, self.n, self.Dx, self.K, C))
-        ws = N.workspace(z.device, need, tag="glm_potential")
-        s_off = self.sites[self.sigma_site][0].start if self.sigma_site is not None else -1
-        pk, p0, p1 = self.sigma_prior
-        trials, per_row = (self.trials.data_ptr(), self.trials_per_row) if self.binomial else (None, 0)
-        N.check(lib.b2_glm_scaled_potential(
-            self.scaled_kind, self.X.data_ptr(), self.y.data_ptr(), trials, per_row, self.n, self.Dx, self.K,
-            int(self.has_bias), z.data_ptr(), C, self.D, self.w_off, self.b_off, s_off, self.s_b, pk, p0, p1,
-            self.sigma, ctypes.byref(self.weight_scale), U.data_ptr(), g.data_ptr(), ws.data_ptr(), ws.numel(),
-            N.stream_ptr(z.device)), "b2_glm_scaled_potential")
-        return U, g
-
-    def _group_value_and_grad(self, lib, z, C, U, g):
-        ge = self.group_effect
-        need = int(lib.b2_glm_group_potential_workspace(self.scaled_kind, self.n, self.Dx, ge.G * (1 + ge.S), C))
-        ws = N.workspace(z.device, need, tag="glm_potential")
-        s_off = self.sites[self.sigma_site][0].start if self.sigma_site is not None else -1
-        pk, p0, p1 = self.sigma_prior
-        trials, per_row = (self.trials.data_ptr(), self.trials_per_row) if self.binomial else (None, 0)
-        N.check(lib.b2_glm_group_potential(
-            self.scaled_kind, self.X.data_ptr(), self.y.data_ptr(), trials, per_row, self.n, self.Dx,
-            int(self.has_bias), z.data_ptr(), C, self.D, self.w_off, self.b_off, s_off, self.s_w, self.s_b, pk, p0, p1,
-            self.sigma, ctypes.byref(self.group_effect), U.data_ptr(), g.data_ptr(), ws.data_ptr(), ws.numel(),
-            N.stream_ptr(z.device)), "b2_glm_group_potential")
+        N.check(lib.b2_glm_potential(ctypes.byref(self.regression), z.data_ptr(), C, self.D, U.data_ptr(),
+                                     g.data_ptr(), ws.data_ptr(), ws.numel(), N.stream_ptr(z.device)),
+                "b2_glm_potential")
         return U, g
 
     def unpack(self, z):

@@ -1,6 +1,6 @@
 """Binomial family: the elementwise site kernels (families 16 / 17), the fused Binomial-regression GLM kernels
 (glm_binomial_tc.cu), the SVI route (``_BinomialLinear``) and the NUTS route (``GlmPotential`` through
-``b2_glm_binomial_potential``).
+``b2_glm_potential``).
 
 CPU tier: the goldens recorded from the unmodified reference (tests/golden/make_golden_binomial.py), the host-built
 functors against them, the lazy-logits routing, recognition, argument checks and the kernels' SASS.  GPU tier: the
@@ -216,7 +216,7 @@ def test_bind_maps_the_reference_binomial():
 
 
 # ---- CPU tier: argument checks --------------------------------------------------------------------------------
-def test_entry_points_validate_arguments_before_any_cuda_call():
+def test_binomial_entry_points_validate_arguments_before_any_cuda_call():
     """The pointers are never dereferenced and no workspace is passed: the checks come first."""
     L = N.lib()
     p = ctypes.c_void_p(4096)
@@ -245,8 +245,9 @@ def test_entry_points_validate_arguments_before_any_cuda_call():
         assert call(p, p, p, 1, p, 10000, D, 0, p, need - 1) == -5, D
 
     def pot(X, y, m, per_row, D, bias, z, Dz, w_off, b_off, s_w=1.0, s_b=1.0, U=p, g=p):
-        return L.b2_glm_binomial_potential(X, y, m, per_row, 10000, D, bias, z, 8, Dz, w_off, b_off, s_w, s_b, U,
-                                           g, None, 0, None)
+        r = N.b2_glm_regression(kind=N.GLM_BINOMIAL, X=X, y=y, N=10000, D=D, K=1, trials=m, trials_per_row=per_row,
+                                has_bias=bias, w_off=w_off, b_off=b_off, s_w=s_w, s_b=s_b, s_off=-1)
+        return L.b2_glm_potential(ctypes.byref(r), z, 8, Dz, U, g, None, 0, None)
 
     assert pot(None, p, p, 1, 10, 1, p, 11, 0, 10) == -4
     assert pot(p, p, None, 1, 10, 1, p, 11, 0, 10) == -4

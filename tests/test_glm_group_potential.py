@@ -1,6 +1,6 @@
 """NUTS / HMC on multilevel regression: a varying intercept by group, ``X @ w + b + alpha[g]``, through
-``GlmPotential`` (``b2_glm_group_potential``), with the group effect scored as G more columns of the fused GLM
-kernel's contraction over ``[X | onehot(g)]``.
+``GlmPotential`` (``b2_glm_potential`` with a group effect), with the group effect scored as G more columns of the
+fused GLM kernel's contraction over ``[X | onehot(g)]``.
 
 CPU tier: which models ``recognise`` routes to ``GlmPotential`` (every likelihood kind, centred and non-centred group
 effects, a constant group scale or each of the four priors on a latent one, the ways a model can write the gather),
@@ -263,26 +263,36 @@ def test_out_of_range_index_is_refused_at_construction():
                              group=dict(pot.group, index=g2))
 
 
-def test_group_entry_point_validates_arguments_before_any_cuda_call():
+def test_group_effect_entry_point_validates_arguments_before_any_cuda_call():
     L = N.lib()
     p = ctypes.c_void_p(4096)
     q = ctypes.c_void_p(4100)
     D, G = 10, 20
 
-    def call(kind=N.GLM_POISSON, X=p, y=p, trials=None, per_row=0, n=10000, Dx=D, bias=1, z=p, Dz=D + G + 2,
-             w_off=0, b_off=D, s_off=-1, s_w=1.0, s_b=10.0, s_prior=0, sp0=0.0, sp1=0.0, sigma=1.0, groups=p,
-             nG=G, a_off=D + 1, noncentred=0, sa_off=D + G + 1, sa_prior=N.SIGMA_HALFCAUCHY, sa_p0=1.0, sa_p1=1.0,
-             s_const=0.0, ge=True, ws=None, nbytes=0):
+    def regression(kind=N.GLM_POISSON, X=p, y=p, trials=None, per_row=0, n=10000, Dx=D, bias=1, w_off=0, b_off=D,
+                   s_off=-1, s_w=1.0, s_b=10.0, s_prior=0, sp0=0.0, sp1=0.0, sigma=1.0, groups=p, nG=G, a_off=D + 1,
+                   noncentred=0, sa_off=D + G + 1, sa_prior=N.SIGMA_HALFCAUCHY, sa_p0=1.0, sa_p1=1.0, s_const=0.0,
+                   tau_off=-1):
         e = N.b2_glm_group_effect()
         e.groups, e.G, e.a_off, e.noncentred = groups, nG, a_off, noncentred
         e.s_off, e.s_prior, e.sp0, e.sp1, e.s_const = sa_off, sa_prior, sa_p0, sa_p1, s_const
-        return L.b2_glm_group_potential(kind, X, y, trials, per_row, n, Dx, bias, z, 4, Dz, w_off, b_off, s_off, s_w,
-                                        s_b, s_prior, sp0, sp1, sigma, ctypes.byref(e) if ge else None, p, p, ws,
-                                        nbytes, None)
+        m = N.b2_glm_regression(kind=kind, X=X, y=y, N=n, D=Dx, K=1, trials=trials, trials_per_row=per_row,
+                                has_bias=bias, w_off=w_off, b_off=b_off, s_w=s_w, s_b=s_b, s_off=s_off,
+                                s_prior=s_prior, sp0=sp0, sp1=sp1, sigma=sigma, group=ctypes.pointer(e))
+        if tau_off >= 0:     # a latent weight scale tau
+            m.scale = ctypes.pointer(N.b2_glm_weight_scale(tau_off=tau_off, lam_off=-1, tau_prior=1, tau_p0=1.0))
+        return m
+
+    def call(z=p, Dz=D + G + 2, null=False, ws=None, nbytes=0, **kw):
+        m = None if null else ctypes.byref(regression(**kw))
+        return L.b2_glm_potential(m, z, 4, Dz, p, p, ws, nbytes, None)
+
+    def workspace(**kw):
+        return L.b2_glm_potential_workspace(ctypes.byref(regression(**kw)), 4)
 
     # z = [w (10), b, alpha (20), log s_a]: valid, so the workspace check is next
     assert call() == -5
-    assert call(X=None) == -4 and call(y=None) == -4 and call(z=None) == -4 and call(ge=False) == -4
+    assert call(X=None) == -4 and call(y=None) == -4 and call(z=None) == -4 and call(null=True) == -4
     assert call(groups=None) == -4 and call(kind=N.GLM_BINOMIAL) == -4
     assert call(kind=N.GLM_CATEGORICAL) == -2 and call(kind=7) == -2
     assert call(kind=N.GLM_BERNOULLI) == -5                                 # any D with a group effect
@@ -313,10 +323,12 @@ def test_group_entry_point_validates_arguments_before_any_cuda_call():
     assert call(**nz, s_prior=N.SIGMA_HALFNORMAL, sp0=1.0) == -5
     assert call(**nz, s_prior=0, sp0=1.0) == -2 and call(**dict(nz, s_off=D + G + 1), s_prior=1, sp0=1.0) == -2
     assert call(kind=N.GLM_NORMAL, sigma=0.0) == -2 and call(kind=N.GLM_NORMAL, sigma=0.6) == -5
-    need = int(L.b2_glm_group_potential_workspace(N.GLM_POISSON, 10000, D, G, 4))
+    # a group effect with a latent weight scale
+    assert call(tau_off=D + G + 2, Dz=D + G + 3) == -2
+    need = int(workspace())
     assert need > 256 and call(ws=p, nbytes=need - 1) == -5
-    assert L.b2_glm_group_potential_workspace(N.GLM_POISSON, 10000, 100, 29, 4) == 256
-    assert L.b2_glm_group_potential_workspace(N.GLM_CATEGORICAL, 10000, D, G, 4) == 256
+    assert workspace(Dx=100, nG=29) == 256
+    assert workspace(kind=N.GLM_CATEGORICAL) == 256
 
 
 # ---- CPU tier: what ptxas makes of the group kernels --------------------------------------------------------------

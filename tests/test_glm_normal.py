@@ -762,15 +762,19 @@ def test_expansion_of_a_slice_is_not_a_per_particle_scale():
         assert dist._per_particle_sigma(sc, loc.lazy) is None
 
 
-def test_potential_entry_point_validates_arguments_before_any_cuda_call():
+def test_linear_regression_entry_point_validates_arguments_before_any_cuda_call():
     L = N.lib()
     p = ctypes.c_void_p(4096)
     q = ctypes.c_void_p(4100)
 
-    def call(X=p, y=p, D=10, bias=1, z=p, Dz=12, w_off=0, b_off=10, s_off=11, s_w=1.0, s_b=10.0,
-             prior=N.SIGMA_HALFNORMAL, sp0=1.0, sp1=1.0, sigma=1.0, ws=None, nbytes=0):
-        return L.b2_glm_normal_potential(X, y, 10000, D, bias, z, 4, Dz, w_off, b_off, s_off, s_w, s_b, prior, sp0,
-                                         sp1, sigma, p, p, ws, nbytes, None)
+    def regression(X=p, y=p, D=10, bias=1, w_off=0, b_off=10, s_off=11, s_w=1.0, s_b=10.0, prior=N.SIGMA_HALFNORMAL,
+                   sp0=1.0, sp1=1.0, sigma=1.0):
+        return N.b2_glm_regression(kind=N.GLM_NORMAL, X=X, y=y, N=10000, D=D, K=1, has_bias=bias, w_off=w_off,
+                                   b_off=b_off, s_w=s_w, s_b=s_b, s_off=s_off, s_prior=prior, sp0=sp0, sp1=sp1,
+                                   sigma=sigma)
+
+    def call(z=p, Dz=12, ws=None, nbytes=0, **kw):
+        return L.b2_glm_potential(ctypes.byref(regression(**kw)), z, 4, Dz, p, p, ws, nbytes, None)
 
     assert call(X=None) == -4 and call(y=None) == -4 and call(z=None) == -4
     assert call(D=0) == -2 and call(D=129, Dz=131, b_off=129, s_off=130) == -2
@@ -784,7 +788,7 @@ def test_potential_entry_point_validates_arguments_before_any_cuda_call():
     assert call() == -5                                          # valid: the workspace check is next
     assert call(prior=N.SIGMA_LOGNORMAL, sp0=-3.0, sp1=0.5) == -5
     assert call(s_off=-1, Dz=11, sigma=0.6) == -5
-    need = int(L.b2_glm_normal_potential_workspace(10000, 10, 4))
+    need = int(L.b2_glm_potential_workspace(ctypes.byref(regression()), 4))
     assert call(ws=p, nbytes=need - 1) == -5
 
 

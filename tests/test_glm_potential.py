@@ -6,6 +6,8 @@ CPU tier: which models ``recognise`` routes to ``GlmPotential`` and which keep t
 ``TracePotential``, determinism, CUDA-graph replay, an HMC trajectory against the oracle integrator, NUTS
 posteriors against the oracle sampler, the routes taken by ``NUTS(model)``, and unmodified Pyro through
 ``bind``."""
+import ctypes
+
 import pytest
 import torch
 import torch.nn.functional as F
@@ -154,6 +156,40 @@ def test_out_of_scope_models_keep_their_route(case):
 def test_intercept_free_logistic_keeps_logistic_potential():
     X, y = _data(300, 16)
     assert isinstance(_recognised(models.logreg_mcmc_model, X, y), LogisticPotential)
+
+
+def test_entry_point_validates_arguments_before_any_cuda_call():
+    """Logistic, softmax and Poisson regression with a constant weight scale: no pointer is dereferenced and no
+    workspace is passed, so every call returns at its first failed check."""
+    L = N.lib()
+    p = ctypes.c_void_p(4096)
+    q = ctypes.c_void_p(4100)
+
+    def call(kind=N.GLM_BERNOULLI, X=p, y=p, n=10000, Dx=16, K=1, bias=1, z=p, C=4, Dz=17, w_off=0, b_off=16,
+             s_off=-1, s_w=1.0, s_b=10.0, U=p, g=p, null=False):
+        m = N.b2_glm_regression(kind=kind, X=X, y=y, N=n, D=Dx, K=K, has_bias=bias, w_off=w_off, b_off=b_off,
+                                s_w=s_w, s_b=s_b, s_off=s_off)
+        return L.b2_glm_potential(None if null else ctypes.byref(m), z, C, Dz, U, g, None, 0, None)
+
+    # z = [w (16), b]: valid, so the workspace check is next
+    assert call() == -5
+    assert call(null=True) == -4 and call(X=None) == -4 and call(y=None) == -4 and call(z=None) == -4
+    assert call(U=None) == -4 and call(g=None) == -4
+    # kinds and widths: Bernoulli D in {4, 8, 16, 32}, softmax D == 32 and 2 <= K <= 16, Poisson 1 <= D <= 128
+    assert call(kind=7) == -2 and call(Dx=10, Dz=11, b_off=10) == -2
+    assert call(kind=N.GLM_POISSON, Dx=10, Dz=11, b_off=10) == -5
+    assert call(kind=N.GLM_POISSON, Dx=129, Dz=130, b_off=129) == -2
+    assert call(kind=N.GLM_CATEGORICAL, Dx=32, K=4, Dz=132, b_off=128) == -5
+    assert call(kind=N.GLM_CATEGORICAL, Dx=16, K=4, Dz=68, b_off=64) == -2
+    assert call(kind=N.GLM_CATEGORICAL, Dx=32, K=17, Dz=561, b_off=544) == -2
+    assert call(n=0) == -2 and call(C=0) == -2
+    # the row: out of it, overlapping, or not exactly the blocks
+    assert call(Dz=18) == -2 and call(Dz=16) == -2 and call(b_off=15) == -2 and call(w_off=1, b_off=0) == -5
+    assert call(w_off=-1) == -2 and call(bias=0, Dz=16) == -5
+    assert call(s_off=17, Dz=18) == -2                              # a noise scale outside linear regression
+    assert call(s_w=0.0) == -2 and call(s_b=0.0) == -2 and call(bias=0, Dz=16, s_b=0.0) == -5
+    # left to the likelihood call, after the workspace check: N (the SIMT Bernoulli kernel takes any) and alignment
+    assert call(n=1 << 31) == -5 and call(X=q) == -5 and call(y=q) == -5
 
 
 # ---- GPU tier ----------------------------------------------------------------------------------------------

@@ -1,13 +1,13 @@
 """NUTS / HMC on regression with a latent weight scale: the hierarchical ``w ~ Normal(0, tau)``, ARD
 ``w ~ Normal(0, lam)`` and horseshoe ``w ~ Normal(0, tau * lam)`` priors, through ``GlmPotential``
-(``b2_glm_scaled_potential``).
+(``b2_glm_potential`` with a latent ``scale``).
 
 CPU tier: which models ``recognise`` routes to ``GlmPotential`` (every likelihood kind, every scale form and prior,
 scale sites drawn before and after the other sites, linear regression with a latent noise scale too), their z
 layout against ``TracePotential``, the near misses that must keep the traced route, and the entry point's argument
 checks.  GPU tier: U and dU/dz against an fp64 restatement and against ``TracePotential``, determinism, CUDA-graph
 replay, HMC trajectories against the oracle integrator, NUTS posteriors against ``TracePotential`` runs, the routes
-``NUTS(model)`` and ``bind.NUTS`` take, and the unchanged native call of a constant weight scale."""
+``NUTS(model)`` and ``bind.NUTS`` take, and the one native call of a constant weight scale."""
 import ctypes
 import math
 
@@ -266,25 +266,29 @@ def test_intercept_free_logistic_with_constant_scale_keeps_logistic_potential():
     assert isinstance(_recognised(model, X, y), LogisticPotential)
 
 
-def test_scaled_entry_point_validates_arguments_before_any_cuda_call():
+def test_latent_scale_entry_point_validates_arguments_before_any_cuda_call():
     L = N.lib()
     p = ctypes.c_void_p(4096)
     q = ctypes.c_void_p(4100)
     D = 10
 
-    def call(kind=N.GLM_POISSON, X=p, y=p, trials=None, per_row=0, n=10000, Dx=D, K=1, bias=1, z=p, Dz=2 * D + 2,
-             w_off=1, b_off=D + 1, s_off=-1, s_b=10.0, s_prior=0, sp0=0.0, sp1=0.0, sigma=1.0, tau=(0, 1, 1.0, 1.0),
-             lam=(D + 2, 2, 1.0, 1.0), scale=True, ws=None, nbytes=0):
+    def regression(kind=N.GLM_POISSON, X=p, y=p, trials=None, per_row=0, n=10000, Dx=D, K=1, bias=1, w_off=1,
+                   b_off=D + 1, s_off=-1, s_b=10.0, s_prior=0, sp0=0.0, sp1=0.0, sigma=1.0, tau=(0, 1, 1.0, 1.0),
+                   lam=(D + 2, 2, 1.0, 1.0)):
         sc = N.b2_glm_weight_scale()
         sc.tau_off, sc.tau_prior, sc.tau_p0, sc.tau_p1 = tau
         sc.lam_off, sc.lam_prior, sc.lam_p0, sc.lam_p1 = lam
-        return L.b2_glm_scaled_potential(kind, X, y, trials, per_row, n, Dx, K, bias, z, 4, Dz, w_off, b_off, s_off,
-                                         s_b, s_prior, sp0, sp1, sigma, ctypes.byref(sc) if scale else None, p, p,
-                                         ws, nbytes, None)
+        return N.b2_glm_regression(kind=kind, X=X, y=y, N=n, D=Dx, K=K, trials=trials, trials_per_row=per_row,
+                                   has_bias=bias, w_off=w_off, b_off=b_off, s_b=s_b, s_off=s_off, s_prior=s_prior,
+                                   sp0=sp0, sp1=sp1, sigma=sigma, scale=ctypes.pointer(sc))
+
+    def call(z=p, Dz=2 * D + 2, null=False, ws=None, nbytes=0, **kw):
+        m = None if null else ctypes.byref(regression(**kw))
+        return L.b2_glm_potential(m, z, 4, Dz, p, p, ws, nbytes, None)
 
     # z = [tau, w (10), b, lam (10)]: valid, so the workspace check is next
     assert call() == -5
-    assert call(X=None) == -4 and call(y=None) == -4 and call(z=None) == -4 and call(scale=False) == -4
+    assert call(X=None) == -4 and call(y=None) == -4 and call(z=None) == -4 and call(null=True) == -4
     assert call(kind=N.GLM_BINOMIAL) == -4                                   # Binomial needs its trials
     assert call(kind=7) == -2 and call(kind=N.GLM_BERNOULLI) == -2          # Bernoulli: D in {4, 8, 16, 32}
     assert call(Dx=129) == -2 and call(n=0) == -2
@@ -319,7 +323,7 @@ def test_scaled_entry_point_validates_arguments_before_any_cuda_call():
                 lam=(KD + K_CAT + 1, 2, 1.0, 1.0)) == -5
     assert call(kind=N.GLM_CATEGORICAL, Dx=32, K=K_CAT, Dz=KD + 32 + K_CAT + 1, w_off=1, b_off=KD + 1,
                 lam=(KD + K_CAT + 1, 2, 1.0, 1.0)) == -2
-    need = int(L.b2_glm_scaled_potential_workspace(N.GLM_POISSON, 10000, D, 1, 4))
+    need = int(L.b2_glm_potential_workspace(ctypes.byref(regression()), 4))
     assert need > 256 and call(ws=p, nbytes=need - 1) == -5
 
 
@@ -638,8 +642,9 @@ def test_bind_nuts_recognises_reference_pyro_models():
 
 
 @pytest.mark.gpu
-def test_constant_scale_makes_the_unchanged_native_call(monkeypatch):
-    """A constant weight scale still calls b2_glm_potential with today's arguments, never the scaled entry point."""
+def test_constant_scale_makes_one_call_with_no_scale_or_group(monkeypatch):
+    """A constant weight scale makes the one b2_glm_potential call with a null scale, a null group and today's
+    scalar arguments."""
     if EMULATE:
         pytest.skip("kernel test")
     import models
@@ -651,19 +656,14 @@ def test_constant_scale_makes_the_unchanged_native_call(monkeypatch):
     real = L.b2_glm_potential
 
     def spy(*a):
-        calls.append(("b2_glm_potential", a))
+        m = a[0]._obj
+        calls.append((m.kind, m.N, m.D, m.K, m.has_bias, a[2], a[3], m.w_off, m.b_off, m.s_w, m.s_b, bool(m.scale),
+                      bool(m.group)))
         return real(*a)
 
-    def scaled(*a):
-        calls.append(("b2_glm_scaled_potential", a))
-        return -1
-
     monkeypatch.setattr(L, "b2_glm_potential", spy)
-    monkeypatch.setattr(L, "b2_glm_scaled_potential", scaled)
     z = 0.3 * torch.randn(8, pot.dim, device=DEV)
     U, G = pot.value_and_grad(z)
     torch.cuda.synchronize()
-    assert [c[0] for c in calls] == ["b2_glm_potential"]
-    a = calls[0][1]
-    assert a[0] == N.GLM_BERNOULLI and a[3:7] == (9000, 32, 1, 1) and a[8:14] == (8, 33, 0, 32, 1.0, 10.0)
+    assert calls == [(N.GLM_BERNOULLI, 9000, 32, 1, 1, 8, 33, 0, 32, 1.0, 10.0, False, False)]
     assert bool(torch.isfinite(U).all())

@@ -1,5 +1,5 @@
 """NUTS / HMC on multilevel regression with varying slopes: ``X @ w + b + alpha[g] + SUM_k beta_k[g] * X[:, c_k]``
-through ``GlmPotential`` (``b2_glm_group_potential`` with ``b2_glm_group_effect.S`` slopes), each slope scored as G
+through ``GlmPotential`` (``b2_glm_potential`` with ``b2_glm_group_effect.S`` slopes), each slope scored as G
 more columns of the fused GLM kernel's contraction, ``x_{c_k} onehot(g)``.
 
 CPU tier: which models ``recognise`` routes to ``GlmPotential`` (every likelihood kind, centred and non-centred slopes,
@@ -275,7 +275,7 @@ def test_models_without_slopes_keep_their_route():
     assert isinstance(pot, GlmPotential) and pot.group_effect.S == 0 and pot.group["slopes"] == []
 
 
-def test_slope_entry_point_validates_arguments_before_any_cuda_call():
+def test_slopes_entry_point_validates_arguments_before_any_cuda_call():
     L = N.lib()
     p = ctypes.c_void_p(4096)
     D, G = 10, 20
@@ -283,8 +283,7 @@ def test_slope_entry_point_validates_arguments_before_any_cuda_call():
     base = dict(Dz=D + 1 + 3 * G + 1, S=2, cols=(3, 7), b_offs=(D + 1 + G, D + 2 + 2 * G), s_offs=(D + 1 + 2 * G, -1),
                 nc=(0, 1), priors=(N.SIGMA_HALFNORMAL, 0), p0=(1.0, 0.0), consts=(0.0, 0.5), Dx=D, nG=G)
 
-    def call(**kw):
-        a = dict(base, **kw)
+    def regression(a):
         e = N.b2_glm_group_effect()
         e.groups, e.G, e.a_off, e.noncentred, e.s_off, e.s_const = p, a["nG"], D + 1, 0, -1, 0.7
         e.S = a["S"]
@@ -292,8 +291,15 @@ def test_slope_entry_point_validates_arguments_before_any_cuda_call():
             s = e.slope[k]
             s.col, s.b_off, s.s_off, s.noncentred = a["cols"][k], a["b_offs"][k], a["s_offs"][k], a["nc"][k]
             s.s_prior, s.sp0, s.sp1, s.s_const = a["priors"][k], a["p0"][k], 1.0, a["consts"][k]
-        return L.b2_glm_group_potential(N.GLM_POISSON, p, p, None, 0, 10000, a["Dx"], 1, p, 4, a["Dz"], 0, D, -1,
-                                        1.0, 10.0, 0, 0.0, 0.0, 1.0, ctypes.byref(e), p, p, None, 0, None)
+        return N.b2_glm_regression(kind=N.GLM_POISSON, X=p, y=p, N=10000, D=a["Dx"], K=1, has_bias=1, w_off=0, b_off=D,
+                                   s_w=1.0, s_b=10.0, s_off=-1, sigma=1.0, group=ctypes.pointer(e))
+
+    def call(**kw):
+        a = dict(base, **kw)
+        return L.b2_glm_potential(ctypes.byref(regression(a)), p, 4, a["Dz"], p, p, None, 0, None)
+
+    def workspace(**kw):
+        return L.b2_glm_potential_workspace(ctypes.byref(regression(dict(base, **kw))), 4)
 
     assert call() == -5                                                     # valid: the workspace check is next
     assert call(S=-1) == -2 and call(S=4) == -2
@@ -311,9 +317,9 @@ def test_slope_entry_point_validates_arguments_before_any_cuda_call():
     assert call(consts=(0.0, 0.0)) == -2 and call(consts=(0.0, -1.0)) == -2
     # S = 0 ignores the slope fields
     assert call(S=0, Dz=D + 1 + G, cols=(99, 99)) == -5
-    # the workspace query's G is the number of group columns
-    assert L.b2_glm_group_potential_workspace(N.GLM_POISSON, 10000, D, 3 * G, 4) > 256
-    assert L.b2_glm_group_potential_workspace(N.GLM_POISSON, 10000, 12, 117, 4) == 256
+    # the workspace counts every group column, G (1 + S)
+    assert workspace() > 256
+    assert workspace(Dx=12, nG=39) == 256
 
 
 # ---- CPU tier: what ptxas makes of the slope kernels (glm_flat_pipeline with SLOPES) ----------------------
