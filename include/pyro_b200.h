@@ -591,6 +591,36 @@ int b2_glm_group_sum(int kind, const float* X, const float* y, const float* tria
                      size_t workspace_bytes, void* stream);
 size_t b2_glm_group_sum_workspace(int kind, int64_t N, int D, int G, int P);
 
+/*
+ * b2_glm_group_slope_sum -- b2_glm_group_sum with S varying slopes by group on columns of X as well:
+ *   eta[p,n] = <X[n,:], W[p,:]> + b[p] + alpha[p, groups[n]] + SUM_k beta_k[p, groups[n]] * X[n, col[k]]
+ * Each slope is G more columns of the one tensor-core pass over [X | onehot(g) | X[:, col[0]] onehot(g) | ..], so
+ * X is still read once and no [P, N] tensor is written; out_dW is [P][D + G (1 + S)], its columns D + (k+1) G ..
+ * D + (k+2) G - 1 the derivatives with respect to beta_k[p, :].  Every other argument, output and the precision
+ * policy are b2_glm_group_sum's; a slope column takes X's precision (rounded to TF32 or split with it).
+ * slopes: 1 <= S <= 3, col[k] distinct in [0, D), beta[k] non-null with row p at beta[k] + p * beta_stride[k]
+ * (G values; a stride of 0 shares one row with every particle), D + G (1 + S) <= 128.  Every argument is checked
+ * before any CUDA call, with b2_glm_group_sum's codes (a NULL slopes or table: B2_ERR_NULL; S, a column or a
+ * stride out of range: B2_ERR_BAD_SHAPE).
+ * workspace: b2_glm_group_slope_sum_workspace() bytes, zero-initialised ONCE by the caller.  Three launches with no
+ * host sync (CUDA graph capturable): the pack of each particle's [w | alpha | beta_1 .. beta_S] row, the kind's
+ * slope kernel and glm_finish_kernel, D + G (1 + S) wide.
+ */
+typedef struct b2_glm_slope_tables {
+  int S;                        /* varying slopes, 1 <= S <= 3 */
+  int col[3];                   /* slope k's covariate: column col[k] of X */
+  const float* beta[3];         /* slope k's table: row p at beta[k] + p * beta_stride[k], G values */
+  int64_t beta_stride[3];       /* 0: one row shared by every particle; otherwise >= G */
+} b2_glm_slope_tables;
+int b2_glm_group_slope_sum(int kind, const float* X, const float* y, const float* trials, int trials_per_row,
+                           const float* sigma, int sigma_stride, const int32_t* groups, int G, const float* W,
+                           int64_t w_stride, const float* alpha, int64_t alpha_stride,
+                           const b2_glm_slope_tables* slopes, const float* b, int64_t N, int D, int P, double scale,
+                           double weight, double sum_coeff, int flags, float* out_sum_p, float* out_total,
+                           float* out_dW, float* out_db, float* out_dsigma, void* workspace, size_t workspace_bytes,
+                           void* stream);
+size_t b2_glm_group_slope_sum_workspace(int kind, int64_t N, int D, int G, int S, int P);
+
 /* ---- optimisers --------------------------------------------------------------------------
  * Multi-tensor fused updates replacing PyroOptim's per-parameter Python loop
  * (pyro/optim/optim.py:117-155).  Per-tensor scalar state lives in DEVICE arrays so a captured

@@ -109,6 +109,13 @@ class b2_glm_regression(ctypes.Structure):
                 ("scale", ctypes.POINTER(b2_glm_weight_scale)), ("group", ctypes.POINTER(b2_glm_group_effect))]
 
 
+class b2_glm_slope_tables(ctypes.Structure):
+    """Mirror of ``b2_glm_slope_tables`` (include/pyro_b200.h): the varying slopes of a site sum, their columns of X
+    and their tables."""
+    _fields_ = [("S", ctypes.c_int32), ("col", ctypes.c_int32 * 3), ("beta", ctypes.c_void_p * 3),
+                ("beta_stride", ctypes.c_int64 * 3)]
+
+
 class b2_nuts_lockstep(ctypes.Structure):
     """Mirror of ``b2_nuts_lockstep`` (include/pyro_b200.h): device pointers of the lockstep tree state."""
     _fields_ = [("zL", ctypes.c_void_p), ("rL", ctypes.c_void_p), ("zR", ctypes.c_void_p),
@@ -173,6 +180,10 @@ SIGNATURES = {
     "b2_glm_group_sum": (_i32, [_i32, _vp, _vp, _vp, _i32, _vp, _i32, _vp, _i32, _vp, _i64, _vp, _i64, _vp, _i64,
                                 _i32, _i32, _f64, _f64, _f64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2_glm_group_sum_workspace": (_sz, [_i32, _i64, _i32, _i32, _i32]),
+    "b2_glm_group_slope_sum": (_i32, [_i32, _vp, _vp, _vp, _i32, _vp, _i32, _vp, _i32, _vp, _i64, _vp, _i64,
+                                      ctypes.POINTER(b2_glm_slope_tables), _vp, _i64, _i32, _i32, _f64, _f64, _f64,
+                                      _i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "b2_glm_group_slope_sum_workspace": (_sz, [_i32, _i64, _i32, _i32, _i32, _i32]),
     "b2_clipped_adam": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _vp]),
     "b2_adagrad_rmsprop": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _vp]),
     "b2_leapfrog_half_kick_drift": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _i32, _vp]),

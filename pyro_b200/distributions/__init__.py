@@ -14,6 +14,7 @@ inside the backend instead of by autograd's ``sum_to_size``.
 Sampling (``rsample``/``sample``) uses torch's generators; fusing it with scoring is the next
 row of the scope table (SURVEY.md 8f rank 1).
 """
+import ctypes
 import math
 import weakref
 from collections import namedtuple
@@ -1054,19 +1055,21 @@ class LinearPredictor:
     ``w``: [D], [P, D] or [P, 1, D] (vectorised particles);  ``b``: None, [], [P] or [P, 1].
 
     ``group`` (a :class:`GroupGather`, or None): a varying intercept by group, ``+ table[..., index]``, which the
-    unchanged model added (pyro_b200/lazy.py); its table has one row, or one per particle.  ``eager`` then computes the
-    predictor the way the model wrote it, so that :meth:`dense` is that value bit for bit.  A consumer that does not
-    score the group (``_weights``) must not see such a predictor: it is scored by ``b2_glm_group_sum`` or
-    materialised."""
+    unchanged model added (pyro_b200/lazy.py); its table has one row, or one per particle.  ``slopes`` (a tuple of up
+    to three :class:`SlopeGather`, each with its ``col``): varying slopes by group on columns of X,
+    ``+ table[..., index] * X[:, col]``, with the group's index and G.  ``eager`` then computes the predictor the way
+    the model wrote it, so that :meth:`dense` is that value bit for bit.  A consumer that does not score the group
+    and the slopes (``_weights``) must not see such a predictor: it is scored by ``b2_glm_group_sum`` (an intercept)
+    or ``b2_glm_group_slope_sum`` (an intercept and slopes), or materialised (slopes without an intercept)."""
 
-    def __init__(self, X, w, b=None, tensor_cores=True, group=None, eager=None):
+    def __init__(self, X, w, b=None, tensor_cores=True, group=None, eager=None, slopes=()):
         # latent values may arrive as lazy-aware SiteValue tensors (pyro_b200/lazy.py): score plain ones
         if type(w).__name__ == "SiteValue":
             w = _ops.plain_value(w)
         if type(b).__name__ == "SiteValue":
             b = _ops.plain_value(b)
         self.X, self.w, self.b = X, w, b
-        self.group, self.eager = group, eager
+        self.group, self.eager, self.slopes = group, eager, tuple(slopes)
         self.tensor_cores = tensor_cores  # False: fp32 SIMT contractions (B2_FLAG_GLM_FP32)
         D = X.shape[-1]
         self.vectorised = w.dim() > 1
@@ -1082,7 +1085,10 @@ class LinearPredictor:
         if self.b is not None:
             out = out + self.b.reshape(self.P, 1)
         out = out if self.vectorised else out.squeeze(0)
-        return out if self.group is None else out + self.group.dense()
+        out = out if self.group is None else out + self.group.dense()
+        for sg in self.slopes:
+            out = out + sg.dense()
+        return out
 
 
 class GroupGather:
@@ -1100,6 +1106,31 @@ class GroupGather:
 
     def dense(self):
         return self.table[..., self.index]
+
+
+class SlopeGather:
+    """Lazy ``table[..., index] * covariate``: a :class:`GroupGather` times a gradient-free fp32 ``[N]`` covariate on the
+    table's device (either side of ``*``).  Added to a lazy ``X @ w + b`` whose X has the covariate as column ``col``
+    (``X[:, col]``, ``X[..., col]``, ``X.select(-1, col)``), it becomes one of the predictor's varying slopes
+    (:class:`LinearPredictor` ``slopes``, which sets ``col``); every other use materialises it."""
+
+    def __init__(self, table, index, covariate):
+        if type(table).__name__ == "SiteValue":
+            table = _ops.plain_value(table)
+        self.table, self.index, self.covariate = table, index, covariate
+        self.col = None
+        self.G = table.shape[-1]
+        self.shape = torch.broadcast_shapes(table.shape[:-1] + index.shape, covariate.shape)
+        self.dtype, self.device = table.dtype, table.device
+
+    def with_col(self, col):
+        out = SlopeGather(self.table, self.index, self.covariate)
+        out.col = col
+        return out
+
+    def dense(self):
+        # a product of two floats is commutative bit for bit: the model's order of the factors does not matter
+        return self.table[..., self.index] * self.covariate
 
 
 # int32 copies of group indices for b2_glm_group_sum and GlmPotential: id(index) -> (weakref, _version, device, G,
@@ -1226,8 +1257,8 @@ def _lazy_as(x, cls):
 
 
 def _weights(lp):
-    """``(W [P, D], b [P] or None)`` of a LinearPredictor without a group effect."""
-    if lp.group is not None:
+    """``(W [P, D], b [P] or None)`` of a LinearPredictor without a group effect or slopes."""
+    if lp.group is not None or lp.slopes:
         raise RuntimeError("pyro_b200: a linear predictor with a group effect reached a kernel that does not score it")
     return lp.w.reshape(lp.P, lp.X.shape[-1]), lp.b.reshape(lp.P) if lp.b is not None else None
 
@@ -1250,8 +1281,8 @@ def _row_scope(lp, value, mask, batch_shape, D):
 
 
 def _per_row_scope(lp, value, mask, batch_shape):
-    """``(X, y, W, b)`` of :func:`_row_scope` for a predictor without a group effect, or None."""
-    rs = _row_scope(lp, value, mask, batch_shape, lp.X.shape[-1]) if lp.group is None else None
+    """``(X, y, W, b)`` of :func:`_row_scope` for a predictor without a group effect or slopes, or None."""
+    rs = _row_scope(lp, value, mask, batch_shape, lp.X.shape[-1]) if lp.group is None and not lp.slopes else None
     return None if rs is None else rs + _weights(lp)
 
 
@@ -1286,10 +1317,73 @@ def _glm_group(meta, X, y, W, b, A, sigma):
 _GlmGroupFn = _FusedSum(_glm_group)
 
 
+def _glm_slope(meta, X, y, W, b, A, sigma, *B):
+    scale, weight, coeff, _, kind, idx, trials, per_row, s_stride, cols = meta
+    N.require_cuda(X, "fused multilevel-regression likelihood")
+    P, D = W.shape
+    G, S = A.shape[-1], len(B)
+    Da = D + G * (1 + S)
+    n = X.shape[0]
+    dev = X.device
+    total = torch.empty((), dtype=torch.float32, device=dev)
+    dWAB = torch.empty((P, Da), dtype=torch.float32, device=dev)     # [d/dw | d/dalpha | d/dbeta_1 ..] per particle
+    db = torch.empty(P, dtype=torch.float32, device=dev)
+    dsig = torch.empty(P, dtype=torch.float32, device=dev) if sigma is not None and sigma.requires_grad else None
+    ws = N.workspace(dev, int(N.lib().b2_glm_group_slope_sum_workspace(kind, n, D, G, S, P)), tag="glm")
+    Wc, Ac = W.contiguous(), A.contiguous()
+    Bc = [t.contiguous() for t in B]
+    bc = b.contiguous() if b is not None else None
+    sc = sigma.contiguous() if sigma is not None else None
+    a_stride = 0 if Ac.numel() == G else G        # one table row shared by every particle, or one per particle
+    b_strides = [0 if t.numel() == G else G for t in Bc]
+    sl = N.b2_glm_slope_tables(S)
+    for k in range(S):
+        sl.col[k], sl.beta[k], sl.beta_stride[k] = cols[k], Bc[k].data_ptr(), b_strides[k]
+    N.check(N.lib().b2_glm_group_slope_sum(
+        kind, X.data_ptr(), y.data_ptr(), _ptr(trials), per_row, _ptr(sc), s_stride, idx.data_ptr(), G,
+        Wc.data_ptr(), D, Ac.data_ptr(), a_stride, ctypes.byref(sl), _ptr(bc), n, D, P, float(scale), float(weight),
+        float(coeff), 0, None, total.data_ptr(), dWAB.data_ptr(), db.data_ptr(), _ptr(dsig), ws.data_ptr(),
+        ws.numel(), N.stream_ptr(dev)), "b2_glm_group_slope_sum")
+
+    def table_grad(k, t, stride):          # block k of the group columns: alpha (0) or beta_k
+        g = dWAB[:, D + k * G:D + (k + 1) * G]
+        return (g.sum(0) if stride == 0 else g).reshape(t.shape)
+    dA = table_grad(0, A, a_stride)
+    dB = [table_grad(k + 1, t, st) for k, (t, st) in enumerate(zip(B, b_strides))]
+    if dsig is not None and s_stride == 0:
+        dsig = dsig.sum().reshape(sigma.shape)      # one sigma shared by every particle
+    return (total, None, None, dWAB[:, :D], db if b is not None else None, dA, dsig) + tuple(dB)
+
+
+_GlmSlopeFn = _FusedSum(_glm_slope)
+
+
+def _slope_sum(kind, lp, value, mask, batch_shape, coeffs, trials=(None, 0), sigma=(None, 0)):
+    """The site sum of a predictor with a group effect and varying slopes through ``b2_glm_group_slope_sum``, or None
+    outside its scope: an intercept, :func:`_row_scope` at D + G (1 + S) columns, and tables of X's dtype and device.
+    An index outside ``[0, G)`` raises IndexError before any launch."""
+    grp, slopes = lp.group, lp.slopes
+    if grp is None:
+        return None                 # slopes without an intercept: the kernel always scores alpha, so materialise
+    D = lp.X.shape[-1]
+    rs = _row_scope(lp, value, mask, batch_shape, D + grp.G * (1 + len(slopes)))
+    tables = (grp.table,) + tuple(sg.table for sg in slopes)
+    if rs is None or any(t.dtype != torch.float32 or t.device != lp.X.device for t in tables):
+        return None
+    idx = group_index_int32(grp.index, grp.G)
+    if idx is None:
+        return None
+    W, b = lp.w.reshape(lp.P, D), lp.b.reshape(lp.P) if lp.b is not None else None
+    meta = coeffs + (kind, idx) + tuple(trials) + (sigma[1], tuple(sg.col for sg in slopes))
+    return _GlmSlopeFn.apply(meta, *rs, W, b, grp.table, sigma[0], *(sg.table for sg in slopes))
+
+
 def _group_sum(kind, lp, value, mask, batch_shape, coeffs, trials=(None, 0), sigma=(None, 0)):
     """The site sum of a predictor with a group effect through ``b2_glm_group_sum``, or None outside its scope:
     :func:`_row_scope` at D + G columns, and a table of X's dtype and device.  An index outside ``[0, G)`` raises
-    IndexError before any launch."""
+    IndexError before any launch.  A predictor with slopes goes to :func:`_slope_sum`."""
+    if lp.slopes:
+        return _slope_sum(kind, lp, value, mask, batch_shape, coeffs, trials, sigma)
     grp = lp.group
     D = lp.X.shape[-1]
     rs = _row_scope(lp, value, mask, batch_shape, D + grp.G)
@@ -1326,7 +1420,7 @@ class _BernoulliLinear(Bernoulli):
 
     def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
         lz = self._lazy
-        if lz.group is not None:
+        if lz.group is not None or lz.slopes:
             out = _group_sum(N.GLM_BERNOULLI, lz, value, mask, self.batch_shape, (scale, weight, sum_coeff, unit))
             return out if out is not None else super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
         X = lz.X
@@ -1623,7 +1717,7 @@ class _PoissonLinear(Poisson):
 
     def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
         lp = self._lazy.lp
-        if lp.group is not None:
+        if lp.group is not None or lp.slopes:
             out = _group_sum(N.GLM_POISSON, lp, value, mask, self.batch_shape, (scale, weight, sum_coeff, unit))
             return out if out is not None else super()._fused_sum(value, mask, scale, weight, sum_coeff, unit)
         args = _per_row_scope(lp, value, mask, self.batch_shape)
@@ -1725,7 +1819,7 @@ class _NormalLinear(Normal):
 
     def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
         lp = self._loc_lazy.lazy
-        if lp.group is not None:
+        if lp.group is not None or lp.slopes:
             sig = _per_particle_sigma(self._scale, lp)
             out = None if sig is None else _group_sum(N.GLM_NORMAL, lp, value, mask, self.batch_shape,
                                                       (scale, weight, sum_coeff, unit), sigma=sig)
@@ -1841,7 +1935,7 @@ class _BinomialLinear(Binomial):
         return self._params[1]
 
     def _fused_sum(self, value, mask, scale, weight, sum_coeff, unit=True):
-        if self._lazy.group is not None:
+        if self._lazy.group is not None or self._lazy.slopes:
             trials = _binomial_trials(self._total_count, self._lazy)
             out = None if trials is None else _group_sum(N.GLM_BINOMIAL, self._lazy, value, mask, self.batch_shape,
                                                          (scale, weight, sum_coeff, unit), trials=trials)
@@ -1862,8 +1956,8 @@ def _binomial_new(cls, total_count=1, probs=None, logits=None, validate_args=Non
 
 
 Binomial.__new__ = staticmethod(_binomial_new)
-__all__ += ["LinearPredictor", "linear_predictor", "ExpLinearPredictor", "GroupGather", "ClassLinearPredictor",
-            "class_linear_predictor", "FactorProduct", "constant"]
+__all__ += ["LinearPredictor", "linear_predictor", "ExpLinearPredictor", "GroupGather", "SlopeGather",
+            "ClassLinearPredictor", "class_linear_predictor", "FactorProduct", "constant"]
 
 from .hmm import GaussianHMM  # noqa: E402,F401
 __all__ += ["GaussianHMM"]

@@ -46,6 +46,15 @@ lazy ``X @ w (+ b)``, before or after the bias and in either order, it becomes t
 four families above score ``X @ w + b + alpha[g]`` with ``b2_glm_group_sum``: G more columns of the one pass over X.
 Any other use of the gather, a second group effect included, materialises it exactly as torch computes it.
 
+Varying slopes have one more: such a gather times a covariate (``beta[..., g] * X[:, c]``, either side of ``*``, with
+``s * eta[..., g]`` as the gather too) is a :class:`SlopeGather` when the covariate is a gradient-free fp32 ``[N]`` view
+on the table's device.  Added to a lazy ``X @ w (+ b)`` whose X has the covariate as column ``c`` (``X[:, c]``,
+``X[..., c]``, ``X.select(-1, c)`` of that very X: same storage, X's row stride, ``c`` elements in), with the group
+effect's index object and G, it becomes one of up to three slopes on distinct columns, in any order with the bias and
+the intercept, and the four families score ``X @ w + b + alpha[g] + SUM_k beta_k[g] * X[:, c_k]`` with
+``b2_glm_group_slope_sum``: G more columns per slope of the same pass.  A product with any other tensor, any other use
+of the product, and a predictor with slopes but no intercept when it is scored, materialise exactly.
+
 This is trace-time pattern matching at the seam where Pyro already passes values around (the replayed
 guide value of pyro/poutine/replay_messenger.py:50-61); nothing in the model is rewritten.
 """
@@ -53,7 +62,7 @@ import torch
 
 from ._lazyparam import LazyExpParam
 from .distributions import (ClassLinearPredictor, ExpLinearPredictor, FactorProduct, GroupGather, LinearPredictor,
-                            _ops)
+                            SlopeGather, _ops)
 
 _VIEW_FUNCS = {"squeeze", "unsqueeze", "reshape", "view", "transpose", "t", "permute", "expand",
                "expand_as", "flatten", "contiguous", "__getitem__", "movedim", "swapaxes", "detach_",
@@ -322,16 +331,54 @@ class LinearPredictorTensor(torch.Tensor):
         predictor, an index of one value per row, and a gather that broadcasts to the predictor's shape with one
         table row, or one per particle."""
         lz = self._lazy
-        if lz.group is not None or gg.index.numel() != lz.X.shape[0] or gg.dtype != lz.dtype or gg.device != lz.device:
+        if lz.group is not None or not self._fits(gg):
             return None
+        if lz.slopes and (gg.index is not lz.slopes[0].index or gg.G != lz.slopes[0].G):
+            return None             # the slopes that came first are by another index or G
+        return LinearPredictorTensor(LinearPredictor(lz.X, lz.w, lz.b, lz.tensor_cores, group=gg, slopes=lz.slopes))
+
+    def _fits(self, gg):
+        """A gather (or slope) ``gg`` of one value per row of this predictor, of its dtype and device, that broadcasts
+        to its shape with one table row, or one per particle."""
+        lz = self._lazy
+        if gg.index.numel() != lz.X.shape[0] or gg.dtype != lz.dtype or gg.device != lz.device:
+            return False
         try:
             if torch.broadcast_shapes(gg.shape, lz.shape) != lz.shape:
-                return None
+                return False
         except RuntimeError:
+            return False
+        return gg.table.numel() // gg.G in (1, lz.P)
+
+    def _with_slope(self, sg):
+        """This ``X @ w (+ b) (+ alpha[g])`` plus the lazy slope ``sg`` as one of its varying slopes, or None: a
+        covariate that is column ``c`` of the predictor's X (its storage, X's row stride, ``c`` elements past X's first
+        element), at most three slopes on distinct columns, and the index object and G of the group effect or of the
+        slopes already there."""
+        lz = self._lazy
+        X, cov = lz.X, sg.covariate
+        if len(lz.slopes) >= 3 or not self._fits(sg):
             return None
-        if gg.table.numel() // gg.G not in (1, lz.P):
+        if cov.untyped_storage().data_ptr() != X.untyped_storage().data_ptr() or cov.stride(0) != X.stride(0):
             return None
-        return LinearPredictorTensor(LinearPredictor(lz.X, lz.w, lz.b, lz.tensor_cores, group=gg))
+        col = cov.storage_offset() - X.storage_offset()
+        if not 0 <= col < X.shape[1] or any(other.col == col for other in lz.slopes):
+            return None
+        first = lz.group if lz.group is not None else (lz.slopes[0] if lz.slopes else None)
+        if first is not None and (sg.index is not first.index or sg.G != first.G):
+            return None
+        return LinearPredictorTensor(LinearPredictor(lz.X, lz.w, lz.b, lz.tensor_cores, group=lz.group,
+                                                     slopes=lz.slopes + (sg.with_col(col),)))
+
+    def _times_covariate(self, c):
+        """``table[..., index] * c`` as a lazy slope, or None: ``c`` a gradient-free fp32 ``[N]`` view (a column of a
+        matrix is one; a tensor with storage of its own can never be a column of X) on the table's device."""
+        gg = self._lazy
+        if (not isinstance(c, torch.Tensor) or isinstance(c, (SiteValue, LinearPredictorTensor, LazyExpParam))
+                or c.dtype != torch.float32 or gg.dtype != torch.float32 or c.dim() != 1
+                or c.numel() != gg.index.numel() or c.requires_grad or c.device != gg.device or c._base is None):
+            return None
+        return LinearPredictorTensor(SlopeGather(gg.table, gg.index, c))
 
     def _scaled(self, s):
         """``s * table[..., index]`` as the gather of the table ``s * table``, or None: ``s`` a number or one scalar
@@ -356,13 +403,16 @@ class LinearPredictorTensor(torch.Tensor):
 
     def _with_bias(self, b):
         lz = self._lazy
-        if isinstance(lz, GroupGather):
+        if isinstance(lz, (GroupGather, SlopeGather)):
             if isinstance(b, LinearPredictorTensor) and isinstance(b._lazy, LinearPredictor):
-                return b._with_group(lz)
+                return b._with_group(lz) if isinstance(lz, GroupGather) else b._with_slope(lz)
             return None
         if isinstance(lz, LinearPredictor) and isinstance(b, LinearPredictorTensor) and isinstance(b._lazy,
                                                                                                   GroupGather):
             return self._with_group(b._lazy)
+        if isinstance(lz, LinearPredictor) and isinstance(b, LinearPredictorTensor) and isinstance(b._lazy,
+                                                                                                  SlopeGather):
+            return self._with_slope(b._lazy)
         if isinstance(lz, (FactorProduct, ExpLinearPredictor)):
             return None
         if isinstance(lz, ClassLinearPredictor):
@@ -387,7 +437,8 @@ class LinearPredictorTensor(torch.Tensor):
             return None
         if bp.numel() == 1 and lz.P > 1:
             bp = bp.reshape(()).expand(lz.P)
-        return LinearPredictorTensor(LinearPredictor(lz.X, lz.w, bp, lz.tensor_cores, group=lz.group))
+        return LinearPredictorTensor(LinearPredictor(lz.X, lz.w, bp, lz.tensor_cores, group=lz.group,
+                                                     slopes=lz.slopes))
 
     @classmethod
     def __torch_dispatch__(cls, func, types, args=(), kwargs=None):
@@ -413,15 +464,21 @@ class LinearPredictorTensor(torch.Tensor):
                 if out is not None:
                     if isinstance(out.lazy, LinearPredictor):
                         out._eager = _eager_call(func, args, kwargs)
-                        if out.lazy.group is not None:
+                        if out.lazy.group is not None or out.lazy.slopes:
                             out.lazy.eager = out._eager      # dense() is the sum in the order the model wrote it
                     return out
             if name in _MUL_FUNCS and len(args) == 2 and not kwargs and isinstance(self._lazy, GroupGather):
-                out = self._scaled(args[1] if args[0] is self else args[0])
+                other = args[1] if args[0] is self else args[0]
+                out = self._scaled(other)
+                if out is None:
+                    out = self._times_covariate(other)
+                    if out is not None:
+                        out._eager = _eager_call(func, args, kwargs)
                 if out is not None:
                     return out
-            # a lazy gather answers nothing else: every other use materialises it
-            if any(isinstance(a, LinearPredictorTensor) and isinstance(a._lazy, GroupGather) for a in args):
+            # a lazy gather or slope answers nothing else: every other use materialises it
+            if any(isinstance(a, LinearPredictorTensor) and isinstance(a._lazy, (GroupGather, SlopeGather))
+                   for a in args):
                 with torch._C.DisableTorchFunctionSubclass():
                     return func(*_plain(args), **{k: _plain(v) for k, v in kwargs.items()})
             if name == "exp" and len(args) == 1 and not kwargs and isinstance(self._lazy, LinearPredictor):
