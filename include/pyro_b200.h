@@ -491,10 +491,19 @@ size_t b2_poisson_product_workspace(int64_t N, int K, int64_t J, int P);
  *   with alpha ~ Normal(0, s_a)[G] (centred) or alpha = s_a * e, e ~ Normal(0, 1)[G] (non-centred), s_a the
  *   constant group->s_const or latent (log s_a at group->s_off, prior as for sigma); each slope k (group->S = 1..3)
  *   has its table, form and scale the same way, on column col_k of X (0 <= col_k < D, the S columns distinct).
- *   The likelihood runs on [X | onehot(g) | x_{col_1} onehot(g) ..], G (1 + S) more columns synthesised in shared
- *   memory from g, so X is read once and no [C, N] tensor is made: every kind but B2_GLM_CATEGORICAL, any D >= 1
- *   with D + G (1 + S) <= 128, and a constant weight scale.  A group index outside [0, G) makes U and the group
- *   effect's gradients NaN.
+ *   Scope: every kind but B2_GLM_CATEGORICAL, 1 <= D <= 128, 1 <= G <= 65536, 0 <= S <= 3, a constant weight
+ *   scale, group->sorted 0 or 1.  X is read once for every chain and no [C, N] tensor is made, by one of two routes
+ *   that the width decides:
+ *     D + G (1 + S) <= 128: the likelihood runs on [X | onehot(g) | x_{col_1} onehot(g) ..], G (1 + S) more columns
+ *       of the contraction synthesised in shared memory from g; group->sorted is not read.
+ *     D + G (1 + S) > 128: not for B2_GLM_BINOMIAL, and only with group->sorted == 1, the caller's promise that
+ *       groups is non-decreasing (a model's rows can be sorted by group once: the posterior does not depend on
+ *       their order).  The contraction
+ *       is D wide; alpha[g] + SUM_k beta_k[g] X[n, col_k] is gathered from group-major tables and added to the
+ *       logits in fp32, and the group gradients are sums over each group's run of rows, in a fixed order.  A
+ *       descending pair of indices breaks the promise and makes U NaN for every chain (nothing is read or written
+ *       out of bounds).  With group->sorted == 0 such a model returns B2_ERR_BAD_SHAPE.
+ *   A group index outside [0, G) makes U and the group effect's gradients NaN on either route.
  * Dz is exactly the sum of the present blocks' widths (w, b, log sigma, log tau, log lam, alpha or e, log s_a, each
  * slope's table and log s_k), none overlapping another or leaving the row.  s_w > 0 (constant weight scale) and,
  * with a bias, s_b > 0; a constant sigma or group scale is positive in fp32; a prior's parameters are positive,
@@ -535,12 +544,13 @@ typedef struct b2_glm_group_effect {
   const int32_t* groups;        /* [N] group of each row, 16-byte aligned */
   int64_t a_off;                /* z columns of alpha (centred) or e (non-centred), G of them */
   int64_t s_off;                /* z column of log s_a, -1 for the constant s_const */
-  int G;                        /* number of groups: 1 <= G, D + G <= 128 */
+  int G;                        /* number of groups: 1 <= G <= 65536 */
   int noncentred;               /* 0: alpha ~ Normal(0, s_a); 1: alpha = s_a * e, e ~ Normal(0, 1) */
   int s_prior;                  /* B2_SIGMA_HALFNORMAL .. B2_SIGMA_LOGNORMAL (latent s_a) */
   double s_const, sp0, sp1;
   int S;                        /* varying slopes, 0 <= S <= 3 */
   b2_glm_group_slope slope[3];  /* the first S are read */
+  int sorted;                   /* 1: the caller promises groups is non-decreasing; 0: no promise */
 } b2_glm_group_effect;
 typedef struct b2_glm_regression {
   int kind;                               /* B2_GLM_BERNOULLI .. B2_GLM_BINOMIAL */

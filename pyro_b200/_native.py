@@ -94,7 +94,7 @@ class b2_glm_group_effect(ctypes.Structure):
     _fields_ = [("groups", ctypes.c_void_p), ("a_off", ctypes.c_int64), ("s_off", ctypes.c_int64),
                 ("G", ctypes.c_int32), ("noncentred", ctypes.c_int32), ("s_prior", ctypes.c_int32),
                 ("s_const", ctypes.c_double), ("sp0", ctypes.c_double), ("sp1", ctypes.c_double),
-                ("S", ctypes.c_int32), ("slope", b2_glm_group_slope * 3)]
+                ("S", ctypes.c_int32), ("slope", b2_glm_group_slope * 3), ("sorted", ctypes.c_int32)]
 
 
 class b2_glm_regression(ctypes.Structure):

@@ -50,6 +50,20 @@
 // logits stay fp32-exact under SPLIT_X and GEMM 2's columns D + kG .. D + (k+1)G - 1 are d loglik / d beta_k.  A
 // row with an index outside [0, G) gets NaN in the slope columns too.
 //
+// Gathered group effects (GATHER, for more groups than the contraction has columns): X @ w + b + alpha[g] + SUM_k
+// beta_k[g] x_{c_k} with GEMM 1 and GEMM 2 over X's D columns only, as the plain kernels; W, dW and the partials are
+// D wide.  The group term e[n, p] = T_0[g_n][p] + SUM_k T_k[g_n][p] X[n, c_k] (GlmGather::tab, group-major [1 + S][G]
+// tables of the chains' values, so a row's 64 chains are one 256-byte line) is built in fp32 into the warpgroup's
+// [64 rows][64 chains] shared area while the tile's g and covariates are still in shared memory, and added to GEMM
+// 1's accumulators before the family's epilogue, so every logit stays fp32-exact and no epilogue changes.  The same
+// area then takes the tile's residuals (TF32-rounded, as GEMM 2 takes them), and the group gradients are run sums
+// of them over rows of equal g: the rows must be sorted by group.  Each warpgroup takes a contiguous range of tiles
+// (gather_range) and walks its rows in order, one thread per chain and block; a run that starts after the range's
+// first row and ends before its last is written once to the group-gradient table GlmGather::gsum [1 + S][G][cp]; the
+// range's first run goes to slot 0 and its last (if another) to slot 1 of GlmGather::slots [Q][2][4][cp], which the
+// potential's finish adds in row order.  GlmGather::status[q] gets bit 0 for an index outside [0, G) (its rows get a
+// NaN term, and no table entry is written for it) and bit 1 for a descending pair, checked across ranges too.
+//
 // Determinism: every CTA writes its partials once (warpgroups summed in a fixed order); no float atomics.
 #pragma once
 #include <cuda.h>
@@ -63,7 +77,7 @@ namespace tcf {
 
 using namespace tc;
 
-template <int DC, bool GROUPS = false>
+template <int DC, bool GROUPS = false, bool GATHER = false>
 struct Cfg {
   static constexpr int kKD = 32 * DC;                          // padded feature count
   static constexpr int kN2 = kKD + 8;                          // GEMM 2 width: dW columns, db, 7 unused
@@ -77,8 +91,9 @@ struct Cfg {
   static constexpr uint32_t WG_XT = WG_XLO + kOp;              // X^T [kb 2][c KD + 8][32 n], n permuted (kt_pos)
   static constexpr uint32_t WG_LAND = WG_XT + 2 * kXtBlock;    // landing buffer [64][D], unswizzled
   static constexpr uint32_t WG_Y = WG_LAND + kOp;              // y [64] (Binomial: two slots of y, trials)
-  static constexpr uint32_t WG_G = WG_Y + 1024;                // group index [64] int32 (GROUPS)
-  static constexpr uint32_t kWGBytes = WG_G + (GROUPS ? 1024 : 0);
+  static constexpr uint32_t WG_G = WG_Y + 1024;                // group index [64] int32 (GROUPS, GATHER)
+  static constexpr uint32_t WG_E = WG_G + 1024;                // GATHER: [64 n][64 p] fp32 group term, then residuals
+  static constexpr uint32_t kWGBytes = WG_G + (GROUPS ? 1024 : 0) + (GATHER ? 1024 + 16384 : 0);
   // CTA layout (operand regions 1024-byte aligned: the 128-byte swizzle pattern is taken from address bits)
   static constexpr uint32_t OFF_WHI = 0;                       // [DC][p 64][32] SW128
   static constexpr uint32_t OFF_WLO = OFF_WHI + kOp;
@@ -100,21 +115,131 @@ __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_
                : "memory");
 }
 
+// GATHER: the [64 n][64 p] shared area of a warpgroup holds entry (n, p) at n * 64 + (p ^ 8 ((n >> 1) & 3)), so
+// that both the accumulator fragment (acc1[i], term_at) and a warp's row of 64 chains are free of bank conflicts
+__device__ __forceinline__ int term_at(int i, int w4, int gid, int t4) {
+  const int n = 8 * (i >> 2) + 2 * t4 + (i & 1), p = 16 * w4 + gid + 8 * ((i >> 1) & 1);
+  return n * kM + (p ^ (t4 << 3));
+}
+
+// GATHER: the tile's group term e[n, p] = T_0[g_n][p] + SUM_k T_k[g_n][p] X[n, c_k] into et, from the landing
+// buffer and the group indices before they are refilled; warp w4 builds rows 16 w4 .. 16 w4 + 15, each lane two
+// chains.  An index outside [0, G) gives NaN, rows past the tile's end 0.
+__device__ __forceinline__ void gather_term(const GlmGather& ga, const float* land, const int32_t* gs, float* et,
+                                            int D, int rows, int slab, int w4, int lane) {
+  const int64_t cb = (int64_t)slab * kM + 2 * lane;
+#pragma unroll 4
+  for (int i = 0; i < 16; ++i) {
+    const int r = 16 * w4 + i;
+    float2 e = make_float2(0.f, 0.f);
+    if (r < rows) {
+      const int gi = gs[r];
+      if ((unsigned)gi < (unsigned)ga.G) {
+        const float* tr = ga.tab + (int64_t)gi * ga.cp + cb;
+        e = *reinterpret_cast<const float2*>(tr);
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+          if (k < ga.S) {
+            const float x = land[r * D + ga.col[k]];
+            const float2 v = *reinterpret_cast<const float2*>(tr + (int64_t)(k + 1) * ga.G * ga.cp);
+            e.x = fmaf(v.x, x, e.x);
+            e.y = fmaf(v.y, x, e.y);
+          }
+      } else {
+        e = make_float2(__int_as_float(0x7fc00000), __int_as_float(0x7fc00000));
+      }
+    }
+    reinterpret_cast<float2*>(et + r * kM)[lane ^ (((r >> 1) & 3) << 2)] = e;
+  }
+}
+
+// GATHER: one thread's walk over its warpgroup's range of rows in order, for chain ch and the group effect's blocks
+// k0 = kb and k1 = kb + 2 (thread t: kb = t >> 6; block 0 the intercept, block k slope k, k <= S): the run sums
+// SUM r[n, ch] (times X[n, c] for a slope) over each run of equal g.  open is 0 before the range's first row, 1
+// while its first run is open and 2 after.
+struct GatherWalk {
+  int q, k0, k1, c0, c1;                       // c0, c1: the blocks' covariate columns, -1 for none
+  int64_t ch;
+  int cur, open, stat;
+  float s0, s1;
+  __device__ __forceinline__ void init(const GlmGather& ga, int qi, int t, int slab) {
+    const int kb = t >> 6;
+    q = qi;
+    k0 = kb;
+    k1 = kb + 2;
+    c0 = kb == 1 ? ga.col[0] : -1;
+    c1 = kb == 0 ? (ga.S >= 2 ? ga.col[1] : -1) : (ga.S >= 3 ? ga.col[2] : -1);
+    ch = (int64_t)slab * kM + (t & 63);
+    cur = open = stat = 0;
+    s0 = s1 = 0.f;
+  }
+  // the open run's sums: where 0 / 1 the range's first / last slot, 2 the table (a valid group only)
+  __device__ __forceinline__ void flush(const GlmGather& ga, int where) {
+    float *d0, *d1;
+    if (where < 2) {
+      float* b = ga.slots + (int64_t)(2 * q + where) * 4 * ga.cp + ch;
+      d0 = b + (int64_t)k0 * ga.cp;
+      d1 = b + (int64_t)k1 * ga.cp;
+    } else {
+      if ((unsigned)cur >= (unsigned)ga.G) return;
+      d0 = ga.gsum + ((int64_t)k0 * ga.G + cur) * ga.cp + ch;
+      d1 = ga.gsum + ((int64_t)k1 * ga.G + cur) * ga.cp + ch;
+    }
+    *d0 = s0;
+    if (k1 <= ga.S) *d1 = s1;
+  }
+  // the tile's rows row0 .. row0 + rows - 1, residuals in et
+  __device__ __forceinline__ void tile(const GlmGather& ga, const float* et, const float* __restrict__ X, int D,
+                                       int64_t row0, int rows) {
+    if (k0 > ga.S) return;
+    const int p = (int)(ch & 63);
+#pragma unroll 4
+    for (int n = 0; n < rows; ++n) {
+      const int64_t row = row0 + n;
+      const int gn = __ldg(ga.idx + row);
+      const float r = et[n * kM + (p ^ (((n >> 1) & 3) << 3))];
+      const float x0 = c0 >= 0 ? __ldg(X + row * D + c0) : 1.f;
+      const float x1 = c1 >= 0 ? __ldg(X + row * D + c1) : 0.f;
+      if ((unsigned)gn >= (unsigned)ga.G) stat |= 1;
+      if (open == 0) {
+        if (row > 0 && __ldg(ga.idx + row - 1) > gn) stat |= 2;
+        open = 1;
+      } else if (gn != cur) {
+        flush(ga, open == 1 ? 0 : 2);
+        if (gn < cur) stat |= 2;
+        open = 2;
+        s0 = s1 = 0.f;
+      }
+      cur = gn;
+      s0 = fmaf(r, x0, s0);
+      s1 = fmaf(r, x1, s1);
+    }
+  }
+  // the range's last run, and its status (one thread of the first slab)
+  __device__ __forceinline__ void finish(const GlmGather& ga, int slab, int t) {
+    if (k0 <= ga.S && open) flush(ga, open == 1 ? 0 : 1);
+    if (t == 0 && slab == 0) ga.status[q] = stat;
+  }
+};
+
 // wgmma accumulator fragment (m64nN, f32): thread (warp w4 of the warpgroup, lane = 4 gid + t4) holds
 // d[4j + 2h + e] = D[16 w4 + gid + 8h][8j + 2 t4 + e].
 // Binomial only (glm_tc_common.cuh): trials are the per-row counts [N] (kRowTrials, bulk-copied behind y) or
 // the one count of every row (kConstTrials).
 // GROUPS: grp.idx[N] the group index of each row, grp.G groups and (SLOPES) grp.S slopes on X's columns grp.col;
 // W is [P][D + G (1 + S)], the partials [gx][P][D + G (1 + S) + 2].  Without SLOPES, S is 0.
-template <class Fam, int DC, bool SPLIT_X, bool GROUPS = false, bool SLOPES = false>
+// GATHER: the group effect of ga (P <= ga.cp), W and the partials D wide.
+template <class Fam, int DC, bool SPLIT_X, bool GROUPS = false, bool SLOPES = false, bool GATHER = false>
 __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, const float* __restrict__ y,
                                                   const float* __restrict__ W, const float* __restrict__ bvec,
                                                   int64_t N, int D, int P, float* __restrict__ partials,
                                                   const float* __restrict__ trials = nullptr,
-                                                  GlmGroups grp = {}) {
-  using C = Cfg<DC, GROUPS>;
+                                                  GlmGroups grp = {}, GlmGather ga = {}) {
+  static_assert(!(GATHER && GROUPS), "one group-effect route per kernel");
+  using C = Cfg<DC, GROUPS, GATHER>;
   constexpr int kKD = C::kKD, kWG = C::kWG;
-  const int32_t* __restrict__ groups = grp.idx;
+  constexpr bool kIdx = GROUPS || GATHER;      // the tiles bring their group indices
+  const int32_t* __restrict__ groups = GATHER ? ga.idx : grp.idx;
   const int G = grp.G;
   const int Da = GROUPS ? D + (SLOPES ? grp.cols() : G) : D;   // columns of the contraction
   pdl_enter();   // lets glm_finish_kernel be resident (blocked in its griddepcontrol.wait) before this kernel ends
@@ -155,7 +280,18 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
     const uint32_t bar = base + C::OFF_BAR + 8u * (uint32_t)wg;
     float* land = reinterpret_cast<float*>(my + C::WG_LAND);
     float* ys = reinterpret_cast<float*>(my + C::WG_Y);
-    int32_t* gs = reinterpret_cast<int32_t*>(my + C::WG_G);   // GROUPS only
+    int32_t* gs = reinterpret_cast<int32_t*>(my + C::WG_G);   // GROUPS, GATHER only
+    // the warpgroup's tiles: it = it0, it0 + kStep, .. < itn, tile row0_of(it); GATHER: the contiguous range of tiles
+    // [tb, tb + itn) of warpgroup q, the others round-robin over the CTAs and then the CTA's warpgroups
+    const int q = blockIdx.x * kWG + wg;
+    int64_t tb = 0, te = 0;
+    if constexpr (GATHER) gather_tiles(q, gridDim.x * kWG, ntiles, tb, te);
+    const int it0 = GATHER ? 0 : wg, itn = GATHER ? (int)(te - tb) : nt;
+    constexpr int kStep = GATHER ? 1 : kWG;
+    auto row0_of = [&](int it) -> int64_t {
+      if constexpr (GATHER) return (tb + it) * kRows;
+      else return (blockIdx.x + (int64_t)it * gridDim.x) * kRows;
+    };
     float bias[2];                             // of particles 16 w4 + gid + 8h
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -169,32 +305,36 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
     if constexpr (Fam::kTrials == kConstTrials) mconst = *trials;
     // tile it -> landing buffer; one thread of the warpgroup issues the loads
     auto load = [&](int it) {
-      const int64_t row0 = (blockIdx.x + (int64_t)it * gridDim.x) * kRows;
+      const int64_t row0 = row0_of(it);
       const int rows = (int)(N - row0 < kRows ? N - row0 : kRows);
       const uint32_t xb = (uint32_t)(rows * D) * 4u, yb = (uint32_t)rows * 4u;
       const uint32_t xbulk = xb & ~15u, ybulk = yb & ~15u;
-      const int yo = Fam::kTrials != kNoTrials ? (((it - wg) / kWG) & 1) * 2 * kRows : 0;
+      const int yo = Fam::kTrials != kNoTrials ? (((it - it0) / kStep) & 1) * 2 * kRows : 0;
       if (rows < kRows || xbulk != xb) {       // the last tile: its remainder and zeros for y past N
         const float* xsrc = X + row0 * D;
         for (uint32_t i = xbulk / 4; i < xb / 4; ++i) land[i] = xsrc[i];
         for (int i = (int)(ybulk / 4); i < kRows; ++i) ys[yo + i] = (i < rows) ? y[row0 + i] : 0.f;
         if constexpr (kRowM)
           for (int i = (int)(ybulk / 4); i < kRows; ++i) ys[yo + kRows + i] = (i < rows) ? trials[row0 + i] : 0.f;
-        if constexpr (GROUPS)
+        if constexpr (kIdx)
           for (int i = (int)(ybulk / 4); i < kRows; ++i) gs[i] = (i < rows) ? groups[row0 + i] : 0;
       }
       // the arrive releases the ordinary stores above to the warpgroup's mbar_wait
-      mbar_expect_tx(bar, xbulk + ((kRowM ? 2 : 1) + (GROUPS ? 1 : 0)) * ybulk);
+      mbar_expect_tx(bar, xbulk + ((kRowM ? 2 : 1) + (kIdx ? 1 : 0)) * ybulk);
       if (xbulk) bulk_load(my_s + C::WG_LAND, X + row0 * D, xbulk, bar);
       if (ybulk) bulk_load(my_s + C::WG_Y + 4 * yo, y + row0, ybulk, bar);
       if constexpr (kRowM)
         if (ybulk) bulk_load(my_s + C::WG_Y + 4 * (yo + kRows), trials + row0, ybulk, bar);
-      if constexpr (GROUPS)
+      if constexpr (kIdx)
         if (ybulk) bulk_load(my_s + C::WG_G, groups + row0, ybulk, bar);
     };
-    if (t == 0 && wg < nt) load(wg);
-    for (int k = 0, it = wg; it < nt; ++k, it += kWG) {
-      const int64_t row0 = (blockIdx.x + (int64_t)it * gridDim.x) * kRows;
+    // GATHER: the walk over the range's rows (one thread per chain p and blocks kb, kb + 2 of the group effect)
+    float* et = reinterpret_cast<float*>(my + C::WG_E);
+    GatherWalk walk;
+    if constexpr (GATHER) walk.init(ga, q, t, slab);
+    if (t == 0 && it0 < itn) load(it0);
+    for (int k = 0, it = it0; it < itn; ++k, it += kStep) {
+      const int64_t row0 = row0_of(it);
       const int rows = (int)(N - row0 < kRows ? N - row0 : kRows);
       mbar_wait(bar, (uint32_t)k & 1u);
       // GEMM 2 of this warpgroup's previous tile has finished reading X^T and the g registers
@@ -271,6 +411,7 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
           }
         }
       }
+      if constexpr (GATHER) gather_term(ga, land, gs, et, D, rows, slab, w4, lane);
       typename Fam::Labels yr;                 // read before the refill
       if constexpr (Fam::kTrials != kNoTrials) {
         const float* slot = ys + (k & 1) * 2 * kRows;
@@ -282,7 +423,7 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
       fence_proxy_async();
       wg_bar(1 + wg);
       // the landing buffer is free: the warpgroup's next tile arrives while this one is contracted
-      if (t == 0 && it + kWG < nt) load(it + kWG);
+      if (t == 0 && it + kStep < itn) load(it + kStep);
       float acc1[32];
       if constexpr (Fam::kBiasInEpilogue) {
         const float zero[2] = {0.f, 0.f};
@@ -290,16 +431,36 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
       } else {
         gemm1<DC, SPLIT_X>(acc1, bias, base + C::OFF_WHI, base + C::OFF_WLO, my_s + C::WG_XOP, my_s + C::WG_XLO);
       }
+      if constexpr (GATHER) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc1[i] += et[term_at(i, w4, gid, t4)];
+      }
       uint32_t g[32];                          // indexed like acc1
       if constexpr (Fam::kBiasInEpilogue)
         Fam::tile_epilogue(acc1, bias, yr, row0, N, t4, rows < kRows, lpa, g);
       else
         Fam::tile_epilogue(acc1, yr, row0, N, t4, rows < kRows, lpa, g);
+      if constexpr (GATHER) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) et[term_at(i, w4, gid, t4)] = __uint_as_float(g[i]);
+      }
       // left running while the next tile is waited for
-      gemm2<C::kN2>(acc2, g, my_s + C::WG_XT, it == wg);
+      gemm2<C::kN2>(acc2, g, my_s + C::WG_XT, it == it0);
+      if constexpr (GATHER) {
+        wg_bar(1 + wg);                        // every residual of the tile is in et
+        walk.tile(ga, et, X, D, row0, rows);
+        wg_bar(1 + wg);                        // et is free for the next tile's term
+      }
     }
     wgmma_wait0();
     fence_regs(acc2);
+    if constexpr (GATHER) {
+      walk.finish(ga, slab, t);
+      if (itn == 0) {                          // a warpgroup without tiles adds zeros to the CTA's partials
+#pragma unroll
+        for (int i = 0; i < C::kN2 / 2; ++i) acc2[i] = 0.f;
+      }
+    }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       auto v = lpa[h];
@@ -309,10 +470,19 @@ __device__ __forceinline__ void glm_flat_pipeline(const float* __restrict__ X, c
     }
   }
   double dterm = 0.0;
-  if constexpr (Fam::kDataTerm) dterm = Fam::template data_term<C::kThreads>(y, trials, N);
-  // CTA results through the warpgroup regions, idle now
-  cta_partials<1, C::kN2, C::kThreads>(reinterpret_cast<float*>(sm + C::OFF_WG), acc2, lpa, wg, nt, slab, P, 1, Da,
-                                       partials, dterm);
+  if constexpr (Fam::kDataTerm) {
+    if constexpr (GATHER) {                    // the CTA's rows are its warpgroups' ranges, one contiguous span
+      int64_t t0, t1, u0, u1;
+      gather_tiles(blockIdx.x * kWG, gridDim.x * kWG, ntiles, t0, u0);
+      gather_tiles(blockIdx.x * kWG + kWG - 1, gridDim.x * kWG, ntiles, u1, t1);
+      dterm = Fam::template data_term<C::kThreads, true>(y, trials, N, t0 * kRows, min(t1 * kRows, N));
+    } else {
+      dterm = Fam::template data_term<C::kThreads>(y, trials, N);
+    }
+  }
+  // CTA results through the warpgroup regions, idle now (GATHER: every warpgroup, a tileless one with zeros)
+  cta_partials<1, C::kN2, C::kThreads>(reinterpret_cast<float*>(sm + C::OFF_WG), acc2, lpa, wg, GATHER ? kWG : nt,
+                                       slab, P, 1, Da, partials, dterm);
 }
 
 }  // namespace tcf

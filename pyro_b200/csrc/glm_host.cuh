@@ -24,6 +24,30 @@ struct GlmGroups {
   __host__ __device__ int cols() const { return idx ? G * (1 + S) : 0; }
 };
 
+// A gathered group effect (glm_flat_pipeline's GATHER, for more groups than the contraction has columns): the same
+// X @ w + b + alpha[g] + SUM_k beta_k[g] X[n, col[k]], with idx sorted, but the group term added to GEMM 1's logits
+// from the group-major tables tab [1 + S][G][cp] (cp >= P chains, a multiple of 64) and the group gradients summed
+// over the rows of each group (run sums): gsum [1 + S][G][cp] for a group inside one warpgroup's range of tiles (the
+// caller zeroes it first), slots [Q][2][4][cp] for the first and last run of warpgroup q's range, status [Q] with bit
+// 0 for an index outside [0, G) and bit 1 for a descending pair.  Q = gx * (warpgroups per CTA).
+struct GlmGather {
+  const int32_t* idx = nullptr;
+  int G = 0;
+  int S = 0;
+  int col[3] = {0, 0, 0};
+  int cp = 0;
+  const float* tab = nullptr;
+  float* gsum = nullptr;
+  float* slots = nullptr;
+  int* status = nullptr;
+};
+
+// warpgroup q's contiguous range of tiles [t0, t1) among Q for ntiles tiles (GATHER); rows [64 t0, min(64 t1, N))
+__host__ __device__ inline void gather_tiles(int q, int Q, int64_t ntiles, int64_t& t0, int64_t& t1) {
+  t0 = (int64_t)q * ntiles / Q;
+  t1 = (int64_t)(q + 1) * ntiles / Q;
+}
+
 // ---- glm.cu ----
 // The second launch of every GLM likelihood call: glm_finish_kernel over the CTA partials [gx][P][K (D + 1) + 1].
 // The Normal noise scale sigma[p * sigma_stride] with n = N rows and out_dsigma are optional.  The per-particle sums
@@ -68,6 +92,17 @@ int glm_binomial_logits(const float* X, const float* y, const float* trials, int
                         const float* b, int64_t N, int D, int P, double scale, double weight, double sum_coeff,
                         int flags, float* out_sum_p, float* out_total, float* out_dW, float* out_db, void* workspace,
                         size_t workspace_bytes, cudaStream_t s, GlmGroups grp);
+
+// ---- glm_group_gather_tc.cu ----
+// The run-sum ranges Q of a gathered call: CTAs times the warpgroups of the kernel that D dispatches to
+int glm_gather_ranges(int64_t N, int D);
+// The likelihood call of kind B2_GLM_BERNOULLI, B2_GLM_POISSON or B2_GLM_NORMAL with a gathered group effect (any
+// other kind: B2_ERR_BAD_SHAPE), X split (every logit fp32-exact): the kind's gather kernel and glm_finish_kernel,
+// D wide, with weight = -1 (dW, db, dsigma are derivatives of -loglik; the run sums of ga are d loglik / d T_k
+// before the finish's factor).  workspace: glm_row_workspace(N, D, P) bytes.
+int glm_gather_likelihood(int kind, const float* X, const float* y, const float* W, const float* b,
+                          const float* sigma, float* dsigma, int64_t N, int D, int P, float* sum_p, float* dW,
+                          float* db, void* workspace, cudaStream_t s, const GlmGather& ga);
 
 // ---- glm_group.cu ----
 // The group kernel of kind B2_GLM_BERNOULLI, B2_GLM_POISSON or B2_GLM_BINOMIAL (row_trials: per-row counts m) with X

@@ -21,7 +21,11 @@
 // the trial counts to its likelihood call as a fixed operand.  A latent weight scale (w ~ Normal(0, tau * lam))
 // changes only the finish's weight terms.  A group effect, a varying intercept alpha[g] and up to three varying
 // slopes beta_k[g] on columns of X, makes each chain's packed weight row [w | alpha | beta_1 ..], and the likelihood
-// runs on [X | onehot(g) | x_{c_1} onehot(g) ..] (glm_flat_tc.cuh GROUPS).
+// runs on [X | onehot(g) | x_{c_1} onehot(g) ..] (glm_flat_tc.cuh GROUPS) when those D + G (1 + S) columns fit in
+// 128.  Past that (rows sorted by group) the group effect is gathered (glm_flat_tc.cuh GATHER,
+// glm_group_gather_tc.cu): the pack writes the group-major tables T_k [1 + S][G][cp] and zeroes the group-gradient
+// table, the likelihood runs D wide and leaves the run sums of each group, and the finish adds the runs that cross
+// the warpgroups' ranges (gather_fixup) before the same prior terms.
 #include <math.h>
 
 #include "b2_common.cuh"
@@ -67,6 +71,45 @@ __global__ void __launch_bounds__(256) glm_potential_pack_kernel(const float* __
   } else {
     bp[c * Kb + (j - KD)] = z[c * Dz + b_off + (j - KD)];
   }
+}
+
+// The gathered route: Wp / bp / sig as glm_potential_pack_kernel<false> (KD = D), then tab[k][a][c] (c < cp) the
+// value of group a in block k for chain c (0 for c >= C), and gsum zeroed
+__global__ void __launch_bounds__(256) glm_potential_gather_pack_kernel(
+    const float* __restrict__ z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int D, int Kb,
+    float* __restrict__ Wp, float* __restrict__ bp, int64_t s_off, float s_const, float* __restrict__ sig,
+    b2_glm_group_effect ge, int cp, float* __restrict__ tab, float* __restrict__ gsum) {
+  const int64_t per = D + Kb, nw = C * per;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (sig != nullptr && i < C) sig[i] = s_off >= 0 ? expf(z[i * Dz + s_off]) : s_const;
+  if (i < nw) {
+    const int64_t c = i / per, j = i - c * per;
+    if (j < D) Wp[c * D + j] = z[c * Dz + w_off + j];
+    else bp[c * Kb + (j - D)] = z[c * Dz + b_off + (j - D)];
+    return;
+  }
+  const int64_t e = i - nw;
+  if (e >= (int64_t)(1 + ge.S) * ge.G * cp) return;
+  const int64_t kg = e / cp, c = e - kg * cp;
+  const int k = (int)(kg / ge.G), a = (int)(kg - (int64_t)k * ge.G);
+  int64_t off = ge.a_off, so = ge.s_off;
+  int nc = ge.noncentred;
+  double sc = ge.s_const;
+#pragma unroll
+  for (int m = 0; m < 3; ++m)
+    if (k == m + 1) {
+      off = ge.slope[m].b_off;
+      so = ge.slope[m].s_off;
+      nc = ge.slope[m].noncentred;
+      sc = ge.slope[m].s_const;
+    }
+  float v = 0.f;
+  if (c < C) {
+    v = z[c * Dz + off + a];
+    if (nc) v *= so >= 0 ? expf(z[c * Dz + so]) : (float)sc;
+  }
+  tab[e] = v;
+  gsum[e] = 0.f;
 }
 
 constexpr double kHalfLog2Pi = 0.91893853320467274178;
@@ -128,15 +171,20 @@ struct GroupBlockSums {
   double t, s, u, h;
 };
 
+// GATHER: dWb[j * stride] is the run sum of group j, d loglik / dv scaled by fac to d(-loglik)/dv; bad: NaN instead
+template <bool GATHER = false>
 __device__ __forceinline__ GroupBlockSums group_block_sums(const b2_glm_group_slope& b, int G, const float* zc,
-                                                           float* gc, const float* dWb, int lane) {
+                                                           float* gc, const float* dWb, int lane,
+                                                           int64_t stride = 1, double fac = 1.0, bool bad = false) {
   GroupBlockSums r;
   r.t = b.s_off >= 0 ? (double)zc[b.s_off] : 0.0;
   r.s = b.s_off >= 0 ? exp(r.t) : b.s_const;
   const double is2 = 1.0 / (r.s * r.s);
   double u = 0.0, h = 0.0;
   for (int j = lane; j < G; j += 32) {
-    const double v = (double)zc[b.b_off + j], g = (double)dWb[j];
+    const double v = (double)zc[b.b_off + j],
+                 g = GATHER ? (bad ? __longlong_as_double(0x7ff8000000000000ll) : fac * (double)dWb[j * stride])
+                            : (double)dWb[j];
     if (b.noncentred) {
       u += 0.5 * v * v + kHalfLog2Pi;
       h += r.s * v * g;
@@ -151,6 +199,88 @@ __device__ __forceinline__ GroupBlockSums group_block_sums(const b2_glm_group_sl
   r.u = warp_sum(u);
   r.h = warp_sum(h);
   return r;
+}
+
+// The gathered route's bookkeeping for chain c: each group's run sums (1 + S blocks) end up in gsum[k][g][c].  A group
+// inside one warpgroup's range is there already (and an empty one 0, from the pack); the runs of the at most 2 Q
+// slots (the first and last run of each range, in row order) are summed by group key here, with a segmented scan of
+// the warp in fp64 over 32 slots at a time, and written over their groups' entries.  The keys ascend along the slots
+// for sorted rows; whatever the rows, every read and write is in bounds.  Returns whether any range saw an index
+// outside [0, G) or a descending pair (status).
+struct GlmGatherFinish {
+  float* gsum;
+  const float* slots;
+  const int* status;
+  const int32_t* idx;
+  int cp, Q;
+  int64_t N;
+};
+
+__device__ __forceinline__ bool gather_fixup(const GlmGatherFinish& gf, int G, int S, int64_t c, int lane) {
+  constexpr unsigned kAll = 0xffffffffu;
+  int st = 0;
+  for (int q = lane; q < gf.Q; q += 32) st |= gf.status[q];
+  st = __reduce_or_sync(kAll, st);
+  const int64_t ntiles = (gf.N + 63) / 64;
+  const int ne = 2 * gf.Q;
+  double carry[4] = {0.0, 0.0, 0.0, 0.0};
+  int ckey = -1;
+  for (int e0 = 0; e0 < ne; e0 += 32) {
+    const int e = e0 + lane;
+    int key = -1;
+    double v[4] = {0.0, 0.0, 0.0, 0.0};
+    if (e < ne) {
+      int64_t t0, t1;
+      gather_tiles(e >> 1, gf.Q, ntiles, t0, t1);
+      if (t0 < t1) {                           // slot 0: the range's first run; slot 1: its last, if another
+        const int f = gf.idx[t0 * 64], l = gf.idx[(t1 * 64 < gf.N ? t1 * 64 : gf.N) - 1];
+        key = (e & 1) == 0 ? f : (f != l ? l : -1);
+        if (key < -1) key = -1;
+        if (key >= 0)
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            if (k <= S) v[k] = (double)gf.slots[((int64_t)e * 4 + k) * gf.cp + c];
+      }
+    }
+    // a slot without a run takes the key before it (they ascend) and adds nothing
+    if (lane == 0 && ckey > key) key = ckey;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_up_sync(kAll, key, o);
+      if (lane >= o && u > key) key = u;
+    }
+    // the previous chunk's last segment is complete when this chunk starts with another key
+    if (lane == 0 && key != ckey && (unsigned)ckey < (unsigned)G)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        if (k <= S) gf.gsum[((int64_t)k * G + ckey) * gf.cp + c] = (float)carry[k];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int ko = __shfl_up_sync(kAll, key, o);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const double vo = __shfl_up_sync(kAll, v[k], o);
+        if (lane >= o && ko == key) v[k] += vo;
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (key == ckey) v[k] += carry[k];
+    const int knext = __shfl_down_sync(kAll, key, 1);
+    if (lane < 31 && knext != key && (unsigned)key < (unsigned)G)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        if (k <= S) gf.gsum[((int64_t)k * G + key) * gf.cp + c] = (float)v[k];
+    ckey = __shfl_sync(kAll, key, 31);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) carry[k] = __shfl_sync(kAll, v[k], 31);
+  }
+  if (lane == 0 && (unsigned)ckey < (unsigned)G)
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (k <= S) gf.gsum[((int64_t)k * G + ckey) * gf.cp + c] = (float)carry[k];
+  __syncwarp();
+  return st != 0;
 }
 
 // lane 0: a group block's terms of U, G log s for a centred one last
@@ -169,17 +299,27 @@ __device__ __forceinline__ void add_group_block_u(const b2_glm_group_slope& b, i
 // and once per chain U += -log p(tau) - t, dU/dt = SUM_j a_j - tau (d log p / d tau)(tau) - 1.  Then come the bias
 // prior, the noise scale's terms and, with a group effect (GROUP: ge), its blocks: the intercept block's U terms
 // before the bias prior and its latent scale's after the noise scale's, then each slope block, in the order of k.
-// LATENT and GROUP are template flags, so each configuration runs only its own code.
-template <bool LATENT, bool GROUP>
-__global__ void __launch_bounds__(256) glm_potential_finish_kernel(
+// LATENT and GROUP are template flags, so each configuration runs only its own code.  GATHER (with GROUP): the
+// gathered route, KD = D, the group blocks' d loglik from gather_fixup's table times -1 (-1 / sigma_c^2 for linear
+// regression, as glm_finish_kernel scales dW), and U NaN for a bad index or a descending pair.
+template <bool LATENT, bool GROUP, bool GATHER = false>
+__device__ __forceinline__ void glm_potential_finish(
     const float* __restrict__ z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int KD, int Kb, double s_w,
     double s_b, const float* __restrict__ sum_p, const float* __restrict__ dW, const float* __restrict__ db,
     float* __restrict__ U, float* __restrict__ grad, const float* __restrict__ sig, const float* __restrict__ dsig,
-    int64_t s_off, int s_prior, double sp0, double sp1, b2_glm_weight_scale ws, b2_glm_group_effect ge) {
+    int64_t s_off, int s_prior, double sp0, double sp1, const b2_glm_weight_scale& ws, const b2_glm_group_effect& ge,
+    const GlmGatherFinish& gf) {
   const int64_t c = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (c >= C) return;
-  const int D = GROUP ? KD - ge.G * (1 + ge.S) : KD;
+  const int D = GROUP && !GATHER ? KD - ge.G * (1 + ge.S) : KD;
+  bool bad = false;
+  double gfac = 1.0;
+  if constexpr (GATHER) {
+    bad = gather_fixup(gf, ge.G, ge.S, c, lane);
+    const double sg = sig != nullptr ? (double)sig[c] : 1.0;
+    gfac = sig != nullptr ? -1.0 / (sg * sg) : -1.0;
+  }
   const double ib = Kb ? 1.0 / (s_b * s_b) : 0.0;
   const float* zc = z + c * Dz;
   float* gc = grad + c * Dz;
@@ -187,7 +327,8 @@ __global__ void __launch_bounds__(256) glm_potential_finish_kernel(
   const double t = LATENT && ws.tau_off >= 0 ? (double)zc[ws.tau_off] : 0.0;
   const b2_glm_group_slope icpt = {ge.a_off, ge.s_off, 0, ge.noncentred, ge.s_prior, ge.s_const, ge.sp0, ge.sp1};
   GroupBlockSums a = {};
-  if (GROUP) a = group_block_sums(icpt, ge.G, zc, gc, dWc + D, lane);
+  if (GATHER) a = group_block_sums<true>(icpt, ge.G, zc, gc, gf.gsum + c, lane, gf.cp, gfac, bad);
+  else if (GROUP) a = group_block_sums(icpt, ge.G, zc, gc, dWc + D, lane);
   // uw: SUM w^2 / s_w^2 for a constant weight scale, the weight and lam terms of U for a latent one; asum: SUM a_j;
   // qb: SUM b^2 / s_b^2
   double uw = 0.0, asum = 0.0, qb = 0.0;
@@ -233,28 +374,57 @@ __global__ void __launch_bounds__(256) glm_potential_finish_kernel(
   }
   for (int k = 0; GROUP && k < ge.S; ++k) {
     const b2_glm_group_slope& sl = ge.slope[k];
-    const GroupBlockSums b = group_block_sums(sl, ge.G, zc, gc, dWc + D + (k + 1) * ge.G, lane);
+    const GroupBlockSums b =
+        GATHER ? group_block_sums<true>(sl, ge.G, zc, gc, gf.gsum + (int64_t)(k + 1) * ge.G * gf.cp + c, lane, gf.cp,
+                                        gfac, bad)
+               : group_block_sums(sl, ge.G, zc, gc, dWc + D + (k + 1) * ge.G, lane);
     if (lane == 0) {
       add_group_block_u(sl, ge.G, b, u);
       if (sl.s_off >= 0) gc[sl.s_off] = (float)latent_scale_terms(sl.s_prior, sl.sp0, sl.sp1, b.t, b.h, u);
     }
   }
-  if (lane == 0) U[c] = (float)u;
+  if (lane == 0) U[c] = GATHER && bad ? __int_as_float(0x7fc00000) : (float)u;
+}
+
+template <bool LATENT, bool GROUP>
+__global__ void __launch_bounds__(256) glm_potential_finish_kernel(
+    const float* __restrict__ z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int KD, int Kb, double s_w,
+    double s_b, const float* __restrict__ sum_p, const float* __restrict__ dW, const float* __restrict__ db,
+    float* __restrict__ U, float* __restrict__ grad, const float* __restrict__ sig, const float* __restrict__ dsig,
+    int64_t s_off, int s_prior, double sp0, double sp1, b2_glm_weight_scale ws, b2_glm_group_effect ge) {
+  glm_potential_finish<LATENT, GROUP>(z, C, Dz, w_off, b_off, KD, Kb, s_w, s_b, sum_p, dW, db, U, grad, sig, dsig,
+                                      s_off, s_prior, sp0, sp1, ws, ge, {});
+}
+
+__global__ void __launch_bounds__(256) glm_potential_gather_finish_kernel(
+    const float* __restrict__ z, int64_t C, int64_t Dz, int64_t w_off, int64_t b_off, int D, int Kb, double s_w,
+    double s_b, const float* __restrict__ sum_p, const float* __restrict__ dW, const float* __restrict__ db,
+    float* __restrict__ U, float* __restrict__ grad, const float* __restrict__ sig, const float* __restrict__ dsig,
+    int64_t s_off, int s_prior, double sp0, double sp1, b2_glm_group_effect ge, GlmGatherFinish gf) {
+  const b2_glm_weight_scale no_scale = {-1, -1, 0, 0, 0.0, 0.0, 0.0, 0.0};
+  glm_potential_finish<false, true, true>(z, C, Dz, w_off, b_off, D, Kb, s_w, s_b, sum_p, dW, db, U, grad, sig, dsig,
+                                          s_off, s_prior, sp0, sp1, no_scale, ge, gf);
 }
 
 // the group columns of the likelihood's contraction, G (1 + S); 0 without a group effect
 inline int glm_group_cols(const b2_glm_regression& m) { return m.group ? m.group->G * (1 + m.group->S) : 0; }
 
+// a group effect past the contraction's 128 columns: the gathered route
+inline bool glm_gathered(const b2_glm_regression& m) { return m.group && m.D + glm_group_cols(m) > 128; }
+
 // The kinds and widths the likelihood kernels take (K == 1 except for softmax).  With a group effect: every kind
-// but softmax, any D with D + G (1 + S) <= 128 columns, and a constant weight scale.
+// but softmax, 1 <= D <= 128, 1 <= G <= 65536, a constant weight scale, and past D + G (1 + S) = 128 columns only
+// with the caller's promise that the rows are sorted by group, and not for Binomial regression (the gathered
+// route has no Binomial kernel).
 inline bool glm_regression_in_scope(const b2_glm_regression& m, int64_t C) {
   if (m.N < 1 || C < 1 || C >= ((int64_t)1 << 31)) return false;
   if (m.group) {
     const b2_glm_group_effect& g = *m.group;
-    if (m.scale || g.S < 0 || g.S > 3 || g.G < 1 || g.G > 128) return false;
+    if (m.scale || g.S < 0 || g.S > 3 || g.G < 1 || g.G > 65536 || (g.sorted != 0 && g.sorted != 1)) return false;
     return (m.kind == B2_GLM_BERNOULLI || m.kind == B2_GLM_POISSON || m.kind == B2_GLM_NORMAL ||
             m.kind == B2_GLM_BINOMIAL) &&
-           m.K == 1 && m.D >= 1 && m.D + glm_group_cols(m) <= 128;
+           m.K == 1 && m.D >= 1 && m.D <= 128 &&
+           (m.D + glm_group_cols(m) <= 128 || (g.sorted == 1 && m.kind != B2_GLM_BINOMIAL));
   }
   if (m.kind == B2_GLM_BERNOULLI) return m.K == 1 && (m.D == 4 || m.D == 8 || m.D == 16 || m.D == 32);
   if (m.kind == B2_GLM_CATEGORICAL) return m.D == 32 && m.K >= 2 && m.K <= 16;
@@ -264,18 +434,22 @@ inline bool glm_regression_in_scope(const b2_glm_regression& m, int64_t C) {
 }
 
 // workspace areas, each 256-byte aligned: [likelihood workspace][Wp][bp][dW][db][sum_p], then for linear
-// regression [sig][dsig]
+// regression [sig][dsig], then for the gathered route [tab][gsum][slots][status] (none grows with N past the
+// likelihood's CTA partials)
 struct GlmPotentialLayout {
-  size_t wp, bp, dw, db, sum_p, sig, dsig, total;
+  size_t wp, bp, dw, db, sum_p, sig, dsig, tab, gsum, slots, status, total;
+  int cp, Q;
 };
 
 inline size_t round256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 // the layout of an in-scope regression
 inline GlmPotentialLayout glm_potential_layout(const b2_glm_regression& m, int64_t C) {
-  const int Da = m.D + glm_group_cols(m);
+  const bool gathered = glm_gathered(m);
+  const int Da = gathered ? m.D : m.D + glm_group_cols(m);
   size_t lik_bytes;
-  switch (m.kind) {
+  if (gathered) lik_bytes = glm_row_workspace(m.N, m.D, (int)C);
+  else switch (m.kind) {
     case B2_GLM_BERNOULLI: lik_bytes = b2_glm_workspace(m.N, Da, (int)C); break;
     case B2_GLM_POISSON: lik_bytes = b2_glm_poisson_workspace(m.N, Da, (int)C); break;
     case B2_GLM_NORMAL: lik_bytes = b2_glm_normal_workspace(m.N, Da, (int)C); break;
@@ -283,7 +457,7 @@ inline GlmPotentialLayout glm_potential_layout(const b2_glm_regression& m, int64
     default: lik_bytes = b2_glm_categorical_workspace(m.N, Da, m.K, (int)C);
   }
   GlmPotentialLayout L;
-  const size_t kd = (size_t)m.K * m.D + glm_group_cols(m), k = (size_t)m.K, c = (size_t)C;
+  const size_t kd = (size_t)Da * m.K, k = (size_t)m.K, c = (size_t)C;
   size_t off = round256(lik_bytes);
   L.wp = off; off += round256(c * kd * sizeof(float));
   L.bp = off; off += round256(c * k * sizeof(float));
@@ -294,6 +468,17 @@ inline GlmPotentialLayout glm_potential_layout(const b2_glm_regression& m, int64
   if (m.kind == B2_GLM_NORMAL) {
     L.sig = off; off += round256(c * sizeof(float));
     L.dsig = off; off += round256(c * sizeof(float));
+  }
+  L.tab = L.gsum = L.slots = L.status = 0;
+  L.cp = L.Q = 0;
+  if (gathered) {
+    L.cp = (int)((C + 63) / 64 * 64);
+    L.Q = glm_gather_ranges(m.N, m.D);
+    const size_t table = (size_t)(1 + m.group->S) * m.group->G * L.cp * sizeof(float);
+    L.tab = off; off += round256(table);
+    L.gsum = off; off += round256(table);
+    L.slots = off; off += round256((size_t)L.Q * 2 * 4 * L.cp * sizeof(float));
+    L.status = off; off += round256((size_t)L.Q * sizeof(int));
   }
   L.total = off;
   return L;
@@ -411,8 +596,8 @@ extern "C" int b2_glm_potential(const b2_glm_regression* mp, const float* z, int
   const b2_glm_regression& m = *mp;
   const GlmPotentialLayout L = glm_potential_layout(m, C);
   if (!workspace || workspace_bytes < L.total) return B2_ERR_WORKSPACE;
-  const bool normal = m.kind == B2_GLM_NORMAL;
-  const int KD = m.K * m.D + glm_group_cols(m), Kb = m.has_bias ? m.K : 0;
+  const bool normal = m.kind == B2_GLM_NORMAL, gathered = glm_gathered(m);
+  const int KD = m.K * m.D + (gathered ? 0 : glm_group_cols(m)), Kb = m.has_bias ? m.K : 0;
   char* ws = reinterpret_cast<char*>(workspace);
   float* Wp = reinterpret_cast<float*>(ws + L.wp);
   float* bp = m.has_bias ? reinterpret_cast<float*>(ws + L.bp) : nullptr;
@@ -432,6 +617,35 @@ extern "C" int b2_glm_potential(const b2_glm_regression* mp, const float* z, int
     for (int k = 0; k < ge.S; ++k) grp.col[k] = ge.slope[k].col;
   }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+
+  if (gathered) {
+    GlmGather ga;
+    ga.idx = ge.groups;
+    ga.G = ge.G;
+    ga.S = ge.S;
+    for (int k = 0; k < ge.S; ++k) ga.col[k] = ge.slope[k].col;
+    ga.cp = L.cp;
+    float* tab = reinterpret_cast<float*>(ws + L.tab);
+    ga.tab = tab;
+    ga.gsum = reinterpret_cast<float*>(ws + L.gsum);
+    ga.slots = reinterpret_cast<float*>(ws + L.slots);
+    ga.status = reinterpret_cast<int*>(ws + L.status);
+    const int64_t npack = C * (KD + Kb) + (int64_t)(1 + ge.S) * ge.G * L.cp;
+    glm_potential_gather_pack_kernel<<<(unsigned)((npack + 255) / 256), 256, 0, s>>>(
+        z, C, Dz, m.w_off, m.b_off, KD, Kb, Wp, bp, m.s_off, (float)m.sigma, sig, ge, L.cp, tab, ga.gsum);
+    count_launch(1);
+    rc = check_launch();
+    if (rc != 0) return rc;
+    rc = glm_gather_likelihood(m.kind, m.X, static_cast<const float*>(m.y), Wp, bp, sig, dsig, m.N, m.D, (int)C,
+                               sum_p, dW, db, ws, s, ga);
+    if (rc != 0) return rc;
+    const GlmGatherFinish gf = {ga.gsum, ga.slots, ga.status, ge.groups, L.cp, L.Q, m.N};
+    glm_potential_gather_finish_kernel<<<(unsigned)((C * 32 + 255) / 256), 256, 0, s>>>(
+        z, C, Dz, m.w_off, m.b_off, KD, Kb, m.s_w, m.s_b, sum_p, dW, db, U, grad, sig, dsig, m.s_off, m.s_prior, m.sp0,
+        m.sp1, ge, gf);
+    count_launch(1);
+    return check_launch();
+  }
 
   const int64_t npack = C * (KD + Kb);
   const auto pack = m.group ? glm_potential_pack_kernel<true> : glm_potential_pack_kernel<false>;

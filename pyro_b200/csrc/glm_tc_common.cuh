@@ -447,6 +447,21 @@ __device__ __forceinline__ double cta_row_sum(int64_t N, F f) {
   return v;
 }
 
+// SUM f(n) over the rows r0 <= n < r1 (one contiguous span of the CTA's rows), as cta_row_sum
+template <int NT, class F>
+__device__ __forceinline__ double span_row_sum(int64_t r0, int64_t r1, F f) {
+  __shared__ double red[NT / 32];
+  double s = 0.0;
+  for (int64_t n = r0 + threadIdx.x; n < r1; n += NT) s += f(n);
+  s = warp_sum(s);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  double v = 0.0;
+#pragma unroll
+  for (int w = 0; w < NT / 32; ++w) v += red[w];
+  return v;
+}
+
 // ---- likelihood families of the GLM tile pipelines ----------------------------------------------------------
 // Fam is the likelihood family: kBiasInEpilogue (the bias is added by the epilogue, which then takes it after
 // acc1, instead of starting GEMM 1's accumulator), kKP (GEMM 1 rows per particle), kYBytes (labels of one
@@ -496,9 +511,13 @@ struct Poisson : Bernoulli {
   static constexpr bool kBiasInEpilogue = true;
   using LpAcc = double;
   static constexpr bool kDataTerm = true;
-  template <int NT>
-  static __device__ __forceinline__ double data_term(const float* __restrict__ y, const float*, int64_t N) {
-    return cta_row_sum<NT>(N, [&](int64_t n) { return log_factorial_f64(__ldg(y + n)); });
+  // SPAN: over the rows [r0, r1) instead of the CTA's round-robin tiles
+  template <int NT, bool SPAN = false>
+  static __device__ __forceinline__ double data_term(const float* __restrict__ y, const float*, int64_t N,
+                                                     int64_t r0 = 0, int64_t r1 = 0) {
+    auto f = [&](int64_t n) { return log_factorial_f64(__ldg(y + n)); };
+    if constexpr (SPAN) return span_row_sum<NT>(r0, r1, f);
+    else return cta_row_sum<NT>(N, f);
   }
   static __device__ __forceinline__ void tile_epilogue(const float (&acc1)[32], const float (&bias)[2],
                                                        const Labels& y, int64_t row0, int64_t N, int t4, bool last,

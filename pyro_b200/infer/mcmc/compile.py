@@ -213,19 +213,21 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
     site's scale equals the drawn ``tau``, ``lam`` or ``tau * lam`` at every probe.  Intercept-free logistic
     regression with a constant weight scale keeps LogisticPotential's route.
 
-    A varying intercept by group (every kind but softmax, with a constant weight scale, any D with D + G <= 128):
+    A varying intercept by group (every kind but softmax, with a constant weight scale, any D with D + G <= 128, or
+    past that with the rows sorted by group, D <= 128 and G <= 65536, but for Binomial regression):
     the group index is the one gradient-free int64 ``[N]`` tensor among the arguments, and the group effect a
     latent ``Normal`` site of shape ``(G,)``, tried after the model without one fails.  The probes decide the form:
     the observation's logits (log-rate, loc) equal ``X @ w + b + alpha[g]`` with ``alpha ~ Normal(0, s_a)``
     (centred), or ``X @ w + b + s_a * eta[g]`` with ``eta ~ Normal(0, 1)`` (non-centred), ``s_a`` a constant or a
     drawn positive scalar site, at every probe.  So how the model writes the gather does not matter.
 
-    Varying slopes (up to three, with a varying intercept, D + G (1 + S) <= 128): further latent ``Normal`` sites of
-    shape ``(G,)``, tried after the intercept-only model fails.  Slope k adds ``beta_k[g] * X[:, c_k]`` to the linear
-    predictor, ``beta_k`` centred or non-centred with its own constant or latent scale, as the intercept.  A probe
-    with only table k non-zero finds ``c_k``: the residual after ``X @ w + b + alpha[g]`` must be ``beta_k[g]`` times
-    a column of X (the lowest such column when columns repeat); then the three probes with every table drawn confirm
-    the whole sum.  So the covariate must be a column of X, whatever the model writes to take it."""
+    Varying slopes (up to three, with a varying intercept, D + G (1 + S) <= 128 or a sorted index): further latent
+    ``Normal`` sites of shape ``(G,)``, tried after the intercept-only model fails.  Slope k adds
+    ``beta_k[g] * X[:, c_k]`` to the linear predictor, ``beta_k`` centred or non-centred with its own constant or
+    latent scale, as the intercept.  A probe with only table k non-zero finds ``c_k``: the residual after
+    ``X @ w + b + alpha[g]`` must be ``beta_k[g]`` times a column of X (the lowest such column when columns repeat);
+    then the three probes with every table drawn confirm the whole sum.  So the covariate must be a column of X,
+    whatever the model writes to take it."""
     if len(observed) != 1 or not 1 <= len(latent) <= 11:
         return None
     (obs_name, obs), = observed.items()
@@ -281,13 +283,18 @@ def _try_glm(poutine, model, args, kwargs, latent, observed):
         # only sites with a group for every index: the probes gather with it
         lo, hi = int(ints[0].min()), int(ints[0].max())
         groups = [name for name, s in shapes.items() if len(s) == 1 and lo >= 0 and hi < s[0]]
-        attempts += [(a, ()) for a in groups if D + shapes[a][0] <= 128]
+        # the one-hot columns fit the contraction, or the rows are sorted by group (the gathered route)
+        ordered = bool((ints[0][1:] >= ints[0][:-1]).all())
+
+        def fits(G, S):
+            return D + G * (1 + S) <= 128 or (ordered and kind != "Binomial" and D <= 128 and G <= 65536)
+        attempts += [(a, ()) for a in groups if fits(shapes[a][0], 0)]
         # then with slopes: the other sites of the intercept's shape (when D == G, bar one that may be the weight)
         for a in groups:
             G = shapes[a][0]
             rest = [name for name in groups if name != a and shapes[name] == (G,)]
             sets = [rest] + ([[b for b in rest if b != w] for w in rest] if D == G else [])
-            attempts += [(a, tuple(b)) for b in sets if 1 <= len(b) <= 3 and D + G * (1 + len(b)) <= 128]
+            attempts += [(a, tuple(b)) for b in sets if 1 <= len(b) <= 3 and fits(G, len(b))]
     for group_site, slope_sites in attempts:
         pot = _glm_roles(poutine, model, args, kwargs, kind, obs_name, obs, order, positive, priors, latent, X, y,
                          scales, shapes, group_site, ints[0] if group_site is not None else None, slope_sites)

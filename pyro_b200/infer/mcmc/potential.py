@@ -133,10 +133,13 @@ class GlmPotential:
     site ``group["site"]``, drawn as ``Normal(0, s_a)`` (centred) or as ``eta ~ Normal(0, 1)`` with
     ``alpha = s_a * eta`` (``group["noncentred"]``).  ``s_a`` is the constant ``group["s_const"]`` or the positive
     scalar site ``group["s_site"]`` with prior ``group["s_prior"]`` (as ``sigma_prior``).  ``group["index"]`` must
-    lie in ``[0, G)``; a private int32 copy is made once.  The likelihood runs on ``[X | onehot(g)]``, so
-    ``D + G <= 128``.  ``group["slopes"]`` lists up to three varying slopes, each a dict with the keys of the intercept
-    (``site``, ``noncentred``, ``s_site``, ``s_const``, ``s_prior``) and ``col``: slope k adds
-    ``beta_k[g] * X[:, col]``, and each takes G more columns of the contraction, so ``D + G (1 + S) <= 128``.
+    lie in ``[0, G)``; a private int32 copy is made once.  ``group["slopes"]`` lists up to three varying slopes,
+    each a dict with the keys of the intercept (``site``, ``noncentred``, ``s_site``, ``s_const``, ``s_prior``) and
+    ``col``: slope k adds ``beta_k[g] * X[:, col]``.  Up to ``D + G (1 + S) <= 128`` columns the group effect is
+    more columns of the one contraction over ``[X | onehot(g) | X[:, col] onehot(g) ..]``.  Past that (up to
+    ``G <= 65536``) it is gathered per row and its gradient summed over each group's rows, which needs the rows
+    sorted by group: an index that is not non-decreasing raises ``ValueError`` there.  Sorting the rows of X, y
+    and the index by group once changes nothing in the posterior.
 
     ``value_and_grad`` is one ``b2_glm_potential`` call on the ``b2_glm_regression`` built once here
     (``regression``): the likelihood of all chains comes from one pass of the fused GLM kernel over X, the chains
@@ -230,11 +233,15 @@ class GlmPotential:
         g = group["index"].detach().to(self.device).reshape(-1)
         if g.numel() != self.n or g.is_floating_point():
             raise ValueError("the group index must be an integer tensor of shape [N]")
+        if G > 65536:
+            raise ValueError("at most 65536 groups")
         try:
             self.groups = group_index_int32(g, G)
         except IndexError as e:
             raise ValueError(str(e)) from None
         ge = N.b2_glm_group_effect()
+        # one check: the gathered route past 128 columns needs the rows sorted by group
+        ge.sorted = int(bool((self.groups[1:] >= self.groups[:-1]).all()))
         ge.groups = self.groups.data_ptr()
         ge.a_off, ge.G, ge.noncentred = sl.start, G, int(bool(group["noncentred"]))
         s_site = group.get("s_site")
@@ -258,6 +265,11 @@ class GlmPotential:
                 e.s_off, e.s_prior, e.sp0, e.sp1 = self.sites[sl["s_site"]][0].start, self._SIGMA_PRIORS[pk], p0, p1
             else:
                 e.s_off, e.s_const = -1, float(sl["s_const"])
+        if self.Dx + G * (1 + ge.S) > 128 and self.binomial:
+            raise ValueError("Binomial regression takes at most 128 columns (D + G (1 + S)) with a group effect")
+        if self.Dx + G * (1 + ge.S) > 128 and not ge.sorted:
+            raise ValueError("past 128 columns (D + G (1 + S) = %d) the rows must be sorted by group"
+                             % (self.Dx + G * (1 + ge.S)))
         return ge
 
     @property
