@@ -631,6 +631,38 @@ int b2_glm_group_slope_sum(int kind, const float* X, const float* y, const float
                            void* stream);
 size_t b2_glm_group_slope_sum_workspace(int kind, int64_t N, int D, int G, int S, int P);
 
+/*
+ * b2_glm_group_gather_sum -- the site sum of b2_glm_group_slope_sum's model (S = 0 without slopes) for any number of
+ * groups up to 65536, with the rows SORTED BY GROUP (groups non-decreasing; the caller's precondition):
+ *   eta[p,n] = <X[n,:], W[p,:]> + b[p] + alpha[p, groups[n]] + SUM_k beta_k[p, groups[n]] * X[n, col[k]]
+ * The contraction runs over X's D columns only; the group term is gathered from group-major tables and added to
+ * each logit in fp32, and the group gradients are summed over each run of rows of equal group, so past
+ * D + G (1 + S) = 128 columns X is still read once and no [P, N] tensor is written.  kind: B2_GLM_BERNOULLI,
+ * B2_GLM_POISSON or B2_GLM_NORMAL (Binomial and Categorical: B2_ERR_BAD_SHAPE).  X is always split hi + lo (every
+ * logit fp32-exact, at any N): B2_FLAG_GLM_3XTF32 changes nothing, and B2_FLAG_GLM_FP32 returns B2_ERR_BAD_SHAPE.
+ * Arguments as for b2_glm_group_slope_sum (no trial counts); slopes: NULL for none, or 0 <= S <= 3 with col[k]
+ * distinct in [0, D) and beta[k] non-null.  1 <= D <= 128, 1 <= G <= 65536, any D + G (1 + S) (narrow models are
+ * taken too), table strides 0 or >= G, N < 2^31, X, y and groups 16-byte aligned.
+ * Outputs: out_sum_p (nullable) [P], out_total, out_dW [P][D], out_db [P] (nullable b: not written), out_dsigma
+ * (Normal, nullable) as for b2_glm_normal_loc, and out_dT [1 + S][P][G]: block 0 d/dalpha, block k d/dbeta_k, each
+ * particle-major; every gradient is weight * scale * d loglik (Normal: d loglik already carries 1 / sigma_p^2), summed
+ * in fp64 and written in fp32, in a fixed order (deterministic, no float atomics).
+ * An index outside [0, G) or a descending pair anywhere makes out_total, every out_dT entry and out_sum_p NaN;
+ * nothing is read or written out of bounds.  Every argument is checked before any CUDA call, with
+ * b2_glm_group_slope_sum's codes.
+ * workspace: b2_glm_group_gather_sum_workspace() bytes, zero-initialised ONCE by the caller; it grows with G, S and P
+ * but not with N beyond the CTA partials.  Four launches with no host sync (CUDA graph capturable): the pack of W and
+ * the group-major tables, the kind's gather kernel, glm_finish_kernel (D wide) and the group finish, which writes
+ * out_dT.
+ */
+int b2_glm_group_gather_sum(int kind, const float* X, const float* y, const float* sigma, int sigma_stride,
+                            const int32_t* groups, int G, const float* W, int64_t w_stride, const float* alpha,
+                            int64_t alpha_stride, const b2_glm_slope_tables* slopes, const float* b, int64_t N, int D,
+                            int P, double scale, double weight, double sum_coeff, int flags, float* out_sum_p,
+                            float* out_total, float* out_dW, float* out_db, float* out_dsigma, float* out_dT,
+                            void* workspace, size_t workspace_bytes, void* stream);
+size_t b2_glm_group_gather_sum_workspace(int kind, int64_t N, int D, int G, int S, int P);
+
 /* ---- optimisers --------------------------------------------------------------------------
  * Multi-tensor fused updates replacing PyroOptim's per-parameter Python loop
  * (pyro/optim/optim.py:117-155).  Per-tensor scalar state lives in DEVICE arrays so a captured

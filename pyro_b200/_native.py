@@ -184,6 +184,10 @@ SIGNATURES = {
                                       ctypes.POINTER(b2_glm_slope_tables), _vp, _i64, _i32, _i32, _f64, _f64, _f64,
                                       _i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "b2_glm_group_slope_sum_workspace": (_sz, [_i32, _i64, _i32, _i32, _i32, _i32]),
+    "b2_glm_group_gather_sum": (_i32, [_i32, _vp, _vp, _vp, _i32, _vp, _i32, _vp, _i64, _vp, _i64,
+                                       ctypes.POINTER(b2_glm_slope_tables), _vp, _i64, _i32, _i32, _f64, _f64, _f64,
+                                       _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "b2_glm_group_gather_sum_workspace": (_sz, [_i32, _i64, _i32, _i32, _i32, _i32]),
     "b2_clipped_adam": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _vp]),
     "b2_adagrad_rmsprop": (_i32, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i64, _vp]),
     "b2_leapfrog_half_kick_drift": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _i32, _vp]),

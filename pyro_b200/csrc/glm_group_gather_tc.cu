@@ -2,7 +2,8 @@
 // columns of the contraction (D + G (1 + S) > 128): glm_flat_pipeline's GATHER mode (glm_flat_tc.cuh), GEMM 1 and
 // GEMM 2 over X's D columns, the group term alpha[g_n] + SUM_k beta_k[g_n] X[n, c_k] added to GEMM 1's logits on
 // the CUDA cores from group-major tables, and the group gradients summed over runs of rows of equal g (the rows
-// sorted by group).  Used by b2_glm_potential (glm_potential.cu), which always runs 3xTF32: X is split here.
+// sorted by group).  Used by b2_glm_potential (glm_potential.cu), which always runs 3xTF32, and by
+// b2_glm_group_gather_sum (glm_group.cu), the SVI site sum: X is split here.
 //
 // One kernel per family (Bernoulli, Poisson, Normal) and atom count DC of D; S is read at run time.  A call is the
 // kernel and glm_finish_kernel (D wide), with no host sync.  There is no Binomial kernel: instantiated on this
@@ -52,8 +53,9 @@ int glm_gather_ranges(int64_t N, int D) {
 }
 
 int glm_gather_likelihood(int kind, const float* X, const float* y, const float* W, const float* b,
-                          const float* sigma, float* dsigma, int64_t N, int D, int P, float* sum_p, float* dW,
-                          float* db, void* workspace, cudaStream_t s, const GlmGather& ga) {
+                          const float* sigma, int sigma_stride, float* dsigma, int64_t N, int D, int P, double scale,
+                          double weight, double sum_coeff, int flags, float* sum_p, float* total, float* dW, float* db,
+                          void* workspace, cudaStream_t s, const GlmGather& ga) {
   using namespace tc;
   const GlmRowWorkspace w = glm_row_areas(workspace, N, D, P);
   int rc;
@@ -64,13 +66,11 @@ int glm_gather_likelihood(int kind, const float* X, const float* y, const float*
     default: return B2_ERR_BAD_SHAPE;
   }
   if (rc != 0) return rc;
-  // the flags and noise-scale arguments of the kind's own likelihood call from the potential
   if (kind == B2_GLM_NORMAL)
-    launch_glm_finish(w.partials, w.ticket, w.gx, P, 1, D, 1.0, -1.0, 1.0, 0, sum_p, nullptr, dW, db, s, sigma, 1, N,
-                      dsigma);
+    launch_glm_finish(w.partials, w.ticket, w.gx, P, 1, D, scale, weight, sum_coeff, flags, sum_p, total, dW, db, s,
+                      sigma, sigma_stride, N, dsigma);
   else
-    launch_glm_finish(w.partials, w.ticket, w.gx, P, 1, D, 1.0, -1.0, 1.0, B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db,
-                      s);
+    launch_glm_finish(w.partials, w.ticket, w.gx, P, 1, D, scale, weight, sum_coeff, flags, sum_p, total, dW, db, s);
   count_launch(2);
   return check_launch();
 }

@@ -48,6 +48,116 @@ __host__ __device__ inline void gather_tiles(int q, int Q, int64_t ntiles, int64
   t1 = (int64_t)(q + 1) * ntiles / Q;
 }
 
+// The finishes' view of a gathered call (b2_glm_potential's and b2_glm_group_gather_sum's): each group's run sums
+// (1 + S blocks) end up in gsum[k][g][c].  A group inside one warpgroup's range is there already (and an empty one 0,
+// from the pack); a group that the first or last run of a range reaches is in the at most 2 Q slots, in row order,
+// and its value is the sum of the slots that carry its key (gather_slot_key).  status[Q] as in GlmGather.
+struct GlmGatherFinish {
+  float* gsum;
+  const float* slots;
+  const int* status;
+  const int32_t* idx;
+  int cp, Q;
+  int64_t N;
+};
+
+// The group key of slot e (0 <= e < 2 Q) of a gathered call, range e / 2 having the tiles [t0, t1), t0 < t1: slot
+// 2q is the first run of range q, slot 2q + 1 its last run if that is another group; -1 for a slot without a run (a
+// range of one run) and for a negative index.  The keys ascend along the slots for sorted rows; any rows are read
+// in bounds.
+__device__ __forceinline__ int gather_run_key(const GlmGatherFinish& gf, int e, int64_t t0, int64_t t1) {
+  const int f = gf.idx[t0 * 64], l = gf.idx[(t1 * 64 < gf.N ? t1 * 64 : gf.N) - 1];
+  const int key = (e & 1) == 0 ? f : (f != l ? l : -1);
+  return key < -1 ? -1 : key;
+}
+
+// the key of slot e over ntiles tiles, -1 for an empty range too
+__device__ __forceinline__ int gather_slot_key(const GlmGatherFinish& gf, int e, int64_t ntiles) {
+  int64_t t0, t1;
+  gather_tiles(e >> 1, gf.Q, ntiles, t0, t1);
+  return t0 < t1 ? gather_run_key(gf, e, t0, t1) : -1;
+}
+
+// The group at the row that places slot e among the slots, run or not: the first row of range e / 2 for even e, its
+// last row for odd e, and the first for both slots of an empty range (clamped to the last row of the data).  These
+// rows never descend along the slots, so for sorted rows the orders ascend, and a slot with a run has its key
+// (gather_slot_key) as its order: b2_glm_group_gather_sum's finish finds a group's slots by binary search on them.
+__device__ __forceinline__ int gather_slot_order(const GlmGatherFinish& gf, int e, int64_t ntiles) {
+  int64_t t0, t1;
+  gather_tiles(e >> 1, gf.Q, ntiles, t0, t1);
+  int64_t r = (e & 1) && t1 > t0 ? (t1 * 64 < gf.N ? t1 * 64 : gf.N) - 1 : t0 * 64;
+  if (r > gf.N - 1) r = gf.N - 1;
+  return gf.idx[r];
+}
+
+// The potential's bookkeeping for chain c (one warp): the slots are summed by group key with a segmented scan of the
+// warp in fp64 over 32 slots at a time, and written over their groups' entries of gsum.  Returns whether any range
+// saw an index outside [0, G) or a descending pair (status).
+__device__ __forceinline__ bool gather_fixup(const GlmGatherFinish& gf, int G, int S, int64_t c, int lane) {
+  constexpr unsigned kAll = 0xffffffffu;
+  int st = 0;
+  for (int q = lane; q < gf.Q; q += 32) st |= gf.status[q];
+  st = __reduce_or_sync(kAll, st);
+  const int64_t ntiles = (gf.N + 63) / 64;
+  const int ne = 2 * gf.Q;
+  double carry[4] = {0.0, 0.0, 0.0, 0.0};
+  int ckey = -1;
+  for (int e0 = 0; e0 < ne; e0 += 32) {
+    const int e = e0 + lane;
+    int key = -1;
+    double v[4] = {0.0, 0.0, 0.0, 0.0};
+    if (e < ne) {
+      int64_t t0, t1;
+      gather_tiles(e >> 1, gf.Q, ntiles, t0, t1);
+      if (t0 < t1) {
+        key = gather_run_key(gf, e, t0, t1);
+        if (key >= 0)
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            if (k <= S) v[k] = (double)gf.slots[((int64_t)e * 4 + k) * gf.cp + c];
+      }
+    }
+    // a slot without a run takes the key before it (they ascend) and adds nothing
+    if (lane == 0 && ckey > key) key = ckey;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_up_sync(kAll, key, o);
+      if (lane >= o && u > key) key = u;
+    }
+    // the previous chunk's last segment is complete when this chunk starts with another key
+    if (lane == 0 && key != ckey && (unsigned)ckey < (unsigned)G)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        if (k <= S) gf.gsum[((int64_t)k * G + ckey) * gf.cp + c] = (float)carry[k];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int ko = __shfl_up_sync(kAll, key, o);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const double vo = __shfl_up_sync(kAll, v[k], o);
+        if (lane >= o && ko == key) v[k] += vo;
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (key == ckey) v[k] += carry[k];
+    const int knext = __shfl_down_sync(kAll, key, 1);
+    if (lane < 31 && knext != key && (unsigned)key < (unsigned)G)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        if (k <= S) gf.gsum[((int64_t)k * G + key) * gf.cp + c] = (float)v[k];
+    ckey = __shfl_sync(kAll, key, 31);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) carry[k] = __shfl_sync(kAll, v[k], 31);
+  }
+  if (lane == 0 && (unsigned)ckey < (unsigned)G)
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (k <= S) gf.gsum[((int64_t)k * G + ckey) * gf.cp + c] = (float)carry[k];
+  __syncwarp();
+  return st != 0;
+}
+
 // ---- glm.cu ----
 // The second launch of every GLM likelihood call: glm_finish_kernel over the CTA partials [gx][P][K (D + 1) + 1].
 // The Normal noise scale sigma[p * sigma_stride] with n = N rows and out_dsigma are optional.  The per-particle sums
@@ -98,11 +208,13 @@ int glm_binomial_logits(const float* X, const float* y, const float* trials, int
 int glm_gather_ranges(int64_t N, int D);
 // The likelihood call of kind B2_GLM_BERNOULLI, B2_GLM_POISSON or B2_GLM_NORMAL with a gathered group effect (any
 // other kind: B2_ERR_BAD_SHAPE), X split (every logit fp32-exact): the kind's gather kernel and glm_finish_kernel,
-// D wide, with weight = -1 (dW, db, dsigma are derivatives of -loglik; the run sums of ga are d loglik / d T_k
-// before the finish's factor).  workspace: glm_row_workspace(N, D, P) bytes.
+// D wide, with the finish's scale, weight, sum_coeff, flags, total and noise scale sigma[p * sigma_stride] (Normal).
+// The run sums of ga are d loglik / d T_k before the finish's factor (weight * scale, and 1 / sigma_p^2 for Normal).
+// workspace: glm_row_workspace(N, D, P) bytes.
 int glm_gather_likelihood(int kind, const float* X, const float* y, const float* W, const float* b,
-                          const float* sigma, float* dsigma, int64_t N, int D, int P, float* sum_p, float* dW,
-                          float* db, void* workspace, cudaStream_t s, const GlmGather& ga);
+                          const float* sigma, int sigma_stride, float* dsigma, int64_t N, int D, int P, double scale,
+                          double weight, double sum_coeff, int flags, float* sum_p, float* total, float* dW, float* db,
+                          void* workspace, cudaStream_t s, const GlmGather& ga);
 
 // ---- glm_group.cu ----
 // The group kernel of kind B2_GLM_BERNOULLI, B2_GLM_POISSON or B2_GLM_BINOMIAL (row_trials: per-row counts m) with X

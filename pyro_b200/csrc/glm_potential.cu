@@ -201,88 +201,6 @@ __device__ __forceinline__ GroupBlockSums group_block_sums(const b2_glm_group_sl
   return r;
 }
 
-// The gathered route's bookkeeping for chain c: each group's run sums (1 + S blocks) end up in gsum[k][g][c].  A group
-// inside one warpgroup's range is there already (and an empty one 0, from the pack); the runs of the at most 2 Q
-// slots (the first and last run of each range, in row order) are summed by group key here, with a segmented scan of
-// the warp in fp64 over 32 slots at a time, and written over their groups' entries.  The keys ascend along the slots
-// for sorted rows; whatever the rows, every read and write is in bounds.  Returns whether any range saw an index
-// outside [0, G) or a descending pair (status).
-struct GlmGatherFinish {
-  float* gsum;
-  const float* slots;
-  const int* status;
-  const int32_t* idx;
-  int cp, Q;
-  int64_t N;
-};
-
-__device__ __forceinline__ bool gather_fixup(const GlmGatherFinish& gf, int G, int S, int64_t c, int lane) {
-  constexpr unsigned kAll = 0xffffffffu;
-  int st = 0;
-  for (int q = lane; q < gf.Q; q += 32) st |= gf.status[q];
-  st = __reduce_or_sync(kAll, st);
-  const int64_t ntiles = (gf.N + 63) / 64;
-  const int ne = 2 * gf.Q;
-  double carry[4] = {0.0, 0.0, 0.0, 0.0};
-  int ckey = -1;
-  for (int e0 = 0; e0 < ne; e0 += 32) {
-    const int e = e0 + lane;
-    int key = -1;
-    double v[4] = {0.0, 0.0, 0.0, 0.0};
-    if (e < ne) {
-      int64_t t0, t1;
-      gather_tiles(e >> 1, gf.Q, ntiles, t0, t1);
-      if (t0 < t1) {                           // slot 0: the range's first run; slot 1: its last, if another
-        const int f = gf.idx[t0 * 64], l = gf.idx[(t1 * 64 < gf.N ? t1 * 64 : gf.N) - 1];
-        key = (e & 1) == 0 ? f : (f != l ? l : -1);
-        if (key < -1) key = -1;
-        if (key >= 0)
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            if (k <= S) v[k] = (double)gf.slots[((int64_t)e * 4 + k) * gf.cp + c];
-      }
-    }
-    // a slot without a run takes the key before it (they ascend) and adds nothing
-    if (lane == 0 && ckey > key) key = ckey;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int u = __shfl_up_sync(kAll, key, o);
-      if (lane >= o && u > key) key = u;
-    }
-    // the previous chunk's last segment is complete when this chunk starts with another key
-    if (lane == 0 && key != ckey && (unsigned)ckey < (unsigned)G)
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        if (k <= S) gf.gsum[((int64_t)k * G + ckey) * gf.cp + c] = (float)carry[k];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int ko = __shfl_up_sync(kAll, key, o);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const double vo = __shfl_up_sync(kAll, v[k], o);
-        if (lane >= o && ko == key) v[k] += vo;
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-      if (key == ckey) v[k] += carry[k];
-    const int knext = __shfl_down_sync(kAll, key, 1);
-    if (lane < 31 && knext != key && (unsigned)key < (unsigned)G)
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        if (k <= S) gf.gsum[((int64_t)k * G + key) * gf.cp + c] = (float)v[k];
-    ckey = __shfl_sync(kAll, key, 31);
-#pragma unroll
-    for (int k = 0; k < 4; ++k) carry[k] = __shfl_sync(kAll, v[k], 31);
-  }
-  if (lane == 0 && (unsigned)ckey < (unsigned)G)
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-      if (k <= S) gf.gsum[((int64_t)k * G + ckey) * gf.cp + c] = (float)carry[k];
-  __syncwarp();
-  return st != 0;
-}
-
 // lane 0: a group block's terms of U, G log s for a centred one last
 __device__ __forceinline__ void add_group_block_u(const b2_glm_group_slope& b, int G, const GroupBlockSums& r,
                                                   double& u) {
@@ -636,8 +554,9 @@ extern "C" int b2_glm_potential(const b2_glm_regression* mp, const float* z, int
     count_launch(1);
     rc = check_launch();
     if (rc != 0) return rc;
-    rc = glm_gather_likelihood(m.kind, m.X, static_cast<const float*>(m.y), Wp, bp, sig, dsig, m.N, m.D, (int)C,
-                               sum_p, dW, db, ws, s, ga);
+    // the flags and noise-scale arguments of the kind's own likelihood call (glm_potential_likelihood)
+    rc = glm_gather_likelihood(m.kind, m.X, static_cast<const float*>(m.y), Wp, bp, sig, 1, dsig, m.N, m.D, (int)C,
+                               1.0, -1.0, 1.0, normal ? 0 : B2_FLAG_GLM_3XTF32, sum_p, nullptr, dW, db, ws, s, ga);
     if (rc != 0) return rc;
     const GlmGatherFinish gf = {ga.gsum, ga.slots, ga.status, ge.groups, L.cp, L.Q, m.N};
     glm_potential_gather_finish_kernel<<<(unsigned)((C * 32 + 255) / 256), 256, 0, s>>>(

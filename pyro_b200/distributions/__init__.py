@@ -1060,7 +1060,8 @@ class LinearPredictor:
     ``+ table[..., index] * X[:, col]``, with the group's index and G.  ``eager`` then computes the predictor the way
     the model wrote it, so that :meth:`dense` is that value bit for bit.  A consumer that does not score the group
     and the slopes (``_weights``) must not see such a predictor: it is scored by ``b2_glm_group_sum`` (an intercept)
-    or ``b2_glm_group_slope_sum`` (an intercept and slopes), or materialised (slopes without an intercept)."""
+    or ``b2_glm_group_slope_sum`` (an intercept and slopes), past 128 columns with a sorted index by
+    ``b2_glm_group_gather_sum``, or materialised (slopes without an intercept)."""
 
     def __init__(self, X, w, b=None, tensor_cores=True, group=None, eager=None, slopes=()):
         # latent values may arrive as lazy-aware SiteValue tensors (pyro_b200/lazy.py): score plain ones
@@ -1134,28 +1135,44 @@ class SlopeGather:
 
 
 # int32 copies of group indices for b2_glm_group_sum and GlmPotential: id(index) -> (weakref, _version, device, G,
-# copy).  A copy is built (one conversion, one host sync for its range check) the first time an index is scored, e.g.
-# in SVI's eager warm-up step, so a graph-captured step reuses it without a sync; a fresh index tensor every step
-# (subsampling) pays the conversion and the check every step.
+# copy, sorted).  A copy is built (one conversion, one host sync for its range check and for whether the index is
+# non-decreasing) the first time an index is scored, e.g. in SVI's eager warm-up step, so a graph-captured step reuses
+# it without a sync; a fresh index tensor every step (subsampling) pays the conversion and the check every step.
 _INDEX32 = {}
+
+
+def _index_entry(index, G):
+    key = id(index)
+    hit = _INDEX32.get(key)
+    if hit is not None and hit[0]() is index and hit[1:4] == (index._version, index.device, G):
+        return hit
+    if N.capturing():
+        return None
+    g = index.detach().reshape(-1)
+    # one host sync for both reductions
+    bad, descends = torch.stack([((g < 0) | (g >= G)).any(), (g[1:] < g[:-1]).any()]).tolist()
+    if bad:
+        raise IndexError("group index outside [0, %d)" % G)
+    copy = g.to(torch.int32, copy=True)
+    hit = (weakref.ref(index, lambda _, k=key: _INDEX32.pop(k, None)), index._version, index.device, G, copy,
+           not descends)
+    _INDEX32[key] = hit
+    return hit
 
 
 def group_index_int32(index, G):
     """The int32 copy of the int64 group index ``index`` ([N], any device), checked once against ``[0, G)``: an index
     outside raises IndexError before anything reads it.  None while a CUDA graph is captured and no copy exists yet
     (the check needs a host sync), so the caller can materialise instead."""
-    key = id(index)
-    hit = _INDEX32.get(key)
-    if hit is not None and hit[0]() is index and hit[1:4] == (index._version, index.device, G):
-        return hit[4]
-    if N.capturing():
-        return None
-    g = index.detach().reshape(-1)
-    if bool(((g < 0) | (g >= G)).any()):
-        raise IndexError("group index outside [0, %d)" % G)
-    copy = g.to(torch.int32, copy=True)
-    _INDEX32[key] = (weakref.ref(index, lambda _, k=key: _INDEX32.pop(k, None)), index._version, index.device, G, copy)
-    return copy
+    hit = _index_entry(index, G)
+    return None if hit is None else hit[4]
+
+
+def group_index_sorted(index, G):
+    """Whether the group index ``index`` is non-decreasing (the rows sorted by group), found in the same check and
+    cached with :func:`group_index_int32`'s copy; None while a CUDA graph is captured and nothing is cached yet."""
+    hit = _index_entry(index, G)
+    return None if hit is None else hit[5]
 
 
 def linear_predictor(X, w, b=None, tensor_cores=True):
@@ -1358,14 +1375,70 @@ def _glm_slope(meta, X, y, W, b, A, sigma, *B):
 _GlmSlopeFn = _FusedSum(_glm_slope)
 
 
+def _glm_gather(meta, X, y, W, b, sigma, *T):
+    scale, weight, coeff, _, kind, idx, s_stride, cols = meta
+    N.require_cuda(X, "fused multilevel-regression likelihood")
+    P, D = W.shape
+    G, S = T[0].shape[-1], len(T) - 1
+    n = X.shape[0]
+    dev = X.device
+    total = torch.empty((), dtype=torch.float32, device=dev)
+    dW = torch.empty((P, D), dtype=torch.float32, device=dev)
+    db = torch.empty(P, dtype=torch.float32, device=dev)
+    dT = torch.empty((1 + S, P, G), dtype=torch.float32, device=dev)   # d/dalpha, d/dbeta_1 .. per particle
+    dsig = torch.empty(P, dtype=torch.float32, device=dev) if sigma is not None and sigma.requires_grad else None
+    ws = N.workspace(dev, int(N.lib().b2_glm_group_gather_sum_workspace(kind, n, D, G, S, P)), tag="glm")
+    Wc, bc = W.contiguous(), b.contiguous() if b is not None else None
+    sc = sigma.contiguous() if sigma is not None else None
+    Tc = [t.contiguous() for t in T]
+    strides = [0 if t.numel() == G else G for t in Tc]   # one table row shared by every particle, or one per particle
+    sl = N.b2_glm_slope_tables(S)
+    for k in range(S):
+        sl.col[k], sl.beta[k], sl.beta_stride[k] = cols[k], Tc[k + 1].data_ptr(), strides[k + 1]
+    N.check(N.lib().b2_glm_group_gather_sum(
+        kind, X.data_ptr(), y.data_ptr(), _ptr(sc), s_stride, idx.data_ptr(), G, Wc.data_ptr(), D, Tc[0].data_ptr(),
+        strides[0], ctypes.byref(sl), _ptr(bc), n, D, P, float(scale), float(weight), float(coeff), 0, None,
+        total.data_ptr(), dW.data_ptr(), db.data_ptr(), _ptr(dsig), dT.data_ptr(), ws.data_ptr(), ws.numel(),
+        N.stream_ptr(dev)), "b2_glm_group_gather_sum")
+    dTs = tuple((dT[k].sum(0) if st == 0 else dT[k]).reshape(t.shape) for k, (t, st) in enumerate(zip(T, strides)))
+    if dsig is not None and s_stride == 0:
+        dsig = dsig.sum().reshape(sigma.shape)      # one sigma shared by every particle
+    return (total, None, None, dW, db if b is not None else None, dsig) + dTs
+
+
+_GlmGatherFn = _FusedSum(_glm_gather)
+
+
+def _gather_sum(kind, lp, value, mask, batch_shape, coeffs, sigma):
+    """The site sum of a predictor with a group effect (and up to three slopes) past 128 columns through
+    ``b2_glm_group_gather_sum``, or None outside its scope: :func:`_row_scope` at X's D columns, logistic, Poisson or
+    linear regression, G <= 65536, tables of X's dtype and device, and a cached index that is sorted (a subsample, or
+    any other unsorted index, materialises)."""
+    grp, slopes = lp.group, lp.slopes
+    D = lp.X.shape[-1]
+    rs = _row_scope(lp, value, mask, batch_shape, D)
+    tables = (grp.table,) + tuple(sg.table for sg in slopes)
+    if (rs is None or kind not in (N.GLM_BERNOULLI, N.GLM_POISSON, N.GLM_NORMAL) or grp.G > 65536
+            or any(t.dtype != torch.float32 or t.device != lp.X.device for t in tables)):
+        return None
+    idx = group_index_int32(grp.index, grp.G)
+    if idx is None or not group_index_sorted(grp.index, grp.G):
+        return None
+    W, b = lp.w.reshape(lp.P, D), lp.b.reshape(lp.P) if lp.b is not None else None
+    meta = coeffs + (kind, idx, sigma[1], tuple(sg.col for sg in slopes))
+    return _GlmGatherFn.apply(meta, *rs, W, b, sigma[0], *tables)
+
+
 def _slope_sum(kind, lp, value, mask, batch_shape, coeffs, trials=(None, 0), sigma=(None, 0)):
     """The site sum of a predictor with a group effect and varying slopes through ``b2_glm_group_slope_sum``, or None
     outside its scope: an intercept, :func:`_row_scope` at D + G (1 + S) columns, and tables of X's dtype and device.
-    An index outside ``[0, G)`` raises IndexError before any launch."""
+    Past 128 columns, :func:`_gather_sum`.  An index outside ``[0, G)`` raises IndexError before any launch."""
     grp, slopes = lp.group, lp.slopes
     if grp is None:
         return None                 # slopes without an intercept: the kernel always scores alpha, so materialise
     D = lp.X.shape[-1]
+    if D + grp.G * (1 + len(slopes)) > 128:
+        return _gather_sum(kind, lp, value, mask, batch_shape, coeffs, sigma)
     rs = _row_scope(lp, value, mask, batch_shape, D + grp.G * (1 + len(slopes)))
     tables = (grp.table,) + tuple(sg.table for sg in slopes)
     if rs is None or any(t.dtype != torch.float32 or t.device != lp.X.device for t in tables):
@@ -1381,11 +1454,14 @@ def _slope_sum(kind, lp, value, mask, batch_shape, coeffs, trials=(None, 0), sig
 def _group_sum(kind, lp, value, mask, batch_shape, coeffs, trials=(None, 0), sigma=(None, 0)):
     """The site sum of a predictor with a group effect through ``b2_glm_group_sum``, or None outside its scope:
     :func:`_row_scope` at D + G columns, and a table of X's dtype and device.  An index outside ``[0, G)`` raises
-    IndexError before any launch.  A predictor with slopes goes to :func:`_slope_sum`."""
+    IndexError before any launch.  A predictor with slopes goes to :func:`_slope_sum`, and past 128 columns to
+    :func:`_gather_sum`."""
     if lp.slopes:
         return _slope_sum(kind, lp, value, mask, batch_shape, coeffs, trials, sigma)
     grp = lp.group
     D = lp.X.shape[-1]
+    if D + grp.G > 128:
+        return _gather_sum(kind, lp, value, mask, batch_shape, coeffs, sigma)
     rs = _row_scope(lp, value, mask, batch_shape, D + grp.G)
     if rs is None or grp.table.dtype != torch.float32 or grp.table.device != lp.X.device:
         return None

@@ -19,7 +19,7 @@ from torch.distributions import biject_to
 
 from ... import _native as N
 from ... import poutine
-from ...distributions import group_index_int32, scale_and_mask
+from ...distributions import group_index_int32, group_index_sorted, scale_and_mask
 from ...primitives import plate
 
 
@@ -240,8 +240,8 @@ class GlmPotential:
         except IndexError as e:
             raise ValueError(str(e)) from None
         ge = N.b2_glm_group_effect()
-        # one check: the gathered route past 128 columns needs the rows sorted by group
-        ge.sorted = int(bool((self.groups[1:] >= self.groups[:-1]).all()))
+        # the gathered route past 128 columns needs the rows sorted by group (found by the same check)
+        ge.sorted = int(bool(group_index_sorted(g, G)))
         ge.groups = self.groups.data_ptr()
         ge.a_off, ge.G, ge.noncentred = sl.start, G, int(bool(group["noncentred"]))
         s_site = group.get("s_site")
